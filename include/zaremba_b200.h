@@ -227,6 +227,14 @@ int    zrb_dp_finish_step(zrb_dp* dp, void* stream);
  * process will write can deadlock when the two streams share a hardware work queue (observed: a 2-GPU run hung).  Use the
  * flag only from a stream that provably does not alias the launching stream's queue, or poll it from a kernel. */
 int  zrb_resident_flag(zrb_ctx* ctx, uint32_t** d_flag, uint32_t* next_value);
+/* The plans the persistent recurrence kernels of a tensor-core context run with, chosen at creation for its max_batch
+ * (so a smaller window reuses them) from the shape and the device's SM count.  h_out[0..7] = forward, h_out[8..15] =
+ * backward, each {ok, KS, U, G, nCTA, GBi, Kc, KcS}: ok = 0 means that direction takes the per-timestep path (the other
+ * seven are then 0); KS = CTAs sharing one set of gate rows, each holding 1/KS of the contraction (K-split); U = hidden
+ * units per CTA; G = 8-row groups of a CTA's weight slice; nCTA = grid size; GBi = 8-row batch groups of the operand
+ * images (the MMA's N is 8 * GBi); Kc = 8-element chunks of the contraction; KcS = Kc / KS.  ZRB_E_INVALID for a
+ * validation-engine context.  Host only, no synchronisation. */
+int  zrb_rec_plans(const zrb_ctx* ctx, int32_t* h_out);
 int  zrb_stream_wait_value32(void* stream, const uint32_t* d_flag, uint32_t value);
 
 /* perplexity's inner step (main.py:91-94) without materialising scores for the caller:

@@ -78,6 +78,7 @@ _SIGNATURES = {
     "zrb_check_health": (C.c_int, [_vp]),
     "zrb_resident_flag": (C.c_int, [_vp, C.POINTER(_vp), C.POINTER(C.c_uint32)]),
     "zrb_stream_wait_value32": (C.c_int, [_vp, _vp, C.c_uint32]),
+    "zrb_rec_plans": (C.c_int, [_vp, _vp]),
     "zrb_dp_create": (C.c_int, [C.c_int32, C.c_int32, C.c_int64, C.POINTER(_vp)]),
     "zrb_dp_destroy": (None, [_vp]),
     "zrb_dp_grad_buffer": (_vp, [_vp]),
@@ -99,6 +100,7 @@ _SIGNATURES = {
 
 PROF_CLASSES = ["embed_fwd", "gemm_in", "rec_fwd", "proj_fwd", "softmax", "proj_bwd", "rec_bwd", "gemm_dx",
                 "gemm_wgrad", "embed_bwd", "clip_sgd", "pack"]
+REC_PLAN_FIELDS = ["ok", "KS", "U", "G", "nCTA", "GBi", "Kc", "KcS"]
 
 _lib = None
 
@@ -138,3 +140,10 @@ def check(rc):
 def ptr(t):
     """Device pointer of a torch tensor (or None)."""
     return None if t is None else C.c_void_p(t.data_ptr())
+
+
+def rec_plans(ctx):
+    """zrb_rec_plans: {"fwd": {field: value}, "bwd": {...}} for a tensor-core context (fields: REC_PLAN_FIELDS)."""
+    out = (C.c_int32 * 16)()
+    check(load().zrb_rec_plans(ctx, out))
+    return {d: dict(zip(REC_PLAN_FIELDS, out[8 * i:8 * i + 8])) for i, d in enumerate(("fwd", "bwd"))}

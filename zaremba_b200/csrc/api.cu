@@ -341,6 +341,13 @@ int zrb_resident_flag(zrb_ctx* c, uint32_t** flag, uint32_t* next_value) {
     return ZRB_OK;
 }
 
+int zrb_rec_plans(const zrb_ctx* c, int32_t* h_out) {
+    ZRB_REQUIRE(c && h_out, "null argument");
+    ZRB_REQUIRE(c->cfg.engine == ZRB_ENGINE_TC && c->tc, "recurrence plans exist only in tensor-core contexts");
+    tc_rec_plans(c, h_out);
+    return ZRB_OK;
+}
+
 int zrb_set_embed_rows_out(zrb_ctx* c, float* rows) {
     ZRB_REQUIRE(c, "null ctx");
     c->embed_rows_out = rows;

@@ -473,6 +473,17 @@ int tc_train_step_layer(zrb_ctx* c, const zrb_params* p, const zrb_params* g, in
 
 bool tc_persistent_bwd(const zrb_ctx* c) { return c->tc && c->tc->bplan.ok; }
 
+void tc_rec_plans(const zrb_ctx* c, int32_t* h_out) {
+    const RecPlan* plans[2] = {&c->tc->fplan, &c->tc->bplan};
+    for (int d = 0; d < 2; ++d) {
+        const RecPlan& p = *plans[d];
+        int32_t* o = h_out + 8 * d;
+        o[0] = p.ok;
+        o[1] = p.ok ? p.KS : 0; o[2] = p.ok ? p.U : 0; o[3] = p.ok ? p.G : 0; o[4] = p.ok ? p.nCTA : 0;
+        o[5] = p.ok ? p.GBi : 0; o[6] = p.ok ? p.Kc : 0; o[7] = p.ok ? p.KcS : 0;
+    }
+}
+
 // ---- unit-level entry points: ONE recurrent layer through the persistent kernels (zrb_lstm_layer_fwd / _bwd) --------
 // They borrow layer slot 0 of the context (images, activations) and leave the model-level weight images stale, so the
 // next model-level call repacks.
