@@ -182,12 +182,11 @@ def test_fused_trainer_at_baseline_shapes(name, engine):
 
 @pytest.mark.parametrize("engine", ENGINES)
 def test_large_fused_trainer_philox_step_against_fp64_oracle(engine):
-    """BASELINE configs[2], train mode at p=0.65 with the library's own Philox masks (fetched through
-    zrb_dropout_mask and replayed into the fp64 oracle): loss, clip norm and every UPDATED weight tensor of the
+    """BASELINE configs[2], train mode at p=0.65 with the library's own Philox masks (the fp64 oracle gets the same
+    masks from the independent generator oracle/philox.py): loss, clip norm and every UPDATED weight tensor of the
     fused `Trainer` step, with a max_norm that makes the clip active."""
     import zaremba_b200
-    from zaremba_b200 import _lib
-    lib = _lib.load()
+    from oracle import philox as PH
     V, H, L, T, B, p = 10000, 1500, 2, 35, 20, 0.65
     torch.manual_seed(1)
     m = zaremba_b200.Model(V, H, L, p, 0.04, engine=engine).to(_dev())
@@ -200,11 +199,7 @@ def test_large_fused_trainer_philox_step_against_fp64_oracle(engine):
     max_norm, lr = 1.0, 1.0                            # the step's norm is ~1.9: coef ~0.53
     seed, step = tr.seed, tr.step
     loss, norm = tr.train_step(x.to(_dev()), y.to(_dev()), lr, max_norm)
-    masks = []
-    for site in range(L + 1):
-        buf = torch.empty(T * B * H, dtype=torch.uint8, device="cuda")
-        _lib.check(lib.zrb_dropout_mask(seed, step, site, T * B * H, p, _lib.ptr(buf), None))
-        masks.append(buf.cpu().numpy().reshape(T, B, H).astype(bool))
+    masks = PH.site_masks(seed, step, L, T, B, H, p)
     assert abs(np.mean([mk.mean() for mk in masks]) - (1 - p)) < 2e-3
     sc, st, cache = O.model_fwd(params, x.numpy(), O.zero_states(L, B, H, np.float64), L, p, masks)
     want_loss = O.nll_loss(sc, y.numpy())

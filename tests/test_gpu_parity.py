@@ -218,18 +218,21 @@ def test_lazy_update_equals_strict_update():
 def test_recurrence_launch_modes_agree():
     """The persistent recurrence kernels are launched as programmatic dependents of the GEMM before them while ONE
     tensor-core context is alive on the device, and cooperatively as soon as a second one exists (tc_common.cuh,
-    rec_launch_programmatic): both launches must give the same bits.  H = 256 takes the K-split (cluster) kernels."""
+    rec_launch_programmatic): both launches must give the same bits.  H = 256 takes the K-split (cluster) kernels.
+    Every window holds distinct tokens: a token that occurs three times would make the embedding scatter's fp32
+    atomics round differently from run to run, whatever the launch mode."""
     import gc
     import zaremba_b200
     V, H, L, T, B = 500, 256, 2, 9, 8
     g = torch.Generator().manual_seed(11)
-    d = torch.randint(0, V, (B, 3 * T + 1), generator=g)
+    xs = [torch.randperm(V, generator=g)[:T * B].view(T, B) for _ in range(3)]
+    ys = [torch.randint(0, V, (T, B), generator=g) for _ in range(3)]
 
     def run(tr):
         out = []
         for i in range(3):
-            x = d[:, i * T:(i + 1) * T].t().contiguous().to(_dev())
-            y = d[:, i * T + 1:(i + 1) * T + 1].t().contiguous().to(_dev())
+            x = xs[i].contiguous().to(_dev())
+            y = ys[i].contiguous().to(_dev())
             loss, norm = tr.train_step(x, y, 1.0, 0.25)
             out.append((loss.item(), norm.item()))
         tr.flush()
@@ -338,42 +341,6 @@ def test_clip_sgd_matches_oracle():
         for i, n in enumerate(names):
             np.testing.assert_allclose(pd[i].cpu().numpy(), pp[n], rtol=1e-5, atol=1e-7)
             np.testing.assert_allclose(gd[i].cpu().numpy(), gg[n], rtol=1e-5, atol=1e-9)
-
-
-@pytest.mark.parametrize("engine", ENGINES)
-def test_philox_dropout_masks_replay_in_oracle(engine):
-    """Train-mode step with the library's own Philox masks: fetch the masks through
-    zrb_dropout_mask, hand them to the oracle, compare scores and gradients; also check
-    the keep rate."""
-    from zaremba_b200 import _lib
-    import zaremba_b200
-    lib = _lib.load()
-    V, H, L, T, B, p = 97, 48, 2, 6, 5, 0.65
-    torch.manual_seed(21)
-    m = zaremba_b200.Model(V, H, L, p, 0.2, engine=engine).to(_dev())
-    m.train()
-    rng = np.random.default_rng(2)
-    x = torch.tensor(rng.integers(0, V, size=(T, B))); y = torch.tensor(rng.integers(0, V, size=(T, B)))
-    states = m.state_init(B)
-    scores, states = m(x, states)
-    loss = _caller_nll_loss(scores, y)
-    loss.backward()
-    seed, step = m._seed, m._drop_step - 1
-    masks = []
-    for site in range(L + 1):
-        buf = torch.empty(T * B * H, dtype=torch.uint8, device="cuda")
-        _lib.check(lib.zrb_dropout_mask(seed, step, site, T * B * H, p, _lib.ptr(buf), None))
-        masks.append(buf.cpu().numpy().reshape(T, B, H).astype(bool))
-    keep = np.mean([mk.mean() for mk in masks])
-    assert abs(keep - (1 - p)) < 0.03
-    assert not np.array_equal(masks[0], masks[1])
-    params = {k: v.detach().cpu().numpy().astype(np.float64) for k, v in m.named_parameters()}
-    sc, _, cache = O.model_fwd(params, x.numpy(), O.zero_states(L, B, H, np.float64), L, p, masks)
-    grads = O.model_bwd(params, cache, O.nll_loss_bwd(sc, y.numpy()), L)
-    tol = TOL[engine]
-    _scale_close(scores.detach().cpu().numpy(), sc, tol["fwd"], "scores (philox masks)")
-    for k, prm in m.named_parameters():
-        _scale_close(prm.grad.cpu().numpy(), grads[k], tol["grad"], f"grad {k}")
 
 
 @pytest.mark.parametrize("engine", ENGINES)
