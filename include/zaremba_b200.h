@@ -243,6 +243,41 @@ int  zrb_eval_step(zrb_ctx* ctx, const zrb_params* p, const int64_t* x, const in
                    int32_t T, int32_t B, const zrb_states* in, const zrb_states* out,
                    float* loss, float* tgt_prob, void* stream);
 
+/* ---- text generation (not in the reference: what a user of a trained model calls next) ----------------
+ * Sampling configuration: Gumbel-max over a kept set (DESIGN.md section 9 states it bit for bit).
+ *   temperature  tau >= 0; 0 = greedy: argmax of the scores, lowest index on ties, no uniforms drawn
+ *   top_k        keep the entries >= the k-th largest score (boundary ties kept); 0 or >= V = no filter
+ *   top_p        in (0, 1]: over the top-k set with p = softmax(z / tau), keep the entries >= v*, the largest score
+ *                whose set {z >= v*} holds at least top_p of the mass (boundary ties kept); 1 = no filter
+ *   seed         with (position, row, entry) the key and counter of the Philox4x32-10 uniforms */
+typedef struct {
+    float    temperature;
+    int32_t  top_k;
+    float    top_p;
+    int32_t  reserved;   /* 0 */
+    uint64_t seed;
+} zrb_sampling;
+
+/* One token per row of scores [B, ld] fp32 (row b at scores + b*ld, V used entries, finite -- not checked):
+ * tokens [B] int64, logprobs [B] fp32 = log softmax(scores[b])[token] at temperature 1 over all V entries (NULL: not
+ * written).  A pure function of (scores, cfg, pos, row): the uniforms of row b at position pos are fixed.  One CTA
+ * per row, no synchronisation.  ZRB_E_INVALID for temperature < 0, top_p <= 0, top_k < 0, B < 1, V < 1, V > 2^27, ld < V. */
+int  zrb_sample(const float* scores, int64_t ld, int32_t B, int32_t V, const zrb_sampling* cfg, uint64_t pos,
+                int64_t* tokens, float* logprobs, void* stream);
+
+/* Continue B prompts by n_new sampled tokens without leaving the device (no host synchronisation):
+ *   prefill  eval-mode forward of prompt [T0,B] int64 from `in` into `out`, in windows of at most max_seq steps;
+ *            only the last step's B rows are projected
+ *   step k   tokens[k] (and logprobs[k]) = zrb_sample of those scores at position pos0 + k; unless k = n_new - 1,
+ *            a T = 1 eval forward of tokens[k] (read on the device) carries out -> out
+ *   tokens [n_new,B] int64, logprobs [n_new,B] fp32 or NULL; in / out may alias.
+ * On return `out` is the state BEFORE the last sampled token is consumed: a second call with prompt = tokens[n_new-1],
+ * in = out and pos0 + n_new continues the same stream exactly.  Pending lazy weight updates are applied first; no
+ * dropout; nothing is kept for zrb_backward.  Both engines; B <= the context's max_batch, any T0. */
+int  zrb_generate(zrb_ctx* ctx, const zrb_params* p, const int64_t* prompt, int32_t T0, int32_t B,
+                  const zrb_states* in, const zrb_states* out, int32_t n_new, const zrb_sampling* cfg,
+                  uint64_t pos0, int64_t* tokens, float* logprobs, void* stream);
+
 /* Same as zrb_train_step_grads + zrb_train_step_update but with HOST token buffers
  * (pinned or pageable) and a host loss: the H2D copies of x, y and the D2H copy of the
  * loss are issued on `stream` inside the call; the call returns after the loss landed. */

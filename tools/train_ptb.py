@@ -62,12 +62,9 @@ if args.recipe:
 
 
 def data_init_text(root):                              # main.py:44-59
-    def read(name):
-        with open(os.path.join(root, name)) as f:
-            return f.read()[1:].split(" ")
-    trn, vld, tst = read("ptb.train.txt"), read("ptb.valid.txt"), read("ptb.test.txt")
-    words = sorted(set(trn))
-    w2i = {w: i for i, w in enumerate(words)}
+    from ptb_vocab import read_words, vocabulary
+    trn, vld, tst = (read_words(root, f"ptb.{s}.txt") for s in ("train", "valid", "test"))
+    words, w2i = vocabulary(trn)
     enc = lambda toks: np.array([w2i[w] for w in toks]).reshape(-1, 1)
     return enc(trn), enc(vld), enc(tst), len(words)
 

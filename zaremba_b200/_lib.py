@@ -35,6 +35,11 @@ class ZrbStates(C.Structure):
     _fields_ = [("h", _vp * MAX_LAYERS), ("c", _vp * MAX_LAYERS)]
 
 
+class ZrbSampling(C.Structure):
+    _fields_ = [("temperature", C.c_float), ("top_k", C.c_int32), ("top_p", C.c_float), ("reserved", C.c_int32),
+                ("seed", C.c_uint64)]
+
+
 class ZrbError(RuntimeError):
     pass
 
@@ -70,6 +75,9 @@ _SIGNATURES = {
                                         _vp, _vp]),
     "zrb_eval_step": (C.c_int, [_vp, C.POINTER(ZrbParams), _vp, _vp, C.c_int32, C.c_int32, C.POINTER(ZrbStates),
                                 C.POINTER(ZrbStates), _vp, _vp, _vp]),
+    "zrb_sample": (C.c_int, [_vp, C.c_int64, C.c_int32, C.c_int32, C.POINTER(ZrbSampling), C.c_uint64, _vp, _vp, _vp]),
+    "zrb_generate": (C.c_int, [_vp, C.POINTER(ZrbParams), _vp, C.c_int32, C.c_int32, C.POINTER(ZrbStates),
+                               C.POINTER(ZrbStates), C.c_int32, C.POINTER(ZrbSampling), C.c_uint64, _vp, _vp, _vp]),
     "zrb_train_step_host": (C.c_int, [_vp, C.POINTER(ZrbParams), C.POINTER(ZrbParams), _vp, _vp, C.c_int32,
                                       C.c_int32, C.POINTER(ZrbStates), C.POINTER(ZrbStates), C.c_uint64,
                                       C.c_uint64, C.c_float, C.c_float, _vp, _vp, _vp]),

@@ -407,6 +407,47 @@ int zrb_eval_step(zrb_ctx* c, const zrb_params* p, const int64_t* x, const int64
                        (cudaStream_t)stream);
 }
 
+int zrb_sample(const float* scores, int64_t ld, int32_t B, int32_t V, const zrb_sampling* cfg, uint64_t pos,
+               int64_t* tokens, float* logprobs, void* stream) {
+    return sample_rows(scores, ld, B, V, cfg, pos, tokens, logprobs, (cudaStream_t)stream);
+}
+
+// eval-mode forward of a [c->T, B] window; only the last step's B rows are projected (scores NULL: none)
+static int forward_last_rows(zrb_ctx* c, const zrb_params* p, const int64_t* x, const zrb_states* in,
+                             const zrb_states* out, float* scores, cudaStream_t s) {
+    if (c->cfg.engine == ZRB_ENGINE_TC) return tc_forward(c, p, x, in, out, scores, s, true);
+    return simt_forward(c, p, x, in, out, scores, s, true);
+}
+
+int zrb_generate(zrb_ctx* c, const zrb_params* p, const int64_t* prompt, int32_t T0, int32_t B, const zrb_states* in,
+                 const zrb_states* out, int32_t n_new, const zrb_sampling* cfg, uint64_t pos0, int64_t* tokens,
+                 float* logprobs, void* stream) {
+    ZRB_REQUIRE(c && p && prompt && in && out && tokens, "null argument");
+    ZRB_REQUIRE(T0 >= 1 && n_new >= 1, "T0=%d and n_new=%d must be >= 1", T0, n_new);
+    ZRB_TRY(check_shapes(c, 1, B));
+    ZRB_TRY(sample_check(cfg, B, c->cfg.vocab));
+    cudaStream_t s = (cudaStream_t)stream;
+    const int V = c->cfg.vocab, S = c->cfg.max_seq;
+    c->B = B; c->train = 0; c->seed = 0; c->step = 0;
+    c->have_fwd = false;
+    // prefill in windows of at most max_seq steps; only the last window projects (its last step)
+    const zrb_states* src = in;
+    for (int t0 = 0; t0 < T0; t0 += S) {
+        c->T = T0 - t0 < S ? T0 - t0 : S;
+        ZRB_TRY(forward_last_rows(c, p, prompt + (size_t)t0 * B, src, out, t0 + c->T == T0 ? c->scores : nullptr, s));
+        src = out;
+    }
+    // decode: sample from the scores of position pos0 + k, feed the token back as the next T = 1 window
+    c->T = 1;
+    for (int k = 0; k < n_new; ++k) {
+        int64_t* tok = tokens + (size_t)k * B;
+        ZRB_TRY(sample_rows(c->scores, V, B, V, cfg, pos0 + (uint64_t)k, tok, logprobs ? logprobs + (size_t)k * B : nullptr,
+                            s));
+        if (k + 1 < n_new) ZRB_TRY(forward_last_rows(c, p, tok, out, out, c->scores, s));
+    }
+    return ZRB_OK;
+}
+
 int zrb_train_step_host(zrb_ctx* c, const zrb_params* p, const zrb_params* g, const int64_t* h_x,
                         const int64_t* h_y, int32_t T, int32_t B, const zrb_states* in, const zrb_states* out,
                         uint64_t seed, uint64_t step, float lr, float max_norm, float* h_loss, float* h_norm,

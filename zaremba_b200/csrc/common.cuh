@@ -100,6 +100,32 @@ __host__ inline MaskSrc make_mask_src(const uint8_t* explicit_mask, uint64_t see
     return m;
 }
 
+// Uniforms of the sampler (zrb_sample): a pure function of (seed, pos, row b, vocabulary entry j).
+//   key     = (seed lo32, seed hi32 XOR pos hi32)
+//   counter = (j / 4, b, 0xFFFFFFFF, pos lo32); entry j reads word r[j % 4]
+//   u       = ((r >> 9) + 0.5) * 2^-23: exact in float32, strictly inside (0, 1)
+// Counter word 2 of a dropout mask is its site (<= ZRB_MAX_LAYERS), never 0xFFFFFFFF: the two streams cannot meet.
+struct SampleSrc {
+    uint32_t k0, k1, c3;
+};
+
+__host__ __device__ inline SampleSrc make_sample_src(uint64_t seed, uint64_t pos) {
+    SampleSrc s;
+    s.k0 = (uint32_t)seed;
+    s.k1 = (uint32_t)(seed >> 32) ^ (uint32_t)(pos >> 32);
+    s.c3 = (uint32_t)pos;
+    return s;
+}
+
+// the four words of entries [4*g, 4*g+3] of row b
+__host__ __device__ inline Philox4 sample_words(const SampleSrc& s, uint32_t g, uint32_t b) {
+    return philox4x32_10(g, b, 0xFFFFFFFFu, s.c3, s.k0, s.k1);
+}
+
+__host__ __device__ inline float sample_uniform(uint32_t r) {
+    return ((float)(r >> 9) + 0.5f) * 1.1920928955078125e-7f;   // 2^-23
+}
+
 // keep flags of the 4 consecutive elements [4*g, 4*g+3] packed in bits 0..3
 __device__ inline uint32_t mask_keep4(const MaskSrc& m, uint64_t g, uint64_t n_total) {
     if (m.explicit_mask) {

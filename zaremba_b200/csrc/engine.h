@@ -82,14 +82,15 @@ struct ProfScope {
     ~ProfScope();
 };
 
+// last_only: project only the last timestep's B rows into scores [B,V] (the decode loop of zrb_generate)
 int simt_forward(zrb_ctx* c, const zrb_params* p, const int64_t* x, const zrb_states* in, const zrb_states* out,
-                 float* scores, cudaStream_t s);
+                 float* scores, cudaStream_t s, bool last_only = false);
 int simt_backward(zrb_ctx* c, const zrb_params* p, const float* dscores, const zrb_params* g, cudaStream_t s);
 
 int tc_ctx_init(zrb_ctx* c);
 void tc_ctx_free(zrb_ctx* c);
 int tc_forward(zrb_ctx* c, const zrb_params* p, const int64_t* x, const zrb_states* in, const zrb_states* out,
-               float* scores, cudaStream_t s);
+               float* scores, cudaStream_t s, bool last_only = false);
 int tc_backward(zrb_ctx* c, const zrb_params* p, const float* dscores, const zrb_params* g, cudaStream_t s);
 int tc_train_step_grads(zrb_ctx* c, const zrb_params* p, const zrb_params* g, const int64_t* x, const int64_t* y,
                         int T, int B, const zrb_states* in, const zrb_states* out, uint64_t seed, uint64_t step,

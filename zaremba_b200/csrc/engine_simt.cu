@@ -7,7 +7,7 @@
 namespace zrb {
 
 int simt_forward(zrb_ctx* c, const zrb_params* p, const int64_t* x, const zrb_states* in, const zrb_states* out,
-                 float* scores, cudaStream_t s) {
+                 float* scores, cudaStream_t s, bool last_only) {
     const int H = c->cfg.hidden, L = c->cfg.layers, V = c->cfg.vocab, T = c->T, B = c->B, N = T * B;
     const size_t bh = (size_t)B * H * sizeof(float);
     ZRB_CUDA(cudaMemcpyAsync(c->x_saved, x, (size_t)N * sizeof(int64_t), cudaMemcpyDeviceToDevice, s));
@@ -42,8 +42,9 @@ int simt_forward(zrb_ctx* c, const zrb_params* p, const int64_t* x, const zrb_st
     }
     if (scores) {  // model.py:109
         ProfScope ps(c, ZRB_PROF_PROJ_FWD, s);
-        ZRB_TRY(gemm_f32(c->act[L], p->fc_w, scores, N, V, H, 0, 1, 1.f, 0.f, s));
-        ZRB_TRY(add_bias1(scores, p->fc_b, N, V, s));
+        const int rows = last_only ? B : N;
+        ZRB_TRY(gemm_f32(c->act[L] + (size_t)(N - rows) * H, p->fc_w, scores, rows, V, H, 0, 1, 1.f, 0.f, s));
+        ZRB_TRY(add_bias1(scores, p->fc_b, rows, V, s));
     }
     return ZRB_OK;
 }

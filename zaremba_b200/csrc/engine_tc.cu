@@ -191,7 +191,7 @@ int tc_flush_updates(zrb_ctx* c, cudaStream_t s) {
 }
 
 int tc_forward(zrb_ctx* c, const zrb_params* p, const int64_t* x, const zrb_states* in, const zrb_states* out,
-               float* scores, cudaStream_t s) {
+               float* scores, cudaStream_t s, bool last_only) {
     zrb_tc_state* t = c->tc;
     const int H = c->cfg.hidden, L = c->cfg.layers, V = c->cfg.vocab, T = c->T, B = c->B, N = T * B;
     const int Hp = t->Hp;
@@ -252,7 +252,9 @@ int tc_forward(zrb_ctx* c, const zrb_params* p, const int64_t* x, const zrb_stat
     }
     if (scores) {
         ProfScope ps(c, ZRB_PROF_PROJ_FWD, s);
-        ZRB_TRY(gemm_f16_tc(t->x_h[L], Hp, 0, t->fc_w_h, Hp, 0, scores, V, N, V, H, 1.f, p->fc_b, 0, s));
+        const int rows = last_only ? B : N;
+        ZRB_TRY(gemm_f16_tc(t->x_h[L] + (size_t)(N - rows) * Hp, Hp, 0, t->fc_w_h, Hp, 0, scores, V, rows, V, H, 1.f,
+                            p->fc_b, 0, s));
     }
     return ZRB_OK;
 }

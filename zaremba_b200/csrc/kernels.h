@@ -61,6 +61,13 @@ int sgd_apply(const TensorList& tl, float lr, const float* scalars, bool write_g
 int clip_sgd(const TensorList& tl, float lr, float max_norm, float* partials, float* scalars, float* norm_out,
              bool write_g, cudaStream_t s);
 
+// ---- sample.cu ---------------------------------------------------------------------------
+// ZRB_E_INVALID for the arguments zrb_sample rejects (checked before anything is enqueued)
+int sample_check(const zrb_sampling* cfg, int B, int V);
+// tokens[b] (and logprobs[b]) from row b of scores [B, ld]: one CTA per row
+int sample_rows(const float* scores, int64_t ld, int B, int V, const zrb_sampling* cfg, uint64_t pos, int64_t* tokens,
+                float* logprobs, cudaStream_t s);
+
 // ---- gemm_simt.cu ------------------------------------------------------------------------
 int gemm_f32(const float* A, const float* B, float* C, int M, int N, int K, int transA, int transB, float alpha,
              float beta, cudaStream_t s);

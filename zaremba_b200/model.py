@@ -178,6 +178,60 @@ class Model(nn.Module):
             states[i] = new_states[i]
         return scores, states
 
+    # ---- text generation (zrb_generate) ---------------------------------------------------
+    def generate(self, prompt, n_new, states=None, temperature=1.0, top_k=0, top_p=1.0, seed=None, pos=0):
+        """Continue the B columns of `prompt` ([T0,B] int64, CPU or CUDA) by `n_new` sampled tokens on the device.
+
+        Prefill and decode loop run in one library call without host synchronisation.  Always eval mode (no dropout,
+        whatever `.training` says), no autograd, and the dropout step is not advanced.  `states` (model layout, None =
+        zeros) enter before the prompt.  Sampling: see `zaremba_b200.sample`; the uniforms of step k are those of
+        position `pos + k`, and `seed=None` draws a seed from torch's global generator.
+
+        Returns (tokens [n_new,B] int64, logprobs [n_new,B] fp32, states).  The returned states are those BEFORE the
+        last token is consumed, so `generate(tokens[-1:], m, states, ..., seed=seed, pos=pos + n_new)` continues the
+        same stream.  The model's library context is reused, never replaced (that would drop a Trainer's pending
+        lazy updates): a B above its max_batch raises; a model without one gets a context for (min(T0, 64), B).
+        """
+        dev = self.embed.W.device
+        if dev.type != "cuda":
+            raise RuntimeError("zaremba_b200.Model runs on a CUDA device only (no CPU fallback): call .to('cuda')")
+        x = torch.as_tensor(prompt).to(device=dev, dtype=torch.int64).contiguous()
+        if x.dim() != 2 or x.numel() == 0:
+            raise ValueError(f"prompt must be a non-empty [T0,B] tensor, got shape {tuple(x.shape)}")
+        if int(n_new) < 1:
+            raise ValueError(f"n_new must be >= 1, got {n_new}")
+        T0, B = x.shape
+        if self._ctx is None:
+            ctx = self._context(min(T0, 64), B)
+        else:
+            ctx = self._ctx
+            if self._ctx_key[2] != dev.index:
+                raise RuntimeError("the model's library context belongs to another device")
+            if B > self._ctx_key[1]:
+                raise ValueError(f"generate: B={B} exceeds the model's library context (max_batch {self._ctx_key[1]}); "
+                                 "generate in batches of at most that many rows")
+        if seed is None:
+            seed = int(torch.randint(0, 2 ** 63 - 1, (1,)).item())
+        from .sampling import sampling_config
+        cfg = sampling_config(temperature, top_k, top_p, seed)
+        if states is None:
+            states = self.state_init(B)
+        lib = _lib.load()
+        with torch.no_grad():
+            self._note_param_versions()
+            ps, keep_w = self._params_struct(self._lib_weights())   # custom layout: permuted once per call
+            st_in, keep_in = self._states_struct(states)
+            shape = (B, self.hidden_size) if self.lstm_type == "custom" else (1, B, self.hidden_size)
+            out_states = [(torch.empty(shape, device=dev), torch.empty(shape, device=dev)) for _ in range(self.layer_num)]
+            st_out, keep_out = self._states_struct(out_states)
+            tokens = torch.empty(int(n_new), B, dtype=torch.int64, device=dev)
+            logprobs = torch.empty(int(n_new), B, dtype=torch.float32, device=dev)
+            with torch.cuda.device(dev):
+                _lib.check(lib.zrb_generate(ctx, C.byref(ps), _lib.ptr(x), T0, B, C.byref(st_in), C.byref(st_out),
+                                            int(n_new), C.byref(cfg), int(pos) & 0xFFFFFFFFFFFFFFFF, _lib.ptr(tokens),
+                                            _lib.ptr(logprobs), torch.cuda.current_stream(dev).cuda_stream))
+        return tokens, logprobs, out_states
+
     # ---- plumbing ------------------------------------------------------------------------
     def ordered_parameters(self):
         """The 3+4L tensors in registration order, as the library's zrb_params expects them
