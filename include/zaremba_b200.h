@@ -307,8 +307,8 @@ int  zrb_train_step_host(zrb_ctx* ctx, const zrb_params* p, const zrb_params* gr
 int  zrb_prof_enable(zrb_ctx* ctx, int32_t on);
 int  zrb_prof_read(zrb_ctx* ctx, float* h_ms, int64_t* h_counts);
 /* Phase timeline of the persistent recurrence kernels (clock64 stamps of CTA 0, 8 per step:
- * barrier seen, operand landed, MMAs issued, accumulator ready, partials received, cell math start/end,
- * arrival), preceded per kernel by 8 launch slots: CTA 0's clock64 at kernel entry / exit, its %globaltimer (ns)
+ * grid barrier seen, MMA chain start, accumulators out, accumulators seen by the cell warps, partial sums landed,
+ * cell math done, before / after the arrival; tools/rec_trace.py), preceded per kernel by 8 launch slots: CTA 0's clock64 at kernel entry / exit, its %globaltimer (ns)
  * at entry / exit, -(earliest CTA entry ns), latest CTA exit ns, 2 spare.  Needs ZRB_REC_TRACE=1 in the environment
  * at context creation.  Returns the number of entries written ([fwd|bwd][8 + T*8]) or a negative error. */
 int  zrb_prof_rec_trace(zrb_ctx* ctx, int64_t* h_out, int32_t max_entries);

@@ -23,7 +23,17 @@ n = _lib.load().zrb_prof_rec_trace(tr.ctx, buf, 2 * E)
 assert n == 2 * E, n
 raw = np.array(buf[:], dtype=np.int64).reshape(2, E)
 launch, a = raw[:, :8], raw[:, 8:].reshape(2, T, 8)
-names = ["barrier_seen", "operand_landed", "mma_issued", "acc_ready", "tmem_drained", "cells_begin/end", "pre_arrive", "arrived"]
+# the 8 clock64 stamps of a step (CTA 0), both kernels:
+#   barrier_seen     loader: the grid barrier of the step has passed, the operand copies are issued
+#   mma_start        MMA warpgroup: the first operand piece has landed, the wgmma chain starts
+#   acc_out          MMA warpgroup: chain drained, accumulators staged or pushed to their owners, arrival on bar_mma
+#   acc_seen         cell warps: bar_mma completed
+#   partials_landed  cell warps: every partial sum of this CTA's rows is in its shared memory (the K-split / cluster
+#                    exchange; right after acc_seen when there is none)
+#   cells_done       cell warps: cell math done, the next step's operand image stored
+#   pre_arrive       after the cell warps' named barrier
+#   arrived          after the release-add on the grid-barrier counter
+names = ["barrier_seen", "mma_start", "acc_out", "acc_seen", "partials_landed", "cells_done", "pre_arrive", "arrived"]
 out = {}
 for d, nm in enumerate(["fwd", "bwd"]):
     x = a[d][2:T - 1]                       # steady-state steps

@@ -96,7 +96,9 @@ template <int S>
 __global__ void __launch_bounds__(kRecThreads, 1) lstm_rec_bwd_kernel(RecBwdArgs a) {
     constexpr int CS = 4 * S;   // cluster size
     extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 127) & ~(uintptr_t)127);
+    // aligned by offsetting smem_raw itself: the compiler then knows every pointer below is a shared-memory one (LDS /
+    // STS, 32-bit addresses) -- a round trip through an integer would leave them generic
+    uint8_t* smem = smem_raw + ((128u - (smem_u32(smem_raw) & 127u)) & 127u);
     const int a_bytes = a.KcS * a.G * 128;     // this CTA's weight slice
     const int b_bytes = a.KcS * a.GBi * 128;   // the part of its gate's dG image this CTA multiplies with
     const int Bp = a.GBi * 8;                  // N of the MMA
@@ -177,27 +179,45 @@ __global__ void __launch_bounds__(kRecThreads, 1) lstm_rec_bwd_kernel(RecBwdArgs
         const int mt = S == 2 && UC > 64 ? 2 : 1;
         const bool push = S == 2 || a.push != 0;
         const uint32_t sR_addr = smem_u32(sR), bar_recv_addr = smem_u32(bar_recv);
+        // accumulator row = cluster-local unit.  Where each of this thread's (at most four) rows goes, worked out once:
+        // its first float in the staging buffer, or its receive row in the owner's shared memory and the owner's mbarrier
+        const int tm = (int)threadIdx.x - kRecMmaWarp * 32;
+        uint32_t row_dst[2][2], row_owner[2][2], row_bar[2][2];
+        bool row_ok[2][2];
+#pragma unroll
+        for (int m = 0; m < 2; ++m)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int row = rec_acc_row(tm, m, h);
+                if (!push) {
+                    row_dst[m][h] = (uint32_t)(row * ldd * 4);
+                    row_owner[m][h] = 0u; row_bar[m][h] = 0u; row_ok[m][h] = true;
+                } else {
+                    const int owner = row / a.U, uo = row - owner * a.U;
+                    row_ok[m][h] = row < UC;
+                    row_owner[m][h] = row_ok[m][h] ? (uint32_t)owner : 0u;   // (rows past the cluster's are never sent)
+                    row_dst[m][h] = sR_addr + (uint32_t)(((int)rank * a.U + uo) * ldr * 4);
+                    row_bar[m][h] = mapa_shared(bar_recv_addr, row_owner[m][h]);
+                }
+            }
         bool dead = false;
         bounded_mbar_wait(bar_a, 0, a.w, dead, kWaitWeights, 0);
         dead = rec_mma_any(dead);
-        // accumulator row = cluster-local unit
-        auto emit = [&](int row, int col, float v0, float v1) {
+        auto emit = [&](int m, int h, int col, float v0, float v1) {
             if (!push) {
-                float* dst = sD + row * ldd + col;
+                float* dst = (float*)((uint8_t*)sD + row_dst[m][h]) + col;
                 dst[0] = v0;
                 dst[1] = v1;
-            } else if (row < UC) {
+            } else if (row_ok[m][h]) {
                 // straight from the registers into the shared memory of the CTA that owns this unit
-                const int owner = row / a.U, uo = row - owner * a.U;
-                const uint32_t dst = mapa_shared(sR_addr + (uint32_t)((((int)rank * a.U + uo) * ldr + col) * 4), owner);
-                st_async_v2(dst, v0, v1, mapa_shared(bar_recv_addr, owner));
+                st_async_v2(mapa_shared(row_dst[m][h] + (uint32_t)col * 4u, row_owner[m][h]), v0, v1, row_bar[m][h]);
             }
         };
         for (int s = 1; s < T && !dead; ++s) {
             rec_mma_step(a.GBi, mt, a_addr, b_addr, lbo_a, lbo_b, ksteps, piece_steps, bar_b, (s - 1) & 1, a.w, dead, s,
                          tr ? &trs[s * 8 + 1] : nullptr, emit);
             if (!dead) mbar_arrive(bar_mma);
-            if (tr && threadIdx.x == kRecMmaWarp * 32) trs[s * 8 + 2] = clock64();
+            if (tr && tm == 0) trs[s * 8 + 2] = clock64();
         }
     } else if (warp < kRecEpiWarps) {
         pdl_wait();
@@ -206,9 +226,11 @@ __global__ void __launch_bounds__(kRecThreads, 1) lstm_rec_bwd_kernel(RecBwdArgs
         const int tid = threadIdx.x;
         bool dead = false;
         const int cells = a.U * B;                     // cell = b * U + u (u fastest: contiguous j)
+        int cb[kRecMaxCell];   // rec_cell
         float dcreg[kRecMaxCell], bsum[kRecMaxCell][4];
 #pragma unroll
         for (int k = 0; k < kRecMaxCell; ++k) {
+            cb[k] = (tid + kRecEpiThreads * k) / a.U;
             dcreg[k] = 0.f;
 #pragma unroll
             for (int q = 0; q < 4; ++q) bsum[k][q] = 0.f;
@@ -232,10 +254,8 @@ __global__ void __launch_bounds__(kRecThreads, 1) lstm_rec_bwd_kernel(RecBwdArgs
                 dyv[kRecMaxCell];
 #pragma unroll
             for (int k = 0; k < kRecMaxCell; ++k) {
-                int cell = tid + kRecEpiThreads * k;
-                int b = cell / a.U, u = cell % a.U;
-                bool ok = cell < cells && u < nu;
                 gi[k] = gf[k] = gg[k] = go[k] = ct[k] = cp[k] = dyv[k] = 0.f;
+                const auto [b, u, ok] = rec_cell(tid, k, cb[k], a.U, cells, nu);
                 if (ok) {
                     const int j = j0 + u;
                     const size_t n = (size_t)t * B + b;
@@ -253,7 +273,6 @@ __global__ void __launch_bounds__(kRecThreads, 1) lstm_rec_bwd_kernel(RecBwdArgs
                 if (tr && tid == 0) trs[s * 8 + 3] = clock64();   // staged partial / my pushes are out
                 if (!push) {
                     asm volatile("bar.sync 1, 256;" ::: "memory");
-                    if (tr && tid == 0) trs[s * 8 + 4] = clock64();
                     if (tid < 4) mbar_arrive_remote_release(mapa_shared(bar_part_addr, tid));
                     {   // wait until all four CTAs of the cluster staged their partials
                         uint32_t n = 0; long long t0 = 0;
@@ -262,17 +281,14 @@ __global__ void __launch_bounds__(kRecThreads, 1) lstm_rec_bwd_kernel(RecBwdArgs
                         }
                     }
                 } else {
-                    if (tr && tid == 0) trs[s * 8 + 4] = clock64();
                     bounded_mbar_wait(bar_recv, (s - 1) & 1, a.w, dead, kWaitRecv, s);   // all CS x U x Bp partial sums of my units have landed
                 }
+                if (tr && tid == 0) trs[s * 8 + 4] = clock64();
             }
-            if (tr && tid == 0) trs[s * 8 + 5] = clock64();
             __half hv[kRecMaxCell][4];
 #pragma unroll
             for (int k = 0; k < kRecMaxCell; ++k) {
-                int cell = tid + kRecEpiThreads * k;
-                int b = cell / a.U, u = cell % a.U;
-                bool ok = cell < cells && u < nu;
+                const auto [b, u, ok] = rec_cell(tid, k, cb[k], a.U, cells, nu);
                 if (!ok) continue;
                 float dh = dyv[k];
                 if (s > 0) {
@@ -311,18 +327,17 @@ __global__ void __launch_bounds__(kRecThreads, 1) lstm_rec_bwd_kernel(RecBwdArgs
                     bsum[k][q] += dg4[q];
                 }
             }
-            if (tr && tid == 0) trs[s * 8 + 6] = clock64();
+            if (tr && tid == 0) trs[s * 8 + 5] = clock64();
             asm volatile("bar.sync 1, 256;" ::: "memory");
             if (tid == 0) {
+                if (tr) trs[s * 8 + 6] = clock64();
                 grid_counter_arrive(a.counter);
                 if (tr) trs[s * 8 + 7] = clock64();
             }
             // off the critical path: row-major image for the batched dgrad / wgrad GEMMs
 #pragma unroll
             for (int k = 0; k < kRecMaxCell; ++k) {
-                int cell = tid + kRecEpiThreads * k;
-                int b = cell / a.U, u = cell % a.U;
-                bool ok = cell < cells && u < nu;
+                const auto [b, u, ok] = rec_cell(tid, k, cb[k], a.U, cells, nu);
                 if (!ok) continue;
                 __half* hrow = a.dG_h + ((size_t)t * B + b) * a.G4p + j0 + u;
 #pragma unroll
@@ -335,9 +350,8 @@ __global__ void __launch_bounds__(kRecThreads, 1) lstm_rec_bwd_kernel(RecBwdArgs
             // one thread per (gate, unit) of this CTA.  bar.sync orders the CTA's own global writes for its readers.
 #pragma unroll
             for (int k = 0; k < kRecMaxCell; ++k) {
-                int cell = tid + kRecEpiThreads * k;
-                int b = cell / a.U, u = cell % a.U;
-                if (cell < cells && u < nu) {
+                const auto [b, u, ok] = rec_cell(tid, k, cb[k], a.U, cells, nu);
+                if (ok) {
 #pragma unroll
                     for (int q = 0; q < 4; ++q) a.db_scratch[((size_t)q * B + b) * H + j0 + u] = bsum[k][q];
                 }

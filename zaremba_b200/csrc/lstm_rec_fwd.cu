@@ -78,7 +78,9 @@ __device__ __forceinline__ void fwd_cluster_sync() {
 template <bool SPLIT>
 __global__ void __launch_bounds__(kRecThreads, 1) lstm_rec_fwd_kernel(RecFwdArgs a) {
     extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 127) & ~(uintptr_t)127);
+    // aligned by offsetting smem_raw itself: the compiler then knows every pointer below is a shared-memory one (LDS /
+    // STS, 32-bit addresses) -- a round trip through an integer would leave them generic
+    uint8_t* smem = smem_raw + ((128u - (smem_u32(smem_raw) & 127u)) & 127u);
     const int a_bytes = a.KcS * a.G * 128;     // this CTA's weight slice
     const int b_bytes = a.KcS * a.GBi * 128;   // the part of the h image this CTA multiplies with
     const int Bp = a.GBi * 8;                  // N of the MMA
@@ -147,28 +149,47 @@ __global__ void __launch_bounds__(kRecThreads, 1) lstm_rec_fwd_kernel(RecFwdArgs
         const int rows_pair = 8 * a.U;                                   // K-split: gate rows of the pair (4 x 2U)
         const int mt = SPLIT && rows_pair > 64 ? 2 : 1;
         const uint32_t sR_addr = smem_u32(sR), bar_recv_addr = smem_u32(bar_recv);
+        // where each of this thread's (at most four) accumulator rows goes, worked out once: its first float in the
+        // staging buffer (no K split), or its receive row in the owner's shared memory and the owner's mbarrier (K split)
+        const int tm = (int)threadIdx.x - kRecMmaWarp * 32;
+        uint32_t row_dst[2][2], row_owner[2][2], row_bar[2][2];
+        bool row_ok[2][2];
+#pragma unroll
+        for (int m = 0; m < 2; ++m)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int row = rec_acc_row(tm, m, h);
+                if (!SPLIT) {
+                    row_dst[m][h] = (uint32_t)(row * ldd * 4);
+                    row_owner[m][h] = 0u; row_bar[m][h] = 0u; row_ok[m][h] = true;
+                } else {
+                    // row = 4 * (unit within the pair) + gate: straight into the shared memory of the owning CTA.
+                    // Receive rows are gate-major (q * U + u): the cell threads of a warp (consecutive u) then read
+                    // addresses ldr floats apart, 4 banks apart, instead of 4 * ldr (2 distinct banks: 16-way conflicts)
+                    const int up = row >> 2, owner = up / a.U, lrow = (row & 3) * a.U + (up - owner * a.U);
+                    row_ok[m][h] = row < rows_pair;
+                    row_owner[m][h] = row_ok[m][h] ? (uint32_t)owner : 0u;   // (rows past the pair's are never sent)
+                    row_dst[m][h] = sR_addr + (uint32_t)(((int)rank * 4 * a.U + lrow) * ldr * 4);
+                    row_bar[m][h] = fwd_mapa(bar_recv_addr, row_owner[m][h]);
+                }
+            }
         bool dead = false;
         bounded_mbar_wait(bar_a, 0, a.w, dead, kWaitWeights, 0);
         dead = rec_mma_any(dead);
-        auto emit = [&](int row, int col, float v0, float v1) {
+        auto emit = [&](int m, int h, int col, float v0, float v1) {
             if (!SPLIT) {
-                float* dst = sD + row * ldd + col;
+                float* dst = (float*)((uint8_t*)sD + row_dst[m][h]) + col;
                 dst[0] = v0;
                 dst[1] = v1;
-            } else if (row < rows_pair) {
-                // row = 4 * (unit within the pair) + gate: straight into the shared memory of the owning CTA.  Receive
-                // rows are gate-major (q * U + u): the cell threads of a warp (consecutive u) then read addresses ldr
-                // floats apart, 4 banks apart, instead of 4 * ldr (2 distinct banks: 16-way conflicts)
-                const int up = row >> 2, owner = up / a.U, lrow = (row & 3) * a.U + (up - owner * a.U);
-                const uint32_t dst = fwd_mapa(sR_addr + (uint32_t)((((int)rank * 4 * a.U + lrow) * ldr + col) * 4), owner);
-                st_async_v2(dst, v0, v1, fwd_mapa(bar_recv_addr, owner));
+            } else if (row_ok[m][h]) {
+                st_async_v2(fwd_mapa(row_dst[m][h] + (uint32_t)col * 4u, row_owner[m][h]), v0, v1, row_bar[m][h]);
             }
         };
         for (int t = 0; t < a.T && !dead; ++t) {
             rec_mma_step(a.GBi, mt, a_addr, b_addr, lbo_a, lbo_b, ksteps, piece_steps, bar_b, t & 1, a.w, dead, t,
                          tr ? &trs[t * 8 + 1] : nullptr, emit);
             if (!dead) mbar_arrive(bar_mma);
-            if (tr && threadIdx.x == kRecMmaWarp * 32) trs[t * 8 + 2] = clock64();
+            if (tr && tm == 0) trs[t * 8 + 2] = clock64();
         }
     } else if (warp < kRecEpiWarps) {
         pdl_wait();
@@ -179,12 +200,13 @@ __global__ void __launch_bounds__(kRecThreads, 1) lstm_rec_fwd_kernel(RecFwdArgs
         bool dead = false;
         const int cells = a.U * B;                     // cell = b * U + u (u fastest: contiguous j)
         const uint64_t n_total = (uint64_t)a.T * B * H;
+        int cb[kRecMaxCell];   // rec_cell
         float creg[kRecMaxCell];
 #pragma unroll
         for (int k = 0; k < kRecMaxCell; ++k) {
-            int cell = tid + kRecEpiThreads * k;
-            int b = cell / a.U, u = cell % a.U;
-            creg[k] = (cell < cells && u < nu) ? a.c0[(size_t)b * H + j0 + u] : 0.f;
+            cb[k] = (tid + kRecEpiThreads * k) / a.U;
+            const auto [b, u, ok] = rec_cell(tid, k, cb[k], a.U, cells, nu);
+            creg[k] = ok ? a.c0[(size_t)b * H + j0 + u] : 0.f;
         }
         const uint32_t recv_bytes = 2u * 4u * (uint32_t)a.U * (uint32_t)Bp * 4u;   // 2 sources x 4U rows x Bp columns
         for (int t = 0; t < a.T; ++t) {
@@ -193,23 +215,19 @@ __global__ void __launch_bounds__(kRecThreads, 1) lstm_rec_fwd_kernel(RecFwdArgs
             float pre[kRecMaxCell][4];
 #pragma unroll
             for (int k = 0; k < kRecMaxCell; ++k) {
-                int cell = tid + kRecEpiThreads * k;
-                int b = cell / a.U, u = cell % a.U;
-                bool ok = cell < cells && u < nu;
+                const auto [b, u, ok] = rec_cell(tid, k, cb[k], a.U, cells, nu);
 #pragma unroll
                 for (int q = 0; q < 4; ++q)
                     pre[k][q] = ok ? __ldg(a.gates + ((size_t)t * B + b) * 4 * H + (size_t)q * H + j0 + u) : 0.f;
             }
             bounded_mbar_wait(bar_mma, t & 1, a.w, dead, kWaitAcc, t);   // staged rows / my pushes are out
             if (tr && tid == 0) trs[t * 8 + 3] = clock64();
-            if (tr && tid == 0) trs[t * 8 + 4] = clock64();
             if (SPLIT) bounded_mbar_wait(bar_recv, t & 1, a.w, dead, kWaitRecv, t);   // both K halves of my 4U rows have landed
+            if (tr && tid == 0) trs[t * 8 + 4] = clock64();
             float o_i[kRecMaxCell], o_f[kRecMaxCell], o_g[kRecMaxCell], o_o[kRecMaxCell], o_h[kRecMaxCell];
 #pragma unroll
             for (int k = 0; k < kRecMaxCell; ++k) {
-                int cell = tid + kRecEpiThreads * k;
-                int b = cell / a.U, u = cell % a.U;
-                bool ok = cell < cells && u < nu;
+                const auto [b, u, ok] = rec_cell(tid, k, cb[k], a.U, cells, nu);
                 o_i[k] = o_f[k] = o_g[k] = o_o[k] = o_h[k] = 0.f;
                 if (!ok) continue;
                 float zi, zf, zg, zo;
@@ -248,9 +266,7 @@ __global__ void __launch_bounds__(kRecThreads, 1) lstm_rec_fwd_kernel(RecFwdArgs
             // off the critical path: what backward and the next layer read after this kernel
 #pragma unroll
             for (int k = 0; k < kRecMaxCell; ++k) {
-                int cell = tid + kRecEpiThreads * k;
-                int b = cell / a.U, u = cell % a.U;
-                bool ok = cell < cells && u < nu;
+                const auto [b, u, ok] = rec_cell(tid, k, cb[k], a.U, cells, nu);
                 if (!ok) continue;
                 const int j = j0 + u;
                 const size_t n = (size_t)t * B + b;

@@ -56,12 +56,16 @@ static __device__ __noinline__ void rec_give_up(unsigned int* flag, unsigned int
         __threadfence_system();
     }
 }
-// one slow-path visit of a spinning thread (every few thousand polls): true = stop waiting (for good)
-__device__ __forceinline__ bool rec_spin_check(const RecWatch& w, long long& t0, int kind, int step) {
+// one slow-path visit of a spinning thread (every few thousand polls): true = stop waiting (for good), because the word
+// is set or because this wait ran out -- the caller then reports it with rec_give_up (a no-op once the word is set)
+__device__ __forceinline__ bool rec_spin_expired(const RecWatch& w, long long& t0) {
     if (ld_relaxed_gpu(w.flag) != 0u) return true;
     const long long now = clock64();
     if (t0 == 0) { t0 = now; return false; }
-    if (now - t0 <= w.spin_cycles) return false;
+    return now - t0 > w.spin_cycles;
+}
+__device__ __forceinline__ bool rec_spin_check(const RecWatch& w, long long& t0, int kind, int step) {
+    if (!rec_spin_expired(w, t0)) return false;
     rec_give_up(w.flag, w.host, kind, step);
     return true;
 }
@@ -95,10 +99,33 @@ __device__ __forceinline__ bool rec_mma_any(bool v) {
     return r != 0;
 }
 
+// The accumulator row that register pair (mt, h) of MMA thread t (0..127) holds: each thread holds four rows at most,
+// so a kernel works out where each of them goes once, before its step loop (tc_common.cuh: wgmma_row).
+__device__ __forceinline__ int rec_acc_row(int t, int mt, int h) { return 64 * mt + wgmma_row(t, h); }
+
+// bounded_mbar_wait for the span where wgmmas are in flight: no call, no write to `dead`.  false = this thread stopped
+// waiting; the caller reports it with rec_give_up once nothing is in flight.
+__device__ __forceinline__ bool rec_chain_wait(uint64_t* bar, uint32_t parity, const RecWatch& w) {
+    uint32_t n = 0;
+    long long t0 = 0;
+    while (!mbar_try_wait(bar, parity)) {
+        if ((++n & 0xFFFu) == 0 && rec_spin_expired(w, t0)) return false;
+    }
+    return true;
+}
+
 // One step of the MMA warpgroup: D[64 MT x 8 NB] = A[64 MT rows x K] * B[8 NB x K]^T, K in ksteps steps of 16 that arrive
 // in kRecPieces pieces (bar_b[pc], phase `parity`).  Both operands are K-major in the canonical no-swizzle layout: 8x8
-// core matrices of 128 B, 8-row groups 128 B apart, the two K halves of a step lbo bytes apart.  Then emit(row, col, v0,
-// v1) for every accumulator pair (columns col, col + 1).  Returns with `dead` set (on every MMA thread) when a wait gave up.
+// core matrices of 128 B, 8-row groups 128 B apart, the two K halves of a step lbo bytes apart.  Then emit(mt, h, col,
+// v0, v1) for every accumulator pair (row rec_acc_row(t, mt, h), columns col, col + 1).  Returns with `dead` set (on
+// every MMA thread) when a wait gave up.
+//
+// The whole step is ONE asynchronous chain: the wgmmas go out back to back, and the only wait for them is the
+// wgmma_wait<0> before the accumulators are read.  ptxas serialises every wgmma (a wait after each) when it finds a
+// call or a branch it cannot prove warp-uniform between them while accumulators are live, so inside the chain: the
+// operand waits call nothing (rec_chain_wait), the warpgroup's vote is the only thing that decides whether the chain
+// goes on, and a warpgroup that gives up issues no further wgmma by running the remaining pieces with zero K steps
+// rather than by leaving the loop.  Everything that depends on one thread (the trace stamp, rec_give_up) is outside.
 template <int NB, int MT, class Emit>
 __device__ __forceinline__ void rec_mma_step_nb(uint32_t a_addr, uint32_t b_addr, uint32_t lbo_a, uint32_t lbo_b, int ksteps,
                                                 int piece_steps, uint64_t* bar_b, uint32_t parity, const RecWatch& w,
@@ -110,18 +137,18 @@ __device__ __forceinline__ void rec_mma_step_nb(uint32_t a_addr, uint32_t b_addr
 #pragma unroll
         for (int i = 0; i < R; ++i) d[mt][i] = 0.f;
     const int t = (int)threadIdx.x - kRecMmaWarp * 32;
-    bool issued = false;
-    for (int pc = 0; pc < kRecPieces; ++pc) {
-        bounded_mbar_wait(&bar_b[pc], parity, w, dead, kWaitOperand, step);
-        dead = rec_mma_any(dead);
-        if (dead) break;
-        if (pc == 0) {
-            if (stamp && t == 0) *stamp = clock64();
-            wgmma_fence();
+    bool lost = dead ? false : !rec_chain_wait(&bar_b[0], parity, w);
+    dead = rec_mma_any(dead || lost);
+    if (stamp && t == 0) *stamp = clock64();   // MMA start: the first piece has landed, nothing is in flight yet
+    wgmma_fence();
 #pragma unroll
-            for (int mt = 0; mt < MT; ++mt) wgmma_fence_acc(d[mt]);
+    for (int mt = 0; mt < MT; ++mt) wgmma_fence_acc(d[mt]);
+    for (int pc = 0; pc < kRecPieces; ++pc) {
+        if (pc > 0) {
+            if (!dead) lost = !rec_chain_wait(&bar_b[pc], parity, w);
+            dead = rec_mma_any(dead || lost);
         }
-        const int k0 = pc * piece_steps, k1 = min(ksteps, k0 + piece_steps);
+        const int k0 = pc * piece_steps, k1 = dead ? k0 : min(ksteps, k0 + piece_steps);
         for (int ks = k0; ks < k1; ++ks) {
             const uint64_t db = make_smem_desc(b_addr + ks * 2 * lbo_b, lbo_b, 128, kSwizzleNone);
 #pragma unroll
@@ -129,15 +156,13 @@ __device__ __forceinline__ void rec_mma_step_nb(uint32_t a_addr, uint32_t b_addr
                 const uint64_t da = make_smem_desc(a_addr + ks * 2 * lbo_a + mt * 1024, lbo_a, 128, kSwizzleNone);
                 Wgmma<NB * 8, 0, 0>::mma(d[mt], da, db, 1u);
             }
-            issued = true;
         }
     }
-    if (issued) {
-        wgmma_commit();
-        wgmma_wait<0>();
-    }
+    wgmma_commit();
+    wgmma_wait<0>();
 #pragma unroll
     for (int mt = 0; mt < MT; ++mt) wgmma_fence_acc(d[mt]);
+    if (lost) rec_give_up(w.flag, w.host, kWaitOperand, step);
     if (dead) return;
 #pragma unroll
     for (int mt = 0; mt < MT; ++mt)
@@ -145,14 +170,15 @@ __device__ __forceinline__ void rec_mma_step_nb(uint32_t a_addr, uint32_t b_addr
         for (int c8 = 0; c8 < NB; ++c8)
 #pragma unroll
             for (int h = 0; h < 2; ++h)
-                emit(64 * mt + wgmma_row(t, h), wgmma_col(t, c8), d[mt][4 * c8 + 2 * h], d[mt][4 * c8 + 2 * h + 1]);
+                emit(mt, h, wgmma_col(t, c8), d[mt][4 * c8 + 2 * h], d[mt][4 * c8 + 2 * h + 1]);
 }
 
-// the same with N = 8 nb (nb = 1..4: batch up to 32) and MT = mt 64-row tiles (1 or 2) chosen at run time
+// the same with N = 8 nb (nb = 1..4: batch up to 32) and MT = mt 64-row tiles (1 or 2) chosen at run time.  Inlined, so
+// that the kernel's arguments and `dead` stay in registers and the chain's bounds are known to be warp-uniform.
 template <class Emit>
-__device__ __noinline__ void rec_mma_step(int nb, int mt, uint32_t a_addr, uint32_t b_addr, uint32_t lbo_a, uint32_t lbo_b,
-                                          int ksteps, int piece_steps, uint64_t* bar_b, uint32_t parity, const RecWatch& w,
-                                          bool& dead, int step, long long* stamp, Emit emit) {
+__device__ __forceinline__ void rec_mma_step(int nb, int mt, uint32_t a_addr, uint32_t b_addr, uint32_t lbo_a, uint32_t lbo_b,
+                                             int ksteps, int piece_steps, uint64_t* bar_b, uint32_t parity, const RecWatch& w,
+                                             bool& dead, int step, long long* stamp, Emit& emit) {
 #define ZRB_REC_MMA(NB, MT) \
     rec_mma_step_nb<NB, MT>(a_addr, b_addr, lbo_a, lbo_b, ksteps, piece_steps, bar_b, parity, w, dead, step, stamp, emit)
     switch (nb + 4 * (mt - 1)) {
@@ -166,6 +192,16 @@ __device__ __noinline__ void rec_mma_step(int nb, int mt, uint32_t a_addr, uint3
     default: ZRB_REC_MMA(4, 2); break;
     }
 #undef ZRB_REC_MMA
+}
+
+// ---- the cell-math warps ----------------------------------------------------------------------------
+// Cell k of cell-math thread tid is cell = tid + kRecEpiThreads * k = b * U + u (u fastest: contiguous j); it exists when
+// cell < cells = U * B and u < nu (the CTA's last units may lie past H).  The kernels divide out b = cell / U once,
+// before their step loops (cb[k]); the unit then costs one multiply-add per use.
+struct RecCell { int b, u; bool ok; };
+__device__ __forceinline__ RecCell rec_cell(int tid, int k, int cb_k, int U, int cells, int nu) {
+    const int cell = tid + kRecEpiThreads * k, u = cell - cb_k * U;
+    return {cb_k, u, cell < cells && u < nu};
 }
 
 // 8 bytes into a peer CTA's shared memory; the bytes are counted on that CTA's mbarrier (complete_tx), so the reader
