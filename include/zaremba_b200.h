@@ -278,6 +278,36 @@ int  zrb_generate(zrb_ctx* ctx, const zrb_params* p, const int64_t* prompt, int3
                   const zrb_states* in, const zrb_states* out, int32_t n_new, const zrb_sampling* cfg,
                   uint64_t pos0, int64_t* tokens, float* logprobs, void* stream);
 
+/* ---- beam search (DESIGN.md section 10 states it bit for bit) ------------------------------------------
+ * Rows and slots: prompt b has K live hypotheses, slot k at row b*K + k; slot 0 is the best.  Per row r with scores z
+ * and cumulative score S_r: m = max z, L = logf(sum_j expf(z_j - m)) (zrb_sample's reductions), logp_j = (z_j - m) - L,
+ * candidate cand_j = S_r + logp_j (float32).  A row whose last token is eos (>= 0) is finished: its one candidate is
+ * j = eos with logp 0 and cand S_r.  The K best candidates of a prompt -- cand descending, ties by the lower flat index
+ * i*V + j, i the row's slot -- become the new slots 0..K-1 in that order. */
+#define ZRB_MAX_BEAMS    32
+
+/* One selection step: scores [B*K_in, ld] fp32 (finite, V used entries per row), cum_in [B*K_in] (NULL: all 0),
+ * tok_in [B*K_in] int64 the rows' last tokens (NULL: none finished).  K_in = K, or K_in = 1 with tok_in = NULL (step 0).
+ * Writes, per new slot (row b*K + k): tokens int64, parents int32 (the slot i it extends), cum_out (S) and logprobs
+ * (logp) fp32.  cum_in and cum_out may alias.  No synchronisation (the candidate scratch is stream-ordered).
+ * ZRB_E_INVALID for B < 1, V < 1, V > 2^26, K < 1, K > ZRB_MAX_BEAMS, K > V, eos outside [-1, V), ld < V, another K_in. */
+int  zrb_beam_step(const float* scores, int64_t ld, int32_t B, int32_t K_in, int32_t K, int32_t V, const float* cum_in,
+                   const int64_t* tok_in, int32_t eos, int64_t* tokens, int32_t* parents, float* cum_out,
+                   float* logprobs, void* stream);
+
+/* The K most likely continuations of B prompts by n_new tokens, without leaving the device (no host synchronisation):
+ *   prefill  eval-mode forward of prompt [T0,B] int64 from `in` (B rows) as zrb_generate, last step projected
+ *   step k   zrb_beam_step on those scores (step 0: B rows, S = 0), then row b*K + k takes its parent's (h, c) of every
+ *            layer; unless k = n_new - 1, a T = 1 eval forward of the B*K new tokens
+ *   tokens [n_new,B,K] int64, logprobs [n_new,B,K] fp32 (or NULL): the hypothesis in final slot k, traced back through
+ *   the parents (eos and 0 after an eos); scores [B,K] fp32 (or NULL): its S, the float32 sum of its logprobs in order.
+ * `out` (B*K rows) holds the states BEFORE each hypothesis's last token is consumed; in / out may alias.  Pending lazy
+ * weight updates are applied first; no dropout; nothing is kept for zrb_backward.  Both engines, any T0.
+ * ZRB_E_INVALID as zrb_beam_step, and for B*K above the context's max_batch, n_new < 1, T0 < 1. */
+int  zrb_beam_search(zrb_ctx* ctx, const zrb_params* p, const int64_t* prompt, int32_t T0, int32_t B,
+                     const zrb_states* in, const zrb_states* out, int32_t n_new, int32_t K, int32_t eos,
+                     int64_t* tokens, float* logprobs, float* scores, void* stream);
+
 /* Same as zrb_train_step_grads + zrb_train_step_update but with HOST token buffers
  * (pinned or pageable) and a host loss: the H2D copies of x, y and the D2H copy of the
  * loss are issued on `stream` inside the call; the call returns after the loss landed. */

@@ -5,6 +5,8 @@
     python tools/generate.py medium.pt --data DIR --prompt "the company said" -n 30 --top_p 0.9
     python tools/generate.py medium.pt --prompt_ids 12,7,401 --batch 4 --temperature 0.8 --top_k 40
     python tools/generate.py --shape large --batch 20 --time     # decode speed with random weights at a BASELINE shape
+    python tools/generate.py medium.pt --data DIR --prompt "the company" -n 20 --beams 8 --eos 0   # beam search
+    python tools/generate.py --shape large --batch 4 --beams 8 --time
 
 The checkpoint is a state_dict with the reference's key names (`train_ptb.py --save`); the model's shape and layout
 are read from it.  `--data` names the directory of ptb.train.txt: words are then mapped with the reference's
@@ -16,6 +18,12 @@ the device time achieves against the bytes a decode step must read -- the fp16 w
 (input and recurrent matrices of every layer, the projection), computed from the shapes -- together with the
 device's name and power limit.  It also times the sampler alone on a [B,V] score matrix (device time), to state its
 share of a step.
+
+--beams K runs `Model.beam_search` instead: the K most likely continuations of each prompt with their summed
+log-probabilities (`--eos ID` freezes a hypothesis at that token; in the PTB vocabulary '<eos>', the newline, is id 0).
+With --time the decode step covers one T = 1 forward of the B*K rows and the two beam kernels (top-K selection per
+row; merge per prompt with the state reorder), whose device time per step is taken from a torch.profiler trace of one
+search call.
 """
 import argparse
 import json
@@ -84,6 +92,8 @@ def main():
     ap.add_argument("--top_k", type=int, default=0)
     ap.add_argument("--top_p", type=float, default=1.0)
     ap.add_argument("--seed", type=int, default=0)
+    ap.add_argument("--beams", type=int, default=0, help="beam search with this many beams instead of sampling")
+    ap.add_argument("--eos", type=int, default=None, help="--beams: token id that ends a hypothesis")
     ap.add_argument("--engine", choices=["tc", "simt"], default="tc")
     ap.add_argument("--time", action="store_true", help="time the decode loop (CUDA events, after warm-up)")
     ap.add_argument("--steps", type=int, default=400, help="decode steps per timed call (--time)")
@@ -120,9 +130,11 @@ def main():
         ids = [w2i["<eos>"] if w2i and "<eos>" in w2i else 0]
     prompt = torch.tensor(ids, dtype=torch.int64).view(-1, 1).expand(-1, B).contiguous()
     kw = dict(temperature=args.temperature, top_k=args.top_k, top_p=args.top_p, seed=args.seed)
+    show = (lambda t: " ".join(words[i] for i in t)) if words else (lambda t: " ".join(map(str, t)))
+    if args.beams:
+        return beams(model, prompt, ids, args, show)
 
     tokens, logprobs, _ = model.generate(prompt, args.n_new, **kw)
-    show = (lambda t: " ".join(words[i] for i in t)) if words else (lambda t: " ".join(map(str, t)))
     for b in range(B):
         col = tokens[:, b].tolist()
         print(f"[{b}] {show(ids)} | {show(col)}   (mean log-prob {logprobs[:, b].mean().item():.3f})")
@@ -147,6 +159,53 @@ def main():
            "achieved_GB_per_s": round(nbytes / (device_step_ms * 1e-3) / 1e9, 1), "sampler_ms": round(sample_ms, 4),
            "sampler_share": round(sample_ms / device_step_ms, 4),
            "sampling": {k: v for k, v in kw.items() if k != "seed"}}
+    print(json.dumps(out))
+    if args.json:
+        os.makedirs(os.path.dirname(os.path.abspath(args.json)), exist_ok=True)
+        with open(args.json, "w") as f:
+            json.dump(out, f, indent=1)
+
+
+def beam_kernel_ms(model, prompt, n, K, eos):
+    """Device ms per decode step of the two beam kernels, from a torch.profiler trace of one search call."""
+    from torch.autograd import DeviceType
+    from torch.profiler import ProfilerActivity, profile
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        model.beam_search(prompt, n, K, eos=eos)
+        torch.cuda.synchronize()
+    us = {"row": 0.0, "merge": 0.0}
+    for e in prof.events():
+        for k in us:
+            if e.device_type == DeviceType.CUDA and f"beam_{k}_kernel" in e.name:
+                us[k] += e.time_range.elapsed_us()
+    return {k: v / 1e3 / n for k, v in us.items()}
+
+
+def beams(model, prompt, ids, args, show):
+    B, K = prompt.shape[1], args.beams
+    model._context(min(prompt.shape[0], 64), B * K)
+    tokens, logprobs, scores, _ = model.beam_search(prompt, args.n_new, K, eos=args.eos)
+    for b in range(B):
+        for k in range(K):
+            print(f"[{b}.{k}] {show(ids)} | {show(tokens[:, b, k].tolist())}   (score {scores[b, k].item():.3f})")
+    if not args.time:
+        return
+    n = args.steps
+    one = prompt[-1:]
+    for _ in range(3):                                        # warm-up: modules, weight images, plans, scratch
+        model.beam_search(one, n, K, eos=args.eos)
+    step_ms = event_ms(lambda: model.beam_search(one, n, K, eos=args.eos), 5) / n
+    device_step_ms = event_ms(lambda: model.beam_search(one, n, K, eos=args.eos), 1, hold=True) / n
+    kern = beam_kernel_ms(model, one, n, K, args.eos)
+    from zaremba_b200 import _lib
+    V, H, L = model.vocab_size, model.hidden_size, model.layer_num
+    out = {"device": torch.cuda.get_device_name(), "power_limit": power_limit(), "engine": args.engine,
+           "V": V, "H": H, "L": L, "B": B, "beams": K, "rows": B * K, "eos": args.eos, "decode_steps": n,
+           "persistent": bool(args.engine == "tc" and _lib.rec_plans(model._ctx)["fwd"]["ok"]),
+           "ms_per_step": round(step_ms, 4), "device_ms_per_step": round(device_step_ms, 4),
+           "beam_row_ms": round(kern["row"], 4), "beam_merge_ms": round(kern["merge"], 4),
+           "beam_share": round((kern["row"] + kern["merge"]) / device_step_ms, 4),
+           "step_bytes": weight_image_bytes(V, H, L) + B * K * V * 4}
     print(json.dumps(out))
     if args.json:
         os.makedirs(os.path.dirname(os.path.abspath(args.json)), exist_ok=True)

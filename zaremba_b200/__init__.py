@@ -4,10 +4,11 @@ ahmetumutdurmus/zaremba behind the reference's `model.Model` interface.
     from zaremba_b200 import Model            # drop-in for the reference's model.py
     from zaremba_b200 import Trainer          # fused train / eval step (main.py:109-117, :86-95)
     from zaremba_b200 import sample           # on-device top-k / top-p sampling (Model.generate: decode loop)
+    from zaremba_b200 import beam_step        # one on-device beam-search step (Model.beam_search: the whole search)
 """
 from .model import Model, Embed, LSTM, Linear  # noqa: F401
 from .trainer import Trainer, minibatch  # noqa: F401
-from .sampling import sample  # noqa: F401
+from .sampling import sample, beam_step  # noqa: F401
 from . import ensemble, parallel  # noqa: F401
 
-__all__ = ["Model", "Embed", "LSTM", "Linear", "Trainer", "minibatch", "sample"]
+__all__ = ["Model", "Embed", "LSTM", "Linear", "Trainer", "minibatch", "sample", "beam_step"]

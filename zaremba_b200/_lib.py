@@ -11,6 +11,7 @@ import os
 from . import build as _build
 
 MAX_LAYERS = 8
+MAX_BEAMS = 32
 ENGINE_SIMT = 0
 ENGINE_TC = 1
 
@@ -78,6 +79,10 @@ _SIGNATURES = {
     "zrb_sample": (C.c_int, [_vp, C.c_int64, C.c_int32, C.c_int32, C.POINTER(ZrbSampling), C.c_uint64, _vp, _vp, _vp]),
     "zrb_generate": (C.c_int, [_vp, C.POINTER(ZrbParams), _vp, C.c_int32, C.c_int32, C.POINTER(ZrbStates),
                                C.POINTER(ZrbStates), C.c_int32, C.POINTER(ZrbSampling), C.c_uint64, _vp, _vp, _vp]),
+    "zrb_beam_step": (C.c_int, [_vp, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _vp, _vp, C.c_int32, _vp,
+                                _vp, _vp, _vp, _vp]),
+    "zrb_beam_search": (C.c_int, [_vp, C.POINTER(ZrbParams), _vp, C.c_int32, C.c_int32, C.POINTER(ZrbStates),
+                                  C.POINTER(ZrbStates), C.c_int32, C.c_int32, C.c_int32, _vp, _vp, _vp, _vp]),
     "zrb_train_step_host": (C.c_int, [_vp, C.POINTER(ZrbParams), C.POINTER(ZrbParams), _vp, _vp, C.c_int32,
                                       C.c_int32, C.POINTER(ZrbStates), C.POINTER(ZrbStates), C.c_uint64,
                                       C.c_uint64, C.c_float, C.c_float, _vp, _vp, _vp]),

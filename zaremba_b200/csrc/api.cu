@@ -448,6 +448,81 @@ int zrb_generate(zrb_ctx* c, const zrb_params* p, const int64_t* prompt, int32_t
     return ZRB_OK;
 }
 
+int zrb_beam_step(const float* scores, int64_t ld, int32_t B, int32_t K_in, int32_t K, int32_t V, const float* cum_in,
+                  const int64_t* tok_in, int32_t eos, int64_t* tokens, int32_t* parents, float* cum_out, float* logprobs,
+                  void* stream) {
+    ZRB_TRY(beam_check(B, K, V, eos));
+    ZRB_REQUIRE(K_in >= 1 && K_in <= ZRB_MAX_BEAMS, "K_in=%d outside [1,%d]", K_in, ZRB_MAX_BEAMS);
+    cudaStream_t s = (cudaStream_t)stream;
+    BeamCand* cands = nullptr;   // stream-ordered scratch: no context here, and no synchronisation
+    ZRB_CUDA(cudaMallocAsync((void**)&cands, (size_t)B * K_in * K * sizeof(BeamCand), s));
+    const int rc = beam_step(scores, ld, B, K_in, K, V, cum_in, tok_in, eos, cands, tokens, parents, cum_out, logprobs,
+                             nullptr, nullptr, 0, 0, s);
+    ZRB_CUDA(cudaFreeAsync(cands, s));
+    return rc;
+}
+
+// zrb_beam_search's scratch (engine.h): the fixed part once, the per-step arrays grown to `entries`
+static int beam_scratch(zrb_ctx* c, int64_t entries) {
+    if (!c->beam_cand) {
+        const size_t BH = (size_t)c->cfg.max_batch * c->cfg.hidden;
+        float* st = nullptr;
+        ZRB_TRY(dalloc(c, &st, 4 * (size_t)c->cfg.layers * BH));
+        for (int l = 0; l < c->cfg.layers; ++l)
+            for (int k = 0; k < 2; ++k) {
+                c->beam_st[k].h[l] = st + (4 * l + 2 * k) * BH;
+                c->beam_st[k].c[l] = st + (4 * l + 2 * k + 1) * BH;
+            }
+        ZRB_TRY(dalloc(c, &c->beam_cum, (size_t)c->cfg.max_batch));
+        ZRB_TRY(dalloc(c, &c->beam_cand, (size_t)c->cfg.max_batch * ZRB_MAX_BEAMS));
+    }
+    if (entries > c->beam_cap) {   // (previous, smaller ones are kept until destroy)
+        ZRB_TRY(dalloc(c, &c->beam_tok, (size_t)entries));
+        ZRB_TRY(dalloc(c, &c->beam_par, (size_t)entries));
+        ZRB_TRY(dalloc(c, &c->beam_lp, (size_t)entries));
+        c->beam_cap = entries;
+    }
+    return ZRB_OK;
+}
+
+int zrb_beam_search(zrb_ctx* c, const zrb_params* p, const int64_t* prompt, int32_t T0, int32_t B, const zrb_states* in,
+                    const zrb_states* out, int32_t n_new, int32_t K, int32_t eos, int64_t* tokens, float* logprobs,
+                    float* scores, void* stream) {
+    ZRB_REQUIRE(c && p && prompt && in && out && tokens, "null argument");
+    ZRB_REQUIRE(T0 >= 1 && n_new >= 1, "T0=%d and n_new=%d must be >= 1", T0, n_new);
+    ZRB_TRY(beam_check(B, K, c->cfg.vocab, eos));
+    ZRB_REQUIRE((int64_t)B * K <= c->cfg.max_batch, "B*K=%lld above the context's max_batch %d", (long long)B * K,
+                c->cfg.max_batch);
+    ZRB_TRY(check_shapes(c, 1, B * K));
+    cudaStream_t s = (cudaStream_t)stream;
+    const int V = c->cfg.vocab, S = c->cfg.max_seq, L = c->cfg.layers, H = c->cfg.hidden, BK = B * K;
+    ZRB_TRY(beam_scratch(c, (int64_t)n_new * BK));
+    const zrb_states* fwd_out = &c->beam_st[0];   // the forward's output rows: B after the prefill, then B*K
+    const zrb_states* gathered = &c->beam_st[1];  // rows reordered by parent, the next forward's input
+    c->B = B; c->train = 0; c->seed = 0; c->step = 0;
+    c->have_fwd = false;
+    const zrb_states* src = in;
+    for (int t0 = 0; t0 < T0; t0 += S) {
+        c->T = T0 - t0 < S ? T0 - t0 : S;
+        ZRB_TRY(forward_last_rows(c, p, prompt + (size_t)t0 * B, src, fwd_out, t0 + c->T == T0 ? c->scores : nullptr, s));
+        src = fwd_out;
+    }
+    // step k: select from the scores of B*K_in rows, gather the parents' states; unless k = n_new - 1, a T = 1 forward
+    // of the new tokens.  The last gather goes straight to `out`.
+    c->T = 1;
+    c->B = BK;
+    for (int k = 0; k < n_new; ++k) {
+        const int K_in = k ? K : 1;
+        const size_t at = (size_t)k * BK;
+        const bool last = k + 1 == n_new;
+        ZRB_TRY(beam_step(c->scores, V, B, K_in, K, V, k ? c->beam_cum : nullptr, k ? c->beam_tok + at - BK : nullptr, eos,
+                          c->beam_cand, c->beam_tok + at, c->beam_par + at, c->beam_cum, c->beam_lp + at, fwd_out,
+                          last ? out : gathered, L, H, s));
+        if (!last) ZRB_TRY(forward_last_rows(c, p, c->beam_tok + at, gathered, fwd_out, c->scores, s));
+    }
+    return beam_backtrack(c->beam_tok, c->beam_par, c->beam_lp, c->beam_cum, n_new, BK, K, tokens, logprobs, scores, s);
+}
+
 int zrb_train_step_host(zrb_ctx* c, const zrb_params* p, const zrb_params* g, const int64_t* h_x,
                         const int64_t* h_y, int32_t T, int32_t B, const zrb_states* in, const zrb_states* out,
                         uint64_t seed, uint64_t step, float lr, float max_norm, float* h_loss, float* h_norm,

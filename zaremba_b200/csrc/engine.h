@@ -62,6 +62,15 @@ struct zrb_ctx {
     float* embed_rows_out = nullptr;       // if set: backward emits the embedding gradient as N masked rows here
                                            // instead of scattering into the dense table gradient (data parallel)
 
+    // zrb_beam_search scratch, allocated on first use; the per-step arrays grow with n_new * B * K
+    zrb::BeamCand* beam_cand = nullptr;    // [max_batch * ZRB_MAX_BEAMS] candidates of one step
+    float* beam_cum = nullptr;             // [max_batch] cumulative scores S
+    zrb_states beam_st[2] = {};            // [max_batch, H] per layer: the forward's output states / the gathered ones
+    int64_t* beam_tok = nullptr;           // [n_new, B*K] per-step tokens, parents and logprobs
+    int32_t* beam_par = nullptr;
+    float* beam_lp = nullptr;
+    int64_t beam_cap = 0;                  // entries of beam_tok / _par / _lp
+
     zrb_tc_state* tc = nullptr;
 
     // optional per-class event timing (zrb_prof_*)

@@ -68,6 +68,25 @@ int sample_check(const zrb_sampling* cfg, int B, int V);
 int sample_rows(const float* scores, int64_t ld, int B, int V, const zrb_sampling* cfg, uint64_t pos, int64_t* tokens,
                 float* logprobs, cudaStream_t s);
 
+// ---- beam.cu -----------------------------------------------------------------------------
+// one candidate of a beam step: cand = S + logp, flat = i*V + j (slot i of the previous step, token j)
+struct BeamCand {
+    float cand, logp;
+    uint32_t flat;
+};
+// ZRB_E_INVALID for the arguments zrb_beam_step / zrb_beam_search reject (B, beam width K, vocabulary V, eos)
+int beam_check(int B, int K, int V, int eos);
+// One selection step (DESIGN.md section 10) over B prompts of K_in rows of scores [B*K_in, ld]: cum_in [B*K_in] (NULL:
+// all 0), tok_in [B*K_in] (NULL: no row finished); outputs [B*K].  cands: B*K_in*K entries of scratch.  With L > 0 the
+// (h, c) rows of every layer are gathered from src (row b*K_in + parent) to dst (row b*K + k); src and dst must not
+// alias.  Two launches.
+int beam_step(const float* scores, int64_t ld, int B, int K_in, int K, int V, const float* cum_in, const int64_t* tok_in,
+              int eos, BeamCand* cands, int64_t* tokens, int32_t* parents, float* cum_out, float* logprobs,
+              const zrb_states* src, const zrb_states* dst, int L, int H, cudaStream_t s);
+// per-step [n_new, BK] tokens / parents / logprobs -> the hypotheses [n_new, B, K] of each final slot; scores = cum
+int beam_backtrack(const int64_t* step_tok, const int32_t* step_par, const float* step_lp, const float* cum, int n_new,
+                   int BK, int K, int64_t* tokens, float* logprobs, float* scores, cudaStream_t s);
+
 // ---- gemm_simt.cu ------------------------------------------------------------------------
 int gemm_f32(const float* A, const float* B, float* C, int M, int N, int K, int transA, int transB, float alpha,
              float beta, cudaStream_t s);

@@ -232,6 +232,60 @@ class Model(nn.Module):
                                             _lib.ptr(logprobs), torch.cuda.current_stream(dev).cuda_stream))
         return tokens, logprobs, out_states
 
+    def beam_search(self, prompt, n_new, beams, states=None, eos=None):
+        """The `beams` most likely continuations of each column of `prompt` ([T0,B] int64) by `n_new` tokens, ranked
+        by the float32 sum of their log-probabilities (zrb_beam_search; DESIGN.md section 10).
+
+        A hypothesis that emits `eos` is finished: it keeps its score, continues with eos at log-probability 0 and
+        stays in the ranking.  Raw sums favour short finished hypotheses; re-rank with the returned logprobs for a
+        length penalty.  Same rules as `generate`: eval mode, no autograd, the dropout step is not advanced, the context
+        is reused and never replaced (B * beams above its max_batch raises); a model without one gets a context for
+        (min(T0, 64), B * beams).  `states` (model layout, batch B, None = zeros) enter before the prompt.
+
+        Returns (tokens [n_new,B,K] int64, logprobs [n_new,B,K] fp32, scores [B,K] fp32, states): hypothesis k of
+        prompt b, best first; states have batch B*K, row b*K + k, and hold each hypothesis BEFORE its last token.
+        """
+        dev = self.embed.W.device
+        if dev.type != "cuda":
+            raise RuntimeError("zaremba_b200.Model runs on a CUDA device only (no CPU fallback): call .to('cuda')")
+        x = torch.as_tensor(prompt).to(device=dev, dtype=torch.int64).contiguous()
+        if x.dim() != 2 or x.numel() == 0:
+            raise ValueError(f"prompt must be a non-empty [T0,B] tensor, got shape {tuple(x.shape)}")
+        if int(n_new) < 1:
+            raise ValueError(f"n_new must be >= 1, got {n_new}")
+        K = int(beams)
+        if not 1 <= K <= min(_lib.MAX_BEAMS, self.vocab_size):
+            raise ValueError(f"beams must be in [1, {min(_lib.MAX_BEAMS, self.vocab_size)}], got {beams}")
+        T0, B = x.shape
+        if self._ctx is None:
+            ctx = self._context(min(T0, 64), B * K)
+        else:
+            ctx = self._ctx
+            if self._ctx_key[2] != dev.index:
+                raise RuntimeError("the model's library context belongs to another device")
+            if B * K > self._ctx_key[1]:
+                raise ValueError(f"beam_search: B*beams={B * K} exceeds the model's library context (max_batch "
+                                 f"{self._ctx_key[1]}); search fewer prompts at a time")
+        if states is None:
+            states = self.state_init(B)
+        lib = _lib.load()
+        with torch.no_grad():
+            self._note_param_versions()
+            ps, keep_w = self._params_struct(self._lib_weights())   # custom layout: permuted once per call
+            st_in, keep_in = self._states_struct(states)
+            shape = (B * K, self.hidden_size) if self.lstm_type == "custom" else (1, B * K, self.hidden_size)
+            out_states = [(torch.empty(shape, device=dev), torch.empty(shape, device=dev)) for _ in range(self.layer_num)]
+            st_out, keep_out = self._states_struct(out_states)
+            tokens = torch.empty(int(n_new), B, K, dtype=torch.int64, device=dev)
+            logprobs = torch.empty(int(n_new), B, K, dtype=torch.float32, device=dev)
+            scores = torch.empty(B, K, dtype=torch.float32, device=dev)
+            with torch.cuda.device(dev):
+                _lib.check(lib.zrb_beam_search(ctx, C.byref(ps), _lib.ptr(x), T0, B, C.byref(st_in), C.byref(st_out),
+                                               int(n_new), K, -1 if eos is None else int(eos), _lib.ptr(tokens),
+                                               _lib.ptr(logprobs), _lib.ptr(scores),
+                                               torch.cuda.current_stream(dev).cuda_stream))
+        return tokens, logprobs, scores, out_states
+
     # ---- plumbing ------------------------------------------------------------------------
     def ordered_parameters(self):
         """The 3+4L tensors in registration order, as the library's zrb_params expects them

@@ -1,4 +1,5 @@
-"""On-device sampling from a score matrix: `sample(scores, ...)` draws one token per row through zrb_sample.
+"""On-device sampling from a score matrix: `sample(scores, ...)` draws one token per row through zrb_sample, and
+`beam_step(scores, ...)` runs one selection step of a beam search through zrb_beam_step.
 
 The draw is Gumbel-max over a kept set (top-k, then top-p over the top-k set), a pure function of
 (scores, seed, pos, row): DESIGN.md section 9 states it bit for bit.  `Model.generate` runs the same kernel inside
@@ -42,3 +43,42 @@ def sample(scores, temperature=1.0, top_k=0, top_p=1.0, seed=0, pos=0):
         _lib.check(_lib.load().zrb_sample(_lib.ptr(s2), s2.stride(0), B, V, C.byref(cfg), int(pos) & 0xFFFFFFFFFFFFFFFF,
                                           _lib.ptr(tokens), _lib.ptr(logprobs), torch.cuda.current_stream(dev).cuda_stream))
     return (tokens[0], logprobs[0]) if squeeze else (tokens, logprobs)
+
+
+def beam_step(scores, beams, cum=None, last_tokens=None, eos=None):
+    """One beam-search selection step over the rows of `scores` ([B*K_in, V] fp32 CUDA tensor, finite).
+
+    cum None is the first step: one row per prompt, cumulative score 0, no last token.  Otherwise row b*K + i is slot i
+    of prompt b (K = `beams`), with cumulative score cum[row] and last token last_tokens[row] (None: no row is finished);
+    a row whose last token is `eos` only extends with eos at log-probability 0.  The `beams` best candidates of each
+    prompt -- S + logp descending, ties by the lower slot * V + token -- become its new slots in that order (DESIGN.md
+    section 10).
+    Returns (tokens int64, parents int32, cum fp32, logprobs fp32), each [B*beams].  No host synchronisation.
+    """
+    if not scores.is_cuda or scores.dtype != torch.float32 or scores.dim() != 2:
+        raise TypeError("beam_step() takes a [rows, V] fp32 CUDA tensor")
+    if scores.stride(1) != 1 or scores.stride(0) < scores.size(1):
+        scores = scores.contiguous()
+    R, V = scores.shape
+    K = int(beams)
+    if cum is None and last_tokens is not None:
+        raise ValueError("the first step (cum None) has no last tokens")
+    K_in = 1 if cum is None else K
+    if R % K_in:
+        raise ValueError(f"{R} rows are not a whole number of prompts of {K_in} slots")
+    B = R // K_in
+    dev = scores.device
+    if cum is not None:
+        cum = cum.to(device=dev, dtype=torch.float32).contiguous()
+    if last_tokens is not None:
+        last_tokens = last_tokens.to(device=dev, dtype=torch.int64).contiguous()
+    tokens = torch.empty(B * K, dtype=torch.int64, device=dev)
+    parents = torch.empty(B * K, dtype=torch.int32, device=dev)
+    cum_out = torch.empty(B * K, dtype=torch.float32, device=dev)
+    logprobs = torch.empty(B * K, dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(_lib.load().zrb_beam_step(_lib.ptr(scores), scores.stride(0), B, K_in, K, V, _lib.ptr(cum),
+                                             _lib.ptr(last_tokens), -1 if eos is None else int(eos), _lib.ptr(tokens),
+                                             _lib.ptr(parents), _lib.ptr(cum_out), _lib.ptr(logprobs),
+                                             torch.cuda.current_stream(dev).cuda_stream))
+    return tokens, parents, cum_out, logprobs
