@@ -98,6 +98,19 @@ int  zrb_dropout_mask(uint64_t seed, uint64_t step, int32_t site, int64_t n, flo
 /* Optional: force explicit keep-masks instead of Philox (L+1 sites, each [T*B*H] bytes,
  * 1 = keep).  Pass NULL to return to Philox.  Used to replay the reference's masks. */
 int  zrb_set_explicit_masks(zrb_ctx* ctx, const uint8_t* const* site_masks);
+/* Variational dropout (Gal & Ghahramani, "A Theoretically Grounded Application of Dropout in Recurrent Neural
+ * Networks", NeurIPS 2016; DESIGN.md section 11 states it bit for bit).  Opt-in; off (the default) the masks are
+ * exactly the ones above.  With on = 1, in train mode:
+ *   - sites 0..L keep their (seed, step, site, p) but element (t, b, j) takes the flag of element b*H + j: the mask of
+ *     time step 0 held fixed over the window;
+ *   - with p_rec > 0, layer l's recurrent operand at every step t (t = 0 included) is m_l * h_{t-1} / (1 - p_rec), one
+ *     mask per layer shared by the four gates, site L + 1 + l, element b*H + j.  The layer's output, the carried (h, c)
+ *     and c are not masked.
+ * Eval mode applies no mask.  zrb_dropout_mask(seed, step, site, B*H, p) gives every mask of the mode.
+ * ZRB_E_INVALID for on not 0 / 1, p_rec outside [0, 1), p_rec > 0 with on = 0; ZRB_E_STATE while explicit masks are
+ * set (and zrb_set_explicit_masks with non-NULL masks returns ZRB_E_STATE while the mode is on).  A change of the mode
+ * invalidates the saved forward: zrb_backward / zrb_train_step_layer then need a new forward first. */
+int  zrb_set_variational_dropout(zrb_ctx* ctx, int32_t on, float p_rec);
 
 /* Model.forward (model.py:103-110): embedding gather, dropout, L x (LSTM layer,
  * dropout), vocabulary projection.

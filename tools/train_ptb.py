@@ -48,6 +48,10 @@ ap.add_argument("--factor_epoch", type=int, default=6)
 ap.add_argument("--factor", type=float, default=1.2)
 ap.add_argument("--max_grad_norm", type=float, default=5)
 ap.add_argument("--seed", type=int, default=0)
+ap.add_argument("--variational", action="store_true",
+                help="variational dropout (Gal & Ghahramani 2016): masks fixed over each window, recurrent dropout")
+ap.add_argument("--recurrent_dropout", type=float, default=None,
+                help="p of the recurrent masks with --variational (default: --dropout)")
 ap.add_argument("--lazy_update", action="store_true",
                 help="Trainer(lazy_update=True): upper-layer / fc weight updates run beside the next step's forward")
 ap.add_argument("--eval_batch_size", type=int, default=None,
@@ -90,7 +94,8 @@ tst_b = zaremba_b200.minibatch(tst, EB, T)
 torch.manual_seed(args.seed)
 
 if args.impl == "ours":
-    model = zaremba_b200.Model(vocab, args.hidden_size, args.layer_num, args.dropout, args.winit).to(dev)
+    model = zaremba_b200.Model(vocab, args.hidden_size, args.layer_num, args.dropout, args.winit,
+                               variational=args.variational, recurrent_dropout=args.recurrent_dropout).to(dev)
     tr = zaremba_b200.Trainer(model, B, T, lazy_update=args.lazy_update)
     # the corpus is staged on the device once (SURVEY 8f#2): 3 x [n_batches, T, B] int64
     trn_x = torch.stack([x for x, _ in trn_b]).contiguous().to(dev)
@@ -115,6 +120,8 @@ if args.impl == "ours":
 else:
     if world > 1:
         raise SystemExit("--impl cudnn is the reference's single-device path")
+    if args.variational:
+        raise SystemExit("--variational is a mode of --impl ours")
     from oracle import torch_port as P
     model = P.TorchLstmLm(vocab, args.hidden_size, args.layer_num, args.dropout, args.winit).to(dev)
     trn_d = [(x.to(dev), y.to(dev)) for x, y in trn_b]

@@ -63,7 +63,13 @@ static int check_shapes(const zrb_ctx* c, int T, int B) {
 
 MaskSrc site_mask(const zrb_ctx* c, int site) {
     const uint8_t* ex = c->explicit_masks_set ? c->explicit_masks[site] : nullptr;
-    return make_mask_src(ex, c->seed, c->step, site, c->cfg.dropout, c->train);
+    MaskSrc m = make_mask_src(ex, c->seed, c->step, site, c->cfg.dropout, c->train);
+    if (c->variational) m.period = (uint32_t)c->B * (uint32_t)c->cfg.hidden;   // element (t, b, j) reads b*H + j
+    return m;
+}
+
+MaskSrc rec_mask(const zrb_ctx* c, int layer) {
+    return make_mask_src(nullptr, c->seed, c->step, c->cfg.layers + 1 + layer, c->p_rec, c->train && c->variational);
 }
 
 static cudaEvent_t prof_event(zrb_ctx* c) {
@@ -206,8 +212,34 @@ int zrb_dropout_mask(uint64_t seed, uint64_t step, int32_t site, int64_t n, floa
 
 int zrb_set_explicit_masks(zrb_ctx* c, const uint8_t* const* site_masks) {
     ZRB_REQUIRE(c, "null ctx");
+    if (site_masks && c->variational) {
+        set_error("explicit masks replay Zaremba's per-step masks: switch the variational mode off first");
+        return ZRB_E_STATE;
+    }
     c->explicit_masks_set = site_masks != nullptr;
     for (int s = 0; s <= c->cfg.layers; ++s) c->explicit_masks[s] = site_masks ? site_masks[s] : nullptr;
+    return ZRB_OK;
+}
+
+int zrb_set_variational_dropout(zrb_ctx* c, int32_t on, float p_rec) {
+    ZRB_REQUIRE(c, "null ctx");
+    ZRB_REQUIRE(on == 0 || on == 1, "on must be 0 or 1 (got %d)", on);
+    ZRB_REQUIRE(p_rec >= 0.f && p_rec < 1.f, "p_rec %f outside [0,1)", p_rec);
+    ZRB_REQUIRE(on || p_rec == 0.f, "p_rec %f needs the variational mode", p_rec);
+    if (c->explicit_masks_set) {
+        set_error("explicit masks are set: the variational mode cannot replay them");
+        return ZRB_E_STATE;
+    }
+    if (on && c->cfg.engine == ZRB_ENGINE_SIMT && !c->hrec[0]) {
+        const size_t n = (size_t)(c->cfg.max_seq + 1) * c->cfg.max_batch * c->cfg.hidden;
+        for (int l = 0; l < c->cfg.layers; ++l) ZRB_TRY(dalloc(c, &c->hrec[l], n));
+    }
+    if ((bool)on != c->variational || p_rec != c->p_rec) {
+        c->have_fwd = false;        // a backward must not regenerate other masks than its forward used
+        c->bwd_next_layer = -1;
+    }
+    c->variational = on != 0;
+    c->p_rec = p_rec;
     return ZRB_OK;
 }
 

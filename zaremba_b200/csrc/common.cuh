@@ -83,12 +83,15 @@ struct MaskSrc {
     uint32_t thresh;               // keep iff (r >> 8) >= thresh, thresh = round(p * 2^24)
     float scale;                   // 1 / (1 - p)
     int active;                    // 0: identity (eval mode or p == 0)
+    uint32_t period;               // 0, or B*H: variational mode, element e takes the flag of e % period (the mask of
+                                   // time step 0 held fixed over the window; DESIGN.md section 11)
 };
 
 __host__ inline MaskSrc make_mask_src(const uint8_t* explicit_mask, uint64_t seed, uint64_t step, int site,
                                       float p, int train) {
     MaskSrc m;
     m.explicit_mask = explicit_mask;
+    m.period = 0;
     m.k0 = (uint32_t)seed;
     m.k1 = (uint32_t)(seed >> 32) ^ (uint32_t)(step >> 32);
     m.c2 = (uint32_t)site;
@@ -104,7 +107,8 @@ __host__ inline MaskSrc make_mask_src(const uint8_t* explicit_mask, uint64_t see
 //   key     = (seed lo32, seed hi32 XOR pos hi32)
 //   counter = (j / 4, b, 0xFFFFFFFF, pos lo32); entry j reads word r[j % 4]
 //   u       = ((r >> 9) + 0.5) * 2^-23: exact in float32, strictly inside (0, 1)
-// Counter word 2 of a dropout mask is its site (<= ZRB_MAX_LAYERS), never 0xFFFFFFFF: the two streams cannot meet.
+// Counter word 2 of a dropout mask is its site (<= 2 * ZRB_MAX_LAYERS with the recurrent sites of the variational
+// mode), never 0xFFFFFFFF: the two streams cannot meet.
 struct SampleSrc {
     uint32_t k0, k1, c3;
 };
@@ -145,11 +149,21 @@ __device__ inline uint32_t mask_keep4(const MaskSrc& m, uint64_t g, uint64_t n_t
     return bits;
 }
 
-// multiplier (0 or scale) for a single element e
-__device__ inline float mask_mul1(const MaskSrc& m, uint64_t e, uint64_t n_total) {
+// the element of the site's Philox stream that element e of the activation reads (variational mode: e % period)
+__device__ inline uint64_t mask_elem(const MaskSrc& m, uint64_t e) { return m.period ? e % m.period : e; }
+
+// multiplier (0 or scale) of stream element e, without the period reduction: the persistent recurrence kernels pass
+// b*H + j themselves and keep the 64-bit remainder out of their code
+__device__ inline float mask_mul1_at(const MaskSrc& m, uint64_t e, uint64_t n_total) {
     if (!m.active) return 1.f;
     uint32_t bits = mask_keep4(m, e >> 2, n_total);
     return ((bits >> (e & 3)) & 1u) ? m.scale : 0.f;
+}
+
+// multiplier (0 or scale) for a single element e
+__device__ inline float mask_mul1(const MaskSrc& m, uint64_t e, uint64_t n_total) {
+    if (!m.active) return 1.f;
+    return mask_mul1_at(m, mask_elem(m, e), n_total);
 }
 
 __device__ inline float sigmoidf_(float z) { return 1.f / (1.f + expf(-z)); }

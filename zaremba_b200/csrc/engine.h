@@ -40,6 +40,10 @@ struct zrb_ctx {
     bool layer_fwd_ok = false;             // zrb_lstm_layer_fwd ran and its activations are still in slot 0
     bool explicit_masks_set = false;
     const uint8_t* explicit_masks[ZRB_MAX_LAYERS + 1] = {};
+    bool variational = false;              // zrb_set_variational_dropout: masks fixed over the window, recurrent sites
+    float p_rec = 0.f;
+    float* hrec[ZRB_MAX_LAYERS] = {};      // validation engine, variational mode: [(T+1)*B, H] h_{t-1} * recurrent mask
+                                           // (block 0: the state entering the window); allocated when first switched on
     int64_t weights_version = 1;           // bumped whenever parameter values change
     float* bwd_dy = nullptr;               // phased backward: grad wrt the next layer's output / scratch
     float* bwd_dx = nullptr;
@@ -82,7 +86,8 @@ struct zrb_ctx {
 
 namespace zrb {
 
-MaskSrc site_mask(const zrb_ctx* c, int site);
+MaskSrc site_mask(const zrb_ctx* c, int site);   // dropout site 0..L (period B*H in the variational mode)
+MaskSrc rec_mask(const zrb_ctx* c, int layer);   // recurrent site L+1+layer of the variational mode (inactive otherwise)
 
 // RAII bracket: records an event pair around the launches of one kernel class
 struct ProfScope {

@@ -27,15 +27,19 @@ int simt_forward(zrb_ctx* c, const zrb_params* p, const int64_t* x, const zrb_st
             ZRB_TRY(gemm_f32(c->act[l], p->w_ih[l], G, N, 4 * H, H, 0, 1, 1.f, 0.f, s));
             ZRB_TRY(add_bias2(G, p->b_ih[l], p->b_hh[l], N, 4 * H, s));
         }
-        MaskSrc m = site_mask(c, l + 1);
+        MaskSrc m = site_mask(c, l + 1), rm = rec_mask(c, l);
         ProfScope ps(c, ZRB_PROF_REC_FWD, s);
+        // variational mode: the recurrent operand is hrec (block t = h_{t-1} * mask), also read by the dW_hh GEMM
+        float* hrec = rm.active ? c->hrec[l] : nullptr;
+        if (hrec) ZRB_TRY(dropout_copy(c->h0s[l], hrec, (int64_t)B * H, rm, s));
         for (int t = 0; t < T; ++t) {
-            const float* h_prev = t ? c->hraw[l] + (size_t)(t - 1) * B * H : c->h0s[l];
+            const float* h_prev = hrec ? hrec + (size_t)t * B * H : t ? c->hraw[l] + (size_t)(t - 1) * B * H : c->h0s[l];
             const float* c_prev = t ? c->cst[l] + (size_t)(t - 1) * B * H : c->c0s[l];
             float* Gt = G + (size_t)t * B * 4 * H;
             ZRB_TRY(gemm_f32(h_prev, p->w_hh[l], Gt, B, 4 * H, H, 0, 1, 1.f, 1.f, s));
             ZRB_TRY(lstm_cell_fwd(Gt, c_prev, c->cst[l] + (size_t)t * B * H, c->hraw[l] + (size_t)t * B * H,
-                                  c->act[l + 1] + (size_t)t * B * H, B, H, (int64_t)t * B * H, (int64_t)N * H, m, s));
+                                  c->act[l + 1] + (size_t)t * B * H, hrec ? hrec + (size_t)(t + 1) * B * H : nullptr, B, H,
+                                  (int64_t)t * B * H, (int64_t)N * H, m, rm, s));
         }
         ZRB_CUDA(cudaMemcpyAsync(out->h[l], c->hraw[l] + (size_t)(T - 1) * B * H, bh, cudaMemcpyDeviceToDevice, s));
         ZRB_CUDA(cudaMemcpyAsync(out->c[l], c->cst[l] + (size_t)(T - 1) * B * H, bh, cudaMemcpyDeviceToDevice, s));
@@ -62,7 +66,7 @@ int simt_backward(zrb_ctx* c, const zrb_params* p, const float* dscores, const z
         ZRB_TRY(colsum(dscores, g->fc_b, nullptr, N, V, s));
     }
     for (int l = L - 1; l >= 0; --l) {
-        MaskSrc m = site_mask(c, l + 1);
+        MaskSrc m = site_mask(c, l + 1), rm = rec_mask(c, l);
         ZRB_CUDA(cudaMemsetAsync(c->dc, 0, bh * sizeof(float), s));
         {
         ProfScope ps(c, ZRB_PROF_REC_BWD, s);
@@ -71,7 +75,7 @@ int simt_backward(zrb_ctx* c, const zrb_params* p, const float* dscores, const z
             float* dGt = c->dG + (size_t)t * B * 4 * H;
             ZRB_TRY(lstm_cell_bwd(dY + (size_t)t * bh, t == T - 1 ? nullptr : c->dh_rec, c->dc,
                                   c->gates[l] + (size_t)t * B * 4 * H, c->cst[l] + (size_t)t * bh, c_prev, dGt, B, H,
-                                  (int64_t)t * bh, (int64_t)N * H, m, s));
+                                  (int64_t)t * bh, (int64_t)N * H, m, rm, s));
             if (t > 0) ZRB_TRY(gemm_f32(dGt, p->w_hh[l], c->dh_rec, B, H, 4 * H, 0, 0, 1.f, 0.f, s));
         }
         }
@@ -81,9 +85,14 @@ int simt_backward(zrb_ctx* c, const zrb_params* p, const float* dscores, const z
         }
         ProfScope ps(c, ZRB_PROF_GEMM_WGRAD, s);
         ZRB_TRY(gemm_f32(c->dG, c->act[l], g->w_ih[l], 4 * H, H, N, 1, 0, 1.f, 0.f, s));
-        // dW_hh = sum_t dG_t^T h_{t-1}: t = 0 pairs with the entering state, t >= 1 with hraw[t-1]
-        ZRB_TRY(gemm_f32(c->dG, c->h0s[l], g->w_hh[l], 4 * H, H, B, 1, 0, 1.f, 0.f, s));
-        if (T > 1)
+        // dW_hh = sum_t dG_t^T h_{t-1}: t = 0 pairs with the entering state, t >= 1 with hraw[t-1]; in the
+        // variational mode the masked operands hrec, one GEMM over all N rows
+        if (rm.active) {
+            ZRB_TRY(gemm_f32(c->dG, c->hrec[l], g->w_hh[l], 4 * H, H, N, 1, 0, 1.f, 0.f, s));
+        } else {
+            ZRB_TRY(gemm_f32(c->dG, c->h0s[l], g->w_hh[l], 4 * H, H, B, 1, 0, 1.f, 0.f, s));
+        }
+        if (T > 1 && !rm.active)
             ZRB_TRY(gemm_f32(c->dG + (size_t)B * 4 * H, c->hraw[l], g->w_hh[l], 4 * H, H, N - B, 1, 0, 1.f, 1.f, s));
         ZRB_TRY(colsum(c->dG, g->b_ih[l], g->b_hh[l], N, 4 * H, s));
         float* tmp = dY; dY = dX; dX = tmp;

@@ -6,6 +6,7 @@
 //   fc_w_h               [V,  Hp]   by the dgrads (dG*W, dS*W): one image serves both
 //   x_h[l]      [N, Hp]  dropout'ed input of layer l (x_h[L] feeds the projection); MN-major B of wgrads
 //   hprev_h[l]  [N+B,Hp] rows 0..B-1 = h entering the window, rows B.. = h_t: row block t is h_{t-1}
+//                        (variational mode: times the layer's recurrent mask, so the dW_hh GEMM needs no change)
 //   dG_h        [N, G4p] kGradScale * dG;  dS_h [N, Vp] kGradScale * dscores
 // Gradient images are scaled by an exact power of two and unscaled by the consuming GEMM's alpha.
 #include "engine.h"
@@ -205,6 +206,7 @@ int tc_forward(zrb_ctx* c, const zrb_params* p, const int64_t* x, const zrb_stat
         for (int l = 0; l < L; ++l) {
             fp.in_h[l] = in->h[l]; fp.in_c[l] = in->c[l]; fp.h0s[l] = c->h0s[l]; fp.c0s[l] = c->c0s[l];
             fp.hprev_h[l] = t->hprev_h[l]; fp.h0_img[l] = t->fplan.ok ? t->h0_img[l] : nullptr;
+            fp.rm[l] = rec_mask(c, l);
         }
         fp.x = x; fp.x_saved = c->x_saved;
         fp.L = L; fp.B = B; fp.H = H; fp.Hp = Hp; fp.GB = t->fplan.GBi; fp.Kc = t->fplan.Kc; fp.N = N;
@@ -221,7 +223,7 @@ int tc_forward(zrb_ctx* c, const zrb_params* p, const int64_t* x, const zrb_stat
             ZRB_TRY(gemm_f16_tc(t->x_h[l], Hp, 0, t->w_ih_h[l], Hp, 0, G, 4 * H, N, 4 * H, H, 1.f, p->b_ih[l], 0, s, nullptr,
                                 p->b_hh[l]));
         }
-        MaskSrc m = site_mask(c, l + 1);
+        MaskSrc m = site_mask(c, l + 1), rm = rec_mask(c, l);
         ProfScope ps(c, ZRB_PROF_REC_FWD, s);
         if (t->fplan.ok) {
             const unsigned int arrivals = (unsigned int)T * (unsigned int)t->fplan.nCTA;
@@ -230,7 +232,7 @@ int tc_forward(zrb_ctx* c, const zrb_params* p, const int64_t* x, const zrb_stat
                 t->cnt_f = 0;
             }
             ZRB_TRY(lstm_rec_fwd(t->fplan, tc_watchdog(c), t->w_img_f[l], t->h0_img[l], t->h_img, G, c->c0s[l], c->cst[l], out->h[l],
-                                 out->c[l], t->hprev_h[l], t->x_h[l + 1], t->counter, t->cnt_f, T, B, H, Hp, m, s,
+                                 out->c[l], t->hprev_h[l], t->x_h[l + 1], t->counter, t->cnt_f, T, B, H, Hp, m, rm, s,
                                  t->trace));
             t->cnt_f += arrivals;
             // deferred update of the NEXT layer's matrices (or of fc.W after the last layer): on the idle SMs, beside
@@ -245,7 +247,7 @@ int tc_forward(zrb_ctx* c, const zrb_params* p, const int64_t* x, const zrb_stat
                                 1.f, nullptr, 1, s));
             ZRB_TRY(lstm_cell_fwd_tc(Gt, c_prev, c->cst[l] + (size_t)tt * B * H, c->hraw[l] + (size_t)tt * B * H,
                                      t->hprev_h[l] + (size_t)(tt + 1) * B * Hp, t->x_h[l + 1] + (size_t)tt * B * Hp, Hp, B,
-                                     H, (int64_t)tt * B * H, (int64_t)N * H, m, s));
+                                     H, (int64_t)tt * B * H, (int64_t)N * H, m, rm, s));
         }
         ZRB_CUDA(cudaMemcpyAsync(out->h[l], c->hraw[l] + (size_t)(T - 1) * B * H, bh, cudaMemcpyDeviceToDevice, s));
         ZRB_CUDA(cudaMemcpyAsync(out->c[l], c->cst[l] + (size_t)(T - 1) * B * H, bh, cudaMemcpyDeviceToDevice, s));
@@ -353,7 +355,7 @@ static int tc_backward_layer(zrb_ctx* c, const zrb_params* p, const zrb_params* 
     float* dX = c->bwd_dx;
     __half* dG_h = (l & 1) ? t->dG_h_alt : t->dG_h;
     {
-        MaskSrc m = site_mask(c, l + 1);
+        MaskSrc m = site_mask(c, l + 1), rm = rec_mask(c, l);
         if (t->bplan.ok) {
             ProfScope ps(c, ZRB_PROF_REC_BWD, s);
             const unsigned int arrivals = (unsigned int)T * (unsigned int)t->bplan.nCTA;
@@ -362,7 +364,7 @@ static int tc_backward_layer(zrb_ctx* c, const zrb_params* p, const zrb_params* 
                 t->cnt_b = 0;
             }
             ZRB_TRY(lstm_rec_bwd(t->bplan, tc_watchdog(c), t->w_img_b[l], t->g_img, dY, c->gates[l], c->cst[l], c->c0s[l], dG_h,
-                                 t->counter + 32, t->cnt_b, T, B, H, G4p, m, s,
+                                 t->counter + 32, t->cnt_b, T, B, H, G4p, m, rm, s,
                                  t->trace ? t->trace + 8 + (size_t)c->cfg.max_seq * 8 : nullptr, g->b_ih[l], g->b_hh[l],
                                  c->resident_flag, ++c->resident_seq, c->dG /* [N,4H] fp32, idle on this path */));
             t->cnt_b += arrivals;
@@ -375,7 +377,7 @@ static int tc_backward_layer(zrb_ctx* c, const zrb_params* p, const zrb_params* 
                 ZRB_TRY(lstm_cell_bwd_tc(dY + (size_t)tt * bh, tt == T - 1 ? nullptr : c->dh_rec, c->dc,
                                          c->gates[l] + (size_t)tt * B * 4 * H, c->cst[l] + (size_t)tt * bh, c_prev,
                                          c->dG + (size_t)tt * B * 4 * H, dG_h + (size_t)tt * B * G4p, G4p, B, H,
-                                         (int64_t)tt * bh, (int64_t)N * H, m, s));
+                                         (int64_t)tt * bh, (int64_t)N * H, m, rm, s));
                 if (tt > 0)  // dh_{t-1}[B,H] = dG_t[B,4H] * W_hh[4H,H]
                     ZRB_TRY(gemm_f16_tc(dG_h + (size_t)tt * B * G4p, G4p, 0, t->w_hh_h[l], Hp, 1, c->dh_rec, H, B, H,
                                         4 * H, inv, nullptr, 0, s));
@@ -518,7 +520,7 @@ int tc_layer_fwd(zrb_ctx* c, const float* w_ih, const float* w_hh, const float* 
     }
     MaskSrc m = make_mask_src(nullptr, 0, 0, 0, 0.f, 0);    // no dropout at this level: the caller applies it (model.py:105,108)
     ZRB_TRY(lstm_rec_fwd(t->fplan, tc_watchdog(c), t->w_img_f[0], t->h0_img[0], t->h_img, c->gates[0], c->c0s[0], c->cst[0], hT, cT,
-                         t->hprev_h[0], t->x_h[1], t->counter, t->cnt_f, T, B, H, Hp, m, s, nullptr, y));
+                         t->hprev_h[0], t->x_h[1], t->counter, t->cnt_f, T, B, H, Hp, m, m, s, nullptr, y));
     t->cnt_f += arrivals;
     c->have_fwd = false;                         // a model-level backward must not follow this
     c->layer_fwd_ok = true;
@@ -540,7 +542,7 @@ int tc_layer_bwd(zrb_ctx* c, const float* dy, float* dx, float* dw_ih, float* dw
     }
     MaskSrc m = make_mask_src(nullptr, 0, 0, 0, 0.f, 0);
     ZRB_TRY(lstm_rec_bwd(t->bplan, tc_watchdog(c), t->w_img_b[0], t->g_img, dy, c->gates[0], c->cst[0], c->c0s[0], t->dG_h, t->counter + 32,
-                         t->cnt_b, T, B, H, G4p, m, s, nullptr, db_ih, db_hh, c->resident_flag, ++c->resident_seq, c->dG));
+                         t->cnt_b, T, B, H, G4p, m, m, s, nullptr, db_ih, db_hh, c->resident_flag, ++c->resident_seq, c->dG));
     t->cnt_b += arrivals;
     const float inv = 1.f / kGradScale;
     if (dx) ZRB_TRY(gemm_f16_tc(t->dG_h, G4p, 0, t->w_ih_h[0], Hp, 1, dx, H, N, H, 4 * H, inv, nullptr, 0, s));

@@ -13,13 +13,16 @@ int embed_dropout_bwd(const float* dA, const int64_t* idx, float* dW, int N, int
                       cudaStream_t s);
 // pre [B,4H] holds x-part + h-part pre-activations (+bias already added); overwritten with
 // activated gates (i,f,g,o).  c_prev/c_out/h_raw/y_out [B,H]; y_out = dropout(h).
-int lstm_cell_fwd(float* pre, const float* c_prev, float* c_out, float* h_raw, float* y_out,
-                  int B, int H, int64_t elem_off, int64_t n_total, MaskSrc m, cudaStream_t s);
-// dG [B,4H] out; dc [B,H] in/out carry; dh_rec [B,H] in (may be null = 0);
+// h_rec [B,H] (or null): h * the recurrent mask rm of element b*H + j (variational mode: the next step's operand)
+int lstm_cell_fwd(float* pre, const float* c_prev, float* c_out, float* h_raw, float* y_out, float* h_rec,
+                  int B, int H, int64_t elem_off, int64_t n_total, MaskSrc m, MaskSrc rm, cudaStream_t s);
+// dG [B,4H] out; dc [B,H] in/out carry; dh_rec [B,H] in (may be null = 0), multiplied by the recurrent mask rm;
 // dy_post [B,H] upstream grad on the post-dropout output
 int lstm_cell_bwd(const float* dy_post, const float* dh_rec, float* dc, const float* gates, const float* c_t,
                   const float* c_prev, float* dG, int B, int H, int64_t elem_off, int64_t n_total, MaskSrc m,
-                  cudaStream_t s);
+                  MaskSrc rm, cudaStream_t s);
+// y[e] = x[e] * (mask multiplier of element e), e < n
+int dropout_copy(const float* x, float* y, int64_t n, MaskSrc m, cudaStream_t s);
 // C[n, j] += bias1[j] + bias2[j]
 int add_bias2(float* C, const float* b1, const float* b2, int N, int M, cudaStream_t s);
 int add_bias1(float* C, const float* b1, int N, int M, cudaStream_t s);

@@ -1,6 +1,8 @@
 // Persistent LSTM recurrence, backward, one launch per layer (sm_90a, thread-block clusters).
 //
 //   for t in T-1..0:  dh_t = mask * dY_t + dG_{t+1} * W_hh ;  cell backward -> dG_t, dc      (SURVEY 8a)
+//   (variational mode: the second term times the cell's recurrent multiplier m * scale(p_rec); the MMA warpgroup
+//   applies it to the partial products it pushes, from flags drawn once before the step loop)
 //
 // The contraction dG_{t+1}[B,4H] * W_hh[4H,H] runs over the 4H gate rows.  A CTA that owned only a few
 // hidden units would fill 16 of the 64 rows of a wgmma tile, so a CLUSTER owns UC units and
@@ -45,7 +47,8 @@ struct RecBwdArgs {
     unsigned int base;
     int T, B, H, G4p, U, G, GB, Kc, nCTA;
     int KcS, GBi;             // K chunks per CTA (Kc / S); 8-row batch groups of the dG images (GB, or 4 when N = 32)
-    MaskSrc m;
+    MaskSrc m;                // the output site's dropout (period B*H: variational mode, fixed over the window)
+    MaskSrc rm;               // variational mode: recurrent mask of element b*H + j; scales the recurrent gradient
     RecWatch w;               // watchdog (rec_common.cuh)
     long long* trace;         // optional (profiling): [8] launch stamps (rec_launch_stamps) + [T][8] clock64 stamps of CTA 0
 };
@@ -200,10 +203,31 @@ __global__ void __launch_bounds__(kRecThreads, 1) lstm_rec_bwd_kernel(RecBwdArgs
                     row_bar[m][h] = mapa_shared(bar_recv_addr, row_owner[m][h]);
                 }
             }
+        // variational mode: the recurrent mask of each (unit = row, batch = column) value this thread emits, drawn once.
+        // Bit 16 m + 4 (col / 8) + 2 h + e (e: column col + e) set = dropped; none set with the mode off.  Every
+        // partial product is multiplied by 0 or scale(p_rec) (a.rm.scale, 1 with the mode off: exact), so the cell
+        // math adds scale * m * (dG_{t+1} W_hh) with no register of its own -- the epilogue is at the register limit.
+        uint32_t rdrop = 0;
+        if (a.rm.active) {
+            for (int m = 0; m < 2; ++m)
+                for (int h = 0; h < 2; ++h) {
+                    const int row = rec_acc_row(tm, m, h), j = jc0 + row;
+                    for (int c8 = 0; c8 < 4; ++c8)
+                        for (int e = 0; e < 2; ++e) {
+                            const int b = wgmma_col(tm, c8) + e;
+                            if (row < UC && j < H && b < B && mask_mul1_at(a.rm, (uint64_t)b * H + j, (uint64_t)B * H) == 0.f)
+                                rdrop |= 1u << (16 * m + 4 * c8 + 2 * h + e);
+                        }
+                }
+        }
+        const float rscale = a.rm.scale;
         bool dead = false;
         bounded_mbar_wait(bar_a, 0, a.w, dead, kWaitWeights, 0);
         dead = rec_mma_any(dead);
         auto emit = [&](int m, int h, int col, float v0, float v1) {
+            const int bit = 16 * m + 4 * (col >> 3) + 2 * h;
+            v0 *= ((rdrop >> bit) & 1u) ? 0.f : rscale;
+            v1 *= ((rdrop >> (bit + 1)) & 1u) ? 0.f : rscale;
             if (!push) {
                 float* dst = (float*)((uint8_t*)sD + row_dst[m][h]) + col;
                 dst[0] = v0;
@@ -264,7 +288,9 @@ __global__ void __launch_bounds__(kRecThreads, 1) lstm_rec_bwd_kernel(RecBwdArgs
                     go[k] = __ldg(grow + 3 * (size_t)H);
                     ct[k] = __ldg(a.cst + n * H + j);
                     cp[k] = t > 0 ? __ldg(a.cst + (n - B) * H + j) : __ldg(a.c0 + (size_t)b * H + j);
-                    dyv[k] = __ldg(a.dy + n * H + j) * mask_mul1(a.m, (uint64_t)n * H + j, n_total);
+                    // (variational mode: element b*H + j of the site's stream, the mask fixed over the window)
+                    dyv[k] = __ldg(a.dy + n * H + j) *
+                             mask_mul1_at(a.m, (uint64_t)(a.m.period ? b : (int)n) * H + j, n_total);
                 }
             }
             if (s > 0) {
@@ -557,7 +583,7 @@ static int launch_rec_bwd(const RecPlan& p, const RecBwdArgs& a, cudaStream_t s)
 
 int lstm_rec_bwd(const RecPlan& p, const RecWatchdog& wd, const __half* w_img, __half* g_img, const float* dy, const float* gates,
                  const float* cst, const float* c0, __half* dG_h, unsigned int* counter, unsigned int counter_base, int T,
-                 int B, int H, int G4p, MaskSrc m, cudaStream_t s, long long* trace, float* db1, float* db2,
+                 int B, int H, int G4p, MaskSrc m, MaskSrc rm, cudaStream_t s, long long* trace, float* db1, float* db2,
                  unsigned int* resident_flag, unsigned int resident_value, float* db_scratch) {
     ZRB_REQUIRE(!db1 || db_scratch, "bias gradients need the scratch buffer");
     RecBwdArgs a;
@@ -566,7 +592,8 @@ int lstm_rec_bwd(const RecPlan& p, const RecWatchdog& wd, const __half* w_img, _
     static const bool pull = getenv("ZRB_BWD_PULL") != nullptr;   // A/B switch: the r01 staging + DSMEM-pull exchange (S = 1)
     a.push = pull ? 0 : 1;
     a.counter = counter; a.db1 = db1; a.db2 = db2; a.db_scratch = db_scratch; a.res_flag = resident_flag; a.res_value = resident_value;
-    a.T = T; a.B = B; a.H = H; a.G4p = G4p; a.U = p.U; a.G = p.G; a.GB = p.GB; a.Kc = p.Kc; a.nCTA = p.nCTA; a.m = m; a.trace = trace;
+    a.T = T; a.B = B; a.H = H; a.G4p = G4p; a.U = p.U; a.G = p.G; a.GB = p.GB; a.Kc = p.Kc; a.nCTA = p.nCTA; a.m = m; a.rm = rm; a.trace = trace;
+    if (!rm.active) a.rm.scale = 1.f;   // (the epilogue multiplies by it unconditionally)
     a.KcS = p.KcS; a.GBi = p.GBi;
     ZRB_REQUIRE(wd.flag && wd.host, "lstm_rec_bwd needs the context's watchdog words");
     a.w = rec_watch_args(wd);

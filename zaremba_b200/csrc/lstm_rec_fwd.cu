@@ -19,8 +19,9 @@
 //   MMA warpgroup   H/16 wgmma m64nNk16 (N = pad8(B)) chained into register accumulators, then each
 //                   accumulator row is staged in shared memory (rec_common.cuh: rec_mma_step)
 //   8 epilogue warps add the x-part pre-activations prefetched during the MMAs to the staged rows,
-//                   apply sigmoid/tanh/cell update/dropout.  The next step's operand image is stored FIRST
-//                   and published (one red.release.gpu on the grid-barrier counter, which is never reset:
+//                   apply sigmoid/tanh/cell update/dropout (variational mode: the operand image holds h * rm, rm
+//                   the cell's recurrent multiplier drawn once before the step loop and kept in a register).
+//                   The next step's operand image is stored FIRST and published (one red.release.gpu on the grid-barrier counter, which is never reset:
 //                   the launch gets its starting value); everything backward needs (activated gates, c_t,
 //                   row-major fp16 h, dropout(h) for the next layer) is stored after the arrival, off the
 //                   critical path.
@@ -56,7 +57,8 @@ struct RecFwdArgs {
     unsigned int base;
     int T, B, H, Hp, U, G, GB, Kc, nCTA;
     int KcS, GBi;             // K chunks per CTA (Kc / KS); 8-row batch groups of the operand image (GB, or 4 when N = 32)
-    MaskSrc m;
+    MaskSrc m;                // the output site's dropout (period B*H: variational mode, fixed over the window)
+    MaskSrc rm;               // variational mode: recurrent mask of element b*H + j on h_{t-1} (operand images, hprev_h)
     RecWatch w;               // watchdog (rec_common.cuh)
     long long* trace;         // optional (profiling): [8] launch stamps (rec_launch_stamps) + [T][8] clock64 stamps of CTA 0
 };
@@ -202,11 +204,18 @@ __global__ void __launch_bounds__(kRecThreads, 1) lstm_rec_fwd_kernel(RecFwdArgs
         const uint64_t n_total = (uint64_t)a.T * B * H;
         int cb[kRecMaxCell];   // rec_cell
         float creg[kRecMaxCell];
+        // the cell's mask multipliers held fixed over the window, drawn once here (variational mode; else 1 and unused):
+        // recurrent rm on the next step's operand, ym on the output when the output site's mask has a period
+        float rm[kRecMaxCell], ym[kRecMaxCell];
+        const uint64_t bh = (uint64_t)B * H;
 #pragma unroll
         for (int k = 0; k < kRecMaxCell; ++k) {
             cb[k] = (tid + kRecEpiThreads * k) / a.U;
             const auto [b, u, ok] = rec_cell(tid, k, cb[k], a.U, cells, nu);
             creg[k] = ok ? a.c0[(size_t)b * H + j0 + u] : 0.f;
+            const uint64_t e = (uint64_t)b * H + j0 + u;
+            rm[k] = ok ? mask_mul1_at(a.rm, e, bh) : 1.f;
+            ym[k] = ok && a.m.period ? mask_mul1_at(a.m, e, bh) : 1.f;
         }
         const uint32_t recv_bytes = 2u * 4u * (uint32_t)a.U * (uint32_t)Bp * 4u;   // 2 sources x 4U rows x Bp columns
         for (int t = 0; t < a.T; ++t) {
@@ -254,7 +263,7 @@ __global__ void __launch_bounds__(kRecThreads, 1) lstm_rec_fwd_kernel(RecFwdArgs
                 // critical path: the next step's operand image [kc][g][r][e], kc = j/8, e = j%8, g = b/8, r = b%8
                 const int j = j0 + u;
                 __half* img = a.h_img + (size_t)(t + 1) * ((size_t)a.Kc * a.GBi * 64);
-                img[((size_t)(j >> 3) * a.GBi + (b >> 3)) * 64 + (b & 7) * 8 + (j & 7)] = __float2half_rn(h);
+                img[((size_t)(j >> 3) * a.GBi + (b >> 3)) * 64 + (b & 7) * 8 + (j & 7)] = __float2half_rn(h * rm[k]);
             }
             if (tr && tid == 0) trs[t * 8 + 5] = clock64();
             asm volatile("bar.sync 1, 256;" ::: "memory");
@@ -273,8 +282,8 @@ __global__ void __launch_bounds__(kRecThreads, 1) lstm_rec_fwd_kernel(RecFwdArgs
                 float* grow = a.gates + n * 4 * H + j;
                 grow[0] = o_i[k]; grow[H] = o_f[k]; grow[2 * (size_t)H] = o_g[k]; grow[3 * (size_t)H] = o_o[k];
                 a.cst[n * H + j] = creg[k];
-                a.hprev_h[((size_t)B + n) * a.Hp + j] = __float2half_rn(o_h[k]);
-                float y = o_h[k] * mask_mul1(a.m, (uint64_t)n * H + j, n_total);
+                a.hprev_h[((size_t)B + n) * a.Hp + j] = __float2half_rn(o_h[k] * rm[k]);
+                float y = o_h[k] * (a.m.period ? ym[k] : mask_mul1_at(a.m, (uint64_t)n * H + j, n_total));
                 a.y_h[n * a.Hp + j] = __float2half_rn(y);
                 if (a.h_f32) a.h_f32[n * H + j] = o_h[k];
                 if (t == a.T - 1) {
@@ -379,8 +388,8 @@ int pack_whh_fwd(const float* W, __half* img, int H, const RecPlan& p, cudaStrea
 
 int lstm_rec_fwd(const RecPlan& p, const RecWatchdog& wd, const __half* w_img, const __half* h0_img, __half* h_img, float* gates,
                  const float* c0, float* cst, float* h_last, float* c_last, __half* hprev_h, __half* y_h,
-                 unsigned int* counter, unsigned int counter_base, int T, int B, int H, int Hp, MaskSrc m, cudaStream_t s,
-                 long long* trace, float* h_f32) {
+                 unsigned int* counter, unsigned int counter_base, int T, int B, int H, int Hp, MaskSrc m, MaskSrc rm,
+                 cudaStream_t s, long long* trace, float* h_f32) {
     static bool attr[64] = {};   // per device: function attributes belong to the device's context
     int dev = 0;
     cudaGetDevice(&dev);
@@ -393,7 +402,7 @@ int lstm_rec_fwd(const RecPlan& p, const RecWatchdog& wd, const __half* w_img, c
     RecFwdArgs a;
     a.w_img = w_img; a.h0_img = h0_img; a.h_img = h_img; a.base = counter_base; a.gates = gates; a.c0 = c0; a.cst = cst; a.h_last = h_last; a.c_last = c_last;
     a.hprev_h = hprev_h; a.y_h = y_h; a.counter = counter; a.h_f32 = h_f32;
-    a.T = T; a.B = B; a.H = H; a.Hp = Hp; a.U = p.U; a.G = p.G; a.GB = p.GB; a.Kc = p.Kc; a.nCTA = p.nCTA; a.m = m;
+    a.T = T; a.B = B; a.H = H; a.Hp = Hp; a.U = p.U; a.G = p.G; a.GB = p.GB; a.Kc = p.Kc; a.nCTA = p.nCTA; a.m = m; a.rm = rm;
     a.KcS = p.KcS; a.GBi = p.GBi;
     a.trace = trace;
     ZRB_REQUIRE(wd.flag && wd.host, "lstm_rec_fwd needs the context's watchdog words");

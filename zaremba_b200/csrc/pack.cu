@@ -34,19 +34,22 @@ __global__ void fwd_prep_kernel(FwdPrep a) {
     for (int l = 0; l < a.L; ++l) {
         const float* __restrict__ h = a.in_h[l];
         const float* __restrict__ c = a.in_c[l];
+        const MaskSrc rm = a.rm[l];   // variational mode: the recurrent operand of step 0 is h0 * rm
         for (int i = tid; i < bh; i += nth) {
             a.h0s[l][i] = h[i];
             a.c0s[l][i] = c[i];
         }
         for (int i = tid; i < bhp; i += nth) {
             const int r = i / a.Hp, col = i % a.Hp;
-            a.hprev_h[l][i] = __float2half_rn(col < a.H ? h[(size_t)r * a.H + col] : 0.f);
+            a.hprev_h[l][i] = __float2half_rn(
+                col < a.H ? h[(size_t)r * a.H + col] * mask_mul1_at(rm, (uint64_t)r * a.H + col, (uint64_t)bh) : 0.f);
         }
         if (a.h0_img[l]) {
             for (int i = tid; i < img_n; i += nth) {
                 const int e = i & 7, r = (i >> 3) & 7, g = (i >> 6) % a.GB, kc = (i >> 6) / a.GB;
                 const int b = g * 8 + r, k = kc * 8 + e;
-                a.h0_img[l][i] = __float2half_rn((b < a.B && k < a.H) ? h[(size_t)b * a.H + k] : 0.f);
+                a.h0_img[l][i] = __float2half_rn(
+                    (b < a.B && k < a.H) ? h[(size_t)b * a.H + k] * mask_mul1_at(rm, (uint64_t)b * a.H + k, (uint64_t)bh) : 0.f);
             }
         }
     }

@@ -28,9 +28,10 @@ __global__ void embed_dropout_fwd_kernel(const float* __restrict__ W, const int6
 #pragma unroll
         for (int i = 0; i < 4; ++i) v[i] = (j0 + i < H) ? src[j0 + i] : 0.f;
         if (m.active) {
-            // rows are H long; H % 4 != 0 makes groups straddle Philox quads -> per-element path
+            // rows are H long; H % 4 != 0 makes groups straddle Philox quads -> per-element path.  (A variational
+            // period B*H is then a multiple of 4 too, so the reduced e0 still starts a quad.)
             if ((H & 3) == 0) {
-                uint32_t bits = mask_keep4(m, e0 >> 2, n_total);
+                uint32_t bits = mask_keep4(m, mask_elem(m, e0) >> 2, n_total);
 #pragma unroll
                 for (int i = 0; i < 4; ++i) v[i] = ((bits >> i) & 1u) ? v[i] * m.scale : 0.f;
             } else {
@@ -85,7 +86,8 @@ int embed_dropout_bwd(const float* dA, const int64_t* idx, float* dW, int N, int
 // ----------------------------------------------------------------------------------------
 __global__ void lstm_cell_fwd_kernel(float* __restrict__ pre, const float* __restrict__ c_prev,
                                      float* __restrict__ c_out, float* __restrict__ h_raw, float* __restrict__ y_out,
-                                     int B, int H, int64_t elem_off, int64_t n_total, MaskSrc m) {
+                                     float* __restrict__ h_rec, int B, int H, int64_t elem_off, int64_t n_total, MaskSrc m,
+                                     MaskSrc rm) {
     int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (tid >= (int64_t)B * H) return;
     int b = (int)(tid / H), j = (int)(tid % H);
@@ -100,12 +102,14 @@ __global__ void lstm_cell_fwd_kernel(float* __restrict__ pre, const float* __res
     c_out[tid] = c;
     h_raw[tid] = h;
     y_out[tid] = h * mask_mul1(m, (uint64_t)(elem_off + tid), (uint64_t)n_total);
+    if (h_rec) h_rec[tid] = h * mask_mul1_at(rm, (uint64_t)tid, (uint64_t)B * H);   // the next step's recurrent operand
 }
 
-int lstm_cell_fwd(float* pre, const float* c_prev, float* c_out, float* h_raw, float* y_out, int B, int H,
-                  int64_t elem_off, int64_t n_total, MaskSrc m, cudaStream_t s) {
+int lstm_cell_fwd(float* pre, const float* c_prev, float* c_out, float* h_raw, float* y_out, float* h_rec, int B, int H,
+                  int64_t elem_off, int64_t n_total, MaskSrc m, MaskSrc rm, cudaStream_t s) {
     int64_t n = (int64_t)B * H;
-    lstm_cell_fwd_kernel<<<cdiv(n, 256), 256, 0, s>>>(pre, c_prev, c_out, h_raw, y_out, B, H, elem_off, n_total, m);
+    lstm_cell_fwd_kernel<<<cdiv(n, 256), 256, 0, s>>>(pre, c_prev, c_out, h_raw, y_out, h_rec, B, H, elem_off, n_total, m,
+                                                      rm);
     ZRB_KERNEL_CHECK();
     return ZRB_OK;
 }
@@ -115,14 +119,14 @@ __global__ void lstm_cell_bwd_kernel(const float* __restrict__ dy_post, const fl
                                      float* __restrict__ dc, const float* __restrict__ gates,
                                      const float* __restrict__ c_t, const float* __restrict__ c_prev,
                                      float* __restrict__ dG, int B, int H, int64_t elem_off, int64_t n_total,
-                                     MaskSrc m) {
+                                     MaskSrc m, MaskSrc rm) {
     int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (tid >= (int64_t)B * H) return;
     int b = (int)(tid / H), j = (int)(tid % H);
     const float* row = gates + (int64_t)b * 4 * H;
     float i = row[j], f = row[H + j], g = row[2 * H + j], o = row[3 * H + j];
     float dh = dy_post[tid] * mask_mul1(m, (uint64_t)(elem_off + tid), (uint64_t)n_total);
-    if (dh_rec) dh += dh_rec[tid];
+    if (dh_rec) dh += dh_rec[tid] * mask_mul1_at(rm, (uint64_t)tid, (uint64_t)B * H);
     float tc = tanhf(c_t[tid]);
     float d_o = dh * tc;
     float dcc = dc[tid] + dh * o * (1.f - tc * tc);
@@ -139,10 +143,22 @@ __global__ void lstm_cell_bwd_kernel(const float* __restrict__ dy_post, const fl
 
 int lstm_cell_bwd(const float* dy_post, const float* dh_rec, float* dc, const float* gates, const float* c_t,
                   const float* c_prev, float* dG, int B, int H, int64_t elem_off, int64_t n_total, MaskSrc m,
-                  cudaStream_t s) {
+                  MaskSrc rm, cudaStream_t s) {
     int64_t n = (int64_t)B * H;
     lstm_cell_bwd_kernel<<<cdiv(n, 256), 256, 0, s>>>(dy_post, dh_rec, dc, gates, c_t, c_prev, dG, B, H, elem_off,
-                                                      n_total, m);
+                                                      n_total, m, rm);
+    ZRB_KERNEL_CHECK();
+    return ZRB_OK;
+}
+
+// y[e] = x[e] * mask multiplier of element e, e < n (the masked state entering the window, variational mode)
+__global__ void dropout_copy_kernel(const float* __restrict__ x, float* __restrict__ y, int64_t n, MaskSrc m) {
+    int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e < n) y[e] = x[e] * mask_mul1(m, (uint64_t)e, (uint64_t)n);
+}
+int dropout_copy(const float* x, float* y, int64_t n, MaskSrc m, cudaStream_t s) {
+    if (n == 0) return ZRB_OK;
+    dropout_copy_kernel<<<cdiv(n, 256), 256, 0, s>>>(x, y, n, m);
     ZRB_KERNEL_CHECK();
     return ZRB_OK;
 }

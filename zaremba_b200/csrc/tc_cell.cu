@@ -8,7 +8,7 @@ namespace zrb {
 __global__ void lstm_cell_fwd_tc_kernel(float* __restrict__ pre, const float* __restrict__ c_prev,
                                         float* __restrict__ c_out, float* __restrict__ h_raw,
                                         __half* __restrict__ h_raw_h, __half* __restrict__ y_h, int64_t ld_h, int B,
-                                        int H, int64_t elem_off, int64_t n_total, MaskSrc m) {
+                                        int H, int64_t elem_off, int64_t n_total, MaskSrc m, MaskSrc rm) {
     int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (tid >= (int64_t)B * H) return;
     int b = (int)(tid / H), j = (int)(tid % H);
@@ -22,15 +22,15 @@ __global__ void lstm_cell_fwd_tc_kernel(float* __restrict__ pre, const float* __
     row[j] = i; row[H + j] = f; row[2 * H + j] = g; row[3 * H + j] = o;
     c_out[tid] = c;
     h_raw[tid] = h;
-    h_raw_h[(int64_t)b * ld_h + j] = __float2half_rn(h);
+    h_raw_h[(int64_t)b * ld_h + j] = __float2half_rn(h * mask_mul1_at(rm, (uint64_t)tid, (uint64_t)B * H));   // next step's operand
     y_h[(int64_t)b * ld_h + j] = __float2half_rn(h * mask_mul1(m, (uint64_t)(elem_off + tid), (uint64_t)n_total));
 }
 
 int lstm_cell_fwd_tc(float* pre, const float* c_prev, float* c_out, float* h_raw, __half* h_raw_h, __half* y_h,
-                     int64_t ld_h, int B, int H, int64_t elem_off, int64_t n_total, MaskSrc m, cudaStream_t s) {
+                     int64_t ld_h, int B, int H, int64_t elem_off, int64_t n_total, MaskSrc m, MaskSrc rm, cudaStream_t s) {
     int64_t n = (int64_t)B * H;
     lstm_cell_fwd_tc_kernel<<<cdiv(n, 256), 256, 0, s>>>(pre, c_prev, c_out, h_raw, h_raw_h, y_h, ld_h, B, H, elem_off,
-                                                         n_total, m);
+                                                         n_total, m, rm);
     ZRB_KERNEL_CHECK();
     return ZRB_OK;
 }
@@ -45,14 +45,14 @@ __global__ void lstm_cell_bwd_tc_kernel(const float* __restrict__ dy_post, const
                                         float* __restrict__ dc, const float* __restrict__ gates,
                                         const float* __restrict__ c_t, const float* __restrict__ c_prev,
                                         float* __restrict__ dG, __half* __restrict__ dG_h, int64_t ld_g, int B, int H,
-                                        int64_t elem_off, int64_t n_total, MaskSrc m) {
+                                        int64_t elem_off, int64_t n_total, MaskSrc m, MaskSrc rm) {
     int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (tid >= (int64_t)B * H) return;
     int b = (int)(tid / H), j = (int)(tid % H);
     const float* row = gates + (int64_t)b * 4 * H;
     float i = row[j], f = row[H + j], g = row[2 * H + j], o = row[3 * H + j];
     float dh = dy_post[tid] * mask_mul1(m, (uint64_t)(elem_off + tid), (uint64_t)n_total);
-    if (dh_rec) dh += dh_rec[tid];
+    if (dh_rec) dh += dh_rec[tid] * mask_mul1_at(rm, (uint64_t)tid, (uint64_t)B * H);
     float tc = tanhf(c_t[tid]);
     float d_o = dh * tc;
     float dcc = dc[tid] + dh * o * (1.f - tc * tc);
@@ -68,10 +68,10 @@ __global__ void lstm_cell_bwd_tc_kernel(const float* __restrict__ dy_post, const
 
 int lstm_cell_bwd_tc(const float* dy_post, const float* dh_rec, float* dc, const float* gates, const float* c_t,
                      const float* c_prev, float* dG, __half* dG_h, int64_t ld_g, int B, int H, int64_t elem_off,
-                     int64_t n_total, MaskSrc m, cudaStream_t s) {
+                     int64_t n_total, MaskSrc m, MaskSrc rm, cudaStream_t s) {
     int64_t n = (int64_t)B * H;
     lstm_cell_bwd_tc_kernel<<<cdiv(n, 256), 256, 0, s>>>(dy_post, dh_rec, dc, gates, c_t, c_prev, dG, dG_h, ld_g, B, H,
-                                                         elem_off, n_total, m);
+                                                         elem_off, n_total, m, rm);
     ZRB_KERNEL_CHECK();
     return ZRB_OK;
 }

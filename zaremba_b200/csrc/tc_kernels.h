@@ -13,12 +13,13 @@ int colsum_h_scratch_floats(int M);
 int colsum_h(const __half* A, int64_t ld, float* out, float* out2, int N, int M, float inv_scale, float* scratch,
              cudaStream_t s);
 
-// cell pointwise with fp16 side outputs (tc_cell.cu)
+// cell pointwise with fp16 side outputs (tc_cell.cu).  rm: recurrent mask of element b*H + j (variational mode), applied
+// to h_raw_h (the next step's operand) forward and to dh_rec backward
 int lstm_cell_fwd_tc(float* pre, const float* c_prev, float* c_out, float* h_raw, __half* h_raw_h, __half* y_h,
-                     int64_t ld_h, int B, int H, int64_t elem_off, int64_t n_total, MaskSrc m, cudaStream_t s);
+                     int64_t ld_h, int B, int H, int64_t elem_off, int64_t n_total, MaskSrc m, MaskSrc rm, cudaStream_t s);
 int lstm_cell_bwd_tc(const float* dy_post, const float* dh_rec, float* dc, const float* gates, const float* c_t,
                      const float* c_prev, float* dG, __half* dG_h, int64_t ld_g, int B, int H, int64_t elem_off,
-                     int64_t n_total, MaskSrc m, cudaStream_t s);
+                     int64_t n_total, MaskSrc m, MaskSrc rm, cudaStream_t s);
 
 // ---- persistent recurrence (lstm_rec_fwd.cu / lstm_rec_bwd.cu) ---------------------------------------
 struct RecPlan {
@@ -47,12 +48,15 @@ int pack_whh_fwd(const float* W, __half* img, int H, const RecPlan& p, cudaStrea
 // the launch starts (the caller adds T * nCTA per launch).
 int lstm_rec_fwd(const RecPlan& p, const RecWatchdog& wd, const __half* w_img, const __half* h0_img, __half* h_img, float* gates,
                  const float* c0, float* cst, float* h_last, float* c_last, __half* hprev_h, __half* y_h,
-                 unsigned int* counter, unsigned int counter_base, int T, int B, int H, int Hp, MaskSrc m, cudaStream_t s,
-                 long long* trace = nullptr, float* h_f32 = nullptr);   // h_f32: optional [N,H] fp32 copy of h_t
+                 unsigned int* counter, unsigned int counter_base, int T, int B, int H, int Hp, MaskSrc m, MaskSrc rm,
+                 cudaStream_t s, long long* trace = nullptr, float* h_f32 = nullptr);   // h_f32: optional [N,H] fp32 copy of h_t
+// m: the output site's mask (period B*H in the variational mode); rm: the recurrent mask of element b*H + j, applied to
+// the operand images and hprev_h (never to h_last, h_f32 or the input of m).
 // Everything the forward needs from the incoming state and tokens in ONE launch (it replaced 9: five device
 // copies, two fp16 conversions, two image packs): h0s/c0s = copies of the incoming (h, c) (the caller may pass
 // the same buffers for the outgoing state), hprev_h rows [0,B) = half(h0) with zeroed pad columns, h0_img = the
-// UMMA-layout image [kc][g][r][e] = half(h0[b = g*8+r, k = kc*8+e]) (null: not built), x_saved = x.
+// UMMA-layout image [kc][g][r][e] = half(h0[b = g*8+r, k = kc*8+e]) (null: not built), x_saved = x.  Variational mode:
+// the half(h0) rows and the image hold h0 * rm[l] (element b*H + k); h0s stays unmasked.
 struct FwdPrep {
     const float* in_h[ZRB_MAX_LAYERS];
     const float* in_c[ZRB_MAX_LAYERS];
@@ -60,6 +64,7 @@ struct FwdPrep {
     float* c0s[ZRB_MAX_LAYERS];
     __half* hprev_h[ZRB_MAX_LAYERS];
     __half* h0_img[ZRB_MAX_LAYERS];
+    MaskSrc rm[ZRB_MAX_LAYERS];
     const int64_t* x;
     int64_t* x_saved;
     int L, B, H, Hp, GB, Kc, N;
@@ -73,7 +78,7 @@ int rec_bwd_plan(int H, int B, RecPlan* plan);   // U = units per CTA, nCTA = 4 
 int pack_whh_bwd(const float* W, __half* img, int H, const RecPlan& p, cudaStream_t s);
 int lstm_rec_bwd(const RecPlan& p, const RecWatchdog& wd, const __half* w_img, __half* g_img, const float* dy, const float* gates,
                  const float* cst, const float* c0, __half* dG_h, unsigned int* counter, unsigned int counter_base, int T,
-                 int B, int H, int G4p, MaskSrc m, cudaStream_t s, long long* trace = nullptr, float* db1 = nullptr,
+                 int B, int H, int G4p, MaskSrc m, MaskSrc rm, cudaStream_t s, long long* trace = nullptr, float* db1 = nullptr,
                  float* db2 = nullptr,    // db1 / db2: bias gradients sum_{t,b} dG [4H] written by the kernel (or null)
                  unsigned int* resident_flag = nullptr, unsigned int resident_value = 0, float* db_scratch = nullptr);
 // resident_flag: CTA 0 stores resident_value there once every CTA of the grid has arrived at the first grid barrier,

@@ -119,12 +119,25 @@ class Model(nn.Module):
 
     Extra keyword `engine`: "tc" (wgmma tensor cores, default) or "simt" (fp32 CUDA cores,
     validation).
+
+    Extra keywords `variational` / `recurrent_dropout`: variational dropout (Gal & Ghahramani 2016; DESIGN.md
+    section 11).  With `variational=True` every dropout mask is drawn once per window and reused at every time step,
+    and the recurrent connection of each layer is dropped with p = `recurrent_dropout` (None: the same p as
+    `dropout`, Gal's setting; 0: no recurrent dropout).  Eval mode applies no mask either way.
     """
 
-    def __init__(self, vocab_size, hidden_size, layer_num, dropout, winit, lstm_type="pytorch", engine="tc"):
+    def __init__(self, vocab_size, hidden_size, layer_num, dropout, winit, lstm_type="pytorch", engine="tc",
+                 variational=False, recurrent_dropout=None):
         super().__init__()
         if lstm_type not in ("pytorch", "custom"):
             raise ValueError(f"lstm_type must be 'pytorch' or 'custom', got {lstm_type!r}")
+        if variational not in (False, True):
+            raise ValueError(f"variational must be True or False, got {variational!r}")
+        if recurrent_dropout is not None and not variational:
+            raise ValueError("recurrent_dropout needs variational=True")
+        p_rec = float(dropout) if (variational and recurrent_dropout is None) else float(recurrent_dropout or 0.0)
+        if not 0.0 <= p_rec < 1.0:
+            raise ValueError(f"recurrent_dropout must be in [0, 1), got {recurrent_dropout!r}")
         if layer_num > _lib.MAX_LAYERS:
             raise ValueError(f"at most {_lib.MAX_LAYERS} layers")
         self.vocab_size = vocab_size
@@ -134,6 +147,8 @@ class Model(nn.Module):
         self.lstm_type = lstm_type
         self.engine = engine
         self.p_drop = float(dropout)
+        self.variational = bool(variational)
+        self.p_rec = p_rec
         self.embed = Embed(vocab_size, hidden_size)
         self.rnns = nn.ModuleList(LSTM(hidden_size, hidden_size, lstm_type) for _ in range(layer_num))
         self.fc = Linear(hidden_size, vocab_size)
@@ -314,7 +329,10 @@ class Model(nn.Module):
 
     def set_explicit_dropout_masks(self, masks):
         """Replay given keep-masks (list of L+1 uint8/bool CUDA tensors [T,B,H]) instead of
-        Philox; None restores Philox.  Used by parity tests with the reference's masks."""
+        Philox; None restores Philox.  Used by parity tests with the reference's masks.  They are Zaremba's per-step
+        masks: a model in the variational mode refuses them."""
+        if masks is not None and self.variational:
+            raise ValueError("explicit dropout masks replay Zaremba's per-step masks; this model uses variational dropout")
         self._explicit_masks = None if masks is None else [m.to(torch.uint8).contiguous() for m in masks]
         if self._ctx is not None:
             self._push_masks()
@@ -342,6 +360,8 @@ class Model(nn.Module):
             _lib.check(lib.zrb_ctx_create(C.byref(cfg), C.byref(h)))
         self._ctx, self._ctx_key = h, key
         self._versions = None
+        if self.variational:
+            _lib.check(lib.zrb_set_variational_dropout(h, 1, self.p_rec))
         if self._explicit_masks is not None:
             self._push_masks()
         return self._ctx
