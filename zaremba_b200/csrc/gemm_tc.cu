@@ -7,13 +7,15 @@
 //                 (6 stages of 128x128 tiles or 4 of 128x256)
 //   warpgroups 1-2  consumers: warpgroup c owns rows [64c, 64c+64) of the 128-row tile, issues wgmma m64nNk16
 //                 (N = tile width) on each landed stage, releases the stage once the next stage's wgmmas are in
-//                 flight, and stores its accumulators (alpha, bias, fp32 stores or split-K atomics) itself
+//                 flight, and stores its accumulators (alpha, bias, fp32 stores or split-K atomics) itself; the two
+//                 warpgroups run kStages-1 K blocks apart, so one's epilogue overlaps the other's wgmmas
 //
 // Every batched contraction of the path runs here: X*W_ih^T, the vocabulary projection, their
 // dgrads (weights read MN-major from the same fp16 image, no transposed copies) and the
 // wgrads (both operands MN-major: contraction over tokens).  Roofline: tensor pipe
 // (2*M*N*K flop per call); operands stream once from HBM/L2 via TMA.
 #include <stdlib.h>
+#include <string.h>
 
 #include "kernels.h"
 #include "tc_common.cuh"
@@ -57,7 +59,16 @@ struct GemmArgs {
     int pdl_tail;     // launched as a programmatic dependent of the kernel before it in the stream (it started while that
                       // kernel was still running and consumes none of its outputs): wait for that kernel before exiting,
                       // so that "this grid completed" keeps implying "everything before it in the stream completed"
+    int epi_direct;   // ZRB_GEMM_EPI=direct: both consumer warpgroups in lockstep, one 4-byte store per element
 };
+
+// Staggered consumers (the default): warpgroup 1 starts its first work item only once warpgroup 0 has issued the
+// wgmmas of kStagger K blocks (or all of its first item, if shorter).  Both stay that far apart -- the producer can
+// only refill a stage that both have released -- so each warpgroup's epilogue runs while the other one issues wgmmas
+// instead of leaving the tensor cores idle.  kStagger < kStages: warpgroup 0 gets there on stages the producer loads
+// before anything is released.
+template <int GBN> constexpr int kStagger = GemmCfg<GBN>::kStages - 1;
+constexpr int kStaggerBar = 1;   // named barrier of the two consumer warpgroups (256 threads)
 
 template <bool A_MN, bool B_MN, int GBN>
 __global__ void __launch_bounds__(kGemmThreads, 1)
@@ -137,6 +148,12 @@ gemm_f16_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_const
         const int t = (int)threadIdx.x - 128 * (1 + wg);
         int s = 0; uint32_t ph = 0;
         float acc[GBN / 2];
+        bool started_wg1 = p.epi_direct || wg == 1;   // (warpgroup 0) has warpgroup 1 been let go
+        if (!p.epi_direct && wg == 1) asm volatile("bar.sync %0, 256;" :: "n"(kStaggerBar) : "memory");
+        int kb_issued = 0;
+        // float2 stores (and float2 atomics for split-K): a quad of lanes writes one whole 32-byte sector of a row
+        const bool pair_store = !p.epi_direct && !p.accumulate && (p.ldc & 1) == 0 && ((uintptr_t)p.C & 7) == 0 &&
+                                ((uintptr_t)p.C2 & 7) == 0;
         for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
             const int tile = w % num_tiles, split = dual ? 0 : w / num_tiles;
             const int kb0 = split * kb_per, kb1 = min(num_kb, kb0 + kb_per);
@@ -166,6 +183,10 @@ gemm_f16_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_const
                     Wgmma<GBN, A_MN ? 1 : 0, B_MN ? 1 : 0>::mma(acc, da, db, 1u);
                 }
                 wgmma_commit();
+                if (!started_wg1 && ++kb_issued == kStagger<GBN>) {
+                    asm volatile("bar.arrive %0, 256;" :: "n"(kStaggerBar) : "memory");
+                    started_wg1 = true;
+                }
                 wgmma_wait<1>();                        // the previous stage's wgmmas are done: hand it back
                 if (prev >= 0) {
                     __syncwarp();
@@ -173,6 +194,10 @@ gemm_f16_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_const
                 }
                 prev = s;
                 if (++s == kStages) { s = 0; ph ^= 1; }
+            }
+            if (!started_wg1) {                         // a first work item shorter than kStagger K blocks
+                asm volatile("bar.arrive %0, 256;" :: "n"(kStaggerBar) : "memory");
+                started_wg1 = true;
             }
             wgmma_wait<0>();
             wgmma_fence_acc(acc);
@@ -190,6 +215,22 @@ gemm_f16_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_const
                 float* const crow = Cout + (int64_t)row * p.ldc;
 #pragma unroll
                 for (int c8 = 0; c8 < GBN / 8; ++c8) {
+                    const int col0 = n0 + wgmma_col(t, c8);   // even
+                    if (pair_store && col0 + 1 < p.N) {
+                        // the same two elements, values and sum-of-squares order as the per-element loop below
+                        const float bv0 = add_bias ? p.bias[col0] + (p.bias2 ? p.bias2[col0] : 0.f) : 0.f;
+                        const float bv1 = add_bias ? p.bias[col0 + 1] + (p.bias2 ? p.bias2[col0 + 1] : 0.f) : 0.f;
+                        const float o0 = p.alpha * acc[4 * c8 + 2 * h] + bv0;
+                        const float o1 = p.alpha * acc[4 * c8 + 2 * h + 1] + bv1;
+                        if (p.splits > 1) {
+                            atomicAdd(reinterpret_cast<float2*>(crow + col0), make_float2(o0, o1));
+                        } else {
+                            *reinterpret_cast<float2*>(crow + col0) = make_float2(o0, o1);
+                            ss += o0 * o0;
+                            ss += o1 * o1;
+                        }
+                        continue;
+                    }
 #pragma unroll
                     for (int e = 0; e < 2; ++e) {
                         const int col = n0 + wgmma_col(t, c8) + e;
@@ -212,6 +253,7 @@ gemm_f16_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_const
                 if (lane == 0) ssq[tile * 8 + cw] = ss;
             }
         }
+        if (!started_wg1) asm volatile("bar.arrive %0, 256;" :: "n"(kStaggerBar) : "memory");   // (a CTA without work)
     }
     // ONE CTA keeps the grid from completing before the primary has: a CTA blocked here holds its SM, and if every
     // CTA waited, the SMs the recurrence leaves idle would each run a single tile and then sit until it ends
@@ -327,8 +369,12 @@ static int dispatch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const CUt
 
 // Tile shape for an [M,N] output with K-block count num_kb: 128x256 when those tiles give every SM (nearly) a
 // full wave, else 128x128; few output tiles but a long contraction (the dgrads) split K.
+// With `retile` (outputs without sum-of-squares slots, ZRB_GEMM_EPI unset), an unsplit 256-wide plan whose last round
+// of the persistent grid is mostly empty switches to 128-wide tiles when those need fewer rounds counted in
+// 256-wide-tile units (X*W_ih^T at Large: 144 tiles = 2 rounds on 132 SMs, vs 282 half tiles = 3 half rounds).  The
+// tile width does not change what is summed per output element, nor in which K order.
 struct TileChoice { int bn, tiles_m, tiles_n, splits; };
-static TileChoice choose_tiles(int M, int N, int num_kb, bool can_split) {
+static TileChoice choose_tiles(int M, int N, int num_kb, bool can_split, bool retile = false) {
     const int nsm = tc_num_sms();
     TileChoice c;
     c.tiles_m = cdiv(M, GBM);
@@ -343,6 +389,9 @@ static TileChoice choose_tiles(int M, int N, int num_kb, bool can_split) {
     c.bn = (t256 >= (nsm * 9) / 10) ? 256 : 128;
     static const int force_bn = [] { const char* e = getenv("ZRB_GEMM_BN"); return e ? atoi(e) : 0; }();   // experiment switch
     if (force_bn == 128 || force_bn == 256) c.bn = force_bn;
+    else if (retile && c.bn == 256 && cdiv(t256, nsm) * 2 > cdiv(c.tiles_m * cdiv(N, 128), nsm) &&
+             c.tiles_m * cdiv(N, 128) * 2 > nsm)   // (never turns a whole plan into a split one)
+        c.bn = 128;
     c.tiles_n = cdiv(N, c.bn);
     // few output tiles but a long contraction: split K in two so that ~all SMs work; partials added into a
     // zeroed C with atomics
@@ -365,7 +414,12 @@ int gemm_f16_tc(const __half* A, int64_t lda, int a_mn, const __half* B, int64_t
     ZRB_REQUIRE(!bias2 || bias, "bias2 needs bias");
     ZRB_REQUIRE(!sumsq_out || !accumulate, "sumsq_out needs a plain store epilogue");
     ZRB_REQUIRE(K > 0, "gemm_f16_tc needs K > 0");
-    const TileChoice tc = choose_tiles(M, N, cdiv(K, GBK), !sumsq_out && ldc == N && !C2 && !accumulate);
+    // ZRB_GEMM_EPI=direct: the lockstep consumers with per-element stores and the tile plan they were tuned with (A/B
+    // comparisons, bit for bit and in time); read at every launch so that one process can run both
+    const char* epi = getenv("ZRB_GEMM_EPI");
+    const bool direct = epi && strcmp(epi, "direct") == 0;
+    const TileChoice tc = choose_tiles(M, N, cdiv(K, GBK), !sumsq_out && ldc == N && !C2 && !accumulate,
+                                       !direct && !sumsq_out && !C2 && !accumulate);
     const int bn = tc.bn;
     CUtensorMap ta, tb;
     if (!a_mn) ZRB_TRY(tc_make_tmap_f16(&ta, A, K, M, lda, GBK, GBM, 1));
@@ -387,6 +441,7 @@ int gemm_f16_tc(const __half* A, int64_t lda, int a_mn, const __half* B, int64_t
     a.a_tiled = a_mn ? nullptr : A_tiled; a.a_nt128 = a_nt128; a.b_tiled = b_mn ? nullptr : B_tiled; a.b_nt128 = b_nt128;
     a.pdl_tail = (pdl && a.splits == 1) ? 1 : 0;    // (a split launch is preceded by a memset: nothing to chain to)
     a.pdl_trigger = (rec_pdl_enabled() && !a.pdl_tail) ? 1 : 0;
+    a.epi_direct = direct ? 1 : 0;
     // split partials are added into a zeroed C: order-independent for two (a+b == b+a)
     if (a.splits > 1 && !accumulate) ZRB_CUDA(cudaMemsetAsync(C, 0, (size_t)M * N * sizeof(float), s));
     return bn == 256 ? dispatch_gemm<256>(ta, tb, tb2, a, a_mn, b_mn, s) : dispatch_gemm<128>(ta, tb, tb2, a, a_mn, b_mn, s);
