@@ -321,6 +321,38 @@ int  zrb_beam_search(zrb_ctx* ctx, const zrb_params* p, const int64_t* prompt, i
                      const zrb_states* in, const zrb_states* out, int32_t n_new, int32_t K, int32_t eos,
                      int64_t* tokens, float* logprobs, float* scores, void* stream);
 
+/* ---- neural-cache evaluation (Grave, Joulin & Usunier, "Improving Neural Language Models with a Continuous Cache",
+ * ICLR 2017; DESIGN.md section 12 states it bit for bit) ---------------------------------------------------------
+ * Per stream b (batch row) the cache holds pairs (k_i, y_i), i the stream's position (tokens fed since the last
+ * reset, counted across calls): k_i = half_rn(h_i), the last layer's output at i, and y_i the target at i.  A query at
+ * position t with target y_t, cache size W, temperature theta >= 0 and weight lambda in [0, 1):
+ *   C_t = { i : max(0, t - W) <= i < t }   (earlier calls and earlier rows of this window; never t itself)
+ *   s_i = theta * <half(h_t), k_i>,  p_cache = sum_{i in C_t, y_i = y_t} exp(s_i - m) / sum_{i in C_t} exp(s_i - m)
+ *   p = (1 - lambda) p_model + lambda p_cache, row loss = -logaddexp(log(1 - lambda) - r, log(lambda) + log(p_cache))
+ *   with r = -log p_model the eval step's row loss; C_t empty (a stream's first token): p = p_model, p_cache = 0.
+ * The window loss reduces the row losses as zrb_eval_step does (summed over the batch, averaged over time); lambda = 0
+ * gives zrb_eval_step's loss bit for bit.  The handle is independent of any context; its position counter lives on the
+ * host (no synchronisation) and a reset only zeroes it.  hidden <= 1536 (the query tile stays in shared memory).
+ * ZRB_E_INVALID for hidden outside [1, 1536], batch, size or max_seq < 1. */
+typedef struct zrb_cache zrb_cache;   /* opaque */
+int  zrb_cache_create(int32_t hidden, int32_t batch, int32_t size, int32_t max_seq, zrb_cache** out);
+int  zrb_cache_reset(zrb_cache* cache);
+void zrb_cache_destroy(zrb_cache* cache);
+/* The unit on its own, with no model: append h [T,B,H] fp32 (rounded to fp16) and targets y [T,B] int64 to the cache,
+ * then cache_prob [T*B] fp32 = p_cache of every row.  ZRB_E_INVALID (handle unchanged) for theta < 0 or not finite,
+ * B other than the cache's, T outside [1, max_seq], and a current device other than the one the cache was created on. */
+int  zrb_cache_step(zrb_cache* cache, const float* h, const int64_t* y, int32_t T, int32_t B, float theta,
+                    float* cache_prob, void* stream);
+/* zrb_eval_step with the cache: the same eval-mode forward (pending lazy updates applied first, no dropout) and row
+ * losses, then the window's last-layer outputs and targets are appended to the cache and every row attends over it.
+ * loss: the window loss of the mixed p; tgt_prob [T*B] (or NULL): p_model, zrb_eval_step's tgt_prob; cache_prob [T*B]
+ * (or NULL): p_cache.  With both, a caller can sweep lambda on the host.  Two launches more than zrb_eval_step (append,
+ * attend and combine; the combine does the loss reduction).
+ * ZRB_E_INVALID (handle unchanged) as zrb_cache_step, for lambda outside [0, 1), and for an H other than the cache's. */
+int  zrb_eval_step_cache(zrb_ctx* ctx, const zrb_params* p, const int64_t* x, const int64_t* y, int32_t T, int32_t B,
+                         const zrb_states* in, const zrb_states* out, zrb_cache* cache, float theta, float lambda,
+                         float* loss, float* tgt_prob, float* cache_prob, void* stream);
+
 /* Same as zrb_train_step_grads + zrb_train_step_update but with HOST token buffers
  * (pinned or pageable) and a host loss: the H2D copies of x, y and the D2H copy of the
  * loss are issued on `stream` inside the call; the call returns after the loss landed. */

@@ -84,6 +84,12 @@ _SIGNATURES = {
                                 _vp, _vp, _vp, _vp]),
     "zrb_beam_search": (C.c_int, [_vp, C.POINTER(ZrbParams), _vp, C.c_int32, C.c_int32, C.POINTER(ZrbStates),
                                   C.POINTER(ZrbStates), C.c_int32, C.c_int32, C.c_int32, _vp, _vp, _vp, _vp]),
+    "zrb_cache_create": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.POINTER(_vp)]),
+    "zrb_cache_reset": (C.c_int, [_vp]),
+    "zrb_cache_destroy": (None, [_vp]),
+    "zrb_cache_step": (C.c_int, [_vp, _vp, _vp, C.c_int32, C.c_int32, C.c_float, _vp, _vp]),
+    "zrb_eval_step_cache": (C.c_int, [_vp, C.POINTER(ZrbParams), _vp, _vp, C.c_int32, C.c_int32, C.POINTER(ZrbStates),
+                                      C.POINTER(ZrbStates), _vp, C.c_float, C.c_float, _vp, _vp, _vp, _vp]),
     "zrb_train_step_host": (C.c_int, [_vp, C.POINTER(ZrbParams), C.POINTER(ZrbParams), _vp, _vp, C.c_int32,
                                       C.c_int32, C.POINTER(ZrbStates), C.POINTER(ZrbStates), C.c_uint64,
                                       C.c_uint64, C.c_float, C.c_float, _vp, _vp, _vp]),

@@ -116,6 +116,7 @@ int tc_train_step_layer(zrb_ctx* c, const zrb_params* p, const zrb_params* g, in
 int tc_rec_trace(zrb_ctx* c, long long* h_out, int max_entries);
 int tc_flush_updates(zrb_ctx* c, cudaStream_t s);   // apply deferred weight updates now (zrb_set_lazy_update)
 bool tc_persistent_bwd(const zrb_ctx* c);
+const __half* tc_last_layer_image(const zrb_ctx* c);   // x_h[L]: fp16 last-layer output of the last forward, pitch pad64(H)
 void tc_rec_plans(const zrb_ctx* c, int32_t* h_out);   // zrb_rec_plans: 2 x {ok, KS, U, G, nCTA, GBi, Kc, KcS}
 int tc_layer_fwd(zrb_ctx* c, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh, const float* x,
                  int T, int B, const float* h0, const float* c0, float* y, float* hT, float* cT, cudaStream_t s);

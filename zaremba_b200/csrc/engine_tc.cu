@@ -261,6 +261,8 @@ int tc_forward(zrb_ctx* c, const zrb_params* p, const int64_t* x, const zrb_stat
     return ZRB_OK;
 }
 
+const __half* tc_last_layer_image(const zrb_ctx* c) { return c->tc->x_h[c->cfg.layers]; }
+
 static bool prof_keeps_pdl() {
     static const bool on = getenv("ZRB_PROF_KEEP_PDL") != nullptr;
     return on;

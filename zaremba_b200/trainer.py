@@ -385,27 +385,47 @@ class Trainer:
         return float(self._hloss[0]), float(self._hloss[1])
 
     # ---- main.py:91-94 --------------------------------------------------------------------
-    def eval_step(self, x, y, want_probs=False):
+    def eval_step(self, x, y, want_probs=False, cache=None, theta=0.0, lam=0.0):
         """Eval-mode forward + loss on device tokens; carries `self.states`.  Returns the loss
         tensor (main.py:92) and, if asked, softmax(scores)[n, y_n] for the ensemble
-        (ensemble.py:100-106)."""
+        (ensemble.py:100-106).
+        cache: a `NeuralCache` -> zrb_eval_step_cache: the window is appended to the cache and the loss is that of
+        (1 - lam) p_model + lam p_cache at temperature theta (DESIGN.md section 12).  With want_probs the return is
+        (loss, p_model, p_cache), [T*B] each, from which any lam can be evaluated on the host."""
         lib = _lib.load()
         T, B = x.shape
         self._check_versions()
         self._pending = False          # zrb_eval_step applies what is pending before it reads the weights
+        if cache is not None:
+            return self._eval_step_cache(lib, x, y, T, B, want_probs, cache, theta, lam)
         _lib.check(lib.zrb_eval_step(self.ctx, C.byref(self._ps), _lib.ptr(x), _lib.ptr(y), T, B,
                                      C.byref(self._st), C.byref(self._st), _lib.ptr(self.loss),
                                      _lib.ptr(self.tgt_prob) if want_probs else None, self._stream()))
         return (self.loss, self.tgt_prob[: T * B]) if want_probs else self.loss
 
-    def perplexity(self, batches):
+    def _eval_step_cache(self, lib, x, y, T, B, want_probs, cache, theta, lam):
+        if not hasattr(self, "cache_prob"):
+            self.cache_prob = torch.zeros_like(self.tgt_prob)
+        _lib.check(lib.zrb_eval_step_cache(self.ctx, C.byref(self._ps), _lib.ptr(x), _lib.ptr(y), T, B,
+                                           C.byref(self._st), C.byref(self._st), cache.handle, float(theta), float(lam),
+                                           _lib.ptr(self.loss), _lib.ptr(self.tgt_prob) if want_probs else None,
+                                           _lib.ptr(self.cache_prob) if want_probs else None, self._stream()))
+        if want_probs:
+            return self.loss, self.tgt_prob[: T * B], self.cache_prob[: T * B]
+        return self.loss
+
+    def perplexity(self, batches, cache=None, theta=0.0, lam=0.0):
         """main.py:86-95 with the per-batch `.item()` sync removed: losses accumulate on the
-        device and are read once."""
+        device and are read once.  cache: a `NeuralCache`, reset together with the states, through which every window
+        is evaluated (eval_step(cache=, theta=, lam=))."""
         self.reset_states()
+        if cache is not None:
+            cache.reset()
         acc = torch.zeros((), device=self.dev, dtype=torch.float64)
         n = 0
         for x, y in batches:
             xd = x.to(self.dev).contiguous(); yd = y.to(self.dev).contiguous()
-            acc += self.eval_step(xd, yd).double() / x.shape[1]
+            loss = self.eval_step(xd, yd) if cache is None else self.eval_step(xd, yd, cache=cache, theta=theta, lam=lam)
+            acc += loss.double() / x.shape[1]
             n += 1
         return math.exp(acc.item() / max(n, 1))
