@@ -52,8 +52,17 @@ typedef struct {
     int32_t max_batch;    /* B  upper bound */
     int32_t engine;       /* ZRB_ENGINE_*   */
     float   dropout;      /* p of nn.Dropout (model.py:87) */
-    int32_t reserved;
+    int32_t flags;        /* ZRB_TIED_EMBEDDING or 0; any other bit: ZRB_E_INVALID */
 } zrb_config;
+
+/* Tied embedding and softmax weights (Press & Wolf, "Using the Output Embedding to Improve Language Models", EACL 2017;
+ * DESIGN.md section 13).  One matrix E [V,H] is both embed.W and fc.W: every zrb_params passed to a tied context, for
+ * parameters and for gradients, must have fc_w == embed_w (ZRB_E_INVALID, before anything is launched, otherwise).
+ * Forward: x0 = E[x], scores = A_L E^T + b.  Gradient: dE = G_proj + G_emb, where G_proj = dS^T A_L is the projection's
+ * weight gradient and, per distinct token id r of the window, e_r = the 2^-40 fixed-point sum of its dropout-masked
+ * embedding-gradient rows converted to fp32 once; dE[r] = fp32(G_proj[r] + e_r) (no float atomics: bit-reproducible).
+ * The clip norm and the update take E once.  zrb_embed_scatter_rows ADDS its sums into the (reduced) gradient. */
+#define ZRB_TIED_EMBEDDING 1
 
 /* The 11 (= 3 + 4L) parameter tensors in the reference's registration order
  * (model.py:83-86; SURVEY 8b): fp32, row-major, contiguous. */
@@ -167,7 +176,9 @@ int  zrb_train_step_layer(zrb_ctx* ctx, const zrb_params* p, const zrb_params* g
  * dropout-masked gradient rows [N,H] there INSTEAD of scattering them into the dense table gradient; ranks
  * all-gather ids and rows (4 MB each instead of a 60 MB all-reduce) and zrb_embed_scatter_rows builds the
  * dense gradient: rows with equal id are summed in index order by the first occurrence, without atomics, so
- * all ranks get identical bits.  Pass NULL to return to the dense scatter. */
+ * all ranks get identical bits.  Pass NULL to return to the dense scatter.  In a ZRB_TIED_EMBEDDING context the
+ * dense gradient already holds the (reduced) projection gradient: zrb_embed_scatter_rows adds the sums of the
+ * ids' rows into it (dE[r] = fp32(G_proj[r] + e_r)) instead of clearing and writing. */
 int  zrb_set_embed_rows_out(zrb_ctx* ctx, float* rows);
 /* Single-process fused step (zrb_train_step_grads/_update with the SAME grads buffers every step): touch only
  * this window's rows of the dense embedding gradient (clear the previous window's rows instead of zero-filling

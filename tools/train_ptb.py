@@ -52,6 +52,8 @@ ap.add_argument("--variational", action="store_true",
                 help="variational dropout (Gal & Ghahramani 2016): masks fixed over each window, recurrent dropout")
 ap.add_argument("--recurrent_dropout", type=float, default=None,
                 help="p of the recurrent masks with --variational (default: --dropout)")
+ap.add_argument("--tied", action="store_true",
+                help="tie the embedding and softmax weights (Press & Wolf 2017): fc.W is embed.W")
 ap.add_argument("--lazy_update", action="store_true",
                 help="Trainer(lazy_update=True): upper-layer / fc weight updates run beside the next step's forward")
 ap.add_argument("--eval_batch_size", type=int, default=None,
@@ -95,7 +97,8 @@ torch.manual_seed(args.seed)
 
 if args.impl == "ours":
     model = zaremba_b200.Model(vocab, args.hidden_size, args.layer_num, args.dropout, args.winit,
-                               variational=args.variational, recurrent_dropout=args.recurrent_dropout).to(dev)
+                               variational=args.variational, recurrent_dropout=args.recurrent_dropout,
+                               tied=args.tied).to(dev)
     tr = zaremba_b200.Trainer(model, B, T, lazy_update=args.lazy_update)
     # the corpus is staged on the device once (SURVEY 8f#2): 3 x [n_batches, T, B] int64
     trn_x = torch.stack([x for x, _ in trn_b]).contiguous().to(dev)
@@ -122,6 +125,8 @@ else:
         raise SystemExit("--impl cudnn is the reference's single-device path")
     if args.variational:
         raise SystemExit("--variational is a mode of --impl ours")
+    if args.tied:
+        raise SystemExit("--tied is a mode of --impl ours (the reference's cudnn path keeps embed.W and fc.W apart)")
     from oracle import torch_port as P
     model = P.TorchLstmLm(vocab, args.hidden_size, args.layer_num, args.dropout, args.winit).to(dev)
     trn_d = [(x.to(dev), y.to(dev)) for x, y in trn_b]

@@ -14,6 +14,7 @@ MAX_LAYERS = 8
 MAX_BEAMS = 32
 ENGINE_SIMT = 0
 ENGINE_TC = 1
+TIED_EMBEDDING = 1   # zrb_config.flags bit ZRB_TIED_EMBEDDING
 
 _f32p = C.POINTER(C.c_float)
 _vp = C.c_void_p
@@ -22,7 +23,7 @@ _vp = C.c_void_p
 class ZrbConfig(C.Structure):
     _fields_ = [("vocab", C.c_int32), ("hidden", C.c_int32), ("layers", C.c_int32),
                 ("max_seq", C.c_int32), ("max_batch", C.c_int32), ("engine", C.c_int32),
-                ("dropout", C.c_float), ("reserved", C.c_int32)]
+                ("dropout", C.c_float), ("flags", C.c_int32)]
 
 
 class ZrbParams(C.Structure):

@@ -61,6 +61,13 @@ static int check_shapes(const zrb_ctx* c, int T, int B) {
     return ZRB_OK;
 }
 
+// a tied context takes E once: fc_w must be embed_w in parameters and gradients alike
+static int check_tied(const zrb_ctx* c, const zrb_params* p) {
+    ZRB_REQUIRE(!c->tied || !p || p->fc_w == p->embed_w, "tied context: fc_w (%p) must equal embed_w (%p)",
+                (void*)p->fc_w, (void*)p->embed_w);
+    return ZRB_OK;
+}
+
 MaskSrc site_mask(const zrb_ctx* c, int site) {
     const uint8_t* ex = c->explicit_masks_set ? c->explicit_masks[site] : nullptr;
     MaskSrc m = make_mask_src(ex, c->seed, c->step, site, c->cfg.dropout, c->train);
@@ -111,6 +118,7 @@ int zrb_ctx_create(const zrb_config* cfg, zrb_ctx** out) {
     ZRB_REQUIRE(cfg->max_seq > 0 && cfg->max_batch > 0, "bad window T=%d B=%d", cfg->max_seq, cfg->max_batch);
     ZRB_REQUIRE(cfg->dropout >= 0.f && cfg->dropout < 1.f, "dropout %f outside [0,1)", cfg->dropout);
     ZRB_REQUIRE(cfg->engine == ZRB_ENGINE_SIMT || cfg->engine == ZRB_ENGINE_TC, "unknown engine %d", cfg->engine);
+    ZRB_REQUIRE((cfg->flags & ~ZRB_TIED_EMBEDDING) == 0, "unknown config flags 0x%x", (unsigned)cfg->flags);
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
         set_error("no CUDA device: libzaremba_b200 has no CPU path");
@@ -118,6 +126,7 @@ int zrb_ctx_create(const zrb_config* cfg, zrb_ctx** out) {
     }
     zrb_ctx* c = new zrb_ctx();
     c->cfg = *cfg;
+    c->tied = (cfg->flags & ZRB_TIED_EMBEDDING) != 0;
     const int H = cfg->hidden, L = cfg->layers, V = cfg->vocab;
     const size_t N = (size_t)cfg->max_seq * cfg->max_batch, BH = (size_t)cfg->max_batch * H;
     int rc = ZRB_OK;
@@ -154,6 +163,10 @@ int zrb_ctx_create(const zrb_config* cfg, zrb_ctx** out) {
         }
     }
     if (rc == ZRB_OK) rc = dalloc(c, &c->emb_first, (size_t)V);
+    if (rc == ZRB_OK && c->tied) {   // fixed-point sums of the embedding rows, every backward
+        rc = dalloc(c, &c->emb_acc, N * H);
+        c->emb_cap_rows = (int64_t)N;
+    }
     if (rc == ZRB_OK) rc = dalloc(c, &c->y_dev, N);
     if (rc == ZRB_OK) rc = dalloc(c, &c->x_dev, N);
     if (rc == ZRB_OK) rc = dalloc(c, &c->scores, N * V);
@@ -247,6 +260,7 @@ int zrb_forward(zrb_ctx* c, const zrb_params* p, const int64_t* x, int32_t T, in
                 const zrb_states* out, float* scores, int32_t train, uint64_t seed, uint64_t step, void* stream) {
     ZRB_REQUIRE(c && p && x && in && out, "null argument");
     ZRB_TRY(check_shapes(c, T, B));
+    ZRB_TRY(check_tied(c, p));
     cudaStream_t s = (cudaStream_t)stream;
     c->T = T; c->B = B; c->train = train ? 1 : 0; c->seed = seed; c->step = step;
     c->have_fwd = false;
@@ -260,6 +274,8 @@ int zrb_forward(zrb_ctx* c, const zrb_params* p, const int64_t* x, int32_t T, in
 
 int zrb_backward(zrb_ctx* c, const zrb_params* p, const float* dscores, const zrb_params* g, void* stream) {
     ZRB_REQUIRE(c && p && dscores && g, "null argument");
+    ZRB_TRY(check_tied(c, p));
+    ZRB_TRY(check_tied(c, g));
     if (!c->have_fwd) {
         set_error("zrb_backward without a preceding zrb_forward");
         return ZRB_E_STATE;
@@ -304,6 +320,7 @@ static TensorList param_list(const zrb_ctx* c, const zrb_params* p, const zrb_pa
         tl.p[k] = p->b_hh[l]; tl.g[k] = g->b_hh[l]; tl.n[k++] = 4 * H;
     }
     tl.p[k] = p->fc_w; tl.g[k] = g->fc_w; tl.n[k++] = V * H;
+    if (c->tied) tl.n[0] = 0;   // E once, at fc.W's slot (zero-length entries are skipped by the norm and the update)
     tl.p[k] = p->fc_b; tl.g[k] = g->fc_b; tl.n[k++] = V;
     tl.count = k;
     return tl;
@@ -316,6 +333,8 @@ int zrb_train_step_grads(zrb_ctx* c, const zrb_params* p, const zrb_params* g, c
     ZRB_REQUIRE(c->cfg.layers * 4 + 3 <= 16, "fused step supports at most 3 layers");
     cudaStream_t s = (cudaStream_t)stream;
     ZRB_TRY(check_shapes(c, T, B));
+    ZRB_TRY(check_tied(c, p));
+    ZRB_TRY(check_tied(c, g));
     if (c->cfg.engine == ZRB_ENGINE_TC) return tc_train_step_grads(c, p, g, x, y, T, B, in, out, seed, step, loss, s);
     ZRB_TRY(zrb_forward(c, p, x, T, B, in, out, c->scores, 1, seed, step, stream));
     {
@@ -332,6 +351,8 @@ int zrb_train_step_begin(zrb_ctx* c, const zrb_params* p, const zrb_params* g, c
                          uint64_t step, float* loss, void* stream) {
     ZRB_REQUIRE(c && p && g && x && y && in && out, "null argument");
     ZRB_TRY(check_shapes(c, T, B));
+    ZRB_TRY(check_tied(c, p));
+    ZRB_TRY(check_tied(c, g));
     if (c->cfg.engine == ZRB_ENGINE_TC)
         return tc_train_step_begin(c, p, g, x, y, T, B, in, out, seed, step, loss, (cudaStream_t)stream);
     ZRB_TRY(zrb_train_step_grads(c, p, g, x, y, T, B, in, out, seed, step, loss, stream));   // validation engine: all at once
@@ -342,6 +363,8 @@ int zrb_train_step_begin(zrb_ctx* c, const zrb_params* p, const zrb_params* g, c
 int zrb_train_step_layer(zrb_ctx* c, const zrb_params* p, const zrb_params* g, int32_t layer, void* stream) {
     ZRB_REQUIRE(c && p && g, "null argument");
     ZRB_REQUIRE(layer >= 0 && layer < c->cfg.layers, "layer %d out of range", layer);
+    ZRB_TRY(check_tied(c, p));
+    ZRB_TRY(check_tied(c, g));
     if (c->cfg.engine == ZRB_ENGINE_TC) return tc_train_step_layer(c, p, g, layer, (cudaStream_t)stream);
     if (layer != c->bwd_next_layer) {
         set_error("backward layers must be visited in order L-1..0");
@@ -396,6 +419,8 @@ int zrb_embed_scatter_rows(zrb_ctx* c, float* grad_embed, const int64_t* ids, co
     }
     ProfScope ps(c, ZRB_PROF_EMBED_BWD, s);
     const int H = c->cfg.hidden, V = c->cfg.vocab;
+    // tied: grad_embed holds the reduced projection gradient, every row of it non-zero and updated densely
+    if (c->tied) return embed_scatter_rows(ids, rows, grad_embed, (int)n_rows, H, V, c->emb_first, c->emb_acc, s, true);
     if (c->emb_sparse && c->emb_prev_grad == grad_embed) {
         ZRB_TRY(embed_zero_rows(grad_embed, c->emb_prev_ids, c->emb_prev_n, H, V, s));   // only the last step's rows are non-zero
     } else {
@@ -419,6 +444,8 @@ int zrb_train_step_update(zrb_ctx* c, const zrb_params* p, const zrb_params* g, 
     ZRB_REQUIRE(c && p && g, "null argument");
     ZRB_TRY(watchdog_check(c));
     ZRB_REQUIRE(c->cfg.layers * 4 + 3 <= 16, "fused step supports at most 3 layers");
+    ZRB_TRY(check_tied(c, p));
+    ZRB_TRY(check_tied(c, g));
     TensorList tl = param_list(c, p, g);
     if (c->cfg.engine == ZRB_ENGINE_TC) return tc_update(c, p, tl, lr, max_norm, norm_out, (cudaStream_t)stream);
     {
@@ -433,6 +460,7 @@ int zrb_eval_step(zrb_ctx* c, const zrb_params* p, const int64_t* x, const int64
                   const zrb_states* in, const zrb_states* out, float* loss, float* tgt_prob, void* stream) {
     ZRB_REQUIRE(c && p && x && y && in && out, "null argument");
     ZRB_TRY(check_shapes(c, T, B));
+    ZRB_TRY(check_tied(c, p));
     ZRB_TRY(zrb_forward(c, p, x, T, B, in, out, c->scores, 0, 0, 0, stream));
     c->have_fwd = false;  // eval keeps nothing for backward
     return softmax_nll(c->scores, y, T * B, c->cfg.vocab, B, c->row_loss, loss, nullptr, tgt_prob,
@@ -458,6 +486,7 @@ int zrb_generate(zrb_ctx* c, const zrb_params* p, const int64_t* prompt, int32_t
     ZRB_REQUIRE(T0 >= 1 && n_new >= 1, "T0=%d and n_new=%d must be >= 1", T0, n_new);
     ZRB_TRY(check_shapes(c, 1, B));
     ZRB_TRY(sample_check(cfg, B, c->cfg.vocab));
+    ZRB_TRY(check_tied(c, p));
     cudaStream_t s = (cudaStream_t)stream;
     const int V = c->cfg.vocab, S = c->cfg.max_seq;
     c->B = B; c->train = 0; c->seed = 0; c->step = 0;
@@ -526,6 +555,7 @@ int zrb_beam_search(zrb_ctx* c, const zrb_params* p, const int64_t* prompt, int3
     ZRB_REQUIRE((int64_t)B * K <= c->cfg.max_batch, "B*K=%lld above the context's max_batch %d", (long long)B * K,
                 c->cfg.max_batch);
     ZRB_TRY(check_shapes(c, 1, B * K));
+    ZRB_TRY(check_tied(c, p));
     cudaStream_t s = (cudaStream_t)stream;
     const int V = c->cfg.vocab, S = c->cfg.max_seq, L = c->cfg.layers, H = c->cfg.hidden, BK = B * K;
     ZRB_TRY(beam_scratch(c, (int64_t)n_new * BK));
@@ -561,6 +591,8 @@ int zrb_train_step_host(zrb_ctx* c, const zrb_params* p, const zrb_params* g, co
                         void* stream) {
     ZRB_REQUIRE(c && h_x && h_y && h_loss, "null argument");
     ZRB_TRY(check_shapes(c, T, B));
+    ZRB_TRY(check_tied(c, p));
+    ZRB_TRY(check_tied(c, g));
     cudaStream_t s = (cudaStream_t)stream;
     size_t nb = (size_t)T * B * sizeof(int64_t);
     ZRB_CUDA(cudaMemcpyAsync(c->x_dev, h_x, nb, cudaMemcpyHostToDevice, s));

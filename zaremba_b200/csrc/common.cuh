@@ -168,6 +168,10 @@ __device__ inline float mask_mul1(const MaskSrc& m, uint64_t e, uint64_t n_total
 
 __device__ inline float sigmoidf_(float z) { return 1.f / (1.f + expf(-z)); }
 
+// one SGD element (main.py:117) with the clipped gradient g = coef * grad: the ONE expression update_pack stores and the
+// tied embedding's gather through a deferred update reads, so that the two agree bit for bit
+__device__ __forceinline__ float sgd_elem(float p, float g, float lr) { return p - lr * g; }
+
 __device__ inline float warp_sum(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

@@ -55,6 +55,7 @@ struct zrb_ctx {
     bool emb_sparse = false;               // touch only the rows of the embedding gradient that can be non-zero
     bool lazy_update = false;              // zrb_set_lazy_update: upper-layer / fc weight updates run beside the next forward
     bool fused_norm = false;               // single process: matrices' part of the clip norm from the wgrad GEMM epilogues
+    bool tied = false;                     // ZRB_TIED_EMBEDDING: embed_w == fc_w in every zrb_params (DESIGN.md section 13)
     int64_t emb_prev_cap = 0;              // capacity of emb_prev_ids (tokens)
     unsigned int* resident_flag = nullptr; // written by the backward recurrence kernel once all its CTAs are resident
     unsigned int resident_seq = 0;         // value the last launch publishes there

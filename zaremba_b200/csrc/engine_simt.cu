@@ -99,6 +99,10 @@ int simt_backward(zrb_ctx* c, const zrb_params* p, const float* dscores, const z
     }
     ProfScope ps(c, ZRB_PROF_EMBED_BWD, s);
     if (c->embed_rows_out) return embed_rows(dY, c->embed_rows_out, N, H, site_mask(c, 0), s);
+    if (c->tied) {   // g->embed_w holds G_proj: add the row sums (the tensor-core engine's fixed-point merge)
+        ZRB_TRY(embed_rows(dY, dX, N, H, site_mask(c, 0), s));
+        return embed_scatter_rows(c->x_saved, dX, g->embed_w, N, H, V, c->emb_first, c->emb_acc, s, true);
+    }
     ZRB_CUDA(cudaMemsetAsync(g->embed_w, 0, (size_t)V * H * sizeof(float), s));
     ZRB_TRY(embed_dropout_bwd(dY, c->x_saved, g->embed_w, N, H, V, site_mask(c, 0), s));
     return ZRB_OK;

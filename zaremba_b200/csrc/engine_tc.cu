@@ -214,7 +214,11 @@ int tc_forward(zrb_ctx* c, const zrb_params* p, const int64_t* x, const zrb_stat
     }
     {
         ProfScope ps(c, ZRB_PROF_EMBED_FWD, s);
-        ZRB_TRY(embed_dropout_fwd(p->embed_w, x, nullptr, t->x_h[0], Hp, N, H, V, site_mask(c, 0), s));
+        // tied: E's update (item L) is still deferred -> gather through it; the update itself rides beside the last
+        // recurrence, before the projection reads fc_w_h
+        const bool through = ride && c->tied && (t->upd_pending & (1u << L));
+        ZRB_TRY(embed_dropout_fwd(p->embed_w, x, nullptr, t->x_h[0], Hp, N, H, V, site_mask(c, 0), s,
+                                  through ? t->upd_tl.g[1 + 4 * L] : nullptr, t->upd_lr, c->scalars));
     }
     for (int l = 0; l < L; ++l) {
         float* G = c->gates[l];
@@ -407,6 +411,13 @@ static int tc_backward_layer(zrb_ctx* c, const zrb_params* p, const zrb_params* 
     if (l > 0) return ZRB_OK;
     ProfScope ps(c, ZRB_PROF_EMBED_BWD, s);
     if (c->embed_rows_out) return embed_rows(dY, c->embed_rows_out, N, H, site_mask(c, 0), s);
+    if (c->tied) {
+        // g->embed_w holds G_proj (the projection's wgrad GEMM overwrote every row): add the fixed-point row sums, with
+        // dX (free now) as the rows buffer; the fused norm's extra slots get the correction from G_proj^2 to dE^2
+        ZRB_TRY(embed_rows(dY, dX, N, H, site_mask(c, 0), s));
+        return embed_scatter_rows(c->x_saved, dX, g->embed_w, N, H, V, c->emb_first, c->emb_acc, s, true,
+                                  c->fused_norm ? c->partials + norm_partials_base() : nullptr, kNormExtra);
+    }
     if (c->emb_sparse && c->emb_prev_grad == g->embed_w) {
         ZRB_TRY(embed_zero_rows(g->embed_w, c->emb_prev_ids, c->emb_prev_n, H, V, s));   // only last window's rows are non-zero
     } else {
@@ -579,9 +590,17 @@ int tc_update(zrb_ctx* c, const zrb_params* p, const TensorList& tl, float lr, f
         c->weights_version++;
         return ZRB_OK;
     }
-    // tensor order of param_list(): embed, (w_ih, w_hh, b_ih, b_hh) x L, fc_w, fc_b
-    const bool rows_only = c->emb_sparse && c->emb_prev_grad == tl.g[0] && c->emb_prev_n > 0;
-    if (rows_only) {
+    // tensor order of param_list(): embed, (w_ih, w_hh, b_ih, b_hh) x L, fc_w, fc_b (tied: embed has n = 0, E is fc_w)
+    const bool rows_only = !c->tied && c->emb_sparse && c->emb_prev_grad == tl.g[0] && c->emb_prev_n > 0;
+    const bool tied_gemm_norm = c->tied && t->wg_ok && t->wg_key == tl.g[1 + 4 * L];
+    if (tied_gemm_norm) {
+        // matrices from the wgrad epilogue slots (E's describe G_proj); the extra slots hold the merge's correction
+        // to dE (tc_backward_layer): no read of the matrices' gradients
+        TensorList dense = tl;
+        for (int l = 0; l < L; ++l) dense.n[1 + 4 * l] = dense.n[2 + 4 * l] = 0;
+        dense.n[1 + 4 * L] = 0;
+        ZRB_TRY(grad_norm(dense, max_norm, c->partials, c->scalars, norm_out, s, true, t->wg_slots));
+    } else if (rows_only) {
         // embedding: only the rows of the last window can be non-zero -> norm and update over those rows
         TensorList dense = tl;
         dense.n[0] = 0;

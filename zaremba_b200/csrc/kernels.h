@@ -6,8 +6,10 @@ namespace zrb {
 
 // ---- pointwise.cu -----------------------------------------------------------------------
 // out[n, :] = W[idx[n], :] * dropout   (model.py:13-14 + :105)
+// pend_g (or null): gather sgd_elem(W, scalars[1] * pend_g, lr), W's deferred update (tied embedding, lazy update)
 int embed_dropout_fwd(const float* W, const int64_t* idx, float* out, __half* out_h, int64_t ld_h,
-                      int N, int H, int V, MaskSrc m, cudaStream_t s);
+                      int N, int H, int V, MaskSrc m, cudaStream_t s, const float* pend_g = nullptr, float lr = 0.f,
+                      const float* scalars = nullptr);
 // dW[idx[n], :] += dA[n, :] * dropout   (dW pre-zeroed)
 int embed_dropout_bwd(const float* dA, const int64_t* idx, float* dW, int N, int H, int V, MaskSrc m,
                       cudaStream_t s);
@@ -34,8 +36,9 @@ int softmax_nll(const float* scores, const int64_t* y, int N, int V, int B, floa
                 float* dscores, float* tgt_prob, cudaStream_t s, __half* ds_h = nullptr, int64_t ld_s = 0,
                 float h_scale = 1.f);
 int embed_rows(const float* dA, float* rows, int N, int H, MaskSrc m, cudaStream_t s);
+// add: dW[id] += the id's sum instead of dW[id] = (tied embedding); sumsq: see embed_finish_add_kernel
 int embed_scatter_rows(const int64_t* ids, const float* rows, float* dW, int n_rows, int H, int V, int* first,
-                       long long* acc, cudaStream_t s);
+                       long long* acc, cudaStream_t s, bool add = false, float* sumsq = nullptr, int nblocks = 0);
 int embed_zero_rows(float* dW, const int64_t* ids, int n, int H, int V, cudaStream_t s);
 int embed_first_table(const int64_t* ids, int* first, int n, int V, cudaStream_t s);
 int embed_rows_sumsq(const float* dW, const int64_t* ids, const int* first, int n, int H, int V, float* partial,

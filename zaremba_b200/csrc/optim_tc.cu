@@ -72,7 +72,7 @@ __global__ void update_pack_kernel(float* __restrict__ p, float* __restrict__ g,
         load_vec<VEC>(g + off, gv);
         load_vec<VEC>(p + off, pv);
 #pragma unroll
-        for (int x = 0; x < VEC; ++x) { gv[x] *= coef; pv[x] -= lr * gv[x]; }
+        for (int x = 0; x < VEC; ++x) { gv[x] *= coef; pv[x] = sgd_elem(pv[x], gv[x], lr); }
         if (sp.write_g) store_vec<VEC>(g + off, gv);
         store_vec<VEC>(p + off, pv);
         if (sp.row_img) {
@@ -109,7 +109,7 @@ __global__ void update_pack_whh_kernel(float* __restrict__ p, float* __restrict_
                 load_vec<VEC>(g + off, gv);
                 load_vec<VEC>(p + off, pv);
 #pragma unroll
-                for (int x = 0; x < VEC; ++x) { gv[x] *= coef; pv[x] -= lr * gv[x]; hv[e][x] = __float2half_rn(pv[x]); }
+                for (int x = 0; x < VEC; ++x) { gv[x] *= coef; pv[x] = sgd_elem(pv[x], gv[x], lr); hv[e][x] = __float2half_rn(pv[x]); }
                 if (sp.write_g) store_vec<VEC>(g + off, gv);
                 store_vec<VEC>(p + off, pv);
                 if (sp.row_img) store_halves<VEC>(sp.row_img + ((int64_t)q * H + j) * sp.ld + c, hv[e]);

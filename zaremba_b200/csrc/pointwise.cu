@@ -10,10 +10,14 @@ namespace zrb {
 // grid: one block per token row; threads stride the row in groups of 4 (one Philox call
 // yields the keep flags of 4 consecutive elements).
 // Algorithmic bytes per token: H*4 read (table row) + H*4 written (+ H*2 fp16 image).
+// PENDING (tied embedding, lazy update): the SGD update of W is still deferred; every gathered element is
+// sgd_elem(W, coef * g, lr) with the coefficient of scalars[1], the value update_pack will store (g is only read).
 // ----------------------------------------------------------------------------------------
+template <bool PENDING>
 __global__ void embed_dropout_fwd_kernel(const float* __restrict__ W, const int64_t* __restrict__ idx,
                                          float* __restrict__ out, __half* __restrict__ out_h, int64_t ld_h, int N,
-                                         int H, int V, MaskSrc m) {
+                                         int H, int V, MaskSrc m, const float* __restrict__ pend_g, float lr,
+                                         const float* __restrict__ scalars) {
     int n = blockIdx.x;
     if (n >= N) return;
     int64_t row = idx[n];
@@ -21,12 +25,17 @@ __global__ void embed_dropout_fwd_kernel(const float* __restrict__ W, const int6
     const float* src = W + row * (int64_t)H;
     int groups = (H + 3) >> 2;
     uint64_t n_total = (uint64_t)N * H;
+    float coef = 0.f;
+    if constexpr (PENDING) coef = scalars[1];
     for (int g = threadIdx.x; g < groups; g += blockDim.x) {
         int j0 = g << 2;
         uint64_t e0 = (uint64_t)n * H + j0;
         float v[4];
 #pragma unroll
-        for (int i = 0; i < 4; ++i) v[i] = (j0 + i < H) ? src[j0 + i] : 0.f;
+        for (int i = 0; i < 4; ++i) {
+            if constexpr (PENDING) v[i] = (j0 + i < H) ? sgd_elem(src[j0 + i], pend_g[row * (int64_t)H + j0 + i] * coef, lr) : 0.f;
+            else v[i] = (j0 + i < H) ? src[j0 + i] : 0.f;
+        }
         if (m.active) {
             // rows are H long; H % 4 != 0 makes groups straddle Philox quads -> per-element path.  (A variational
             // period B*H is then a multiple of 4 too, so the reduced e0 still starts a quad.)
@@ -50,10 +59,11 @@ __global__ void embed_dropout_fwd_kernel(const float* __restrict__ W, const int6
 }
 
 int embed_dropout_fwd(const float* W, const int64_t* idx, float* out, __half* out_h, int64_t ld_h, int N, int H,
-                      int V, MaskSrc m, cudaStream_t s) {
+                      int V, MaskSrc m, cudaStream_t s, const float* pend_g, float lr, const float* scalars) {
     if (N == 0) return ZRB_OK;
     int threads = H >= 1024 ? 256 : 128;
-    embed_dropout_fwd_kernel<<<N, threads, 0, s>>>(W, idx, out, out_h, ld_h, N, H, V, m);
+    if (pend_g) embed_dropout_fwd_kernel<true><<<N, threads, 0, s>>>(W, idx, out, out_h, ld_h, N, H, V, m, pend_g, lr, scalars);
+    else embed_dropout_fwd_kernel<false><<<N, threads, 0, s>>>(W, idx, out, out_h, ld_h, N, H, V, m, nullptr, 0.f, nullptr);
     ZRB_KERNEL_CHECK();
     return ZRB_OK;
 }
@@ -450,8 +460,41 @@ __global__ void embed_finish_kernel(const int64_t* __restrict__ ids, const int* 
     for (int j = threadIdx.x; j < H; j += blockDim.x)
         dW[id * (int64_t)H + j] = (float)((double)acc[(int64_t)n * H + j] * (1.0 / 1099511627776.0));
 }
+// Tied embedding (DESIGN.md section 13): dW already holds the projection's weight gradient G; the id's sum e is added,
+// dW[id] = fp32(G[id] + e).  sumsq (or null): the `nblocks` blocks grid-stride over the tokens and block k writes
+// sumsq[k] = sum over its distinct ids' elements of (new^2 - old^2), so that a clip norm whose matrix part came from
+// sums of squares of G (the wgrad GEMM epilogues) becomes that of the merged gradient without reading it again.
+__global__ void embed_finish_add_kernel(const int64_t* __restrict__ ids, const int* __restrict__ first,
+                                        const long long* __restrict__ acc, float* __restrict__ dW, int n_rows, int H,
+                                        int V, float* __restrict__ sumsq) {
+    __shared__ double sh[8];
+    // new^2 - old^2 cancels in part when |e| << |G|: the squares of two fp32 values are exact in fp64 and the sum is
+    // kept there, so the correction's error is one fp32 rounding of each block's total, not one per element
+    double ss = 0.0;
+    for (int n = blockIdx.x; n < n_rows; n += gridDim.x) {
+        const int64_t id = ids[n];
+        if (id < 0 || id >= V || first[id] != n) continue;
+        for (int j = threadIdx.x; j < H; j += blockDim.x) {
+            const float old = dW[id * (int64_t)H + j];
+            const float e = (float)((double)acc[(int64_t)n * H + j] * (1.0 / 1099511627776.0));
+            const float nw = old + e;
+            dW[id * (int64_t)H + j] = nw;
+            ss += (double)nw * nw - (double)old * old;
+        }
+    }
+    if (!sumsq) return;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
+    if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = ss;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double t = 0.0;
+        for (int i = 0; i < (int)(blockDim.x >> 5); ++i) t += sh[i];
+        sumsq[blockIdx.x] = (float)t;
+    }
+}
 int embed_scatter_rows(const int64_t* ids, const float* rows, float* dW, int n_rows, int H, int V, int* first,
-                       long long* acc, cudaStream_t s) {
+                       long long* acc, cudaStream_t s, bool add, float* sumsq, int nblocks) {
     if (!n_rows) return ZRB_OK;
     ZRB_CUDA(cudaMemsetAsync(first, 0x7f, (size_t)V * sizeof(int), s));           // 0x7f7f7f7f > any row index
     ZRB_CUDA(cudaMemsetAsync(acc, 0, (size_t)n_rows * H * sizeof(long long), s));
@@ -459,7 +502,8 @@ int embed_scatter_rows(const int64_t* ids, const float* rows, float* dW, int n_r
     ZRB_KERNEL_CHECK();
     embed_accum_kernel<<<n_rows, 256, 0, s>>>(ids, rows, first, acc, n_rows, H, V);
     ZRB_KERNEL_CHECK();
-    embed_finish_kernel<<<n_rows, 256, 0, s>>>(ids, first, acc, dW, n_rows, H, V);
+    if (add) embed_finish_add_kernel<<<sumsq ? nblocks : n_rows, 256, 0, s>>>(ids, first, acc, dW, n_rows, H, V, sumsq);
+    else embed_finish_kernel<<<n_rows, 256, 0, s>>>(ids, first, acc, dW, n_rows, H, V);
     ZRB_KERNEL_CHECK();
     return ZRB_OK;
 }

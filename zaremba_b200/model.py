@@ -124,15 +124,25 @@ class Model(nn.Module):
     section 11).  With `variational=True` every dropout mask is drawn once per window and reused at every time step,
     and the recurrent connection of each layer is dropped with p = `recurrent_dropout` (None: the same p as
     `dropout`, Gal's setting; 0: no recurrent dropout).  Eval mode applies no mask either way.
+
+    Extra keyword `tied`: tie the embedding and softmax weights (Press & Wolf 2017; DESIGN.md section 13).  `fc.W` is
+    then the same `nn.Parameter` as `embed.W` (one [V,H] matrix E, `fc.b` stays separate), `parameters()` yields the
+    2 + 4L distinct tensors, and the library takes E's one merged gradient.  `reset_parameters` walks `parameters()`,
+    so with the same seed E and the LSTM tensors equal an untied model's `embed.W` and LSTM tensors, and `fc.b` is
+    drawn where the untied model draws `fc.W`.  `state_dict()` carries both keys (torch's rule for a shared parameter),
+    so a tied checkpoint also loads into an untied model; loading one whose `embed.W` and `fc.W` differ into a tied
+    model raises ValueError.
     """
 
     def __init__(self, vocab_size, hidden_size, layer_num, dropout, winit, lstm_type="pytorch", engine="tc",
-                 variational=False, recurrent_dropout=None):
+                 variational=False, recurrent_dropout=None, *, tied=False):
         super().__init__()
         if lstm_type not in ("pytorch", "custom"):
             raise ValueError(f"lstm_type must be 'pytorch' or 'custom', got {lstm_type!r}")
         if variational not in (False, True):
             raise ValueError(f"variational must be True or False, got {variational!r}")
+        if not isinstance(tied, bool):
+            raise ValueError(f"tied must be True or False, got {tied!r}")
         if recurrent_dropout is not None and not variational:
             raise ValueError("recurrent_dropout needs variational=True")
         p_rec = float(dropout) if (variational and recurrent_dropout is None) else float(recurrent_dropout or 0.0)
@@ -149,9 +159,12 @@ class Model(nn.Module):
         self.p_drop = float(dropout)
         self.variational = bool(variational)
         self.p_rec = p_rec
+        self.tied = tied
         self.embed = Embed(vocab_size, hidden_size)
         self.rnns = nn.ModuleList(LSTM(hidden_size, hidden_size, lstm_type) for _ in range(layer_num))
         self.fc = Linear(hidden_size, vocab_size)
+        if tied:
+            self.fc.W = self.embed.W
         self.dropout = nn.Dropout(p=dropout)     # kept for repr / state parity; masks come from the library
         self.reset_parameters()
         self._ctx = None
@@ -174,6 +187,12 @@ class Model(nn.Module):
 
     def detach(self, states):
         return [(h.detach(), c.detach()) for (h, c) in states]
+
+    def load_state_dict(self, state_dict, strict=True, assign=False):
+        if self.tied and "embed.W" in state_dict and "fc.W" in state_dict and \
+                not torch.equal(torch.as_tensor(state_dict["embed.W"]).cpu(), torch.as_tensor(state_dict["fc.W"]).cpu()):
+            raise ValueError("checkpoint has different embed.W and fc.W: it cannot load into a tied model (tied=True)")
+        return super().load_state_dict(state_dict, strict=strict, assign=assign)
 
     def forward(self, x, states):
         dev = self.embed.W.device
@@ -304,11 +323,12 @@ class Model(nn.Module):
     # ---- plumbing ------------------------------------------------------------------------
     def ordered_parameters(self):
         """The 3+4L tensors in registration order, as the library's zrb_params expects them
-        (pytorch names / gate order; the custom layout is permuted by `_lib_weights`)."""
+        (pytorch names / gate order; the custom layout is permuted by `_lib_weights`).  Tied: the 2+4L distinct
+        tensors, E once (no fc.W entry)."""
         out = [self.embed.W]
         for r in self.rnns:
             out += list(r.tensors())
-        out += [self.fc.W, self.fc.b]
+        out += [self.fc.b] if self.tied else [self.fc.W, self.fc.b]
         return out
 
     def _lib_weights(self):
@@ -316,7 +336,7 @@ class Model(nn.Module):
         if self.lstm_type == "custom":
             # (i,f,o,n) -> (i,f,g,o) row-block permutation: a differentiable copy, so autograd
             # routes the gradients back into the custom layout
-            ws = [w if i in (0, len(ws) - 2, len(ws) - 1) else _ifon_to_ifgo(w) for i, w in enumerate(ws)]
+            ws = [_ifon_to_ifgo(w) if 1 <= i <= 4 * self.layer_num else w for i, w in enumerate(ws)]
         return ws
 
     def _next_dropout_key(self):
@@ -354,7 +374,8 @@ class Model(nn.Module):
             self._destroy_ctx()
         lib = _lib.load()
         cfg = _lib.ZrbConfig(self.vocab_size, self.hidden_size, self.layer_num, key[0], key[1],
-                             _lib.ENGINE_TC if self.engine == "tc" else _lib.ENGINE_SIMT, self.p_drop, 0)
+                             _lib.ENGINE_TC if self.engine == "tc" else _lib.ENGINE_SIMT, self.p_drop,
+                             _lib.TIED_EMBEDDING if self.tied else 0)
         h = C.c_void_p()
         with torch.cuda.device(self.embed.W.device):
             _lib.check(lib.zrb_ctx_create(C.byref(cfg), C.byref(h)))
@@ -390,8 +411,8 @@ class Model(nn.Module):
             ps.w_hh[l] = ts[2 + 4 * l].data_ptr()
             ps.b_ih[l] = ts[3 + 4 * l].data_ptr()
             ps.b_hh[l] = ts[4 + 4 * l].data_ptr()
-        ps.fc_w = ts[1 + 4 * L].data_ptr()
-        ps.fc_b = ts[2 + 4 * L].data_ptr()
+        ps.fc_w = ts[0].data_ptr() if self.tied else ts[1 + 4 * L].data_ptr()   # tied: E is fc.W too
+        ps.fc_b = ts[-1].data_ptr()
         return ps, ts
 
     def _states_struct(self, states):

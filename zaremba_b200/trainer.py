@@ -90,7 +90,10 @@ class Trainer:
         self.world = (dist.get_world_size(process_group)
                       if data_parallel and dist.is_available() and dist.is_initialized() else 1)
         params = model.ordered_parameters()
-        sizes = [p.numel() for p in params]
+        # flat layout: the library's order, except that a tied E sits next to fc.b, so that the bucket the projection
+        # backward completes (E's G_proj part, fc.b) is one range
+        layout = params[1:-1] + [params[0], params[-1]] if model.tied else params
+        sizes = [p.numel() for p in layout]
         # one flat parameter buffer and one flat gradient buffer; the nn.Parameters become views
         self.flat_p = torch.empty(sum(sizes), device=dev, dtype=torch.float32)
         # DP transport: "ce" = copy engines over NVLink peer memory (dp_ce.cu, overlaps with backward),
@@ -113,7 +116,7 @@ class Trainer:
             self.flat_g = torch.zeros(sum(sizes), device=dev, dtype=torch.float32)
         off = 0
         with torch.no_grad():
-            for p, n in zip(params, sizes):
+            for p, n in zip(layout, sizes):
                 view = self.flat_p[off:off + n].view_as(p)
                 view.copy_(p)
                 p.data = view
@@ -137,15 +140,17 @@ class Trainer:
         self.seed = (int(torch.initial_seed()) + rank * 0x9E3779B97F4A7C15) & 0xFFFFFFFFFFFFFFFF
         # data-parallel buckets of the flat gradient buffer, in the order backward completes them:
         # [fc.W, fc.b], layer L-1, ..., layer 1, [embed.W + layer 0]
+        # (tied: [E, fc.b], layer L-1, ..., layer 1, [layer 0]; E's embedding part travels as rows, added afterwards)
         L = model.layer_num
         offs = [0]
         for n in sizes:
             offs.append(offs[-1] + n)
-        self._buckets = [(offs[1 + 4 * L], offs[-1])]
+        r0 = 0 if model.tied else 1            # where layer 0 starts in the flat layout
+        self._buckets = [(offs[4 * L], offs[-1])] if model.tied else [(offs[1 + 4 * L], offs[-1])]
         for l in range(L - 1, 0, -1):
-            self._buckets.append((offs[1 + 4 * l], offs[1 + 4 * (l + 1)]))
-        self._buckets.append((0, offs[1 + 4]))
-        self._embed_end = offs[1]
+            self._buckets.append((offs[r0 + 4 * l], offs[r0 + 4 * (l + 1)]))
+        self._buckets.append((0, offs[r0 + 4]))
+        self._embed_end = offs[r0]             # all-reduced with the rest from here (tied: E's projection part too)
         self._comm_stream = torch.cuda.Stream(device=dev) if self.world > 1 else None
         # (reducing finished buckets with NCCL underneath the rest of backward was removed: NCCL's channels evict part
         # of the persistent recurrence grid; the copy-engine transport is the one that overlaps)
@@ -228,6 +233,8 @@ class Trainer:
         lo, hi = self._buckets[nb - 1]
         # tail: layer-0 gradients through one NCCL all-reduce (alone on the GPU); the embedding gradient as rows
         allreduce_sum_(self.flat_g[self._embed_end:hi], self.pg)
+        if self.model.tied:
+            self._ce_join(lib)
         self._exchange_embedding_rows(lib, x, T, B)
         _lib.check(lib.zrb_dp_finish_step(self._dp, st))
         _lib.check(lib.zrb_set_embed_rows_out(self.ctx, None))
@@ -346,13 +353,24 @@ class Trainer:
         self._pending = True
         return self.loss, self.norm
 
+    def _ce_join(self, lib):
+        """Tied model on the copy-engine transport: E's gradient lies in bucket 0, which the transport reduces on its
+        own streams (peers pull my shard, my shard is reduced in place, the peers' reduced shards are copied in), and
+        the scatter (zrb_embed_scatter_rows) then ADDS the embedding rows into that same range in place.  So the add
+        must wait until (1) this rank's reduction and gathers of every bucket have finished (zrb_dp_finish_step: the compute stream
+        waits for them), and (2) every peer has pulled this rank's reduced shards (zrb_dp_begin_step: the peers' "done"
+        flags) -- otherwise a peer could copy a row that already holds e_r and add e_r a second time."""
+        st = self._stream()
+        _lib.check(lib.zrb_dp_finish_step(self._dp, st))
+        _lib.check(lib.zrb_dp_begin_step(self._dp, st))
+
     def _exchange_embedding_rows(self, lib, x, T, B):
         """Sparse form of the embedding gradient: all-gather every rank's N token ids and N masked gradient rows
         (4 MB per rank instead of a 60 MB dense all-reduce) and scatter them deterministically into the dense buffer."""
         N = T * B
         dist.all_gather_into_tensor(self._rows_all[: self.world * N], self._rows[:N], group=self.pg)
         dist.all_gather_into_tensor(self._ids_all[: self.world * N], x.reshape(-1), group=self.pg)
-        _lib.check(lib.zrb_embed_scatter_rows(self.ctx, _lib.ptr(self.flat_g), _lib.ptr(self._ids_all),
+        _lib.check(lib.zrb_embed_scatter_rows(self.ctx, _lib.ptr(self.model.embed.W.grad), _lib.ptr(self._ids_all),
                                               _lib.ptr(self._rows_all), self.world * N, self._stream()))
 
     def train_step_host(self, x, y, lr, max_norm):
