@@ -364,6 +364,35 @@ int  zrb_eval_step_cache(zrb_ctx* ctx, const zrb_params* p, const int64_t* x, co
                          const zrb_states* in, const zrb_states* out, zrb_cache* cache, float theta, float lambda,
                          float* loss, float* tgt_prob, float* cache_prob, void* stream);
 
+/* ---- dynamic evaluation (Krause, Kahembwe, Murray & Renals, "Dynamic Evaluation of Neural Sequence Models", ICML 2018;
+ * DESIGN.md section 14 states it bit for bit) --------------------------------------------------------------------------
+ * theta = the P distinct parameter elements (a tied E once), theta_g = `global`, a snapshot taken when the pass starts.
+ * Per window s ([T,B], states carried as in perplexity):
+ *   1. score: the eval-mode forward at theta_s (no dropout, whatever the context's dropout / variational / explicit-mask
+ *      settings); loss = zrb_eval_step's window loss, bit for bit.
+ *   2. gradient: g_s = d loss / d theta of that same eval-mode function, entering states detached -- bit for bit what
+ *      zrb_train_step_grads writes in a context created with dropout = 0 from the same weights, window and states.
+ *   3. update: theta += a * (theta_g - theta) - lr * u, elementwise, in the fp32 order of DESIGN.md section 14:
+ *        RMS rule (rms given):  u = g / (r + eps), a = min(1, lambda * r / rbar)
+ *        SGD rule (rms NULL):   u = g,             a = min(1, lambda)
+ *      r = the RMS statistic, rbar = *rms_mean (device), the mean of r over all P elements.  An element with r = 0 gets
+ *      a = 0 and u = g / eps.  The clip of a at 1 (a parameter never moves past theta_g) is this library's choice.
+ * Statistics: MS = (1/K) sum_k g_k^2 over K windows, each g_k as in step 2 at theta_g with no update, states carried from
+ * zero.  zrb_grad_stats_step: the window's g into `grads` and ms += g*g (fp32, one fma; p unchanged).
+ * zrb_grad_stats_finish: r = sqrtf(ms / K) in place and *rms_mean = fp32(fixed-order fp64 sum of r / P): bit-reproducible.
+ * zrb_dyneval_step: steps 1-3 in one call; afterwards `grads` holds the raw g_s and the fp16 weight images are current.
+ * All zrb_params of a tied context must have fc_w == embed_w; loss may be NULL.  Pending lazy updates are applied first.
+ * ZRB_E_INVALID, before anything is launched and with every buffer unchanged, for lr or lambda negative or not finite,
+ * eps <= 0 or not finite under the RMS rule, rms_mean NULL with rms given, windows < 1, and the tied rule. */
+int  zrb_grad_stats_step(zrb_ctx* ctx, const zrb_params* p, const zrb_params* grads, const zrb_params* ms,
+                         const int64_t* x, const int64_t* y, int32_t T, int32_t B, const zrb_states* in,
+                         const zrb_states* out, float* loss, void* stream);
+int  zrb_grad_stats_finish(zrb_ctx* ctx, const zrb_params* ms, int64_t windows, float* rms_mean, void* stream);
+int  zrb_dyneval_step(zrb_ctx* ctx, const zrb_params* p, const zrb_params* grads, const zrb_params* global,
+                      const zrb_params* rms, const float* rms_mean, const int64_t* x, const int64_t* y, int32_t T,
+                      int32_t B, const zrb_states* in, const zrb_states* out, float lr, float lambda, float eps,
+                      float* loss, void* stream);
+
 /* Same as zrb_train_step_grads + zrb_train_step_update but with HOST token buffers
  * (pinned or pageable) and a host loss: the H2D copies of x, y and the D2H copy of the
  * loss are issued on `stream` inside the call; the call returns after the loss landed. */

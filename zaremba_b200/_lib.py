@@ -91,6 +91,12 @@ _SIGNATURES = {
     "zrb_cache_step": (C.c_int, [_vp, _vp, _vp, C.c_int32, C.c_int32, C.c_float, _vp, _vp]),
     "zrb_eval_step_cache": (C.c_int, [_vp, C.POINTER(ZrbParams), _vp, _vp, C.c_int32, C.c_int32, C.POINTER(ZrbStates),
                                       C.POINTER(ZrbStates), _vp, C.c_float, C.c_float, _vp, _vp, _vp, _vp]),
+    "zrb_grad_stats_step": (C.c_int, [_vp, C.POINTER(ZrbParams), C.POINTER(ZrbParams), C.POINTER(ZrbParams), _vp, _vp,
+                                      C.c_int32, C.c_int32, C.POINTER(ZrbStates), C.POINTER(ZrbStates), _vp, _vp]),
+    "zrb_grad_stats_finish": (C.c_int, [_vp, C.POINTER(ZrbParams), C.c_int64, _vp, _vp]),
+    "zrb_dyneval_step": (C.c_int, [_vp, C.POINTER(ZrbParams), C.POINTER(ZrbParams), C.POINTER(ZrbParams),
+                                   C.POINTER(ZrbParams), _vp, _vp, _vp, C.c_int32, C.c_int32, C.POINTER(ZrbStates),
+                                   C.POINTER(ZrbStates), C.c_float, C.c_float, C.c_float, _vp, _vp]),
     "zrb_train_step_host": (C.c_int, [_vp, C.POINTER(ZrbParams), C.POINTER(ZrbParams), _vp, _vp, C.c_int32,
                                       C.c_int32, C.POINTER(ZrbStates), C.POINTER(ZrbStates), C.c_uint64,
                                       C.c_uint64, C.c_float, C.c_float, _vp, _vp, _vp]),

@@ -1,5 +1,6 @@
 // C ABI of libzaremba_b200.so: context, orchestration of the forward / backward / loss /
 // update kernels.  See include/zaremba_b200.h for the contract of every entry point.
+#include <math.h>
 #include <stdarg.h>
 #include <string.h>
 
@@ -465,6 +466,73 @@ int zrb_eval_step(zrb_ctx* c, const zrb_params* p, const int64_t* x, const int64
     c->have_fwd = false;  // eval keeps nothing for backward
     return softmax_nll(c->scores, y, T * B, c->cfg.vocab, B, c->row_loss, loss, nullptr, tgt_prob,
                        (cudaStream_t)stream);
+}
+
+// ---- dynamic evaluation (DESIGN.md section 14) ----------------------------------------------------------------------
+// g = the gradient of the eval-mode window loss at p: the fused gradient path with no dropout (c->train = 0)
+static int eval_grads(zrb_ctx* c, const zrb_params* p, const zrb_params* g, const int64_t* x, const int64_t* y, int T,
+                      int B, const zrb_states* in, const zrb_states* out, float* loss, cudaStream_t s) {
+    if (c->cfg.engine == ZRB_ENGINE_TC) return tc_eval_grads(c, p, g, x, y, T, B, in, out, loss, s);
+    ZRB_TRY(zrb_forward(c, p, x, T, B, in, out, c->scores, 0, 0, 0, s));
+    {
+        ProfScope ps(c, ZRB_PROF_SOFTMAX, s);
+        ZRB_TRY(softmax_nll(c->scores, y, T * B, c->cfg.vocab, B, c->row_loss, loss, c->dscores, nullptr, s));
+    }
+    return simt_backward(c, p, c->dscores, g, s);
+}
+
+int zrb_grad_stats_step(zrb_ctx* c, const zrb_params* p, const zrb_params* g, const zrb_params* ms, const int64_t* x,
+                        const int64_t* y, int32_t T, int32_t B, const zrb_states* in, const zrb_states* out, float* loss,
+                        void* stream) {
+    ZRB_REQUIRE(c && p && g && ms && x && y && in && out, "null argument");
+    ZRB_REQUIRE(c->cfg.layers * 4 + 3 <= 16, "gradient statistics support at most 3 layers");
+    ZRB_TRY(check_shapes(c, T, B));
+    ZRB_TRY(check_tied(c, p));
+    ZRB_TRY(check_tied(c, g));
+    ZRB_TRY(check_tied(c, ms));
+    cudaStream_t s = (cudaStream_t)stream;
+    ZRB_TRY(eval_grads(c, p, g, x, y, T, B, in, out, loss, s));
+    return sq_accumulate(param_list(c, ms, g), s);
+}
+
+int zrb_grad_stats_finish(zrb_ctx* c, const zrb_params* ms, int64_t windows, float* rms_mean, void* stream) {
+    ZRB_REQUIRE(c && ms && rms_mean, "null argument");
+    ZRB_REQUIRE(windows >= 1, "windows=%lld must be >= 1", (long long)windows);
+    ZRB_REQUIRE(c->cfg.layers * 4 + 3 <= 16, "gradient statistics support at most 3 layers");
+    ZRB_TRY(check_tied(c, ms));
+    if (!c->stats_partials) ZRB_TRY(dalloc(c, &c->stats_partials, kStatsPartials));
+    return stats_finish(param_list(c, ms, ms), windows, c->stats_partials, rms_mean, (cudaStream_t)stream);
+}
+
+int zrb_dyneval_step(zrb_ctx* c, const zrb_params* p, const zrb_params* g, const zrb_params* global,
+                     const zrb_params* rms, const float* rms_mean, const int64_t* x, const int64_t* y, int32_t T,
+                     int32_t B, const zrb_states* in, const zrb_states* out, float lr, float lambda, float eps,
+                     float* loss, void* stream) {
+    ZRB_REQUIRE(c && p && g && global && x && y && in && out, "null argument");
+    ZRB_REQUIRE(c->cfg.layers * 4 + 3 <= 16, "dynamic evaluation supports at most 3 layers");
+    ZRB_REQUIRE(isfinite(lr) && lr >= 0.f, "lr %f must be finite and >= 0", lr);
+    ZRB_REQUIRE(isfinite(lambda) && lambda >= 0.f, "lambda %f must be finite and >= 0", lambda);
+    ZRB_REQUIRE(!rms || rms_mean, "the RMS rule needs rms_mean");
+    ZRB_REQUIRE(!rms || (isfinite(eps) && eps > 0.f), "eps %f must be finite and > 0 under the RMS rule", eps);
+    ZRB_TRY(check_shapes(c, T, B));
+    ZRB_TRY(check_tied(c, p));
+    ZRB_TRY(check_tied(c, g));
+    ZRB_TRY(check_tied(c, global));
+    ZRB_TRY(check_tied(c, rms));
+    cudaStream_t s = (cudaStream_t)stream;
+    ZRB_TRY(eval_grads(c, p, g, x, y, T, B, in, out, loss, s));
+    const TensorList tl = param_list(c, p, g), tg = param_list(c, global, global);
+    TensorList tr = tl;
+    if (rms) tr = param_list(c, rms, rms);
+    DynArgs a;
+    a.lr = lr; a.lam = lambda; a.eps = eps; a.rbar = rms ? rms_mean : nullptr;
+    if (c->cfg.engine == ZRB_ENGINE_TC) return tc_dyneval_update(c, p, tl, tg.p, rms ? tr.p : nullptr, a, s);
+    {
+        ProfScope ps(c, ZRB_PROF_CLIP_SGD, s);
+        ZRB_TRY(dyneval_apply(tl, tg.p, rms ? tr.p : nullptr, a, s));
+    }
+    c->weights_version++;
+    return ZRB_OK;
 }
 
 int zrb_sample(const float* scores, int64_t ld, int32_t B, int32_t V, const zrb_sampling* cfg, uint64_t pos,

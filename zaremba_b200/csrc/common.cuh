@@ -172,6 +172,25 @@ __device__ inline float sigmoidf_(float z) { return 1.f / (1.f + expf(-z)); }
 // tied embedding's gather through a deferred update reads, so that the two agree bit for bit
 __device__ __forceinline__ float sgd_elem(float p, float g, float lr) { return p - lr * g; }
 
+// one element of the dynamic-evaluation update (DESIGN.md section 14), in this fixed fp32 order (intrinsics, so that no
+// kernel contracts it differently):  d = tg - p;  u = g / (r + eps) (RMS rule) or g (SGD rule, RMS = false);
+// a = min(1, (lam * r) / rbar) or min(1, lam);  p + fma(a, d, -(lr * u)).  tg = the trained weight theta_g, r = its RMS
+// statistic, rbar = the mean of r over all parameters.  The ONE expression every kernel that applies the rule calls.
+template <bool RMS>
+__device__ __forceinline__ float dyneval_elem(float p, float g, float tg, float r, float lr, float lam, float eps,
+                                              float rbar) {
+    const float d = __fsub_rn(tg, p);
+    const float u = RMS ? __fdiv_rn(g, __fadd_rn(r, eps)) : g;
+    const float a = fminf(1.f, RMS ? __fdiv_rn(__fmul_rn(lam, r), rbar) : lam);
+    return __fadd_rn(p, __fmaf_rn(a, d, -__fmul_rn(lr, u)));
+}
+
+// scalars of the dynamic-evaluation update; rbar is read on the device (zrb_grad_stats_finish writes it)
+struct DynArgs {
+    float lr, lam, eps;
+    const float* rbar;   // null: the SGD rule
+};
+
 __device__ inline float warp_sum(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

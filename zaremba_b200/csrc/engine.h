@@ -76,6 +76,8 @@ struct zrb_ctx {
     float* beam_lp = nullptr;
     int64_t beam_cap = 0;                  // entries of beam_tok / _par / _lp
 
+    double* stats_partials = nullptr;      // zrb_grad_stats_finish: kStatsPartials fp64 block sums (allocated on first use)
+
     zrb_tc_state* tc = nullptr;
 
     // optional per-class event timing (zrb_prof_*)
@@ -125,5 +127,10 @@ int tc_layer_bwd(zrb_ctx* c, const float* dy, float* dx, float* dw_ih, float* dw
                  cudaStream_t s);   // the persistent backward recurrence kernel is in use for this context
 int tc_update(zrb_ctx* c, const zrb_params* p, const TensorList& tl, float lr, float max_norm, float* norm_out,
               cudaStream_t s);
+// dynamic evaluation (DESIGN.md section 14): eval-mode gradients, and the update with the dynamic rule
+int tc_eval_grads(zrb_ctx* c, const zrb_params* p, const zrb_params* g, const int64_t* x, const int64_t* y, int T, int B,
+                  const zrb_states* in, const zrb_states* out, float* loss, cudaStream_t s);
+int tc_dyneval_update(zrb_ctx* c, const zrb_params* p, const TensorList& tl, float* const* tg, float* const* r,
+                      const DynArgs& a, cudaStream_t s);
 
 }  // namespace zrb

@@ -465,6 +465,28 @@ int tc_train_step_grads(zrb_ctx* c, const zrb_params* p, const zrb_params* g, co
     return tc_backward_from_image(c, p, g, s);
 }
 
+// the gradient of the eval-mode loss (DESIGN.md section 14): the fused gradient path with c->train = 0, so that every
+// site_mask / rec_mask is off while tc_forward still keeps the activations; pending lazy updates are applied first (the
+// forward runs outside a train step).  No clip norm follows, so the wgrad epilogues write no sum-of-squares slots.
+int tc_eval_grads(zrb_ctx* c, const zrb_params* p, const zrb_params* g, const int64_t* x, const int64_t* y, int T, int B,
+                  const zrb_states* in, const zrb_states* out, float* loss, cudaStream_t s) {
+    c->T = T; c->B = B; c->train = 0; c->seed = 0; c->step = 0;
+    c->have_fwd = false;
+    ZRB_TRY(tc_forward(c, p, x, in, out, c->scores, s));
+    c->have_fwd = true;
+    {
+        ProfScope ps(c, ZRB_PROF_SOFTMAX, s);
+        ZRB_TRY(softmax_nll(c->scores, y, T * B, c->cfg.vocab, B, c->row_loss, loss, nullptr, nullptr, s, c->tc->dS_h,
+                            c->tc->Vp, kGradScale));
+    }
+    const bool fused = c->fused_norm;
+    c->fused_norm = false;
+    const int rc = tc_backward_from_image(c, p, g, s);
+    c->fused_norm = fused;
+    c->tc->wg_ok = false;
+    return rc;
+}
+
 int tc_train_step_begin(zrb_ctx* c, const zrb_params* p, const zrb_params* g, const int64_t* x, const int64_t* y,
                         int T, int B, const zrb_states* in, const zrb_states* out, uint64_t seed, uint64_t step,
                         float* loss, cudaStream_t s) {
@@ -650,6 +672,46 @@ int tc_update(zrb_ctx* c, const zrb_params* p, const TensorList& tl, float lr, f
                              c->keep_clipped, s));
     push(f + 1);
     ZRB_TRY(sgd_apply(rest, lr, c->scalars, c->keep_clipped, s));
+    t->wg_ok = false;
+    c->weights_version++;
+    t->packed_version = c->weights_version;      // images are current
+    t->packed_params = *p;
+    return ZRB_OK;
+}
+
+// The dynamic-evaluation update (DESIGN.md section 14): tc_update's schedule with the dynamic rule, no norm and no lazy
+// deferral.  The matrices go through update_pack's kernels, which rebuild their fp16 images from registers; the rest
+// through the list kernel.  tg / r: theta_g and the RMS statistic in param_list() order (r null: the SGD rule).
+int tc_dyneval_update(zrb_ctx* c, const zrb_params* p, const TensorList& tl, float* const* tg, float* const* r,
+                      const DynArgs& a, cudaStream_t s) {
+    zrb_tc_state* t = c->tc;
+    const int H = c->cfg.hidden, L = c->cfg.layers, V = c->cfg.vocab;
+    ZRB_TRY(tc_flush_updates(c, s));
+    ProfScope ps(c, ZRB_PROF_CLIP_SGD, s);
+    bool fuse = true;
+    for (int i = 0; i < tl.count && fuse; ++i)
+        fuse = ((((uintptr_t)tl.p[i]) | ((uintptr_t)tl.g[i]) | ((uintptr_t)tg[i]) | (r ? (uintptr_t)r[i] : 0)) & 3) == 0;
+    if (!fuse) {   // images rebuilt by the next forward's pack
+        ZRB_TRY(dyneval_apply(tl, tg, r, a, s));
+        c->weights_version++;
+        return ZRB_OK;
+    }
+    TensorList rest = tl;   // entries with an image get length 0 here (skipped by the list kernel)
+    const bool persistent = t->fplan.ok && t->bplan.ok;
+    for (int l = 0; l < L; ++l) {
+        const int b = 1 + 4 * l;
+        ZRB_TRY(update_pack_dyn(tl.p[b], tl.g[b], tg[b], r ? r[b] : nullptr, 4 * H, H, a, t->w_ih_h[l], t->Hp, nullptr,
+                                nullptr, nullptr, nullptr, s));
+        ZRB_TRY(update_pack_dyn(tl.p[b + 1], tl.g[b + 1], tg[b + 1], r ? r[b + 1] : nullptr, 4 * H, H, a,
+                                persistent ? nullptr : t->w_hh_h[l], t->Hp, t->fplan.ok ? t->w_img_f[l] : nullptr,
+                                &t->fplan, t->bplan.ok ? t->w_img_b[l] : nullptr, &t->bplan, s));
+        rest.n[b] = rest.n[b + 1] = 0;
+    }
+    const int f = 1 + 4 * L;
+    ZRB_TRY(update_pack_dyn(tl.p[f], tl.g[f], tg[f], r ? r[f] : nullptr, V, H, a, t->fc_w_h, t->Hp, nullptr, nullptr,
+                            nullptr, nullptr, s));
+    rest.n[f] = 0;
+    ZRB_TRY(dyneval_apply(rest, tg, r, a, s));
     t->wg_ok = false;
     c->weights_version++;
     t->packed_version = c->weights_version;      // images are current

@@ -66,6 +66,15 @@ int grad_norm(const TensorList& tl, float max_norm, float* partials, float* scal
 int sgd_apply(const TensorList& tl, float lr, const float* scalars, bool write_g, cudaStream_t s);
 int clip_sgd(const TensorList& tl, float lr, float max_norm, float* partials, float* scalars, float* norm_out,
              bool write_g, cudaStream_t s);
+// Dynamic evaluation (DESIGN.md section 14) over tensors with no fp16 image: tl.p / tl.g as above, tg / r the same
+// tensors of theta_g and of the RMS statistic (r ignored under the SGD rule, a.rbar null).  Zero-length entries are skipped.
+int dyneval_apply(const TensorList& tl, float* const* tg, float* const* r, const DynArgs& a, cudaStream_t s);
+// ms += g * g (one fma per element) over the list: tl.p = ms, tl.g = the window's gradient
+int sq_accumulate(const TensorList& tl, cudaStream_t s);
+// r = sqrt(ms / windows) in place over the list (tl.p), and rbar = fp32(fixed-order fp64 sum of r / P): one partial per
+// block in `partials` (>= kStatsPartials doubles), then one final reduce.  Bit-reproducible run to run.
+constexpr int kStatsPartials = 2048;
+int stats_finish(const TensorList& tl, int64_t windows, double* partials, float* rbar, cudaStream_t s);
 
 // ---- sample.cu ---------------------------------------------------------------------------
 // ZRB_E_INVALID for the arguments zrb_sample rejects (checked before anything is enqueued)

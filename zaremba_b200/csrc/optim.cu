@@ -190,4 +190,153 @@ int clip_sgd(const TensorList& tl, float lr, float max_norm, float* partials, fl
     return sgd_apply(tl, lr, scalars, write_g, s);
 }
 
+// ---- dynamic evaluation (DESIGN.md section 14) ---------------------------------------------------------------------
+// Tensors without an fp16 image (biases, fc.b, the untied embedding; every tensor on the validation engine).  Block
+// (x, y) streams share x of tensor y; no coalescing, so theta_g and r need not be laid out like p.
+struct DynRuns {
+    float* p[16];
+    const float* g[16];
+    const float* tg[16];
+    const float* r[16];
+    int64_t n[16];
+};
+
+// the non-empty entries of the list; returns their count and sets *bx to the blocks per tensor (cap: no more in all)
+static int dyn_runs(const TensorList& tl, float* const* tg, float* const* r, DynRuns* d, int* bx, int cap) {
+    int k = 0;
+    int64_t longest = 0;
+    for (int t = 0; t < tl.count; ++t) {
+        if (tl.n[t] == 0) continue;
+        d->p[k] = tl.p[t]; d->g[k] = tl.g[t]; d->n[k] = tl.n[t];
+        d->tg[k] = tg ? tg[t] : nullptr;
+        d->r[k] = r ? r[t] : nullptr;
+        longest = tl.n[t] > longest ? tl.n[t] : longest;
+        ++k;
+    }
+    int64_t b = (longest / 4 + kThreads - 1) / kThreads;
+    if (b < 1) b = 1;
+    const int c = cap / (k > 0 ? k : 1);
+    *bx = (int)(b > c ? c : b);
+    return k;
+}
+
+template <bool RMS>
+__global__ void dyneval_list_kernel(DynRuns d, DynArgs a) {
+    float* __restrict__ p = d.p[blockIdx.y];
+    const float* __restrict__ g = d.g[blockIdx.y];
+    const float* __restrict__ tg = d.tg[blockIdx.y];
+    const float* __restrict__ r = d.r[blockIdx.y];
+    const int64_t n = d.n[blockIdx.y];
+    const float rbar = RMS ? *a.rbar : 0.f;
+    const int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x, stride = (int64_t)gridDim.x * blockDim.x;
+    int64_t j0 = 0;
+    if (((((uintptr_t)p) | ((uintptr_t)g) | ((uintptr_t)tg) | (RMS ? (uintptr_t)r : 0)) & 15) == 0) {
+        const int64_t n4 = n >> 2;
+        for (int64_t i = tid; i < n4; i += stride) {
+            float4 pv = __ldcs(reinterpret_cast<const float4*>(p) + i), gv = __ldcs(reinterpret_cast<const float4*>(g) + i);
+            float4 tv = __ldcs(reinterpret_cast<const float4*>(tg) + i), rv = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (RMS) rv = __ldcs(reinterpret_cast<const float4*>(r) + i);
+            pv.x = dyneval_elem<RMS>(pv.x, gv.x, tv.x, rv.x, a.lr, a.lam, a.eps, rbar);
+            pv.y = dyneval_elem<RMS>(pv.y, gv.y, tv.y, rv.y, a.lr, a.lam, a.eps, rbar);
+            pv.z = dyneval_elem<RMS>(pv.z, gv.z, tv.z, rv.z, a.lr, a.lam, a.eps, rbar);
+            pv.w = dyneval_elem<RMS>(pv.w, gv.w, tv.w, rv.w, a.lr, a.lam, a.eps, rbar);
+            __stcs(reinterpret_cast<float4*>(p) + i, pv);
+        }
+        j0 = n4 << 2;
+    }
+    for (int64_t j = j0 + tid; j < n; j += stride)
+        p[j] = dyneval_elem<RMS>(p[j], g[j], tg[j], RMS ? r[j] : 0.f, a.lr, a.lam, a.eps, rbar);
+}
+
+int dyneval_apply(const TensorList& tl, float* const* tg, float* const* r, const DynArgs& a, cudaStream_t s) {
+    DynRuns d;
+    int bx = 1;
+    const int k = dyn_runs(tl, tg, a.rbar ? r : nullptr, &d, &bx, kNormBlocks * 2);
+    if (!k) return ZRB_OK;
+    if (a.rbar) dyneval_list_kernel<true><<<dim3(bx, k), kThreads, 0, s>>>(d, a);
+    else dyneval_list_kernel<false><<<dim3(bx, k), kThreads, 0, s>>>(d, a);
+    ZRB_KERNEL_CHECK();
+    return ZRB_OK;
+}
+
+// ms += g * g, one fma per element, one streaming pass
+__global__ void sq_accumulate_kernel(DynRuns d) {
+    float* __restrict__ ms = d.p[blockIdx.y];
+    const float* __restrict__ g = d.g[blockIdx.y];
+    const int64_t n = d.n[blockIdx.y];
+    const int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x, stride = (int64_t)gridDim.x * blockDim.x;
+    int64_t j0 = 0;
+    if (((((uintptr_t)ms) | ((uintptr_t)g)) & 15) == 0) {
+        const int64_t n4 = n >> 2;
+        for (int64_t i = tid; i < n4; i += stride) {
+            float4 m = __ldcs(reinterpret_cast<const float4*>(ms) + i), v = __ldcs(reinterpret_cast<const float4*>(g) + i);
+            m.x = __fmaf_rn(v.x, v.x, m.x); m.y = __fmaf_rn(v.y, v.y, m.y);
+            m.z = __fmaf_rn(v.z, v.z, m.z); m.w = __fmaf_rn(v.w, v.w, m.w);
+            __stcs(reinterpret_cast<float4*>(ms) + i, m);
+        }
+        j0 = n4 << 2;
+    }
+    for (int64_t j = j0 + tid; j < n; j += stride) ms[j] = __fmaf_rn(g[j], g[j], ms[j]);
+}
+
+int sq_accumulate(const TensorList& tl, cudaStream_t s) {
+    DynRuns d;
+    int bx = 1;
+    const int k = dyn_runs(tl, nullptr, nullptr, &d, &bx, kNormBlocks * 2);
+    if (!k) return ZRB_OK;
+    sq_accumulate_kernel<<<dim3(bx, k), kThreads, 0, s>>>(d);
+    ZRB_KERNEL_CHECK();
+    return ZRB_OK;
+}
+
+// block-wide fp64 sum in a fixed order (xor tree in each warp, then the warps' sums in index order)
+__device__ __forceinline__ double block_sum_f64(double v, double* sh) {
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = v;
+    __syncthreads();
+    double t = 0.0;
+    if (threadIdx.x == 0)
+        for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t += sh[w];
+    return t;
+}
+
+// r = sqrt(ms / K) in place; partials[y * gridDim.x + x] = fp64 sum of the r this block wrote
+__global__ void stats_sqrt_kernel(DynRuns d, float kf, double* __restrict__ partials) {
+    __shared__ double sh[kThreads / 32];
+    float* __restrict__ ms = d.p[blockIdx.y];
+    const int64_t n = d.n[blockIdx.y];
+    const int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x, stride = (int64_t)gridDim.x * blockDim.x;
+    double acc = 0.0;
+    for (int64_t j = tid; j < n; j += stride) {
+        const float r = __fsqrt_rn(__fdiv_rn(ms[j], kf));
+        ms[j] = r;
+        acc += (double)r;
+    }
+    const double t = block_sum_f64(acc, sh);
+    if (threadIdx.x == 0) partials[blockIdx.y * gridDim.x + blockIdx.x] = t;
+}
+
+// rbar = fp32(sum of the partials in a fixed order / P): one block
+__global__ void stats_mean_kernel(const double* __restrict__ partials, int n, double P, float* __restrict__ rbar) {
+    __shared__ double sh[kThreads / 32];
+    double acc = 0.0;
+    for (int i = threadIdx.x; i < n; i += blockDim.x) acc += partials[i];
+    const double t = block_sum_f64(acc, sh);
+    if (threadIdx.x == 0) *rbar = (float)(t / P);
+}
+
+int stats_finish(const TensorList& tl, int64_t windows, double* partials, float* rbar, cudaStream_t s) {
+    DynRuns d;
+    int bx = 1;
+    const int k = dyn_runs(tl, nullptr, nullptr, &d, &bx, kStatsPartials);
+    int64_t P = 0;
+    for (int i = 0; i < k; ++i) P += d.n[i];
+    if (!k) return ZRB_OK;
+    stats_sqrt_kernel<<<dim3(bx, k), kThreads, 0, s>>>(d, (float)windows, partials);
+    ZRB_KERNEL_CHECK();
+    stats_mean_kernel<<<1, kThreads, 0, s>>>(partials, bx * k, (double)P, rbar);
+    ZRB_KERNEL_CHECK();
+    return ZRB_OK;
+}
+
 }  // namespace zrb

@@ -1,4 +1,5 @@
-// SGD update fused with the rebuild of the fp16 operand images (tensor-core engine).
+// Weight update -- the train step's SGD, or dynamic evaluation's rule -- fused with the rebuild of the fp16 operand
+// images (tensor-core engine).
 // The update pass already holds every new weight in registers; writing its fp16 images from there
 // removes the separate pack pass (which re-read 348 MB of fp32 weights per step at the Large config).
 #include "tc_kernels.h"
@@ -57,12 +58,47 @@ __device__ __forceinline__ void store_vec(float* p, const float (&v)[VEC]) {
     __stcs(reinterpret_cast<typename VecT<VEC>::type*>(p), t);
 }
 
-// matrix [rows, cols] (cols % VEC == 0): g *= coef; p -= lr*g; row-major fp16 image of the new p.
-template <int VEC>
-__global__ void update_pack_kernel(float* __restrict__ p, float* __restrict__ g, int rows, int cols, float lr,
-                                   const float* __restrict__ scalars, PackSpec sp) {
+// The element rule of the update kernels.  SgdRule: g *= coef (clip_grad_norm_, coef = scalars[1]); p -= lr*g, with g
+// stored back when PackSpec::write_g asks.  DynRule: the dynamic-evaluation update (dyneval_elem), which also reads
+// theta_g and r at the element's offset and never stores g.
+struct SgdRule {
+    float lr;
+    const float* scalars;
+    float coef;
+    static constexpr bool kMayWriteG = true;
+    __device__ __forceinline__ void init() { coef = scalars[1]; }
+    template <int VEC>
+    __device__ __forceinline__ void apply(int64_t, float (&pv)[VEC], float (&gv)[VEC]) const {
+#pragma unroll
+        for (int x = 0; x < VEC; ++x) { gv[x] *= coef; pv[x] = sgd_elem(pv[x], gv[x], lr); }
+    }
+};
+
+template <bool RMS>
+struct DynRule {
+    const float* tg;     // theta_g, same layout as p
+    const float* r;      // RMS statistic, same layout as p (RMS rule only)
+    DynArgs a;
+    float rbar;
+    static constexpr bool kMayWriteG = false;
+    __device__ __forceinline__ void init() { rbar = RMS ? *a.rbar : 0.f; }
+    template <int VEC>
+    __device__ __forceinline__ void apply(int64_t off, float (&pv)[VEC], float (&gv)[VEC]) const {
+        float tv[VEC], rv[VEC];
+        load_vec<VEC>(tg + off, tv);
+        if constexpr (RMS) load_vec<VEC>(r + off, rv);
+#pragma unroll
+        for (int x = 0; x < VEC; ++x)
+            pv[x] = dyneval_elem<RMS>(pv[x], gv[x], tv[x], RMS ? rv[x] : 0.f, a.lr, a.lam, a.eps, rbar);
+    }
+};
+
+// matrix [rows, cols] (cols % VEC == 0): the rule's update of p; row-major fp16 image of the new p.
+template <int VEC, class Rule>
+__global__ void update_pack_kernel(float* __restrict__ p, float* __restrict__ g, int rows, int cols, Rule rule,
+                                   PackSpec sp) {
     pdl_prologue(sp);
-    const float coef = scalars[1];
+    rule.init();
     const int cv = cols / VEC;
     const int64_t total = (int64_t)rows * cv;
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
@@ -71,9 +107,8 @@ __global__ void update_pack_kernel(float* __restrict__ p, float* __restrict__ g,
         float gv[VEC], pv[VEC];
         load_vec<VEC>(g + off, gv);
         load_vec<VEC>(p + off, pv);
-#pragma unroll
-        for (int x = 0; x < VEC; ++x) { gv[x] *= coef; pv[x] = sgd_elem(pv[x], gv[x], lr); }
-        if (sp.write_g) store_vec<VEC>(g + off, gv);
+        rule.template apply<VEC>(off, pv, gv);
+        if (Rule::kMayWriteG && sp.write_g) store_vec<VEC>(g + off, gv);
         store_vec<VEC>(p + off, pv);
         if (sp.row_img) {
             __half hh[VEC];
@@ -88,11 +123,10 @@ __global__ void update_pack_kernel(float* __restrict__ p, float* __restrict__ g,
 // W_hh [4H, H] with both recurrent images: a thread owns an 8-row x VEC-column tile (rows j..j+7 of one gate
 // block), so the backward image -- whose 16-byte vectors hold 8 consecutive K indices (= rows) of one unit
 // (= column) -- is written with full 16-byte stores instead of 2-byte scatters.
-template <int VEC>
-__global__ void update_pack_whh_kernel(float* __restrict__ p, float* __restrict__ g, int H, float lr,
-                                       const float* __restrict__ scalars, PackSpec sp) {
+template <int VEC, class Rule>
+__global__ void update_pack_whh_kernel(float* __restrict__ p, float* __restrict__ g, int H, Rule rule, PackSpec sp) {
     pdl_prologue(sp);
-    const float coef = scalars[1];
+    rule.init();
     const int cv = H / VEC, jb_n = (H + 7) >> 3;
     const int64_t total = (int64_t)4 * jb_n * cv;
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
@@ -108,9 +142,10 @@ __global__ void update_pack_whh_kernel(float* __restrict__ p, float* __restrict_
                 float gv[VEC], pv[VEC];
                 load_vec<VEC>(g + off, gv);
                 load_vec<VEC>(p + off, pv);
+                rule.template apply<VEC>(off, pv, gv);
 #pragma unroll
-                for (int x = 0; x < VEC; ++x) { gv[x] *= coef; pv[x] = sgd_elem(pv[x], gv[x], lr); hv[e][x] = __float2half_rn(pv[x]); }
-                if (sp.write_g) store_vec<VEC>(g + off, gv);
+                for (int x = 0; x < VEC; ++x) hv[e][x] = __float2half_rn(pv[x]);
+                if (Rule::kMayWriteG && sp.write_g) store_vec<VEC>(g + off, gv);
                 store_vec<VEC>(p + off, pv);
                 if (sp.row_img) store_halves<VEC>(sp.row_img + ((int64_t)q * H + j) * sp.ld + c, hv[e]);
                 if (sp.fwd_img) {   // slice of the CTA owning unit j, row 4u+q; K indices c..c+VEC-1 share a K chunk
@@ -142,9 +177,9 @@ __global__ void update_pack_whh_kernel(float* __restrict__ p, float* __restrict_
     pdl_epilogue(sp);
 }
 
-template <int VEC>
-static int update_pack_launch(float* p, float* g, int rows, int cols, float lr, const float* scalars, const PackSpec& sp,
-                              bool whh, cudaStream_t s) {
+template <int VEC, class Rule>
+static int update_pack_launch(float* p, float* g, int rows, int cols, const Rule& rule, const PackSpec& sp, bool whh,
+                              cudaStream_t s) {
     int64_t total = whh ? (int64_t)4 * ((cols + 7) / 8) * (cols / VEC) : (int64_t)rows * (cols / VEC);
     const int threads = whh ? 128 : 256;
     int blocks = (int)((total + threads - 1) / threads);
@@ -158,20 +193,22 @@ static int update_pack_launch(float* p, float* g, int rows, int cols, float lr, 
         at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
         at[0].val.programmaticStreamSerializationAllowed = 1;
         cfg.attrs = at; cfg.numAttrs = 1;
-        if (whh) ZRB_CUDA(cudaLaunchKernelEx(&cfg, update_pack_whh_kernel<VEC>, p, g, cols, lr, scalars, sp));
-        else ZRB_CUDA(cudaLaunchKernelEx(&cfg, update_pack_kernel<VEC>, p, g, rows, cols, lr, scalars, sp));
+        if (whh) ZRB_CUDA(cudaLaunchKernelEx(&cfg, update_pack_whh_kernel<VEC, Rule>, p, g, cols, rule, sp));
+        else ZRB_CUDA(cudaLaunchKernelEx(&cfg, update_pack_kernel<VEC, Rule>, p, g, rows, cols, rule, sp));
         count_launch();
         return ZRB_OK;
     }
-    if (whh) update_pack_whh_kernel<VEC><<<blocks, threads, 0, s>>>(p, g, cols, lr, scalars, sp);
-    else update_pack_kernel<VEC><<<blocks, threads, 0, s>>>(p, g, rows, cols, lr, scalars, sp);
+    if (whh) update_pack_whh_kernel<VEC, Rule><<<blocks, threads, 0, s>>>(p, g, cols, rule, sp);
+    else update_pack_kernel<VEC, Rule><<<blocks, threads, 0, s>>>(p, g, rows, cols, rule, sp);
     ZRB_KERNEL_CHECK();
     return ZRB_OK;
 }
 
-int update_pack(float* p, float* g, int rows, int cols, float lr, const float* scalars, __half* row_img, int64_t ld,
-                __half* fwd_img, const RecPlan* fp, __half* bwd_img, const RecPlan* bp, bool write_g, cudaStream_t s,
-                bool pdl) {
+// align: OR of every pointer the rule streams besides p and g (their alignment picks the access width too)
+template <class Rule>
+static int update_pack_rule(float* p, float* g, int rows, int cols, const Rule& rule, uintptr_t align, __half* row_img,
+                            int64_t ld, __half* fwd_img, const RecPlan* fp, __half* bwd_img, const RecPlan* bp,
+                            bool write_g, cudaStream_t s, bool pdl) {
     PackSpec sp;
     sp.write_g = write_g ? 1 : 0;
     sp.pdl = pdl ? 1 : 0;
@@ -181,10 +218,31 @@ int update_pack(float* p, float* g, int rows, int cols, float lr, const float* s
     sp.bwd_img = bwd_img; sp.bS = bp ? bp->KS : 1; sp.bUC = bp ? 4 * bp->KS * bp->U : 4; sp.bG = bp ? bp->G : 1;
     sp.bKc = bp ? bp->KcS : 1;
     const bool whh = (fwd_img || bwd_img) && rows == 4 * cols;
-    const bool al16 = ((((uintptr_t)p) | ((uintptr_t)g)) & 15) == 0, al8 = ((((uintptr_t)p) | ((uintptr_t)g)) & 7) == 0;
-    if (cols % 4 == 0 && al16) return update_pack_launch<4>(p, g, rows, cols, lr, scalars, sp, whh, s);
-    if (cols % 2 == 0 && al8) return update_pack_launch<2>(p, g, rows, cols, lr, scalars, sp, whh, s);
-    return update_pack_launch<1>(p, g, rows, cols, lr, scalars, sp, whh, s);
+    const uintptr_t all = ((uintptr_t)p) | ((uintptr_t)g) | align;
+    const bool al16 = (all & 15) == 0, al8 = (all & 7) == 0;
+    if (cols % 4 == 0 && al16) return update_pack_launch<4>(p, g, rows, cols, rule, sp, whh, s);
+    if (cols % 2 == 0 && al8) return update_pack_launch<2>(p, g, rows, cols, rule, sp, whh, s);
+    return update_pack_launch<1>(p, g, rows, cols, rule, sp, whh, s);
+}
+
+int update_pack(float* p, float* g, int rows, int cols, float lr, const float* scalars, __half* row_img, int64_t ld,
+                __half* fwd_img, const RecPlan* fp, __half* bwd_img, const RecPlan* bp, bool write_g, cudaStream_t s,
+                bool pdl) {
+    SgdRule rule;
+    rule.lr = lr; rule.scalars = scalars; rule.coef = 0.f;
+    return update_pack_rule(p, g, rows, cols, rule, 0, row_img, ld, fwd_img, fp, bwd_img, bp, write_g, s, pdl);
+}
+
+int update_pack_dyn(float* p, float* g, const float* tg, const float* r, int rows, int cols, const DynArgs& a,
+                    __half* row_img, int64_t ld, __half* fwd_img, const RecPlan* fp, __half* bwd_img, const RecPlan* bp,
+                    cudaStream_t s) {
+    const uintptr_t align = ((uintptr_t)tg) | ((uintptr_t)r);
+    if (a.rbar) {
+        DynRule<true> rule{tg, r, a, 0.f};
+        return update_pack_rule(p, g, rows, cols, rule, align, row_img, ld, fwd_img, fp, bwd_img, bp, false, s, false);
+    }
+    DynRule<false> rule{tg, nullptr, a, 0.f};
+    return update_pack_rule(p, g, rows, cols, rule, align, row_img, ld, fwd_img, fp, bwd_img, bp, false, s, false);
 }
 
 }  // namespace zrb

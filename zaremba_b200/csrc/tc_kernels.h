@@ -74,6 +74,11 @@ int fwd_prep(const FwdPrep& a, cudaStream_t s);
 int update_pack(float* p, float* g, int rows, int cols, float lr, const float* scalars, __half* row_img, int64_t ld,
                 __half* fwd_img, const RecPlan* fp, __half* bwd_img, const RecPlan* bp, bool write_g, cudaStream_t s,
                 bool pdl = false);   // pdl: programmatic dependent of the (forward recurrence) kernel enqueued before it
+// the same kernels with the dynamic-evaluation rule (dyneval_elem): theta_g tg and r at p's offsets (r unused under the
+// SGD rule, a.rbar null); g is read, never written; the same images
+int update_pack_dyn(float* p, float* g, const float* tg, const float* r, int rows, int cols, const DynArgs& a,
+                    __half* row_img, int64_t ld, __half* fwd_img, const RecPlan* fp, __half* bwd_img, const RecPlan* bp,
+                    cudaStream_t s);
 int rec_bwd_plan(int H, int B, RecPlan* plan);   // U = units per CTA, nCTA = 4 * clusters
 int pack_whh_bwd(const float* W, __half* img, int H, const RecPlan& p, cudaStream_t s);
 int lstm_rec_bwd(const RecPlan& p, const RecWatchdog& wd, const __half* w_img, __half* g_img, const float* dy, const float* gates,

@@ -447,3 +447,116 @@ class Trainer:
             acc += loss.double() / x.shape[1]
             n += 1
         return math.exp(acc.item() / max(n, 1))
+
+    # ---- dynamic evaluation (DESIGN.md section 14) -------------------------------------------------------------------
+    def _single_replica(self, what):
+        if self.world > 1:
+            raise ValueError(f"{what} adapts one replica: create the Trainer with data_parallel=False")
+
+    def _check_flat(self, flat):
+        if flat.shape != self.flat_p.shape or flat.dtype != torch.float32 or flat.device != self.flat_p.device or \
+                not flat.is_contiguous():
+            raise ValueError(f"expected a contiguous flat fp32 tensor of {self.flat_p.numel()} elements on {self.dev}")
+
+    def _flat_params_struct(self, flat):
+        """zrb_params over a flat tensor in flat_p's layout (theta_g, the statistics): views at the parameters' offsets."""
+        self._check_flat(flat)
+        base = self.flat_p.data_ptr()
+        views = [flat[(p.data_ptr() - base) // 4:][:p.numel()].view_as(p) for p in self.model.ordered_parameters()]
+        return self.model._params_struct(views)[0]
+
+    def gradient_stats(self, batches):
+        """The RMS rule's statistics over `batches` ((x, y) [T,B] windows, one B for all): per window the eval-mode
+        gradient at the current weights (no update), states carried from zero; ms += g^2, then r = sqrt(ms / K) and
+        r-bar.  The weights are unchanged; pending lazy updates are applied first; the Trainer's states are reset.
+        The windows may have another [T,B] than the evaluation ones.  Windows larger than the Trainer's own [T,B] make
+        the model re-create its context for the larger shape, and the Trainer then keeps running in that context, whose
+        recurrence plans were chosen for the larger batch.  To keep the Trainer's own plans, compute such statistics on
+        a Trainer of their shape: a `GradStats` serves every Trainer of the same model configuration (the flat layout
+        depends only on the model).  Returns a `GradStats`."""
+        from .dyneval import GradStats
+        self._single_replica("gradient_stats")
+        batches = list(batches)
+        if not batches:
+            raise ValueError("gradient_stats needs at least one window")
+        Bs = {x.shape[1] for x, _ in batches}
+        if len(Bs) != 1:
+            raise ValueError(f"all statistics windows must have one batch size (got {sorted(Bs)})")
+        B = Bs.pop()
+        T = max(x.shape[0] for x, _ in batches)
+        lib = _lib.load()
+        self.flush()
+        self._check_versions()
+        if T > self.T or B > self.B:     # a larger context for these windows (the Trainer's own still fit in it)
+            self.model._context(max(T, self.T), max(B, self.B))
+        ctx = self.ctx
+        self.reset_states()
+        states = self.states if B == self.B else self.model.state_init(B)
+        st, keep_s = self.model._states_struct(states)
+        ms = torch.zeros_like(self.flat_p)
+        ms_s = self._flat_params_struct(ms)
+        mean = torch.zeros((), device=self.dev)
+        loss = torch.zeros((), device=self.dev)
+        for x, y in batches:
+            xd = x.to(self.dev).contiguous(); yd = y.to(self.dev).contiguous()
+            _lib.check(lib.zrb_grad_stats_step(ctx, C.byref(self._ps), C.byref(self._gs), C.byref(ms_s), _lib.ptr(xd),
+                                               _lib.ptr(yd), xd.shape[0], B, C.byref(st), C.byref(st), _lib.ptr(loss),
+                                               self._stream()))
+        _lib.check(lib.zrb_grad_stats_finish(ctx, C.byref(ms_s), len(batches), _lib.ptr(mean), self._stream()))
+        self.reset_states()
+        return GradStats(ms, mean, len(batches))
+
+    def dynamic_eval_step(self, x, y, theta_g, lr, lam=0.0, stats=None, eps=2e-5):
+        """One window of dynamic evaluation (zrb_dyneval_step): the eval-mode loss at the current weights, then
+        theta += a * (theta_g - theta) - lr * u with the RMS rule (stats: a `GradStats`) or the SGD rule (stats None).
+        theta_g: flat tensor in flat_p's layout.  Carries `self.states` (so B must not exceed the Trainer's batch);
+        returns the 0-d loss tensor (no host sync).  Afterwards `.grad` holds the window's raw gradient."""
+        self._single_replica("dynamic_eval_step")
+        lib = _lib.load()
+        T, B = x.shape
+        if B > self.B:
+            raise ValueError(f"window batch {B} exceeds the Trainer's batch {self.B} (its states hold {self.B} rows)")
+        if stats is not None and (stats.mean.numel() != 1 or stats.mean.dtype != torch.float32
+                                  or stats.mean.device != self.flat_p.device):
+            raise ValueError(f"stats.mean must be one fp32 element on {self.dev}")
+        self._check_flat(theta_g)          # every call; the structs below only hold the pointers
+        if stats is not None:
+            self._check_flat(stats.rms)
+        key = (theta_g.data_ptr(), None if stats is None else stats.rms.data_ptr())
+        if getattr(self, "_dyn_key", None) != key:
+            self._dyn_structs = (self._flat_params_struct(theta_g),
+                                 None if stats is None else self._flat_params_struct(stats.rms))
+            self._dyn_key = key
+        gl, rms = self._dyn_structs
+        self._check_versions()
+        self._pending = False          # the call applies what is pending before it reads the weights
+        _lib.check(lib.zrb_dyneval_step(self.ctx, C.byref(self._ps), C.byref(self._gs), C.byref(gl),
+                                        None if rms is None else C.byref(rms),
+                                        None if stats is None else _lib.ptr(stats.mean), _lib.ptr(x), _lib.ptr(y), T, B,
+                                        C.byref(self._st), C.byref(self._st), float(lr), float(lam), float(eps),
+                                        _lib.ptr(self.loss), self._stream()))
+        return self.loss
+
+    def dynamic_perplexity(self, batches, lr, lam=0.0, stats=None, eps=2e-5, restore=True):
+        """`perplexity` with dynamic evaluation: applies pending updates, snapshots theta_g = the current weights,
+        resets the states, adapts after every window and returns exp(mean over windows of loss / B).  restore: put
+        theta_g back afterwards (and tell the library)."""
+        self._single_replica("dynamic_perplexity")
+        self.flush()
+        self._check_versions()
+        theta_g = self.flat_p.clone()
+        self.reset_states()
+        acc = torch.zeros((), device=self.dev, dtype=torch.float64)
+        n = 0
+        try:
+            for x, y in batches:
+                xd = x.to(self.dev).contiguous(); yd = y.to(self.dev).contiguous()
+                loss = self.dynamic_eval_step(xd, yd, theta_g, lr, lam, stats, eps)
+                acc += loss.double() / x.shape[1]
+                n += 1
+            return math.exp(acc.item() / max(n, 1))
+        finally:
+            if restore:
+                with torch.no_grad():
+                    self.flat_p.copy_(theta_g)
+                self.params_changed()
