@@ -15,6 +15,28 @@
 
 #include "tc_kernels.h"
 
+// One grid-barrier word of the persistent recurrence kernels.  The word is never reset between launches: each launch
+// gets the value it starts from as its base, and its T * nCTA arrivals advance the word.
+struct GridBarrier {
+    unsigned int* word = nullptr;
+    unsigned int base = 0;   // the word's value when the next launch starts
+    // claim T * nCTA arrivals: enqueue launch(word, base), after resetting the word when the arrivals could wrap it (once
+    // per ~900k launches; the reset stays before the launch, so nothing lands between a recurrence kernel and its
+    // programmatic dependents).  The base advances only once the launch is enqueued: after a failed launch the next
+    // one must not wait for arrivals that never came.
+    template <typename Launch>
+    int claim(int T, int nCTA, cudaStream_t s, Launch&& launch) {
+        const unsigned int arrivals = (unsigned int)T * (unsigned int)nCTA;
+        if (base > 0xF0000000u - arrivals) {
+            ZRB_CUDA(cudaMemsetAsync(word, 0, sizeof(unsigned int), s));
+            base = 0;
+        }
+        ZRB_TRY(launch(word, base));
+        base += arrivals;
+        return ZRB_OK;
+    }
+};
+
 struct zrb_tc_state {
     int Hp = 0, G4p = 0, Vp = 0;
     int device = 0;
@@ -46,8 +68,7 @@ struct zrb_tc_state {
     __half* w_img_f[ZRB_MAX_LAYERS] = {};
     __half* h0_img[ZRB_MAX_LAYERS] = {};   // image of the state entering the window (step 0's B operand)
     __half* h_img = nullptr;
-    unsigned int* counter = nullptr;       // [0]: forward grid barrier, [32]: backward; never reset between launches,
-    unsigned int cnt_f = 0, cnt_b = 0;     // their values when the next launch starts
+    GridBarrier fwd_bar, bwd_bar;          // words 0 and 32 of one allocation; shared by the model- and layer-level calls
     zrb::RecPlan bplan{};
     __half* w_img_b[ZRB_MAX_LAYERS] = {};
     __half* g_img = nullptr;
@@ -61,7 +82,13 @@ struct zrb_tc_state {
 
 namespace zrb {
 
-static bool prof_keeps_pdl();
+// whether work may run as a programmatic dependent beside a recurrence kernel: not while zrb_prof_enable brackets the
+// kernel classes with events (a record would sit between the two launches), unless ZRB_PROF_KEEP_PDL=1
+static bool pdl_beside_rec(const zrb_ctx* c) {
+    if (!c->prof_on) return true;
+    static const bool keep = getenv("ZRB_PROF_KEEP_PDL") != nullptr;
+    return keep;
+}
 static int pad64(int n) { return (n + 63) / 64 * 64; }
 
 template <typename T>
@@ -122,7 +149,10 @@ int tc_ctx_init(zrb_ctx* c) {
             ZRB_TRY(tc_alloc(c, &t->h0_img[l], (size_t)fp.Kc * fp.GBi * 64));
         }
         ZRB_TRY(tc_alloc(c, &t->h_img, (size_t)(c->cfg.max_seq + 1) * fp.Kc * fp.GBi * 64));
-        ZRB_TRY(tc_alloc(c, &t->counter, 64));
+        unsigned int* words = nullptr;
+        ZRB_TRY(tc_alloc(c, &words, 64));
+        t->fwd_bar.word = words;
+        t->bwd_bar.word = words + 32;
     }
     if (getenv("ZRB_REC_TRACE")) ZRB_TRY(tc_alloc(c, &t->trace, (size_t)2 * (8 + c->cfg.max_seq * 8)));
     ZRB_TRY(rec_bwd_plan(H, c->cfg.max_batch, &t->bplan));
@@ -198,7 +228,7 @@ int tc_forward(zrb_ctx* c, const zrb_params* p, const int64_t* x, const zrb_stat
     const int Hp = t->Hp;
     const size_t bh = (size_t)B * H * sizeof(float);
     // deferred updates ride beside the forward recurrences of a fused train step; any other forward applies them first
-    const bool ride = t->upd_pending && t->in_train_step && t->fplan.ok && (!c->prof_on || prof_keeps_pdl());
+    const bool ride = t->upd_pending && t->in_train_step && t->fplan.ok && pdl_beside_rec(c);
     if (t->upd_pending && !ride) ZRB_TRY(tc_flush_updates(c, s));
     ZRB_TRY(tc_pack_weights(c, p, s));
     {   // state copies (in / out may be the same buffers), fp16 h0 rows and images, saved tokens: one launch
@@ -230,15 +260,11 @@ int tc_forward(zrb_ctx* c, const zrb_params* p, const int64_t* x, const zrb_stat
         MaskSrc m = site_mask(c, l + 1), rm = rec_mask(c, l);
         ProfScope ps(c, ZRB_PROF_REC_FWD, s);
         if (t->fplan.ok) {
-            const unsigned int arrivals = (unsigned int)T * (unsigned int)t->fplan.nCTA;
-            if (t->cnt_f > 0xF0000000u - arrivals) {   // far from wrapping: once per ~900k launches
-                ZRB_CUDA(cudaMemsetAsync(t->counter, 0, sizeof(unsigned int), s));
-                t->cnt_f = 0;
-            }
-            ZRB_TRY(lstm_rec_fwd(t->fplan, tc_watchdog(c), t->w_img_f[l], t->h0_img[l], t->h_img, G, c->c0s[l], c->cst[l], out->h[l],
-                                 out->c[l], t->hprev_h[l], t->x_h[l + 1], t->counter, t->cnt_f, T, B, H, Hp, m, rm, s,
-                                 t->trace));
-            t->cnt_f += arrivals;
+            ZRB_TRY(t->fwd_bar.claim(T, t->fplan.nCTA, s, [&](unsigned int* word, unsigned int base) {
+                return lstm_rec_fwd(t->fplan, tc_watchdog(c), t->w_img_f[l], t->h0_img[l], t->h_img, G, c->c0s[l], c->cst[l],
+                                    out->h[l], out->c[l], t->hprev_h[l], t->x_h[l + 1], word, base, T, B, H, Hp, m, rm, s,
+                                    t->trace);
+            }));
             // deferred update of the NEXT layer's matrices (or of fc.W after the last layer): on the idle SMs, beside
             // this recurrence; their consumers (the next input GEMM / the projection) are enqueued behind them
             if (ride) ZRB_TRY(tc_issue_update(c, l + 1, true, s));
@@ -266,11 +292,6 @@ int tc_forward(zrb_ctx* c, const zrb_params* p, const int64_t* x, const zrb_stat
 }
 
 const __half* tc_last_layer_image(const zrb_ctx* c) { return c->tc->x_h[c->cfg.layers]; }
-
-static bool prof_keeps_pdl() {
-    static const bool on = getenv("ZRB_PROF_KEEP_PDL") != nullptr;
-    return on;
-}
 
 // next block of sum-of-squares slots for an [M,N] weight gradient, or null when the step does not fuse the norm
 static float* wgrad_sumsq(zrb_ctx* c, int M, int N, int K) {
@@ -308,7 +329,7 @@ static int tc_backward_head(zrb_ctx* c, const zrb_params* p, const zrb_params* g
         // dW[V,H] = dS^T[V,N] * A[N,H]     (both operands MN-major: contraction over tokens).  Nothing downstream in
         // backward reads it: with deferral on it runs underneath the first backward recurrence instead of before it.
         t->pending = 0;
-        if (t->defer_wgrad && t->bplan.ok && (!c->prof_on || prof_keeps_pdl())) t->pending = 1;
+        if (t->defer_wgrad && t->bplan.ok && pdl_beside_rec(c)) t->pending = 1;
         else ZRB_TRY(gemm_f16_tc(t->dS_h, Vp, 1, t->x_h[L], Hp, 1, g->fc_w, H, V, H, N, inv, nullptr, 0, s,
                                  wgrad_sumsq(c, V, H, N)));
     }
@@ -364,16 +385,12 @@ static int tc_backward_layer(zrb_ctx* c, const zrb_params* p, const zrb_params* 
         MaskSrc m = site_mask(c, l + 1), rm = rec_mask(c, l);
         if (t->bplan.ok) {
             ProfScope ps(c, ZRB_PROF_REC_BWD, s);
-            const unsigned int arrivals = (unsigned int)T * (unsigned int)t->bplan.nCTA;
-            if (t->cnt_b > 0xF0000000u - arrivals) {
-                ZRB_CUDA(cudaMemsetAsync(t->counter + 32, 0, sizeof(unsigned int), s));
-                t->cnt_b = 0;
-            }
-            ZRB_TRY(lstm_rec_bwd(t->bplan, tc_watchdog(c), t->w_img_b[l], t->g_img, dY, c->gates[l], c->cst[l], c->c0s[l], dG_h,
-                                 t->counter + 32, t->cnt_b, T, B, H, G4p, m, rm, s,
-                                 t->trace ? t->trace + 8 + (size_t)c->cfg.max_seq * 8 : nullptr, g->b_ih[l], g->b_hh[l],
-                                 c->resident_flag, ++c->resident_seq, c->dG /* [N,4H] fp32, idle on this path */));
-            t->cnt_b += arrivals;
+            ZRB_TRY(t->bwd_bar.claim(T, t->bplan.nCTA, s, [&](unsigned int* word, unsigned int base) {
+                return lstm_rec_bwd(t->bplan, tc_watchdog(c), t->w_img_b[l], t->g_img, dY, c->gates[l], c->cst[l], c->c0s[l],
+                                    dG_h, word, base, T, B, H, G4p, m, rm, s,
+                                    t->trace ? t->trace + 8 + (size_t)c->cfg.max_seq * 8 : nullptr, g->b_ih[l], g->b_hh[l],
+                                    c->resident_flag, ++c->resident_seq, c->dG /* [N,4H] fp32, idle on this path */);
+            }));
             ZRB_TRY(tc_issue_pending(c, g, s));   // runs on the SMs the cluster kernel leaves idle
         } else {
             ProfScope ps(c, ZRB_PROF_REC_BWD, s);
@@ -395,7 +412,7 @@ static int tc_backward_layer(zrb_ctx* c, const zrb_params* p, const zrb_params* 
         }
         // dW_ih, dW_hh: nothing downstream in backward reads them -> for l > 0 they run underneath the next layer's
         // recurrence (which writes the other dG buffer); the bias gradients come out of the recurrence kernel itself
-        if (t->defer_wgrad && t->bplan.ok && l > 0 && (!c->prof_on || prof_keeps_pdl())) {
+        if (t->defer_wgrad && t->bplan.ok && l > 0 && pdl_beside_rec(c)) {
             t->pending = 2;
             t->pending_layer = l;
         } else {
@@ -548,15 +565,11 @@ int tc_layer_fwd(zrb_ctx* c, const float* w_ih, const float* w_hh, const float* 
     fp.L = 1; fp.B = B; fp.H = H; fp.Hp = Hp; fp.GB = t->fplan.GBi; fp.Kc = t->fplan.Kc; fp.N = 0;
     ZRB_TRY(fwd_prep(fp, s));
     ZRB_TRY(gemm_f16_tc(t->x_h[0], Hp, 0, t->w_ih_h[0], Hp, 0, c->gates[0], 4 * H, N, 4 * H, H, 1.f, b_ih, 0, s, nullptr, b_hh));
-    const unsigned int arrivals = (unsigned int)T * (unsigned int)t->fplan.nCTA;
-    if (t->cnt_f > 0xF0000000u - arrivals) {
-        ZRB_CUDA(cudaMemsetAsync(t->counter, 0, sizeof(unsigned int), s));
-        t->cnt_f = 0;
-    }
     MaskSrc m = make_mask_src(nullptr, 0, 0, 0, 0.f, 0);    // no dropout at this level: the caller applies it (model.py:105,108)
-    ZRB_TRY(lstm_rec_fwd(t->fplan, tc_watchdog(c), t->w_img_f[0], t->h0_img[0], t->h_img, c->gates[0], c->c0s[0], c->cst[0], hT, cT,
-                         t->hprev_h[0], t->x_h[1], t->counter, t->cnt_f, T, B, H, Hp, m, m, s, nullptr, y));
-    t->cnt_f += arrivals;
+    ZRB_TRY(t->fwd_bar.claim(T, t->fplan.nCTA, s, [&](unsigned int* word, unsigned int base) {
+        return lstm_rec_fwd(t->fplan, tc_watchdog(c), t->w_img_f[0], t->h0_img[0], t->h_img, c->gates[0], c->c0s[0], c->cst[0],
+                            hT, cT, t->hprev_h[0], t->x_h[1], word, base, T, B, H, Hp, m, m, s, nullptr, y);
+    }));
     c->have_fwd = false;                         // a model-level backward must not follow this
     c->layer_fwd_ok = true;
     return ZRB_OK;
@@ -570,15 +583,11 @@ int tc_layer_bwd(zrb_ctx* c, const float* dy, float* dx, float* dw_ih, float* dw
         set_error("zrb_lstm_layer_bwd without a preceding zrb_lstm_layer_fwd");
         return ZRB_E_STATE;
     }
-    const unsigned int arrivals = (unsigned int)T * (unsigned int)t->bplan.nCTA;
-    if (t->cnt_b > 0xF0000000u - arrivals) {
-        ZRB_CUDA(cudaMemsetAsync(t->counter + 32, 0, sizeof(unsigned int), s));
-        t->cnt_b = 0;
-    }
     MaskSrc m = make_mask_src(nullptr, 0, 0, 0, 0.f, 0);
-    ZRB_TRY(lstm_rec_bwd(t->bplan, tc_watchdog(c), t->w_img_b[0], t->g_img, dy, c->gates[0], c->cst[0], c->c0s[0], t->dG_h, t->counter + 32,
-                         t->cnt_b, T, B, H, G4p, m, m, s, nullptr, db_ih, db_hh, c->resident_flag, ++c->resident_seq, c->dG));
-    t->cnt_b += arrivals;
+    ZRB_TRY(t->bwd_bar.claim(T, t->bplan.nCTA, s, [&](unsigned int* word, unsigned int base) {
+        return lstm_rec_bwd(t->bplan, tc_watchdog(c), t->w_img_b[0], t->g_img, dy, c->gates[0], c->cst[0], c->c0s[0], t->dG_h,
+                            word, base, T, B, H, G4p, m, m, s, nullptr, db_ih, db_hh, c->resident_flag, ++c->resident_seq, c->dG);
+    }));
     const float inv = 1.f / kGradScale;
     if (dx) ZRB_TRY(gemm_f16_tc(t->dG_h, G4p, 0, t->w_ih_h[0], Hp, 1, dx, H, N, H, 4 * H, inv, nullptr, 0, s));
     ZRB_TRY(gemm_f16_tc(t->dG_h, G4p, 1, t->x_h[0], Hp, 1, dw_ih, H, 4 * H, H, N, inv, nullptr, 0, s, nullptr, nullptr, false,
@@ -647,7 +656,7 @@ int tc_update(zrb_ctx* c, const zrb_params* p, const TensorList& tl, float lr, f
     const bool persistent = t->fplan.ok && t->bplan.ok;
     // lazy update: layer 0 (needed by the very next kernels) now; layers >= 1 and fc.W beside the forward recurrences of
     // the next step (tc_forward), or at the next call that is not a fused train step (tc_flush_updates)
-    const bool lazy = c->lazy_update && persistent && (!c->prof_on || prof_keeps_pdl());
+    const bool lazy = c->lazy_update && persistent && pdl_beside_rec(c);
     if (lazy) {
         t->upd_tl = tl;
         t->upd_lr = lr;

@@ -429,35 +429,6 @@ __global__ void pack_whh_bwd_kernel(const float* __restrict__ W, __half* __restr
     }
 }
 
-static bool rec_bwd_no_coop() {
-    // Profilers (Nsight Compute) refuse cooperative + cluster launches; under one (detected through the injection
-    // environment it sets up) or with ZRB_NO_COOP=1 the kernel is launched as a plain cluster launch after an occupancy
-    // check that the whole grid fits the device.  Without the cooperative guarantee another context holding SMs (MPS, a
-    // concurrent kernel) could leave CTAs unscheduled; the barrier waits are bounded: after ~3 s the kernel gives up and reports it (rec_common.cuh: RecWatch) instead of hanging.
-    static const bool v = getenv("ZRB_NO_COOP") != nullptr || getenv("CUDA_INJECTION64_PATH") != nullptr ||
-                          getenv("NV_COMPUTE_PROFILER_PERFWORKS_DIR") != nullptr || getenv("NVTX_INJECTION64_PATH") != nullptr;
-    return v;
-}
-
-template <int S>
-static int rec_bwd_max_clusters(int smem) {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(4 * S * 64);
-    cfg.blockDim = dim3(kRecThreads);
-    cfg.dynamicSmemBytes = (size_t)smem;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = 4 * S; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-    cfg.attrs = at; cfg.numAttrs = 1;
-    int n = 0;
-    if (cudaFuncSetAttribute(lstm_rec_bwd_kernel<S>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess ||
-        cudaOccupancyMaxActiveClusters(&n, lstm_rec_bwd_kernel<S>, &cfg) != cudaSuccess) {
-        (void)cudaGetLastError();
-        return 0;
-    }
-    return n;
-}
-
 int rec_bwd_plan(int H, int B, RecPlan* plan) {
     int nsm = tc_num_sms();
     plan->GB = (B + 7) / 8;
@@ -479,10 +450,11 @@ int rec_bwd_plan(int H, int B, RecPlan* plan) {
                 const int G = UC / 8;
                 const size_t smem = rec_smem_bytes(KcS, G, GBi);
                 if (smem <= 227 * 1024 && 8 * U * (GBi * 8 + 4) <= 2 * 64 * (GBi * 8 + 1)) {
-                    if (rec_bwd_max_clusters<2>((int)smem) < ncl) continue;   // the GPCs cannot hold that many 8-CTA clusters
+                    // the GPCs cannot hold that many 8-CTA clusters
+                    if (rec_max_clusters((const void*)lstm_rec_bwd_kernel<2>, 8, (int)smem, 8 * 64) < ncl) continue;
                     plan->KS = 2; plan->U = U; plan->G = G; plan->nCTA = ncl * 8; plan->smem = (int)smem;
-                    plan->Kc = Kc; plan->KcS = KcS; plan->GBi = GBi; plan->ok = 1;
-                    return ZRB_OK;
+                    plan->Kc = Kc; plan->KcS = KcS; plan->GBi = GBi;
+                    return rec_plan_finish(plan, (const void*)lstm_rec_bwd_kernel<2>, 8);
                 }
             }
     }
@@ -499,8 +471,8 @@ int rec_bwd_plan(int H, int B, RecPlan* plan) {
         int G = UC / 8;
         size_t smem = rec_smem_bytes(plan->Kc, G, plan->GB);
         if (smem <= 227 * 1024 && U * B <= kRecMaxCell * kRecEpiThreads) {
-            plan->U = U; plan->G = G; plan->nCTA = ncl * 4; plan->smem = (int)smem; plan->ok = 1;
-            return ZRB_OK;
+            plan->U = U; plan->G = G; plan->nCTA = ncl * 4; plan->smem = (int)smem;
+            return rec_plan_finish(plan, (const void*)lstm_rec_bwd_kernel<1>, 4);
         }
     }
     return ZRB_OK;
@@ -510,74 +482,6 @@ int pack_whh_bwd(const float* W, __half* img, int H, const RecPlan& p, cudaStrea
     const int CS = 4 * p.KS;
     pack_whh_bwd_kernel<<<tc_num_sms() * 4, 256, 0, s>>>(W, img, H, CS * p.U, p.G, p.KcS, p.KS, p.nCTA / CS);
     ZRB_KERNEL_CHECK();
-    return ZRB_OK;
-}
-
-template <int S>
-static int launch_rec_bwd(const RecPlan& p, const RecBwdArgs& a, cudaStream_t s) {
-    constexpr int CS = 4 * S;
-    static bool attr[64] = {};   // per device: function attributes belong to the device's context
-    int dev = 0;
-    cudaGetDevice(&dev);
-    dev &= 63;
-    if (!attr[dev]) {
-        ZRB_CUDA(cudaFuncSetAttribute(lstm_rec_bwd_kernel<S>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        attr[dev] = true;
-    }
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(p.nCTA);
-    cfg.blockDim = dim3(kRecThreads);
-    cfg.dynamicSmemBytes = (size_t)p.smem;
-    cfg.stream = s;
-    cudaLaunchAttribute attrs[2];
-    attrs[0].id = cudaLaunchAttributeClusterDimension;
-    attrs[0].val.clusterDim.x = CS; attrs[0].val.clusterDim.y = 1; attrs[0].val.clusterDim.z = 1;
-    cfg.attrs = attrs;
-    // The grid barrier needs all nCTA CTAs co-resident.  Either the cooperative attribute makes the driver guarantee it
-    // (or refuse the launch), or -- one context on the device, or under a profiler (rec_bwd_no_coop()) -- a plain cluster
-    // launch checked against the occupancy query, with the programmatic attribute so that the CTAs start behind the
-    // preceding GEMM's trigger (tc_common.cuh, rec_launch_programmatic()).
-    const bool programmatic = rec_launch_programmatic(dev) && !a.trace;
-    const bool no_coop = programmatic || rec_bwd_no_coop();
-    cudaError_t e = cudaSuccess;
-    if (!no_coop) {
-        attrs[1].id = cudaLaunchAttributeCooperative;
-        attrs[1].val.cooperative = 1;
-        cfg.numAttrs = 2;
-        e = cudaLaunchKernelEx(&cfg, lstm_rec_bwd_kernel<S>, a);
-        if (e == cudaErrorCooperativeLaunchTooLarge) {
-            (void)cudaGetLastError();
-            set_error("lstm_rec_bwd: the %d-CTA grid cannot be co-resident on this device (cooperative launch too large)",
-                      p.nCTA);
-            return ZRB_E_CUDA;
-        }
-        if (e != cudaSuccess) (void)cudaGetLastError();   // e.g. not supported under a tool: try the checked plain launch
-    }
-    if (no_coop || e != cudaSuccess) {
-        cfg.numAttrs = 1;
-        static int seen_dev = -1, seen_smem = -1, seen_max = 0;   // the query is a host call: once per (device, footprint)
-        if (seen_dev != dev || seen_smem != p.smem) {
-            int max_clusters = 0;
-            cudaError_t oe = cudaOccupancyMaxActiveClusters(&max_clusters, lstm_rec_bwd_kernel<S>, &cfg);
-            if (oe != cudaSuccess) { (void)cudaGetLastError(); max_clusters = 0; }
-            seen_dev = dev; seen_smem = p.smem; seen_max = max_clusters;
-        }
-        if (seen_max * CS < p.nCTA) {
-            set_error("lstm_rec_bwd: %d clusters of %d needed, the device can hold %d at once", p.nCTA / CS, CS, seen_max);
-            return ZRB_E_CUDA;
-        }
-        if (programmatic) {
-            attrs[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-            attrs[1].val.programmaticStreamSerializationAllowed = 1;
-            cfg.numAttrs = 2;
-        }
-        e = cudaLaunchKernelEx(&cfg, lstm_rec_bwd_kernel<S>, a);
-    }
-    if (e != cudaSuccess) {
-        set_error("lstm_rec_bwd launch failed: %s", cudaGetErrorString(e));
-        return ZRB_E_CUDA;
-    }
-    count_launch();
     return ZRB_OK;
 }
 
@@ -599,7 +503,8 @@ int lstm_rec_bwd(const RecPlan& p, const RecWatchdog& wd, const __half* w_img, _
     a.w = rec_watch_args(wd);
     a.base += rec_fault_base("bwd");   // (tests only)
     if (trace) ZRB_CUDA(cudaMemsetAsync(trace + 4, 0x80, 2 * sizeof(long long), s));
-    return p.KS == 2 ? launch_rec_bwd<2>(p, a, s) : launch_rec_bwd<1>(p, a, s);
+    void* args[] = {&a};
+    return rec_launch(p, args, trace != nullptr, s, "lstm_rec_bwd");
 }
 
 }  // namespace zrb

@@ -1,4 +1,4 @@
-// Persistent LSTM recurrence, forward, one launch per layer (sm_90a, cooperative launch).
+// Persistent LSTM recurrence, forward, one launch per layer (sm_90a; launch modes: rec_launch below).
 //
 //   for t in 0..T-1:   gates_t = XG_t + h_{t-1} * W_hh^T ;  (i,f,g,o) ;  c_t, h_t     (model.py:34-45)
 //
@@ -325,16 +325,113 @@ size_t rec_smem_bytes(int Kc, int G, int GB) {
     return (size_t)Kc * G * 128 + (size_t)Kc * GB * 128 + 2 * 64 * (GB * 8 + 1) * 4 + 128 /*align*/ + 128 /*bars*/;
 }
 
+int rec_max_clusters(const void* kernel, int cluster, int smem, int nCTA) {
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(nCTA);
+    cfg.blockDim = dim3(kRecThreads);
+    cfg.dynamicSmemBytes = (size_t)smem;
+    cudaLaunchAttribute at[1];
+    at[0].id = cudaLaunchAttributeClusterDimension;
+    at[0].val.clusterDim.x = cluster; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
+    cfg.attrs = at; cfg.numAttrs = 1;
+    int n = 0;
+    if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess ||
+        cudaOccupancyMaxActiveClusters(&n, kernel, &cfg) != cudaSuccess) {
+        (void)cudaGetLastError();
+        return 0;
+    }
+    return n;
+}
+
+int rec_plan_finish(RecPlan* plan, const void* kernel, int cluster) {
+    plan->kernel = kernel;
+    plan->cluster = cluster;
+    plan->max_clusters = rec_max_clusters(kernel, cluster, plan->smem, plan->nCTA);
+    plan->ok = 1;
+    return ZRB_OK;
+}
+
 static bool rec_no_coop() {
     // Profilers (Nsight Compute) refuse cooperative + cluster launches; under one (detected through the injection
-    // environment it sets up) or with ZRB_NO_COOP=1 cluster kernels are launched without the cooperative attribute,
-    // after an occupancy check that the whole grid fits the device
+    // environment it sets up) or with ZRB_NO_COOP=1 cluster kernels take the checked plain launch
     static const bool v = getenv("ZRB_NO_COOP") != nullptr || getenv("CUDA_INJECTION64_PATH") != nullptr ||
                           getenv("NV_COMPUTE_PROFILER_PERFWORKS_DIR") != nullptr || getenv("NVTX_INJECTION64_PATH") != nullptr;
     return v;
 }
 
+// How both persistent recurrence kernels are launched.  Their grid barrier needs all nCTA CTAs co-resident:
+//   cooperative   -- the driver guarantees it or refuses the launch (cudaErrorCooperativeLaunchTooLarge: an error, no
+//                    fallback).  Always for the unclustered forward, which has no plain mode; for cluster grids unless one
+//                    of the next two applies.
+//   programmatic  -- a plain cluster launch, checked against the plan's occupancy answer, with the programmatic-
+//                    serialization attribute: the GEMM enqueued before it triggers at its start, so the recurrence CTAs
+//                    take SMs as the GEMM's CTAs retire and fetch their resident weight slices while its tail is still
+//                    running (pdl_wait in the kernels).  9 us per train step at the Large config; the cooperative
+//                    attribute suppresses the early start (measured: no gain with both attributes).  Decided at every
+//                    launch by rec_launch_programmatic (tc_common.cuh: while ONE tensor-core context is alive on the
+//                    device, since a second context can appear at any time), never for a traced launch.
+//   checked plain -- the same launch without the programmatic attribute: under a profiler (rec_no_coop), or when a
+//                    cooperative cluster launch fails for another reason than the grid's size.
+// A plain launch is only as safe as the occupancy check: two persistent grids launched at the same time from two
+// streams could each get part of the device and spin on their barriers until the bounded waits give up and fail the
+// zrb context (rec_common.cuh: RecWatch).
+int rec_launch(const RecPlan& p, void** args, bool trace, cudaStream_t s, const char* name) {
+    if (p.cluster == 1) {
+        ZRB_CUDA(cudaLaunchCooperativeKernel(p.kernel, dim3(p.nCTA), dim3(kRecThreads), args, (size_t)p.smem, s));
+        count_launch();
+        return ZRB_OK;
+    }
+    int dev = 0;
+    cudaGetDevice(&dev);
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(p.nCTA);
+    cfg.blockDim = dim3(kRecThreads);
+    cfg.dynamicSmemBytes = (size_t)p.smem;
+    cfg.stream = s;
+    cudaLaunchAttribute attrs[2];
+    attrs[0].id = cudaLaunchAttributeClusterDimension;
+    attrs[0].val.clusterDim.x = p.cluster; attrs[0].val.clusterDim.y = 1; attrs[0].val.clusterDim.z = 1;
+    cfg.attrs = attrs;
+    const bool programmatic = rec_launch_programmatic(dev) && !trace;
+    const bool plain = programmatic || rec_no_coop();
+    cudaError_t e = cudaSuccess;
+    if (!plain) {
+        attrs[1].id = cudaLaunchAttributeCooperative;
+        attrs[1].val.cooperative = 1;
+        cfg.numAttrs = 2;
+        e = cudaLaunchKernelExC(&cfg, p.kernel, args);
+        if (e == cudaErrorCooperativeLaunchTooLarge) {
+            (void)cudaGetLastError();
+            set_error("%s: the %d-CTA grid cannot be co-resident on this device", name, p.nCTA);
+            return ZRB_E_CUDA;
+        }
+        if (e != cudaSuccess) (void)cudaGetLastError();   // e.g. not supported under a tool: try the checked plain launch
+    }
+    if (plain || e != cudaSuccess) {
+        if (p.max_clusters * p.cluster < p.nCTA) {
+            set_error("%s: %d clusters of %d needed, the device can hold %d at once", name, p.nCTA / p.cluster, p.cluster,
+                      p.max_clusters);
+            return ZRB_E_CUDA;
+        }
+        cfg.numAttrs = 1;
+        if (programmatic) {
+            attrs[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+            attrs[1].val.programmaticStreamSerializationAllowed = 1;
+            cfg.numAttrs = 2;
+        }
+        e = cudaLaunchKernelExC(&cfg, p.kernel, args);
+    }
+    if (e != cudaSuccess) {
+        set_error("%s launch failed: %s", name, cudaGetErrorString(e));
+        return ZRB_E_CUDA;
+    }
+    count_launch();
+    return ZRB_OK;
+}
+
 int rec_fwd_plan(int H, int B, RecPlan* plan) {
+    // [KS == 2]; naming <false> first keeps the order of the two kernels in the cubin
+    const void* const kernel[2] = {(const void*)lstm_rec_fwd_kernel<false>, (const void*)lstm_rec_fwd_kernel<true>};
     int nsm = tc_num_sms();
     plan->GB = (B + 7) / 8;
     plan->ok = 0;
@@ -356,8 +453,8 @@ int rec_fwd_plan(int H, int B, RecPlan* plan) {
                 // two M = 64 tiles read 16 row groups per K chunk: the last chunk reaches (16-G)*128 B past the slice, into the h buffer
                 if (smem <= 227 * 1024 && 2 * 4 * U * (GBi * 8 + 4) <= 2 * 64 * (GBi * 8 + 1)) {
                     plan->KS = 2; plan->U = U; plan->G = G; plan->nCTA = 2 * npair; plan->smem = (int)smem;
-                    plan->Kc = Kc; plan->KcS = KcS; plan->GBi = GBi; plan->ok = 1;
-                    return ZRB_OK;
+                    plan->Kc = Kc; plan->KcS = KcS; plan->GBi = GBi;
+                    return rec_plan_finish(plan, kernel[1], 2);
                 }
             }
     }
@@ -373,8 +470,8 @@ int rec_fwd_plan(int H, int B, RecPlan* plan) {
         // the M=64 wgmma reads 8 row groups per K chunk: the last chunk reaches (8-G)*128 B past the
         // slice, which lands in the h image buffer that follows it
         if (smem <= 227 * 1024 && U * B <= kRecMaxCell * kRecEpiThreads) {
-            plan->U = U; plan->G = G; plan->nCTA = n; plan->smem = (int)smem; plan->ok = 1;
-            return ZRB_OK;
+            plan->U = U; plan->G = G; plan->nCTA = n; plan->smem = (int)smem;
+            return rec_plan_finish(plan, kernel[0], 1);
         }
     }
     return ZRB_OK;
@@ -390,15 +487,6 @@ int lstm_rec_fwd(const RecPlan& p, const RecWatchdog& wd, const __half* w_img, c
                  const float* c0, float* cst, float* h_last, float* c_last, __half* hprev_h, __half* y_h,
                  unsigned int* counter, unsigned int counter_base, int T, int B, int H, int Hp, MaskSrc m, MaskSrc rm,
                  cudaStream_t s, long long* trace, float* h_f32) {
-    static bool attr[64] = {};   // per device: function attributes belong to the device's context
-    int dev = 0;
-    cudaGetDevice(&dev);
-    dev &= 63;
-    if (!attr[dev]) {
-        ZRB_CUDA(cudaFuncSetAttribute(lstm_rec_fwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        ZRB_CUDA(cudaFuncSetAttribute(lstm_rec_fwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-        attr[dev] = true;
-    }
     RecFwdArgs a;
     a.w_img = w_img; a.h0_img = h0_img; a.h_img = h_img; a.base = counter_base; a.gates = gates; a.c0 = c0; a.cst = cst; a.h_last = h_last; a.c_last = c_last;
     a.hprev_h = hprev_h; a.y_h = y_h; a.counter = counter; a.h_f32 = h_f32;
@@ -409,64 +497,8 @@ int lstm_rec_fwd(const RecPlan& p, const RecWatchdog& wd, const __half* w_img, c
     a.w = rec_watch_args(wd);
     a.base += rec_fault_base("fwd");   // (tests only)
     if (trace) ZRB_CUDA(cudaMemsetAsync(trace + 4, 0x80, 2 * sizeof(long long), s));
-    if (p.KS == 1) {
-        void* args[] = {&a};
-        ZRB_CUDA(cudaLaunchCooperativeKernel((void*)lstm_rec_fwd_kernel<false>, dim3(p.nCTA), dim3(kRecThreads), args,
-                                             (size_t)p.smem, s));
-        count_launch();
-        return ZRB_OK;
-    }
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(p.nCTA);
-    cfg.blockDim = dim3(kRecThreads);
-    cfg.dynamicSmemBytes = (size_t)p.smem;
-    cfg.stream = s;
-    cudaLaunchAttribute attrs[2];
-    attrs[0].id = cudaLaunchAttributeClusterDimension;
-    attrs[0].val.clusterDim.x = 2; attrs[0].val.clusterDim.y = 1; attrs[0].val.clusterDim.z = 1;
-    cfg.attrs = attrs;
-    cudaError_t e = cudaSuccess;
-    // cooperative, or plain + programmatic behind the input GEMM: tc_common.cuh, rec_launch_programmatic()
-    const bool programmatic = rec_launch_programmatic(dev) && !trace;
-    const bool plain = programmatic || rec_no_coop();
-    if (!plain) {
-        attrs[1].id = cudaLaunchAttributeCooperative;
-        attrs[1].val.cooperative = 1;
-        cfg.numAttrs = 2;
-        e = cudaLaunchKernelEx(&cfg, lstm_rec_fwd_kernel<true>, a);
-        if (e == cudaErrorCooperativeLaunchTooLarge) {
-            (void)cudaGetLastError();
-            set_error("lstm_rec_fwd: the %d-CTA grid cannot be co-resident on this device", p.nCTA);
-            return ZRB_E_CUDA;
-        }
-        if (e != cudaSuccess) (void)cudaGetLastError();
-    }
-    if (plain || e != cudaSuccess) {
-        cfg.numAttrs = 1;
-        static int seen_dev = -1, seen_smem = -1, seen_max = 0;   // the query is a host call: once per (device, footprint)
-        if (seen_dev != dev || seen_smem != p.smem) {
-            int max_clusters = 0;
-            cudaError_t oe = cudaOccupancyMaxActiveClusters(&max_clusters, lstm_rec_fwd_kernel<true>, &cfg);
-            if (oe != cudaSuccess) { (void)cudaGetLastError(); max_clusters = 0; }
-            seen_dev = dev; seen_smem = p.smem; seen_max = max_clusters;
-        }
-        if (seen_max * 2 < p.nCTA) {
-            set_error("lstm_rec_fwd: %d CTA pairs needed, the device can hold %d at once", p.nCTA / 2, seen_max);
-            return ZRB_E_CUDA;
-        }
-        if (programmatic) {
-            attrs[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-            attrs[1].val.programmaticStreamSerializationAllowed = 1;
-            cfg.numAttrs = 2;
-        }
-        e = cudaLaunchKernelEx(&cfg, lstm_rec_fwd_kernel<true>, a);
-    }
-    if (e != cudaSuccess) {
-        set_error("lstm_rec_fwd launch failed: %s", cudaGetErrorString(e));
-        return ZRB_E_CUDA;
-    }
-    count_launch();
-    return ZRB_OK;
+    void* args[] = {&a};
+    return rec_launch(p, args, trace != nullptr, s, "lstm_rec_fwd");
 }
 
 }  // namespace zrb

@@ -12,16 +12,9 @@
 #include "common.cuh"
 
 namespace zrb {
-// host: how the persistent recurrence kernels are launched.
-//   cooperative  -- the driver guarantees that the whole grid is co-resident (the grid barrier needs it) or refuses;
-//   programmatic -- a plain cluster launch, checked against cudaOccupancyMaxActiveClusters, with the programmatic-
-//                   serialization attribute: the GEMM enqueued before it triggers at its start, so the recurrence CTAs
-//                   take SMs as the GEMM's CTAs retire and fetch their resident weight slices while its tail is still
-//                   running (pdl_wait in the kernels).  9 us per train step at the Large config; the cooperative
-//                   attribute suppresses the early start (measured: no gain with both attributes).
-// A plain launch is only as safe as the occupancy check: two persistent grids launched at the same time from two
-// streams could each get part of the device and spin on their barriers (until the bounded waits give up and fail the zrb context).  So the default
-// is programmatic only while ONE tensor-core context is alive on the device -- a process that holds several (an ensemble,
+// host: whether rec_launch (lstm_rec_fwd.cu, where the launch modes of the persistent recurrence kernels are described)
+// launches a cluster grid programmatically.  A plain launch is only as safe as its occupancy check, so the default is
+// programmatic only while ONE tensor-core context is alive on the device -- a process that holds several (an ensemble,
 // two trainers) gets the cooperative launch.  ZRB_REC_PDL=0 forces cooperative, =1 forces programmatic.
 static inline int rec_pdl_env() {
     static const int mode = [] { const char* e = getenv("ZRB_REC_PDL"); return e ? (atoi(e) != 0 ? 1 : 0) : -1; }();

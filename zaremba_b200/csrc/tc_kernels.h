@@ -33,8 +33,19 @@ struct RecPlan {
     int KS;      // K-split: CTAs that share one set of output rows, each holding 1/KS of the contraction (clusters)
     int KcS;     // K chunks per CTA (Kc / KS)
     int GBi;     // 8-row batch groups of the operand images (GB, or padded so that the MMA's N is a multiple of 16)
+    const void* kernel;   // the instantiation launched: lstm_rec_fwd_kernel<KS == 2> / lstm_rec_bwd_kernel<KS>
+    int cluster;          // CTAs per thread-block cluster: 1 (unsplit forward), 2, 4 or 8
+    int max_clusters;     // cudaOccupancyMaxActiveClusters at this cluster size and smem (0: the query failed)
 };
 size_t rec_smem_bytes(int Kc, int G, int GB);
+// cudaOccupancyMaxActiveClusters of `kernel` on a grid of nCTA in clusters of `cluster`, after raising its dynamic
+// shared-memory limit; 0 if either call fails, with the error cleared
+int rec_max_clusters(const void* kernel, int cluster, int smem, int nCTA);
+// the plan fits: record the kernel it launches, its cluster size and occupancy answer, and set ok
+int rec_plan_finish(RecPlan* plan, const void* kernel, int cluster);
+// launch the plan's kernel with args = {&RecFwdArgs} or {&RecBwdArgs}; the launch modes are described at the definition
+// (lstm_rec_fwd.cu).  trace: the launch records a trace (never programmatic); name: for error messages
+int rec_launch(const RecPlan& p, void** args, bool trace, cudaStream_t s, const char* name);
 // Where a persistent kernel that gave up on a wait (rec_common.cuh: RecWatch) reports it: `flag` is the device word the
 // spinning threads poll, `host` a mapped host word the host reads without synchronising.  Owned by the context.
 struct RecWatchdog {
@@ -45,7 +56,7 @@ int rec_fwd_plan(int H, int B, RecPlan* plan);
 int pack_whh_fwd(const float* W, __half* img, int H, const RecPlan& p, cudaStream_t s);
 // h0_img: the B operand of step 0 (image of the state entering the window, built by fwd_prep); h_img slot t+1 is
 // written by step t.  The grid-barrier counter is never reset between launches: `counter_base` is its value when
-// the launch starts (the caller adds T * nCTA per launch).
+// the launch starts (engine_tc.cu: GridBarrier).
 int lstm_rec_fwd(const RecPlan& p, const RecWatchdog& wd, const __half* w_img, const __half* h0_img, __half* h_img, float* gates,
                  const float* c0, float* cst, float* h_last, float* c_last, __half* hprev_h, __half* y_h,
                  unsigned int* counter, unsigned int counter_base, int T, int B, int H, int Hp, MaskSrc m, MaskSrc rm,
