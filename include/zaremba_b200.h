@@ -120,6 +120,15 @@ int  zrb_set_explicit_masks(zrb_ctx* ctx, const uint8_t* const* site_masks);
  * set (and zrb_set_explicit_masks with non-NULL masks returns ZRB_E_STATE while the mode is on).  A change of the mode
  * invalidates the saved forward: zrb_backward / zrb_train_step_layer then need a new forward first. */
 int  zrb_set_variational_dropout(zrb_ctx* ctx, int32_t on, float p_rec);
+/* Weight-dropped LSTM (Merity, Keskar & Socher, "Regularizing and Optimizing LSTM Language Models", ICLR 2018;
+ * DESIGN.md section 15 states it bit for bit): DropConnect on the hidden-to-hidden matrices.  Opt-in; p = 0 (the
+ * default) changes nothing.  In a train-mode call with step s, layer l uses W_eff = fp32(W_hh * m_l * scale) in place of
+ * W_hh at every time step and batch row, scale = float32(1 / (1 - p)), m_l = zrb_dropout_mask(seed, s, 2L + 1 + l,
+ * 4H*H, p) with element r*H + k = W_hh[r, k].  The gradient is dW_hh = fp32(scale * m_l * dW_eff) (0 where the mask
+ * drops); the clip norm is taken over it.  `seed` holds no rank: every data-parallel rank draws the same mask.  Eval mode
+ * and zrb_lstm_layer_fwd / _bwd use the raw W_hh.  ZRB_E_INVALID for p outside [0, 1) or not finite.  A change of the
+ * mode invalidates the saved forward, as zrb_set_variational_dropout does. */
+int  zrb_set_weight_drop(zrb_ctx* ctx, float p, uint64_t seed);
 
 /* Model.forward (model.py:103-110): embedding gather, dropout, L x (LSTM layer,
  * dropout), vocabulary projection.

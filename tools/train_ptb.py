@@ -54,6 +54,8 @@ ap.add_argument("--recurrent_dropout", type=float, default=None,
                 help="p of the recurrent masks with --variational (default: --dropout)")
 ap.add_argument("--tied", action="store_true",
                 help="tie the embedding and softmax weights (Press & Wolf 2017): fc.W is embed.W")
+ap.add_argument("--weight_drop", type=float, default=0.0,
+                help="weight-dropped LSTM (Merity et al. 2018): DropConnect with this p on the hidden-to-hidden matrices")
 ap.add_argument("--lazy_update", action="store_true",
                 help="Trainer(lazy_update=True): upper-layer / fc weight updates run beside the next step's forward")
 ap.add_argument("--eval_batch_size", type=int, default=None,
@@ -98,7 +100,7 @@ torch.manual_seed(args.seed)
 if args.impl == "ours":
     model = zaremba_b200.Model(vocab, args.hidden_size, args.layer_num, args.dropout, args.winit,
                                variational=args.variational, recurrent_dropout=args.recurrent_dropout,
-                               tied=args.tied).to(dev)
+                               tied=args.tied, weight_drop=args.weight_drop).to(dev)
     tr = zaremba_b200.Trainer(model, B, T, lazy_update=args.lazy_update)
     # the corpus is staged on the device once (SURVEY 8f#2): 3 x [n_batches, T, B] int64
     trn_x = torch.stack([x for x, _ in trn_b]).contiguous().to(dev)
@@ -127,6 +129,8 @@ else:
         raise SystemExit("--variational is a mode of --impl ours")
     if args.tied:
         raise SystemExit("--tied is a mode of --impl ours (the reference's cudnn path keeps embed.W and fc.W apart)")
+    if args.weight_drop:
+        raise SystemExit("--weight_drop is a mode of --impl ours")
     from oracle import torch_port as P
     model = P.TorchLstmLm(vocab, args.hidden_size, args.layer_num, args.dropout, args.winit).to(dev)
     trn_d = [(x.to(dev), y.to(dev)) for x, y in trn_b]

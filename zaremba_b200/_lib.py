@@ -57,6 +57,7 @@ _SIGNATURES = {
     "zrb_dropout_mask": (C.c_int, [C.c_uint64, C.c_uint64, C.c_int32, C.c_int64, C.c_float, _vp, _vp]),
     "zrb_set_explicit_masks": (C.c_int, [_vp, C.POINTER(_vp)]),
     "zrb_set_variational_dropout": (C.c_int, [_vp, C.c_int32, C.c_float]),
+    "zrb_set_weight_drop": (C.c_int, [_vp, C.c_float, C.c_uint64]),
     "zrb_forward": (C.c_int, [_vp, C.POINTER(ZrbParams), _vp, C.c_int32, C.c_int32, C.POINTER(ZrbStates),
                               C.POINTER(ZrbStates), _vp, C.c_int32, C.c_uint64, C.c_uint64, _vp]),
     "zrb_backward": (C.c_int, [_vp, C.POINTER(ZrbParams), _vp, C.POINTER(ZrbParams), _vp]),

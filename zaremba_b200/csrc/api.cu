@@ -80,6 +80,10 @@ MaskSrc rec_mask(const zrb_ctx* c, int layer) {
     return make_mask_src(nullptr, c->seed, c->step, c->cfg.layers + 1 + layer, c->p_rec, c->train && c->variational);
 }
 
+MaskSrc wd_mask(const zrb_ctx* c, int layer) {
+    return make_mask_src(nullptr, c->wd_seed, c->step, 2 * c->cfg.layers + 1 + layer, c->p_wd, c->train);
+}
+
 static cudaEvent_t prof_event(zrb_ctx* c) {
     if (!c->prof_pool.empty()) {
         cudaEvent_t e = c->prof_pool.back();
@@ -254,6 +258,22 @@ int zrb_set_variational_dropout(zrb_ctx* c, int32_t on, float p_rec) {
     }
     c->variational = on != 0;
     c->p_rec = p_rec;
+    return ZRB_OK;
+}
+
+int zrb_set_weight_drop(zrb_ctx* c, float p, uint64_t seed) {
+    ZRB_REQUIRE(c, "null ctx");
+    ZRB_REQUIRE(isfinite(p) && p >= 0.f && p < 1.f, "weight-drop p %f outside [0,1)", p);
+    if (p > 0.f && c->cfg.engine == ZRB_ENGINE_SIMT && !c->whh_wd[0]) {
+        const size_t n = (size_t)4 * c->cfg.hidden * c->cfg.hidden;
+        for (int l = 0; l < c->cfg.layers; ++l) ZRB_TRY(dalloc(c, &c->whh_wd[l], n));
+    }
+    if (p != c->p_wd || seed != c->wd_seed) {
+        c->have_fwd = false;        // a backward must not regenerate another mask than its forward used
+        c->bwd_next_layer = -1;
+    }
+    c->p_wd = p;
+    c->wd_seed = seed;
     return ZRB_OK;
 }
 

@@ -107,8 +107,8 @@ __host__ inline MaskSrc make_mask_src(const uint8_t* explicit_mask, uint64_t see
 //   key     = (seed lo32, seed hi32 XOR pos hi32)
 //   counter = (j / 4, b, 0xFFFFFFFF, pos lo32); entry j reads word r[j % 4]
 //   u       = ((r >> 9) + 0.5) * 2^-23: exact in float32, strictly inside (0, 1)
-// Counter word 2 of a dropout mask is its site (<= 2 * ZRB_MAX_LAYERS with the recurrent sites of the variational
-// mode), never 0xFFFFFFFF: the two streams cannot meet.
+// Counter word 2 of a dropout mask is its site (<= 3 * ZRB_MAX_LAYERS = 24 with the recurrent sites of the variational
+// mode and the weight-drop sites), never 0xFFFFFFFF: the two streams cannot meet.
 struct SampleSrc {
     uint32_t k0, k1, c3;
 };
@@ -158,6 +158,20 @@ __device__ inline float mask_mul1_at(const MaskSrc& m, uint64_t e, uint64_t n_to
     if (!m.active) return 1.f;
     uint32_t bits = mask_keep4(m, e >> 2, n_total);
     return ((bits >> (e & 3)) & 1u) ? m.scale : 0.f;
+}
+
+// multipliers (0 or scale; 1 when inactive) of the four consecutive stream elements e0 .. e0+3, for any e0: one Philox
+// call per quad they touch (two when e0 % 4 != 0).  Philox masks only (the weight-drop sites have no explicit masks).
+__device__ inline void mask_mul4_at(const MaskSrc& m, uint64_t e0, float out[4]) {
+    if (!m.active) {
+        out[0] = out[1] = out[2] = out[3] = 1.f;
+        return;
+    }
+    const uint32_t sh = (uint32_t)(e0 & 3);
+    uint32_t bits = mask_keep4(m, e0 >> 2, ~0ull) >> sh;
+    if (sh) bits |= mask_keep4(m, (e0 >> 2) + 1, ~0ull) << (4 - sh);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) out[i] = ((bits >> i) & 1u) ? m.scale : 0.f;
 }
 
 // multiplier (0 or scale) for a single element e

@@ -44,7 +44,11 @@ struct zrb_ctx {
     float p_rec = 0.f;
     float* hrec[ZRB_MAX_LAYERS] = {};      // validation engine, variational mode: [(T+1)*B, H] h_{t-1} * recurrent mask
                                            // (block 0: the state entering the window); allocated when first switched on
-    int64_t weights_version = 1;           // bumped whenever parameter values change
+    float p_wd = 0.f;                      // zrb_set_weight_drop: DropConnect on W_hh (DESIGN.md section 15)
+    uint64_t wd_seed = 0;
+    float* whh_wd[ZRB_MAX_LAYERS] = {};    // validation engine, weight drop: [4H, H] fp32(W_hh * mask * scale) of the
+                                           // last train-mode forward; allocated when first switched on
+    int64_t weights_version = 1;          // bumped whenever parameter values change
     float* bwd_dy = nullptr;               // phased backward: grad wrt the next layer's output / scratch
     float* bwd_dx = nullptr;
     int bwd_next_layer = -1;
@@ -91,6 +95,8 @@ namespace zrb {
 
 MaskSrc site_mask(const zrb_ctx* c, int site);   // dropout site 0..L (period B*H in the variational mode)
 MaskSrc rec_mask(const zrb_ctx* c, int layer);   // recurrent site L+1+layer of the variational mode (inactive otherwise)
+MaskSrc wd_mask(const zrb_ctx* c, int layer);    // weight-drop site 2L+1+layer over W_hh's 4H*H elements (inactive:
+                                                 // eval mode or p_wd = 0)
 
 // RAII bracket: records an event pair around the launches of one kernel class
 struct ProfScope {

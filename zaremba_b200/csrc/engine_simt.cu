@@ -27,16 +27,19 @@ int simt_forward(zrb_ctx* c, const zrb_params* p, const int64_t* x, const zrb_st
             ZRB_TRY(gemm_f32(c->act[l], p->w_ih[l], G, N, 4 * H, H, 0, 1, 1.f, 0.f, s));
             ZRB_TRY(add_bias2(G, p->b_ih[l], p->b_hh[l], N, 4 * H, s));
         }
-        MaskSrc m = site_mask(c, l + 1), rm = rec_mask(c, l);
+        MaskSrc m = site_mask(c, l + 1), rm = rec_mask(c, l), wm = wd_mask(c, l);
         ProfScope ps(c, ZRB_PROF_REC_FWD, s);
         // variational mode: the recurrent operand is hrec (block t = h_{t-1} * mask), also read by the dW_hh GEMM
         float* hrec = rm.active ? c->hrec[l] : nullptr;
         if (hrec) ZRB_TRY(dropout_copy(c->h0s[l], hrec, (int64_t)B * H, rm, s));
+        // weight drop: the recurrent matrix is whh_wd = fp32(W_hh * mask * scale), also read by the backward
+        const float* w_hh = wm.active ? c->whh_wd[l] : p->w_hh[l];
+        if (wm.active) ZRB_TRY(weight_drop(p->w_hh[l], c->whh_wd[l], (int64_t)4 * H * H, wm, nullptr, s));
         for (int t = 0; t < T; ++t) {
             const float* h_prev = hrec ? hrec + (size_t)t * B * H : t ? c->hraw[l] + (size_t)(t - 1) * B * H : c->h0s[l];
             const float* c_prev = t ? c->cst[l] + (size_t)(t - 1) * B * H : c->c0s[l];
             float* Gt = G + (size_t)t * B * 4 * H;
-            ZRB_TRY(gemm_f32(h_prev, p->w_hh[l], Gt, B, 4 * H, H, 0, 1, 1.f, 1.f, s));
+            ZRB_TRY(gemm_f32(h_prev, w_hh, Gt, B, 4 * H, H, 0, 1, 1.f, 1.f, s));
             ZRB_TRY(lstm_cell_fwd(Gt, c_prev, c->cst[l] + (size_t)t * B * H, c->hraw[l] + (size_t)t * B * H,
                                   c->act[l + 1] + (size_t)t * B * H, hrec ? hrec + (size_t)(t + 1) * B * H : nullptr, B, H,
                                   (int64_t)t * B * H, (int64_t)N * H, m, rm, s));
@@ -66,7 +69,8 @@ int simt_backward(zrb_ctx* c, const zrb_params* p, const float* dscores, const z
         ZRB_TRY(colsum(dscores, g->fc_b, nullptr, N, V, s));
     }
     for (int l = L - 1; l >= 0; --l) {
-        MaskSrc m = site_mask(c, l + 1), rm = rec_mask(c, l);
+        MaskSrc m = site_mask(c, l + 1), rm = rec_mask(c, l), wm = wd_mask(c, l);
+        const float* w_hh = wm.active ? c->whh_wd[l] : p->w_hh[l];
         ZRB_CUDA(cudaMemsetAsync(c->dc, 0, bh * sizeof(float), s));
         {
         ProfScope ps(c, ZRB_PROF_REC_BWD, s);
@@ -76,7 +80,7 @@ int simt_backward(zrb_ctx* c, const zrb_params* p, const float* dscores, const z
             ZRB_TRY(lstm_cell_bwd(dY + (size_t)t * bh, t == T - 1 ? nullptr : c->dh_rec, c->dc,
                                   c->gates[l] + (size_t)t * B * 4 * H, c->cst[l] + (size_t)t * bh, c_prev, dGt, B, H,
                                   (int64_t)t * bh, (int64_t)N * H, m, rm, s));
-            if (t > 0) ZRB_TRY(gemm_f32(dGt, p->w_hh[l], c->dh_rec, B, H, 4 * H, 0, 0, 1.f, 0.f, s));
+            if (t > 0) ZRB_TRY(gemm_f32(dGt, w_hh, c->dh_rec, B, H, 4 * H, 0, 0, 1.f, 0.f, s));
         }
         }
         {
@@ -94,6 +98,7 @@ int simt_backward(zrb_ctx* c, const zrb_params* p, const float* dscores, const z
         }
         if (T > 1 && !rm.active)
             ZRB_TRY(gemm_f32(c->dG + (size_t)B * 4 * H, c->hraw[l], g->w_hh[l], 4 * H, H, N - B, 1, 0, 1.f, 1.f, s));
+        if (wm.active) ZRB_TRY(weight_drop(g->w_hh[l], g->w_hh[l], (int64_t)4 * H * H, wm, nullptr, s));   // scale * m * dW_eff
         ZRB_TRY(colsum(c->dG, g->b_ih[l], g->b_hh[l], N, 4 * H, s));
         float* tmp = dY; dY = dX; dX = tmp;
     }

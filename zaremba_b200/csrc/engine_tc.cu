@@ -78,6 +78,15 @@ struct zrb_tc_state {
     bool wg_ok = false;
     int wg_slots = 0;
     const float* wg_key = nullptr;
+    // which weights the W_hh images of each layer (w_img_f / w_img_b, or w_hh_h on the per-timestep path) hold
+    // (DESIGN.md section 15): the raw W_hh, W_hh under the weight-drop mask of (seed, step, p), or nothing usable (the
+    // update of the weight-drop mode, or the unit-level calls, left them behind p)
+    enum WhhKind { kWhhRaw = 0, kWhhMasked, kWhhStale };
+    struct WhhImage {
+        WhhKind kind = kWhhRaw;
+        uint64_t seed = 0, step = 0;
+        float p = 0.f;
+    } whh_img[ZRB_MAX_LAYERS];
 };
 
 namespace zrb {
@@ -173,6 +182,35 @@ void tc_ctx_free(zrb_ctx* c) {
     c->tc = nullptr;
 }
 
+// the W_hh images layer l's call needs: raw outside the weight-drop mode and in eval mode, else masked with this step's
+// mask (DESIGN.md section 15)
+static zrb_tc_state::WhhImage whh_wanted(const zrb_ctx* c, int l) {
+    zrb_tc_state::WhhImage w;
+    if (wd_mask(c, l).active) {
+        w.kind = zrb_tc_state::kWhhMasked;
+        w.seed = c->wd_seed; w.step = c->step; w.p = c->p_wd;
+    }
+    return w;
+}
+static bool whh_current(const zrb_ctx* c, int l) {
+    const zrb_tc_state::WhhImage &have = c->tc->whh_img[l], want = whh_wanted(c, l);
+    if (have.kind != want.kind) return false;
+    return want.kind == zrb_tc_state::kWhhRaw || (have.seed == want.seed && have.step == want.step && have.p == want.p);
+}
+
+// build layer l's W_hh images from W with the mask the call needs; row_image: also the row image w_hh_h when the
+// persistent kernels do not need it (it is read only on the per-timestep path)
+static int tc_pack_whh(zrb_ctx* c, const float* W, int l, bool row_image, cudaStream_t s) {
+    zrb_tc_state* t = c->tc;
+    const int H = c->cfg.hidden;
+    const MaskSrc m = wd_mask(c, l);
+    if (row_image || !t->bplan.ok) ZRB_TRY(convert_pad_f16(W, H, t->w_hh_h[l], t->Hp, 4 * H, H, 1.f, s, m));
+    if (t->fplan.ok) ZRB_TRY(pack_whh_fwd(W, t->w_img_f[l], H, t->fplan, s, m));
+    if (t->bplan.ok) ZRB_TRY(pack_whh_bwd(W, t->w_img_b[l], H, t->bplan, s, m));
+    t->whh_img[l] = whh_wanted(c, l);
+    return ZRB_OK;
+}
+
 // rebuild the fp16 weight images when parameter values changed (main.py:116-117 / zrb_clip_sgd)
 static int tc_pack_weights(zrb_ctx* c, const zrb_params* p, cudaStream_t s) {
     zrb_tc_state* t = c->tc;
@@ -181,14 +219,29 @@ static int tc_pack_weights(zrb_ctx* c, const zrb_params* p, cudaStream_t s) {
     const int H = c->cfg.hidden, L = c->cfg.layers, V = c->cfg.vocab;
     for (int l = 0; l < L; ++l) {
         ZRB_TRY(convert_pad_f16(p->w_ih[l], H, t->w_ih_h[l], t->Hp, 4 * H, H, 1.f, s));
-        ZRB_TRY(convert_pad_f16(p->w_hh[l], H, t->w_hh_h[l], t->Hp, 4 * H, H, 1.f, s));
-        if (t->fplan.ok) ZRB_TRY(pack_whh_fwd(p->w_hh[l], t->w_img_f[l], H, t->fplan, s));
-        if (t->bplan.ok) ZRB_TRY(pack_whh_bwd(p->w_hh[l], t->w_img_b[l], H, t->bplan, s));
+        ZRB_TRY(tc_pack_whh(c, p->w_hh[l], l, true, s));
     }
     ZRB_TRY(convert_pad_f16(p->fc_w, H, t->fc_w_h, t->Hp, V, H, 1.f, s));
     t->packed_version = c->weights_version;
     t->packed_params = *p;
     return ZRB_OK;
+}
+
+// the SGD update of layer l's W_hh.  Outside the weight-drop mode it rebuilds the layer's fp16 images from registers (the
+// next forward needs no pack); in it, it updates p (and g) only, and the next forward packs the images with its own mask.
+static int tc_update_whh(zrb_ctx* c, int l, float* p, float* g, float lr, bool pdl, cudaStream_t s) {
+    zrb_tc_state* t = c->tc;
+    const int H = c->cfg.hidden;
+    if (c->p_wd > 0.f) {
+        t->whh_img[l].kind = zrb_tc_state::kWhhStale;
+        return update_pack(p, g, 4 * H, H, lr, c->scalars, nullptr, t->Hp, nullptr, &t->fplan, nullptr, &t->bplan,
+                           c->keep_clipped, s, pdl);
+    }
+    const bool persistent = t->fplan.ok && t->bplan.ok;
+    t->whh_img[l] = zrb_tc_state::WhhImage{};
+    return update_pack(p, g, 4 * H, H, lr, c->scalars, persistent ? nullptr : t->w_hh_h[l], t->Hp,
+                       t->fplan.ok ? t->w_img_f[l] : nullptr, &t->fplan, t->bplan.ok ? t->w_img_b[l] : nullptr, &t->bplan,
+                       c->keep_clipped, s, pdl);
 }
 
 // apply deferred update item `item` (see zrb_tc_state::upd_pending); pdl: as a programmatic dependent of the forward
@@ -199,14 +252,11 @@ static int tc_issue_update(zrb_ctx* c, int item, bool pdl, cudaStream_t s) {
     if (!(t->upd_pending & (1u << item))) return ZRB_OK;
     t->upd_pending &= ~(1u << item);
     const TensorList& tl = t->upd_tl;
-    const bool persistent = t->fplan.ok && t->bplan.ok;
     if (item < L) {
         const int l = item, b = 1 + 4 * l;
         ZRB_TRY(update_pack(tl.p[b], tl.g[b], 4 * H, H, t->upd_lr, c->scalars, t->w_ih_h[l], t->Hp, nullptr, nullptr,
                             nullptr, nullptr, c->keep_clipped, s, pdl));
-        return update_pack(tl.p[b + 1], tl.g[b + 1], 4 * H, H, t->upd_lr, c->scalars, persistent ? nullptr : t->w_hh_h[l],
-                           t->Hp, t->fplan.ok ? t->w_img_f[l] : nullptr, &t->fplan,
-                           t->bplan.ok ? t->w_img_b[l] : nullptr, &t->bplan, c->keep_clipped, s, pdl);
+        return tc_update_whh(c, l, tl.p[b + 1], tl.g[b + 1], t->upd_lr, pdl, s);
     }
     const int f = 1 + 4 * L;
     return update_pack(tl.p[f], tl.g[f], V, H, t->upd_lr, c->scalars, t->fc_w_h, t->Hp, nullptr, nullptr, nullptr,
@@ -252,6 +302,13 @@ int tc_forward(zrb_ctx* c, const zrb_params* p, const int64_t* x, const zrb_stat
     }
     for (int l = 0; l < L; ++l) {
         float* G = c->gates[l];
+        if (!whh_current(c, l)) {
+            // weight drop (DESIGN.md section 15): this step's masked images, or the raw ones after a masked step.  After
+            // the layer's deferred update (enqueued beside the previous recurrence), before its input GEMM: never between
+            // that GEMM and its programmatic-dependent recurrence
+            ProfScope ps(c, ZRB_PROF_PACK, s);
+            ZRB_TRY(tc_pack_whh(c, p->w_hh[l], l, false, s));
+        }
         {
             ProfScope ps(c, ZRB_PROF_GEMM_IN, s);
             ZRB_TRY(gemm_f16_tc(t->x_h[l], Hp, 0, t->w_ih_h[l], Hp, 0, G, 4 * H, N, 4 * H, H, 1.f, p->b_ih[l], 0, s, nullptr,
@@ -293,11 +350,10 @@ int tc_forward(zrb_ctx* c, const zrb_params* p, const int64_t* x, const zrb_stat
 
 const __half* tc_last_layer_image(const zrb_ctx* c) { return c->tc->x_h[c->cfg.layers]; }
 
-// next block of sum-of-squares slots for an [M,N] weight gradient, or null when the step does not fuse the norm
-static float* wgrad_sumsq(zrb_ctx* c, int M, int N, int K) {
+// next block of n sum-of-squares slots, or null when the step does not fuse the norm
+static float* wgrad_slots(zrb_ctx* c, int n) {
     zrb_tc_state* t = c->tc;
     if (!t->wg_ok) return nullptr;
-    const int n = gemm_f16_tc_sumsq_slots(M, N, K);
     if (t->wg_slots + n > kNormGemm) {
         t->wg_ok = false;   // does not fit: the update takes the norm over the whole buffers instead
         return nullptr;
@@ -306,6 +362,8 @@ static float* wgrad_sumsq(zrb_ctx* c, int M, int N, int K) {
     t->wg_slots += n;
     return out;
 }
+// ... for an [M,N] weight gradient written by gemm_f16_tc
+static float* wgrad_sumsq(zrb_ctx* c, int M, int N, int K) { return wgrad_slots(c, gemm_f16_tc_sumsq_slots(M, N, K)); }
 
 // backward from the scaled fp16 image dS_h already in place
 // projection backward: afterwards fc.W / fc.b gradients are complete and c->bwd_dy holds d loss / d act[L]
@@ -337,13 +395,18 @@ static int tc_backward_head(zrb_ctx* c, const zrb_params* p, const zrb_params* g
 }
 
 // the two weight gradients of layer l from dG (scaled fp16, [N,G4p]): ONE launch, dG is the shared A operand
+// Weight drop (DESIGN.md section 15): the GEMM leaves dW_eff in g->w_hh[l]; the masking pass that follows it in stream
+// order makes it scale * m * dW_eff in place and writes its sums of squares into the norm slots instead of the GEMM.
 static int tc_layer_wgrads(zrb_ctx* c, const zrb_params* g, int l, const __half* dG_h, bool pdl, cudaStream_t s) {
     zrb_tc_state* t = c->tc;
     const int H = c->cfg.hidden, N = c->T * c->B;
+    const MaskSrc wm = wd_mask(c, l);
     float* ss1 = wgrad_sumsq(c, 4 * H, H, N);
-    float* ss2 = wgrad_sumsq(c, 4 * H, H, N);
-    return gemm_f16_tc(dG_h, t->G4p, 1, t->x_h[l], t->Hp, 1, g->w_ih[l], H, 4 * H, H, N, 1.f / kGradScale, nullptr, 0, s,
-                       ss1, nullptr, pdl, t->hprev_h[l], g->w_hh[l], ss2);
+    float* ss2 = wm.active ? nullptr : wgrad_sumsq(c, 4 * H, H, N);
+    ZRB_TRY(gemm_f16_tc(dG_h, t->G4p, 1, t->x_h[l], t->Hp, 1, g->w_ih[l], H, 4 * H, H, N, 1.f / kGradScale, nullptr, 0, s,
+                        ss1, nullptr, pdl, t->hprev_h[l], g->w_hh[l], ss2));
+    if (!wm.active) return ZRB_OK;
+    return weight_drop(g->w_hh[l], g->w_hh[l], (int64_t)4 * H * H, wm, wgrad_slots(c, kWeightDropBlocks), s);
 }
 
 // launch what tc_backward_head / the previous layer deferred, as a programmatic dependent of the recurrence kernel
@@ -554,6 +617,7 @@ int tc_layer_fwd(zrb_ctx* c, const float* w_ih, const float* w_hh, const float* 
     ZRB_TRY(tc_flush_updates(c, s));
     c->T = T; c->B = B; c->train = 0;
     t->packed_version = 0;                       // slot 0 is about to hold this call's weights
+    t->whh_img[0].kind = zrb_tc_state::kWhhStale;
     ZRB_TRY(convert_pad_f16(w_ih, H, t->w_ih_h[0], Hp, 4 * H, H, 1.f, s));
     ZRB_TRY(pack_whh_fwd(w_hh, t->w_img_f[0], H, t->fplan, s));
     ZRB_TRY(pack_whh_bwd(w_hh, t->w_img_b[0], H, t->bplan, s));
@@ -671,9 +735,7 @@ int tc_update(zrb_ctx* c, const zrb_params* p, const TensorList& tl, float lr, f
         }
         ZRB_TRY(update_pack(tl.p[b], tl.g[b], 4 * H, H, lr, c->scalars, t->w_ih_h[l], t->Hp, nullptr, nullptr, nullptr,
                             nullptr, c->keep_clipped, s));
-        ZRB_TRY(update_pack(tl.p[b + 1], tl.g[b + 1], 4 * H, H, lr, c->scalars, persistent ? nullptr : t->w_hh_h[l],
-                            t->Hp, t->fplan.ok ? t->w_img_f[l] : nullptr, &t->fplan,
-                            t->bplan.ok ? t->w_img_b[l] : nullptr, &t->bplan, c->keep_clipped, s));
+        ZRB_TRY(tc_update_whh(c, l, tl.p[b + 1], tl.g[b + 1], lr, false, s));
     }
     const int f = 1 + 4 * L;
     if (lazy) t->upd_pending |= 1u << L;
@@ -714,6 +776,7 @@ int tc_dyneval_update(zrb_ctx* c, const zrb_params* p, const TensorList& tl, flo
         ZRB_TRY(update_pack_dyn(tl.p[b + 1], tl.g[b + 1], tg[b + 1], r ? r[b + 1] : nullptr, 4 * H, H, a,
                                 persistent ? nullptr : t->w_hh_h[l], t->Hp, t->fplan.ok ? t->w_img_f[l] : nullptr,
                                 &t->fplan, t->bplan.ok ? t->w_img_b[l] : nullptr, &t->bplan, s));
+        t->whh_img[l] = zrb_tc_state::WhhImage{};   // the raw weights: evaluation applies no weight drop
         rest.n[b] = rest.n[b + 1] = 0;
     }
     const int f = 1 + 4 * L;

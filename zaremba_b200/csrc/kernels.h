@@ -25,6 +25,10 @@ int lstm_cell_bwd(const float* dy_post, const float* dh_rec, float* dc, const fl
                   MaskSrc rm, cudaStream_t s);
 // y[e] = x[e] * (mask multiplier of element e), e < n
 int dropout_copy(const float* x, float* y, int64_t n, MaskSrc m, cudaStream_t s);
+// weight drop (DESIGN.md section 15): y[e] = x[e] * (mask multiplier of element e), n % 4 == 0, x == y allowed (the
+// gradient pass).  sumsq (or null): kWeightDropBlocks partial sums of y^2 (fixed order; the clip norm's slots)
+constexpr int kWeightDropBlocks = 264;
+int weight_drop(const float* x, float* y, int64_t n, MaskSrc m, float* sumsq, cudaStream_t s);
 // C[n, j] += bias1[j] + bias2[j]
 int add_bias2(float* C, const float* b1, const float* b2, int N, int M, cudaStream_t s);
 int add_bias1(float* C, const float* b1, int N, int M, cudaStream_t s);

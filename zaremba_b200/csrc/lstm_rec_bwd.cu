@@ -403,8 +403,10 @@ __global__ void __launch_bounds__(kRecThreads, 1) lstm_rec_bwd_kernel(RecBwdArgs
 // w_img[cluster][rank][kcl][g][rr][e] = half(W_hh[gate*H + (khalf*KcS + kcl)*8 + e, cluster*UC + g*8 + rr]) with
 // rank = gate*S + khalf: one warp per (cluster, rank, kcl) reads 8 rows x UC contiguous floats and writes one contiguous
 // 16*UC-byte block.
+// m active (weight drop): W[r, j] * the multiplier of element r*H + j, four consecutive u per lane (one Philox call per
+// quad of mask elements; rows8 is a multiple of 8, so a quad of u never changes e)
 __global__ void pack_whh_bwd_kernel(const float* __restrict__ W, __half* __restrict__ img, int H, int UC, int G, int KcS,
-                                    int S, int nCluster) {
+                                    int S, int nCluster, MaskSrc m) {
     __shared__ __half tile[8][8 * 128];
     const int warp_in_block = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int CS = 4 * S;
@@ -416,11 +418,26 @@ __global__ void pack_whh_bwd_kernel(const float* __restrict__ W, __half* __restr
         const int gate = r / S, khalf = r % S;
         __half* t = tile[warp_in_block];
         const int rows8 = G * 8;
-        for (int idx = lane; idx < 8 * rows8; idx += 32) {
-            int e = idx / rows8, u = idx % rows8;            // u fastest: contiguous global reads
-            int k = (khalf * KcS + kcl) * 8 + e, j = cl * UC + u;
-            float v = (k < H && u < UC && j < H) ? W[((size_t)gate * H + k) * H + j] : 0.f;
-            t[u * 8 + e] = __float2half_rn(v);
+        if (m.active) {
+            for (int idx = lane * 4; idx < 8 * rows8; idx += 128) {
+                const int e = idx / rows8, u0 = idx % rows8;
+                const int k = (khalf * KcS + kcl) * 8 + e, j0 = cl * UC + u0;
+                const size_t row = (size_t)gate * H + k;
+                float mul[4] = {0.f, 0.f, 0.f, 0.f};
+                if (k < H && u0 < UC && j0 < H) mask_mul4_at(m, row * H + j0, mul);
+#pragma unroll
+                for (int q = 0; q < 4; ++q) {
+                    const int u = u0 + q, j = j0 + q;
+                    t[u * 8 + e] = __float2half_rn((k < H && u < UC && j < H) ? W[row * H + j] * mul[q] : 0.f);
+                }
+            }
+        } else {
+            for (int idx = lane; idx < 8 * rows8; idx += 32) {
+                int e = idx / rows8, u = idx % rows8;            // u fastest: contiguous global reads
+                int k = (khalf * KcS + kcl) * 8 + e, j = cl * UC + u;
+                float v = (k < H && u < UC && j < H) ? W[((size_t)gate * H + k) * H + j] : 0.f;
+                t[u * 8 + e] = __float2half_rn(v);
+            }
         }
         __syncwarp();
         __half* dst = img + (((size_t)cl * CS + r) * KcS + kcl) * ((size_t)G * 64);
@@ -478,9 +495,9 @@ int rec_bwd_plan(int H, int B, RecPlan* plan) {
     return ZRB_OK;
 }
 
-int pack_whh_bwd(const float* W, __half* img, int H, const RecPlan& p, cudaStream_t s) {
+int pack_whh_bwd(const float* W, __half* img, int H, const RecPlan& p, cudaStream_t s, MaskSrc m) {
     const int CS = 4 * p.KS;
-    pack_whh_bwd_kernel<<<tc_num_sms() * 4, 256, 0, s>>>(W, img, H, CS * p.U, p.G, p.KcS, p.KS, p.nCTA / CS);
+    pack_whh_bwd_kernel<<<tc_num_sms() * 4, 256, 0, s>>>(W, img, H, CS * p.U, p.G, p.KcS, p.KS, p.nCTA / CS, m);
     ZRB_KERNEL_CHECK();
     return ZRB_OK;
 }

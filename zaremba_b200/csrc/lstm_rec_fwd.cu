@@ -301,10 +301,32 @@ __global__ void __launch_bounds__(kRecThreads, 1) lstm_rec_fwd_kernel(RecFwdArgs
 // ---- weight / state image builders ---------------------------------------------------------------
 // w_img[cta][kcl][g][r][e] = half(W_hh[q*H + j, k]) with cta = cluster * KS + rank, row i = g*8 + r = 4*uc + q,
 // uc = unit within the cluster (UC = KS * U units), j = cluster*UC + uc, k = (rank*KcS + kcl)*8 + e
+// m active (weight drop): W[r, k] * the multiplier of element r*H + k; a thread then writes 4 consecutive e (one quad of
+// k), so that each quad of mask elements costs one Philox call
 __global__ void pack_whh_fwd_kernel(const float* __restrict__ W, __half* __restrict__ img, int H, int UC, int G, int KcS,
-                                    int KS, int nCTA) {
+                                    int KS, int nCTA, MaskSrc m) {
     const size_t per_cta = (size_t)KcS * G * 64;
     const size_t total = per_cta * nCTA;
+    if (m.active) {
+        for (size_t idx = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) * 4; idx < total;
+             idx += (size_t)gridDim.x * blockDim.x * 4) {
+            int cta = (int)(idx / per_cta);
+            size_t r0 = idx % per_cta;
+            int e0 = (int)(r0 & 7), r = (int)((r0 >> 3) & 7);
+            int g = (int)((r0 >> 6) % G), kcl = (int)((r0 >> 6) / G);
+            int i = g * 8 + r, uc = i >> 2, q = i & 3;
+            int cluster = cta / KS, rank = cta % KS;
+            int j = cluster * UC + uc, k0 = (rank * KcS + kcl) * 8 + e0;
+            const bool row_ok = uc < UC && j < H;
+            const size_t row = (size_t)q * H + j;
+            float mul[4] = {0.f, 0.f, 0.f, 0.f};
+            if (row_ok && k0 < H) mask_mul4_at(m, row * H + k0, mul);
+#pragma unroll
+            for (int t = 0; t < 4; ++t)
+                img[idx + t] = __float2half_rn(row_ok && k0 + t < H ? W[row * H + k0 + t] * mul[t] : 0.f);
+        }
+        return;
+    }
     for (size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
          idx += (size_t)gridDim.x * blockDim.x) {
         int cta = (int)(idx / per_cta);
@@ -477,8 +499,8 @@ int rec_fwd_plan(int H, int B, RecPlan* plan) {
     return ZRB_OK;
 }
 
-int pack_whh_fwd(const float* W, __half* img, int H, const RecPlan& p, cudaStream_t s) {
-    pack_whh_fwd_kernel<<<tc_num_sms() * 4, 256, 0, s>>>(W, img, H, p.KS * p.U, p.G, p.KcS, p.KS, p.nCTA);
+int pack_whh_fwd(const float* W, __half* img, int H, const RecPlan& p, cudaStream_t s, MaskSrc m) {
+    pack_whh_fwd_kernel<<<tc_num_sms() * 4, 256, 0, s>>>(W, img, H, p.KS * p.U, p.G, p.KcS, p.KS, p.nCTA, m);
     ZRB_KERNEL_CHECK();
     return ZRB_OK;
 }

@@ -4,11 +4,27 @@
 
 namespace zrb {
 
-// dst[r, 0..cols) = half(scale * src[r, 0..cols)), dst pitch ld_dst (>= cols), pad columns zeroed
+// dst[r, 0..cols) = half(scale * src[r, 0..cols)), dst pitch ld_dst (>= cols), pad columns zeroed.
+// m active (weight drop, DESIGN.md section 15): dst[r, c] = half(scale * fp32(src[r, c] * mul(r*ld_src + c))), four
+// consecutive columns per thread so that each quad of mask elements costs one Philox call (ld_dst % 4 == 0)
 __global__ void convert_pad_kernel(const float* __restrict__ src, int64_t ld_src, __half* __restrict__ dst,
-                                   int64_t ld_dst, int rows, int cols, float scale) {
+                                   int64_t ld_dst, int rows, int cols, float scale, MaskSrc m) {
     int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     int64_t total = (int64_t)rows * ld_dst;
+    if (m.active) {
+        for (i *= 4; i < total; i += (int64_t)gridDim.x * blockDim.x * 4) {
+            const int r = (int)(i / ld_dst), c0 = (int)(i % ld_dst);
+            float mul[4];
+            mask_mul4_at(m, (uint64_t)r * ld_src + c0, mul);
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+                float v = c0 + k < cols ? src[(int64_t)r * ld_src + c0 + k] * mul[k] * scale : 0.f;
+                v = fminf(fmaxf(v, -65504.f), 65504.f);
+                dst[i + k] = __float2half_rn(v);
+            }
+        }
+        return;
+    }
     for (; i < total; i += (int64_t)gridDim.x * blockDim.x) {
         int r = (int)(i / ld_dst), c = (int)(i % ld_dst);
         float v = c < cols ? src[(int64_t)r * ld_src + c] * scale : 0.f;
@@ -18,12 +34,13 @@ __global__ void convert_pad_kernel(const float* __restrict__ src, int64_t ld_src
 }
 
 int convert_pad_f16(const float* src, int64_t ld_src, __half* dst, int64_t ld_dst, int rows, int cols, float scale,
-                    cudaStream_t s) {
+                    cudaStream_t s, MaskSrc m) {
     int64_t total = (int64_t)rows * ld_dst;
     if (!total) return ZRB_OK;
+    ZRB_REQUIRE(!m.active || (ld_dst % 4 == 0 && !m.explicit_mask), "masked convert_pad_f16 needs ld_dst %% 4 == 0");
     int blocks = (int)((total + 255) / 256);
     if (blocks > 132 * 16) blocks = 132 * 16;
-    convert_pad_kernel<<<blocks, 256, 0, s>>>(src, ld_src, dst, ld_dst, rows, cols, scale);
+    convert_pad_kernel<<<blocks, 256, 0, s>>>(src, ld_src, dst, ld_dst, rows, cols, scale, m);
     ZRB_KERNEL_CHECK();
     return ZRB_OK;
 }

@@ -173,6 +173,50 @@ int dropout_copy(const float* x, float* y, int64_t n, MaskSrc m, cudaStream_t s)
     return ZRB_OK;
 }
 
+// Weight drop (DESIGN.md section 15): y[e] = x[e] * mul(e) over n4 quads, one Philox call per quad; x may be y (the
+// gradient pass, in place).  sumsq (or null): block b writes the sum of y^2 over its grid-stride share to sumsq[b], a
+// fixed summation order, so the clip norm does not re-read the gradient.
+__global__ void __launch_bounds__(256) weight_drop_kernel(const float* x, float* y, int64_t n4, MaskSrc m,
+                                                          float* __restrict__ sumsq) {
+    __shared__ float sh[8];
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    const bool vec = ((((uintptr_t)x) | ((uintptr_t)y)) & 15) == 0;
+    float acc = 0.f;
+    for (int64_t q = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; q < n4; q += stride) {
+        float mul[4];
+        mask_mul4_at(m, (uint64_t)q * 4, mul);
+        float4 v;
+        if (vec) {
+            v = reinterpret_cast<const float4*>(x)[q];
+        } else {
+            v.x = x[4 * q]; v.y = x[4 * q + 1]; v.z = x[4 * q + 2]; v.w = x[4 * q + 3];
+        }
+        v.x *= mul[0]; v.y *= mul[1]; v.z *= mul[2]; v.w *= mul[3];
+        if (vec) {
+            reinterpret_cast<float4*>(y)[q] = v;
+        } else {
+            y[4 * q] = v.x; y[4 * q + 1] = v.y; y[4 * q + 2] = v.z; y[4 * q + 3] = v.w;
+        }
+        acc += v.x * v.x + v.y * v.y + v.z * v.z + v.w * v.w;
+    }
+    if (!sumsq) return;
+    acc = warp_sum(acc);
+    if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = acc;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        float t = 0.f;
+#pragma unroll
+        for (int w = 0; w < 8; ++w) t += sh[w];
+        sumsq[blockIdx.x] = t;
+    }
+}
+int weight_drop(const float* x, float* y, int64_t n, MaskSrc m, float* sumsq, cudaStream_t s) {
+    ZRB_REQUIRE(n % 4 == 0 && !m.explicit_mask, "weight_drop: n=%lld must be a multiple of 4", (long long)n);
+    weight_drop_kernel<<<kWeightDropBlocks, 256, 0, s>>>(x, y, n / 4, m, sumsq);
+    ZRB_KERNEL_CHECK();
+    return ZRB_OK;
+}
+
 // ----------------------------------------------------------------------------------------
 __global__ void add_bias_kernel(float* __restrict__ C, const float* __restrict__ b1, const float* __restrict__ b2,
                                 int64_t total, int M) {

@@ -7,8 +7,9 @@ namespace zrb {
 
 constexpr float kGradScale = 1024.f;   // fp16 gradient images hold kGradScale * value (exact power of two)
 
+// m (weight drop, DESIGN.md section 15; inactive by default): src element r*ld_src + c times its multiplier first
 int convert_pad_f16(const float* src, int64_t ld_src, __half* dst, int64_t ld_dst, int rows, int cols, float scale,
-                    cudaStream_t s);
+                    cudaStream_t s, MaskSrc m = MaskSrc{});
 int colsum_h_scratch_floats(int M);
 int colsum_h(const __half* A, int64_t ld, float* out, float* out2, int N, int M, float inv_scale, float* scratch,
              cudaStream_t s);
@@ -53,7 +54,8 @@ struct RecWatchdog {
     unsigned int* host = nullptr;
 };
 int rec_fwd_plan(int H, int B, RecPlan* plan);
-int pack_whh_fwd(const float* W, __half* img, int H, const RecPlan& p, cudaStream_t s);
+// m (weight drop, DESIGN.md section 15; inactive by default): the image of fp32(W[r, k] * multiplier of r*H + k)
+int pack_whh_fwd(const float* W, __half* img, int H, const RecPlan& p, cudaStream_t s, MaskSrc m = MaskSrc{});
 // h0_img: the B operand of step 0 (image of the state entering the window, built by fwd_prep); h_img slot t+1 is
 // written by step t.  The grid-barrier counter is never reset between launches: `counter_base` is its value when
 // the launch starts (engine_tc.cu: GridBarrier).
@@ -91,7 +93,7 @@ int update_pack_dyn(float* p, float* g, const float* tg, const float* r, int row
                     __half* row_img, int64_t ld, __half* fwd_img, const RecPlan* fp, __half* bwd_img, const RecPlan* bp,
                     cudaStream_t s);
 int rec_bwd_plan(int H, int B, RecPlan* plan);   // U = units per CTA, nCTA = 4 * clusters
-int pack_whh_bwd(const float* W, __half* img, int H, const RecPlan& p, cudaStream_t s);
+int pack_whh_bwd(const float* W, __half* img, int H, const RecPlan& p, cudaStream_t s, MaskSrc m = MaskSrc{});
 int lstm_rec_bwd(const RecPlan& p, const RecWatchdog& wd, const __half* w_img, __half* g_img, const float* dy, const float* gates,
                  const float* cst, const float* c0, __half* dG_h, unsigned int* counter, unsigned int counter_base, int T,
                  int B, int H, int G4p, MaskSrc m, MaskSrc rm, cudaStream_t s, long long* trace = nullptr, float* db1 = nullptr,

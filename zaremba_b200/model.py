@@ -132,13 +132,24 @@ class Model(nn.Module):
     drawn where the untied model draws `fc.W`.  `state_dict()` carries both keys (torch's rule for a shared parameter),
     so a tied checkpoint also loads into an untied model; loading one whose `embed.W` and `fc.W` differ into a tied
     model raises ValueError.
+
+    Extra keyword `weight_drop`: the weight-dropped LSTM (Merity et al. 2018; DESIGN.md section 15), DropConnect with
+    this p on every layer's hidden-to-hidden matrix.  In train mode each forward draws one mask per layer and uses
+    W_hh * mask / (1 - p) at every time step; the gradient reaching `weight_hh_l0` is masked alike.  Eval mode uses the
+    raw W_hh.  The masks are seeded by `torch.initial_seed()` when the library context is created (no rank in it: every
+    data-parallel rank draws the same mask).  Not with lstm_type "custom".
     """
 
     def __init__(self, vocab_size, hidden_size, layer_num, dropout, winit, lstm_type="pytorch", engine="tc",
-                 variational=False, recurrent_dropout=None, *, tied=False):
+                 variational=False, recurrent_dropout=None, *, tied=False, weight_drop=0.0):
         super().__init__()
         if lstm_type not in ("pytorch", "custom"):
             raise ValueError(f"lstm_type must be 'pytorch' or 'custom', got {lstm_type!r}")
+        if isinstance(weight_drop, bool) or not isinstance(weight_drop, (int, float)) or \
+                not 0.0 <= float(weight_drop) < 1.0:
+            raise ValueError(f"weight_drop must be a number in [0, 1), got {weight_drop!r}")
+        if weight_drop and lstm_type == "custom":
+            raise ValueError("weight_drop applies to lstm_type 'pytorch' only")
         if variational not in (False, True):
             raise ValueError(f"variational must be True or False, got {variational!r}")
         if not isinstance(tied, bool):
@@ -160,6 +171,7 @@ class Model(nn.Module):
         self.variational = bool(variational)
         self.p_rec = p_rec
         self.tied = tied
+        self.weight_drop = float(weight_drop)
         self.embed = Embed(vocab_size, hidden_size)
         self.rnns = nn.ModuleList(LSTM(hidden_size, hidden_size, lstm_type) for _ in range(layer_num))
         self.fc = Linear(hidden_size, vocab_size)
@@ -383,6 +395,8 @@ class Model(nn.Module):
         self._versions = None
         if self.variational:
             _lib.check(lib.zrb_set_variational_dropout(h, 1, self.p_rec))
+        if self.weight_drop:
+            _lib.check(lib.zrb_set_weight_drop(h, self.weight_drop, int(torch.initial_seed()) & 0xFFFFFFFFFFFFFFFF))
         if self._explicit_masks is not None:
             self._push_masks()
         return self._ctx
