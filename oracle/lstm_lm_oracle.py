@@ -222,10 +222,11 @@ def ensemble_nll_loss(scores_list, y):
 # ----------------------------------------------------------------------------
 # backward (what autograd derives for model.py:103-110; SURVEY.md section 8a)
 # ----------------------------------------------------------------------------
-def lstm_layer_bwd(dy, cache, x, W_ih, W_hh):
+def lstm_layer_bwd(dy, cache, x, W_ih, W_hh, record=None):
     """dy [T,B,H] upstream grad on the layer's outputs.  States entering the
     window are detached (model.py:100-101) so no grad flows past t=0.
-    Returns dx, dW_ih, dW_hh, db (db_ih == db_hh)."""
+    Returns dx, dW_ih, dW_hh, db (db_ih == db_hh).  `record` (a dict or None)
+    receives "dG": the gate gradients d loss / d preactivation [T,B,4H]."""
     T, B, H = dy.shape
     dt = dy.dtype
     dW_ih = np.zeros_like(W_ih)
@@ -234,6 +235,8 @@ def lstm_layer_bwd(dy, cache, x, W_ih, W_hh):
     dx = np.zeros_like(x)
     dh_rec = np.zeros((B, H), dtype=dt)
     dc = np.zeros((B, H), dtype=dt)
+    if record is not None:
+        record["dG"] = np.zeros((T, B, 4 * H), dtype=dt)
     for t in range(T - 1, -1, -1):
         h_prev, c_prev, i, f, g, o, c = cache[t]
         dh = dy[t] + dh_rec
@@ -245,6 +248,8 @@ def lstm_layer_bwd(dy, cache, x, W_ih, W_hh):
         df = dc * c_prev
         dG = np.concatenate([di * i * (1.0 - i), df * f * (1.0 - f),
                              dg * (1.0 - g * g), do * o * (1.0 - o)], axis=1)
+        if record is not None:
+            record["dG"][t] = dG
         dc = dc * f
         dx[t] = dG @ W_ih
         dh_rec = dG @ W_hh
@@ -254,8 +259,10 @@ def lstm_layer_bwd(dy, cache, x, W_ih, W_hh):
     return dx, dW_ih, dW_hh, db
 
 
-def model_bwd(params, cache, dscores, layer_num):
-    """Gradients of every parameter given d loss / d scores [T*B,V]."""
+def model_bwd(params, cache, dscores, layer_num, record=None):
+    """Gradients of every parameter given d loss / d scores [T*B,V].  `record`
+    (a dict or None) receives, per layer l, record[l] = {"dy": the gradient
+    reaching the layer's outputs [T,B,H], "dG": its gate gradients [T,B,4H]}."""
     p = cache["dropout"]
     masks = cache["masks"]
     fc_in = cache["fc_in"]
@@ -267,9 +274,12 @@ def model_bwd(params, cache, dscores, layer_num):
     da = (dscores @ params["fc.W"]).reshape(T, B, H)
     for l in range(layer_num - 1, -1, -1):
         da = apply_dropout(da, None if masks is None else masks[l + 1], p)
+        rec = None
+        if record is not None:
+            rec = record[l] = {"dy": da}
         dx, dWi, dWh, db = lstm_layer_bwd(
             da, cache["layer_cache"][l], cache["layer_in"][l],
-            params[f"rnns.{l}.weight_ih_l0"], params[f"rnns.{l}.weight_hh_l0"])
+            params[f"rnns.{l}.weight_ih_l0"], params[f"rnns.{l}.weight_hh_l0"], rec)
         grads[f"rnns.{l}.weight_ih_l0"] = dWi
         grads[f"rnns.{l}.weight_hh_l0"] = dWh
         grads[f"rnns.{l}.bias_ih_l0"] = db
