@@ -218,6 +218,27 @@ int  zrb_set_keep_clipped_grads(zrb_ctx* ctx, int32_t on);
 int  zrb_set_lazy_update(zrb_ctx* ctx, int32_t on);
 int  zrb_flush_updates(zrb_ctx* ctx, void* stream);
 
+/* Iterate averaging (NT-ASGD of Merity, Keskar & Socher 2018; DESIGN.md section 16 states it bit for bit).  Opt-in;
+ * off, nothing changes.  zrb_set_average(ctx, avg) with avg non-NULL starts averaging into the tensors of `avg` (laid
+ * out like the parameters; tied: avg->fc_w == avg->embed_w) with n = 0 and leaves their contents alone; NULL stops it.
+ * Every zrb_train_step_update (and zrb_train_step_host) while it is on sets n = n + 1, applies the SGD update exactly as
+ * without averaging, then for every element of every parameter: a = p' at n = 1, else a = a + (p' - a) * mu with
+ * mu = fp32(1 / n) and fp32 operations in that order (torch.optim.ASGD(lambd=0, t0=0) created at the start).  The
+ * average is dense under the rows-only embedding update too, and it is taken of the raw W_hh under weight drop.  The
+ * parameters are never changed by it.  zrb_clip_sgd, zrb_dyneval_step and every eval call leave n alone.  Pending lazy
+ * updates are applied first (on the legacy default stream), with the averaging of the steps they belong to.
+ * ZRB_E_INVALID for a NULL tensor, average tensors that overlap each other, an untied pair in a tied context, and while
+ * swapped; zrb_train_step_update returns ZRB_E_INVALID, before anything is launched, when an average tensor overlaps a
+ * parameter or gradient it was given. */
+int  zrb_set_average(zrb_ctx* ctx, const zrb_params* avg);
+/* n: the number of train-step updates averaged since zrb_set_average (0 while averaging is off). */
+int  zrb_average_count(const zrb_ctx* ctx, int64_t* n);
+/* Exchange the parameters p and the average bit for bit, and write the fp16 weight images of the values now in p in
+ * the same pass (the W_hh images hold the raw weights), so that eval calls need no pack.  The context records that it is
+ * swapped; a second call swaps back exactly.  While swapped every zrb_train_step_* call returns ZRB_E_INVALID (training
+ * the average and swapping back would corrupt both).  ZRB_E_INVALID when n = 0 and when an average tensor overlaps p. */
+int  zrb_swap_average(zrb_ctx* ctx, const zrb_params* p, void* stream);
+
 /* Watchdog of the persistent recurrence kernels.  Every wait inside them is bounded (~3 s; ZRB_SPIN_CYCLES overrides).  A
  * wait that runs out -- a lost wake-up, or a grid that never became co-resident -- does not trap: the kernel stops
  * waiting everywhere, finishes with garbage in its outputs and leaves a code in a host-mapped word.  The next call on

@@ -56,6 +56,14 @@ ap.add_argument("--tied", action="store_true",
                 help="tie the embedding and softmax weights (Press & Wolf 2017): fc.W is embed.W")
 ap.add_argument("--weight_drop", type=float, default=0.0,
                 help="weight-dropped LSTM (Merity et al. 2018): DropConnect with this p on the hidden-to-hidden matrices")
+ap.add_argument("--asgd", action="store_true",
+                help="NT-ASGD (Merity et al. 2018): start averaging the weights once validation stops improving "
+                     "(AWD-LSTM's non-monotone trigger); validate, test and save with the average from then on")
+ap.add_argument("--nonmono", type=int, default=5,
+                help="--asgd: trigger when more than this many validations exist and this one is worse than the best "
+                     "of all but the last NONMONO")
+ap.add_argument("--asgd_from", type=int, default=None,
+                help="start averaging at the start of this epoch (1-based), whatever validation does")
 ap.add_argument("--lazy_update", action="store_true",
                 help="Trainer(lazy_update=True): upper-layer / fc weight updates run beside the next step's forward")
 ap.add_argument("--eval_batch_size", type=int, default=None,
@@ -120,8 +128,17 @@ if args.impl == "ours":
         return tr.perplexity(batches)
 
     def state_dict():
+        if tr.averaged_steps:
+            return {k: v.cpu() for k, v in tr.average_state_dict().items()}
         tr.flush()
         return {k: v.detach().cpu() for k, v in model.state_dict().items()}
+
+    def averaged_perplexity(batches):
+        """perplexity with the averaged weights once averaging has run (AWD-LSTM validates and tests the average)"""
+        if not tr.averaged_steps:
+            return perplexity(batches)
+        with tr.averaged_weights():
+            return perplexity(batches)
 else:
     if world > 1:
         raise SystemExit("--impl cudnn is the reference's single-device path")
@@ -131,6 +148,8 @@ else:
         raise SystemExit("--tied is a mode of --impl ours (the reference's cudnn path keeps embed.W and fc.W apart)")
     if args.weight_drop:
         raise SystemExit("--weight_drop is a mode of --impl ours")
+    if args.asgd or args.asgd_from is not None:
+        raise SystemExit("--asgd / --asgd_from are modes of --impl ours")
     from oracle import torch_port as P
     model = P.TorchLstmLm(vocab, args.hidden_size, args.layer_num, args.dropout, args.winit).to(dev)
     trn_d = [(x.to(dev), y.to(dev)) for x, y in trn_b]
@@ -153,16 +172,24 @@ else:
                 losses.append(P.softmax_nll_times_batch(logits, y.to(dev)).item() / EB)
         return float(np.exp(np.mean(losses)))
 
+    averaged_perplexity = perplexity
+
     def state_dict():
         return {k: v.detach().cpu() for k, v in model.reference_state_dict().items()}
 
 lr, tic, words_seen = args.learning_rate, timeit.default_timer(), 0
 val_curve, epoch_secs = [], []
+asgd_epoch = None                                      # 1-based epoch at whose start averaging began
 n_epochs = args.total_epochs if args.epochs is None else min(args.epochs, args.total_epochs)
 for epoch in range(n_epochs):
     if epoch > args.factor_epoch:                      # main.py:105-106
         lr = lr / args.factor
     e_words = [0]
+    if args.asgd_from is not None and asgd_epoch is None and epoch + 1 >= args.asgd_from:
+        tr.start_averaging()
+        asgd_epoch = epoch + 1
+        if rank == 0:
+            print(f"averaging the weights from epoch {asgd_epoch} on (--asgd_from)", flush=True)
 
     def log(i, loss, norm, epoch=epoch):
         if loss != loss:                               # NaN: the run is dead, do not burn the remaining epochs
@@ -187,12 +214,19 @@ for epoch in range(n_epochs):
     torch.cuda.synchronize()
     epoch_secs.append(time.perf_counter() - t0)
     words_seen += len(trn_b) * T * B * world
-    val = perplexity(vld_b)
+    val = averaged_perplexity(vld_b)
+    # AWD-LSTM's non-monotone trigger: more than nonmono earlier validations, and this one worse than the best of all
+    # but the last nonmono of them.  Every rank computes the same validation, so every rank starts together.
+    if args.asgd and asgd_epoch is None and len(val_curve) > args.nonmono and val > min(val_curve[:-args.nonmono]):
+        tr.start_averaging()
+        asgd_epoch = epoch + 2
+        if rank == 0:
+            print(f"validation stopped improving: averaging the weights from epoch {asgd_epoch} on", flush=True)
     val_curve.append(val)
     if rank == 0:
         print("Epoch : {:d} || Validation set perplexity : {:.3f}".format(epoch + 1, val))
         print("*************************************************\n", flush=True)
-tst_ppl = perplexity(tst_b)
+tst_ppl = averaged_perplexity(tst_b)
 if rank == 0:
     print("Test set perplexity : {:.3f}".format(tst_ppl))
     print("Training is over.")
@@ -205,7 +239,8 @@ if rank == 0:
                "train_seconds_per_epoch_median": float(np.median(epoch_secs)),
                "train_tokens_per_s_median_epoch": steps * T * B * world / float(np.median(epoch_secs)),
                "total_wall_s": timeit.default_timer() - tic, "gpu": torch.cuda.get_device_name(0),
-               "data": os.path.basename(args.data or args.ids)}
+               "data": os.path.basename(args.data or args.ids),
+               "asgd_start_epoch": asgd_epoch, "averaged_steps": tr.averaged_steps if args.impl == "ours" else 0}
         os.makedirs(os.path.dirname(os.path.abspath(args.json)), exist_ok=True)
         json.dump(out, open(args.json, "w"), indent=1)
     if args.save:

@@ -103,6 +103,9 @@ _SIGNATURES = {
                                       C.c_uint64, C.c_float, C.c_float, _vp, _vp, _vp]),
     "zrb_set_lazy_update": (C.c_int, [_vp, C.c_int32]),
     "zrb_flush_updates": (C.c_int, [_vp, _vp]),
+    "zrb_set_average": (C.c_int, [_vp, C.POINTER(ZrbParams)]),
+    "zrb_average_count": (C.c_int, [_vp, C.POINTER(C.c_int64)]),
+    "zrb_swap_average": (C.c_int, [_vp, C.POINTER(ZrbParams), _vp]),
     "zrb_check_health": (C.c_int, [_vp]),
     "zrb_resident_flag": (C.c_int, [_vp, C.POINTER(_vp), C.POINTER(C.c_uint32)]),
     "zrb_stream_wait_value32": (C.c_int, [_vp, _vp, C.c_uint32]),

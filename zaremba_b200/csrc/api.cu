@@ -329,6 +329,79 @@ int zrb_clip_sgd(zrb_ctx* c, int32_t n, float* const* params, float* const* grad
     return ZRB_OK;
 }
 
+static TensorList param_list(const zrb_ctx* c, const zrb_params* p, const zrb_params* g);
+
+// ---- iterate averaging (DESIGN.md section 16) -----------------------------------------------------------------------
+static bool ranges_overlap(const float* a, int64_t na, const float* b, int64_t nb) {
+    if (na == 0 || nb == 0) return false;
+    const uintptr_t a0 = (uintptr_t)a, a1 = a0 + (uintptr_t)na * sizeof(float);
+    const uintptr_t b0 = (uintptr_t)b, b1 = b0 + (uintptr_t)nb * sizeof(float);
+    return a0 < b1 && b0 < a1;
+}
+
+// ZRB_E_INVALID when an average tensor overlaps a tensor of `tl` (its p, and its g when with_g)
+static int check_avg_alias(const TensorList& ta, const TensorList& tl, bool with_g) {
+    for (int i = 0; i < ta.count; ++i)
+        for (int j = 0; j < tl.count; ++j) {
+            const bool hit = ranges_overlap(ta.p[i], ta.n[i], tl.p[j], tl.n[j]) ||
+                             (with_g && ranges_overlap(ta.p[i], ta.n[i], tl.g[j], tl.n[j]));
+            ZRB_REQUIRE(!hit, "average tensor %d overlaps %s tensor %d", i, with_g ? "a parameter or gradient" : "parameter",
+                        j);
+        }
+    return ZRB_OK;
+}
+
+static int check_not_swapped(const zrb_ctx* c) {
+    ZRB_REQUIRE(!c->avg_swapped, "the parameters hold the average (zrb_swap_average): swap back before training");
+    return ZRB_OK;
+}
+
+int zrb_set_average(zrb_ctx* c, const zrb_params* avg) {
+    ZRB_REQUIRE(c, "null ctx");
+    ZRB_REQUIRE(!c->avg_swapped, "the parameters hold the average (zrb_swap_average): swap back first");
+    if (avg) {
+        ZRB_REQUIRE(avg->embed_w && avg->fc_w && avg->fc_b, "null average tensor");
+        for (int l = 0; l < c->cfg.layers; ++l)
+            ZRB_REQUIRE(avg->w_ih[l] && avg->w_hh[l] && avg->b_ih[l] && avg->b_hh[l], "null average tensor of layer %d", l);
+        ZRB_TRY(check_tied(c, avg));
+        const TensorList ta = param_list(c, avg, avg);
+        for (int i = 0; i < ta.count; ++i)
+            for (int j = i + 1; j < ta.count; ++j)
+                ZRB_REQUIRE(!ranges_overlap(ta.p[i], ta.n[i], ta.p[j], ta.n[j]), "average tensors %d and %d overlap", i, j);
+    }
+    // deferred updates belong to the steps before: they average (or not) with the n they were issued with
+    if (c->cfg.engine == ZRB_ENGINE_TC) ZRB_TRY(tc_flush_updates(c, nullptr));
+    c->avg_on = avg != nullptr;
+    if (avg) c->avg = *avg;
+    c->avg_n = 0;
+    return ZRB_OK;
+}
+
+int zrb_average_count(const zrb_ctx* c, int64_t* n) {
+    ZRB_REQUIRE(c && n, "null argument");
+    *n = c->avg_on ? c->avg_n : 0;
+    return ZRB_OK;
+}
+
+int zrb_swap_average(zrb_ctx* c, const zrb_params* p, void* stream) {
+    ZRB_REQUIRE(c && p, "null argument");
+    ZRB_TRY(watchdog_check(c));
+    ZRB_TRY(check_tied(c, p));
+    ZRB_REQUIRE(c->avg_on && c->avg_n > 0, "no average to swap in: no train step has been averaged since zrb_set_average");
+    const TensorList tl = param_list(c, p, p), ta = param_list(c, &c->avg, &c->avg);
+    ZRB_TRY(check_avg_alias(ta, tl, false));
+    cudaStream_t s = (cudaStream_t)stream;
+    if (c->cfg.engine == ZRB_ENGINE_TC) {
+        ZRB_TRY(tc_swap_average(c, p, tl, ta.p, s));
+    } else {
+        ProfScope ps(c, ZRB_PROF_PACK, s);
+        ZRB_TRY(swap_apply(tl, ta.p, s));
+        c->weights_version++;
+    }
+    c->avg_swapped = !c->avg_swapped;
+    return ZRB_OK;
+}
+
 static TensorList param_list(const zrb_ctx* c, const zrb_params* p, const zrb_params* g) {
     TensorList tl;
     const int64_t H = c->cfg.hidden, V = c->cfg.vocab;
@@ -352,6 +425,7 @@ int zrb_train_step_grads(zrb_ctx* c, const zrb_params* p, const zrb_params* g, c
                          uint64_t step, float* loss, void* stream) {
     ZRB_REQUIRE(c && p && g && x && y && in && out, "null argument");
     ZRB_REQUIRE(c->cfg.layers * 4 + 3 <= 16, "fused step supports at most 3 layers");
+    ZRB_TRY(check_not_swapped(c));
     cudaStream_t s = (cudaStream_t)stream;
     ZRB_TRY(check_shapes(c, T, B));
     ZRB_TRY(check_tied(c, p));
@@ -371,6 +445,7 @@ int zrb_train_step_begin(zrb_ctx* c, const zrb_params* p, const zrb_params* g, c
                          int32_t T, int32_t B, const zrb_states* in, const zrb_states* out, uint64_t seed,
                          uint64_t step, float* loss, void* stream) {
     ZRB_REQUIRE(c && p && g && x && y && in && out, "null argument");
+    ZRB_TRY(check_not_swapped(c));
     ZRB_TRY(check_shapes(c, T, B));
     ZRB_TRY(check_tied(c, p));
     ZRB_TRY(check_tied(c, g));
@@ -384,6 +459,7 @@ int zrb_train_step_begin(zrb_ctx* c, const zrb_params* p, const zrb_params* g, c
 int zrb_train_step_layer(zrb_ctx* c, const zrb_params* p, const zrb_params* g, int32_t layer, void* stream) {
     ZRB_REQUIRE(c && p && g, "null argument");
     ZRB_REQUIRE(layer >= 0 && layer < c->cfg.layers, "layer %d out of range", layer);
+    ZRB_TRY(check_not_swapped(c));
     ZRB_TRY(check_tied(c, p));
     ZRB_TRY(check_tied(c, g));
     if (c->cfg.engine == ZRB_ENGINE_TC) return tc_train_step_layer(c, p, g, layer, (cudaStream_t)stream);
@@ -467,13 +543,33 @@ int zrb_train_step_update(zrb_ctx* c, const zrb_params* p, const zrb_params* g, 
     ZRB_REQUIRE(c->cfg.layers * 4 + 3 <= 16, "fused step supports at most 3 layers");
     ZRB_TRY(check_tied(c, p));
     ZRB_TRY(check_tied(c, g));
+    ZRB_TRY(check_not_swapped(c));
     TensorList tl = param_list(c, p, g);
-    if (c->cfg.engine == ZRB_ENGINE_TC) return tc_update(c, p, tl, lr, max_norm, norm_out, (cudaStream_t)stream);
-    {
-        ProfScope ps(c, ZRB_PROF_CLIP_SGD, (cudaStream_t)stream);
-        ZRB_TRY(clip_sgd(tl, lr, max_norm, c->partials, c->scalars, norm_out, c->keep_clipped, (cudaStream_t)stream));
+    cudaStream_t s = (cudaStream_t)stream;
+    // iterate averaging: this update is number n = avg_n + 1, mu = fp32(1 / n) rounded once from double
+    AvgStep as{};
+    const AvgStep* avg = nullptr;
+    if (c->avg_on) {
+        const TensorList ta = param_list(c, &c->avg, &c->avg);
+        ZRB_TRY(check_avg_alias(ta, tl, true));
+        for (int i = 0; i < ta.count; ++i) as.a[i] = ta.p[i];
+        as.mu = (float)(1.0 / (double)(c->avg_n + 1));
+        as.first = c->avg_n == 0;
+        avg = &as;
     }
-    c->weights_version++;
+    if (c->cfg.engine == ZRB_ENGINE_TC) {
+        ZRB_TRY(tc_update(c, p, tl, lr, max_norm, norm_out, avg, s));
+    } else {
+        ProfScope ps(c, ZRB_PROF_CLIP_SGD, s);
+        if (avg) {
+            ZRB_TRY(grad_norm(tl, max_norm, c->partials, c->scalars, norm_out, s));
+            ZRB_TRY(sgd_avg_apply(tl, avg->a, lr, c->scalars, c->keep_clipped, avg->mu, avg->first, s));
+        } else {
+            ZRB_TRY(clip_sgd(tl, lr, max_norm, c->partials, c->scalars, norm_out, c->keep_clipped, s));
+        }
+        c->weights_version++;
+    }
+    if (avg) c->avg_n++;
     return ZRB_OK;
 }
 

@@ -49,6 +49,10 @@ struct zrb_ctx {
     float* whh_wd[ZRB_MAX_LAYERS] = {};    // validation engine, weight drop: [4H, H] fp32(W_hh * mask * scale) of the
                                            // last train-mode forward; allocated when first switched on
     int64_t weights_version = 1;          // bumped whenever parameter values change
+    bool avg_on = false;                   // zrb_set_average: iterate averaging into `avg` (DESIGN.md section 16)
+    zrb_params avg{};
+    int64_t avg_n = 0;                     // train-step updates averaged so far
+    bool avg_swapped = false;              // zrb_swap_average: the parameters hold the average
     float* bwd_dy = nullptr;               // phased backward: grad wrt the next layer's output / scratch
     float* bwd_dx = nullptr;
     int bwd_next_layer = -1;
@@ -132,7 +136,9 @@ int tc_layer_fwd(zrb_ctx* c, const float* w_ih, const float* w_hh, const float* 
 int tc_layer_bwd(zrb_ctx* c, const float* dy, float* dx, float* dw_ih, float* dw_hh, float* db_ih, float* db_hh,
                  cudaStream_t s);   // the persistent backward recurrence kernel is in use for this context
 int tc_update(zrb_ctx* c, const zrb_params* p, const TensorList& tl, float lr, float max_norm, float* norm_out,
-              cudaStream_t s);
+              const AvgStep* avg, cudaStream_t s);
+// iterate averaging (DESIGN.md section 16): exchange the tensors of tl (param_list() over p) with a, images rebuilt
+int tc_swap_average(zrb_ctx* c, const zrb_params* p, const TensorList& tl, float* const* a, cudaStream_t s);
 // dynamic evaluation (DESIGN.md section 14): eval-mode gradients, and the update with the dynamic rule
 int tc_eval_grads(zrb_ctx* c, const zrb_params* p, const zrb_params* g, const int64_t* x, const int64_t* y, int T, int B,
                   const zrb_states* in, const zrb_states* out, float* loss, cudaStream_t s);

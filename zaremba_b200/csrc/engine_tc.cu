@@ -58,6 +58,8 @@ struct zrb_tc_state {
     unsigned upd_pending = 0;
     float upd_lr = 0.f;
     zrb::TensorList upd_tl{};
+    bool upd_avg_on = false;      // ... and averaged with upd_avg, the average step of that train step (section 16)
+    zrb::AvgStep upd_avg{};
     bool in_train_step = false;   // tc_forward is running as the first half of a fused train step
     float* colsum_scratch = nullptr;   // row-split partials of the bias-gradient column sums
     int64_t packed_version = 0;
@@ -227,21 +229,34 @@ static int tc_pack_weights(zrb_ctx* c, const zrb_params* p, cudaStream_t s) {
     return ZRB_OK;
 }
 
+// the train step's update of one matrix: update_pack, or with iterate averaging on (avg non-null) update_pack_avg,
+// which also averages the new p into a (DESIGN.md section 16)
+static int tc_update_pack(zrb_ctx* c, const AvgStep* avg, float* a, float* p, float* g, int rows, int cols, float lr,
+                          __half* row_img, __half* fwd_img, const RecPlan* fp, __half* bwd_img, const RecPlan* bp,
+                          bool pdl, cudaStream_t s) {
+    const int64_t ld = c->tc->Hp;
+    if (!avg)
+        return update_pack(p, g, rows, cols, lr, c->scalars, row_img, ld, fwd_img, fp, bwd_img, bp, c->keep_clipped, s,
+                           pdl);
+    return update_pack_avg(p, g, a, avg->mu, avg->first, rows, cols, lr, c->scalars, row_img, ld, fwd_img, fp, bwd_img,
+                           bp, c->keep_clipped, s, pdl);
+}
+
 // the SGD update of layer l's W_hh.  Outside the weight-drop mode it rebuilds the layer's fp16 images from registers (the
 // next forward needs no pack); in it, it updates p (and g) only, and the next forward packs the images with its own mask.
-static int tc_update_whh(zrb_ctx* c, int l, float* p, float* g, float lr, bool pdl, cudaStream_t s) {
+static int tc_update_whh(zrb_ctx* c, int l, float* p, float* g, float lr, const AvgStep* avg, float* a, bool pdl,
+                         cudaStream_t s) {
     zrb_tc_state* t = c->tc;
     const int H = c->cfg.hidden;
     if (c->p_wd > 0.f) {
         t->whh_img[l].kind = zrb_tc_state::kWhhStale;
-        return update_pack(p, g, 4 * H, H, lr, c->scalars, nullptr, t->Hp, nullptr, &t->fplan, nullptr, &t->bplan,
-                           c->keep_clipped, s, pdl);
+        return tc_update_pack(c, avg, a, p, g, 4 * H, H, lr, nullptr, nullptr, &t->fplan, nullptr, &t->bplan, pdl, s);
     }
     const bool persistent = t->fplan.ok && t->bplan.ok;
     t->whh_img[l] = zrb_tc_state::WhhImage{};
-    return update_pack(p, g, 4 * H, H, lr, c->scalars, persistent ? nullptr : t->w_hh_h[l], t->Hp,
-                       t->fplan.ok ? t->w_img_f[l] : nullptr, &t->fplan, t->bplan.ok ? t->w_img_b[l] : nullptr, &t->bplan,
-                       c->keep_clipped, s, pdl);
+    return tc_update_pack(c, avg, a, p, g, 4 * H, H, lr, persistent ? nullptr : t->w_hh_h[l],
+                          t->fplan.ok ? t->w_img_f[l] : nullptr, &t->fplan, t->bplan.ok ? t->w_img_b[l] : nullptr,
+                          &t->bplan, pdl, s);
 }
 
 // apply deferred update item `item` (see zrb_tc_state::upd_pending); pdl: as a programmatic dependent of the forward
@@ -252,15 +267,17 @@ static int tc_issue_update(zrb_ctx* c, int item, bool pdl, cudaStream_t s) {
     if (!(t->upd_pending & (1u << item))) return ZRB_OK;
     t->upd_pending &= ~(1u << item);
     const TensorList& tl = t->upd_tl;
+    const AvgStep* avg = t->upd_avg_on ? &t->upd_avg : nullptr;
+    float* const* a = t->upd_avg.a;
     if (item < L) {
         const int l = item, b = 1 + 4 * l;
-        ZRB_TRY(update_pack(tl.p[b], tl.g[b], 4 * H, H, t->upd_lr, c->scalars, t->w_ih_h[l], t->Hp, nullptr, nullptr,
-                            nullptr, nullptr, c->keep_clipped, s, pdl));
-        return tc_update_whh(c, l, tl.p[b + 1], tl.g[b + 1], t->upd_lr, pdl, s);
+        ZRB_TRY(tc_update_pack(c, avg, a[b], tl.p[b], tl.g[b], 4 * H, H, t->upd_lr, t->w_ih_h[l], nullptr, nullptr,
+                               nullptr, nullptr, pdl, s));
+        return tc_update_whh(c, l, tl.p[b + 1], tl.g[b + 1], t->upd_lr, avg, a[b + 1], pdl, s);
     }
     const int f = 1 + 4 * L;
-    return update_pack(tl.p[f], tl.g[f], V, H, t->upd_lr, c->scalars, t->fc_w_h, t->Hp, nullptr, nullptr, nullptr,
-                       nullptr, c->keep_clipped, s, pdl);
+    return tc_update_pack(c, avg, a[f], tl.p[f], tl.g[f], V, H, t->upd_lr, t->fc_w_h, nullptr, nullptr, nullptr, nullptr,
+                          pdl, s);
 }
 
 int tc_flush_updates(zrb_ctx* c, cudaStream_t s) {
@@ -670,18 +687,24 @@ int tc_rec_trace(zrb_ctx* c, long long* h_out, int max_entries) {
 }
 
 // clip + SGD (main.py:114-117).  The update pass also writes the fp16 operand images of the new weights,
-// so the next forward needs no pack pass.
+// so the next forward needs no pack pass.  avg (or null): iterate averaging, every tensor's new value averaged into
+// avg->a[i] in the same passes (DESIGN.md section 16).
 int tc_update(zrb_ctx* c, const zrb_params* p, const TensorList& tl, float lr, float max_norm, float* norm_out,
-              cudaStream_t s) {
+              const AvgStep* avg, cudaStream_t s) {
     zrb_tc_state* t = c->tc;
     const int H = c->cfg.hidden, L = c->cfg.layers, V = c->cfg.vocab;
     ZRB_TRY(tc_flush_updates(c, s));   // (a second update without a forward in between)
     bool fuse = true;   // update_pack picks 16 / 8 / 4-byte accesses from the matrix width and alignment
     for (int i = 0; i < tl.count && fuse; ++i)
-        fuse = ((((uintptr_t)tl.p[i]) | ((uintptr_t)tl.g[i])) & 3) == 0;
+        fuse = ((((uintptr_t)tl.p[i]) | ((uintptr_t)tl.g[i]) | (avg ? (uintptr_t)avg->a[i] : 0)) & 3) == 0;
     ProfScope ps(c, ZRB_PROF_CLIP_SGD, s);
     if (!fuse) {
-        ZRB_TRY(clip_sgd(tl, lr, max_norm, c->partials, c->scalars, norm_out, c->keep_clipped, s));
+        if (avg) {
+            ZRB_TRY(grad_norm(tl, max_norm, c->partials, c->scalars, norm_out, s));
+            ZRB_TRY(sgd_avg_apply(tl, avg->a, lr, c->scalars, c->keep_clipped, avg->mu, avg->first, s));
+        } else {
+            ZRB_TRY(clip_sgd(tl, lr, max_norm, c->partials, c->scalars, norm_out, c->keep_clipped, s));
+        }
         c->weights_version++;
         return ZRB_OK;
     }
@@ -710,12 +733,22 @@ int tc_update(zrb_ctx* c, const zrb_params* p, const TensorList& tl, float lr, f
         ZRB_TRY(grad_norm(dense, max_norm, c->partials, c->scalars, norm_out, s, true, gemm_norm ? t->wg_slots : 0));
         ZRB_TRY(embed_rows_update(tl.p[0], tl.g[0], c->emb_prev_ids, c->emb_first, c->emb_prev_n, H, V, lr, c->scalars,
                                   c->keep_clipped, s));
+        if (avg) {   // the average is dense: every row moves toward the new embedding
+            TensorList e{};
+            e.p[0] = tl.p[0]; e.n[0] = tl.n[0]; e.count = 1;
+            ZRB_TRY(avg_apply(e, avg->a, avg->mu, avg->first, s));
+        }
     } else {
         ZRB_TRY(grad_norm(tl, max_norm, c->partials, c->scalars, norm_out, s));
     }
     TensorList rest;
     rest.count = 0;
-    auto push = [&](int i) { rest.p[rest.count] = tl.p[i]; rest.g[rest.count] = tl.g[i]; rest.n[rest.count] = tl.n[i]; rest.count++; };
+    float* rest_a[16] = {};   // the averages of rest's tensors
+    auto push = [&](int i) {
+        rest.p[rest.count] = tl.p[i]; rest.g[rest.count] = tl.g[i]; rest.n[rest.count] = tl.n[i];
+        rest_a[rest.count] = avg ? avg->a[i] : nullptr;
+        rest.count++;
+    };
     if (!rows_only) push(0);
     const bool persistent = t->fplan.ok && t->bplan.ok;
     // lazy update: layer 0 (needed by the very next kernels) now; layers >= 1 and fc.W beside the forward recurrences of
@@ -724,6 +757,8 @@ int tc_update(zrb_ctx* c, const zrb_params* p, const TensorList& tl, float lr, f
     if (lazy) {
         t->upd_tl = tl;
         t->upd_lr = lr;
+        t->upd_avg_on = avg != nullptr;
+        if (avg) t->upd_avg = *avg;
     }
     for (int l = 0; l < L; ++l) {
         const int b = 1 + 4 * l;
@@ -733,16 +768,19 @@ int tc_update(zrb_ctx* c, const zrb_params* p, const TensorList& tl, float lr, f
             t->upd_pending |= 1u << l;
             continue;
         }
-        ZRB_TRY(update_pack(tl.p[b], tl.g[b], 4 * H, H, lr, c->scalars, t->w_ih_h[l], t->Hp, nullptr, nullptr, nullptr,
-                            nullptr, c->keep_clipped, s));
-        ZRB_TRY(tc_update_whh(c, l, tl.p[b + 1], tl.g[b + 1], lr, false, s));
+        float* const a0 = avg ? avg->a[b] : nullptr;
+        float* const a1 = avg ? avg->a[b + 1] : nullptr;
+        ZRB_TRY(tc_update_pack(c, avg, a0, tl.p[b], tl.g[b], 4 * H, H, lr, t->w_ih_h[l], nullptr, nullptr, nullptr, nullptr,
+                               false, s));
+        ZRB_TRY(tc_update_whh(c, l, tl.p[b + 1], tl.g[b + 1], lr, avg, a1, false, s));
     }
     const int f = 1 + 4 * L;
     if (lazy) t->upd_pending |= 1u << L;
-    else ZRB_TRY(update_pack(tl.p[f], tl.g[f], V, H, lr, c->scalars, t->fc_w_h, t->Hp, nullptr, nullptr, nullptr, nullptr,
-                             c->keep_clipped, s));
+    else ZRB_TRY(tc_update_pack(c, avg, avg ? avg->a[f] : nullptr, tl.p[f], tl.g[f], V, H, lr, t->fc_w_h, nullptr, nullptr,
+                                nullptr, nullptr, false, s));
     push(f + 1);
-    ZRB_TRY(sgd_apply(rest, lr, c->scalars, c->keep_clipped, s));
+    if (avg) ZRB_TRY(sgd_avg_apply(rest, rest_a, lr, c->scalars, c->keep_clipped, avg->mu, avg->first, s));
+    else ZRB_TRY(sgd_apply(rest, lr, c->scalars, c->keep_clipped, s));
     t->wg_ok = false;
     c->weights_version++;
     t->packed_version = c->weights_version;      // images are current
@@ -784,6 +822,43 @@ int tc_dyneval_update(zrb_ctx* c, const zrb_params* p, const TensorList& tl, flo
                             nullptr, nullptr, s));
     rest.n[f] = 0;
     ZRB_TRY(dyneval_apply(rest, tg, r, a, s));
+    t->wg_ok = false;
+    c->weights_version++;
+    t->packed_version = c->weights_version;      // images are current
+    t->packed_params = *p;
+    return ZRB_OK;
+}
+
+// Exchange the weights with their average (DESIGN.md section 16), tl = param_list() over p, a = the averages in its
+// order.  The matrices go through update_pack's kernels, which write the fp16 images of the weights now in p; the rest
+// through the list kernel.  The W_hh images then hold the raw weights, as after the dynamic-evaluation update.
+int tc_swap_average(zrb_ctx* c, const zrb_params* p, const TensorList& tl, float* const* a, cudaStream_t s) {
+    zrb_tc_state* t = c->tc;
+    const int H = c->cfg.hidden, L = c->cfg.layers, V = c->cfg.vocab;
+    ZRB_TRY(tc_flush_updates(c, s));
+    ProfScope ps(c, ZRB_PROF_PACK, s);
+    bool fuse = true;
+    for (int i = 0; i < tl.count && fuse; ++i) fuse = ((((uintptr_t)tl.p[i]) | ((uintptr_t)a[i])) & 3) == 0;
+    if (!fuse) {   // images rebuilt by the next forward's pack
+        ZRB_TRY(swap_apply(tl, a, s));
+        c->weights_version++;
+        return ZRB_OK;
+    }
+    TensorList rest = tl;   // entries with an image get length 0 here (skipped by the list kernel)
+    const bool persistent = t->fplan.ok && t->bplan.ok;
+    for (int l = 0; l < L; ++l) {
+        const int b = 1 + 4 * l;
+        ZRB_TRY(swap_pack(tl.p[b], a[b], 4 * H, H, t->w_ih_h[l], t->Hp, nullptr, nullptr, nullptr, nullptr, s));
+        ZRB_TRY(swap_pack(tl.p[b + 1], a[b + 1], 4 * H, H, persistent ? nullptr : t->w_hh_h[l], t->Hp,
+                          t->fplan.ok ? t->w_img_f[l] : nullptr, &t->fplan, t->bplan.ok ? t->w_img_b[l] : nullptr,
+                          &t->bplan, s));
+        t->whh_img[l] = zrb_tc_state::WhhImage{};
+        rest.n[b] = rest.n[b + 1] = 0;
+    }
+    const int f = 1 + 4 * L;
+    ZRB_TRY(swap_pack(tl.p[f], a[f], V, H, t->fc_w_h, t->Hp, nullptr, nullptr, nullptr, nullptr, s));
+    rest.n[f] = 0;
+    ZRB_TRY(swap_apply(rest, a, s));
     t->wg_ok = false;
     c->weights_version++;
     t->packed_version = c->weights_version;      // images are current

@@ -80,6 +80,21 @@ int sq_accumulate(const TensorList& tl, cudaStream_t s);
 constexpr int kStatsPartials = 2048;
 int stats_finish(const TensorList& tl, int64_t windows, double* partials, float* rbar, cudaStream_t s);
 
+// ---- average_tc.cu: iterate averaging (DESIGN.md section 16) ------------------------------------------------------
+// The average of one train-step update: a[i] averages tl.p[i] (param_list() order); mu = fp32(1 / n), first: n = 1
+struct AvgStep {
+    float* a[16];
+    float mu;
+    bool first;
+};
+// sgd_apply's update, then a[i] = first ? p : a + (p - a) * mu over the new p (zero-length entries skipped)
+int sgd_avg_apply(const TensorList& tl, float* const* a, float lr, const float* scalars, bool write_g, float mu,
+                  bool first, cudaStream_t s);
+// the average alone over tl.p (tl.g unused): the embedding under the rows-only update
+int avg_apply(const TensorList& tl, float* const* a, float mu, bool first, cudaStream_t s);
+// exchange tl.p[i] and a[i] element by element
+int swap_apply(const TensorList& tl, float* const* a, cudaStream_t s);
+
 // ---- sample.cu ---------------------------------------------------------------------------
 // ZRB_E_INVALID for the arguments zrb_sample rejects (checked before anything is enqueued)
 int sample_check(const zrb_sampling* cfg, int B, int V);

@@ -9,6 +9,7 @@ identical to a single process at `--batch_size B * world_size`.
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 import math
 import os
@@ -324,6 +325,7 @@ class Trainer:
     def _train_step(self, x, y, lr, max_norm):
         lib = _lib.load()
         T, B = x.shape
+        self._check_not_swapped()
         self._check_versions()
         if self.world > 1 and self.transport == "ce":
             self._grads_ce(lib, x, y, T, B)
@@ -383,6 +385,7 @@ class Trainer:
         if T != self.T or B != self.B:
             hx = torch.empty(T, B, dtype=torch.int64).pin_memory(); hy = torch.empty_like(hx).pin_memory()
         hx.copy_(x); hy.copy_(y)
+        self._check_not_swapped()
         if self.world == 1:
             self._check_versions()
             with self._own_stream():
@@ -447,6 +450,72 @@ class Trainer:
             acc += loss.double() / x.shape[1]
             n += 1
         return math.exp(acc.item() / max(n, 1))
+
+    # ---- iterate averaging, NT-ASGD (DESIGN.md section 16) -----------------------------------------------------------
+    def _check_not_swapped(self):
+        if getattr(self, "_swapped", False):
+            raise RuntimeError("train_step inside averaged_weights(): the parameters hold the average")
+
+    def start_averaging(self):
+        """Average the weights over every following train step (zrb_set_average): after n steps `flat_avg` holds the
+        mean of the n weight vectors those steps produced, as torch.optim.ASGD(lambd=0, t0=0) created now would.  The
+        weights themselves train exactly as without averaging.  Calling it again restarts at n = 0.  Under data
+        parallelism every rank calls it at the same step (the ranks' averages stay identical; nothing is exchanged)."""
+        self._check_not_swapped()
+        if getattr(self, "flat_avg", None) is None:
+            self.flat_avg = torch.zeros_like(self.flat_p)
+        self._avg_s = self._flat_params_struct(self.flat_avg)
+        self.flush()
+        _lib.check(_lib.load().zrb_set_average(self.ctx, C.byref(self._avg_s)))
+
+    def stop_averaging(self):
+        """Stop averaging; `flat_avg` keeps the average so far."""
+        self._check_not_swapped()
+        self.flush()
+        _lib.check(_lib.load().zrb_set_average(self.ctx, None))
+
+    @property
+    def averaged_steps(self):
+        """n: the train steps averaged since start_averaging() (0 while averaging is off)."""
+        n = C.c_int64()
+        _lib.check(_lib.load().zrb_average_count(self.ctx, C.byref(n)))
+        return n.value
+
+    @contextlib.contextmanager
+    def averaged_weights(self):
+        """`with trainer.averaged_weights():` the parameters hold the average (zrb_swap_average exchanges them with
+        `flat_avg` and rebuilds the fp16 weight images in the same pass); perplexity, eval_step, generation, beam search,
+        the cache and dynamic evaluation see it.  On exit the weights are swapped back bit for bit.  train_step inside the
+        block raises RuntimeError."""
+        self._check_not_swapped()
+        lib = _lib.load()
+        self.flush()
+        self._check_versions()
+        _lib.check(lib.zrb_swap_average(self.ctx, C.byref(self._ps), self._stream()))
+        self._swapped = True
+        try:
+            yield self
+        finally:
+            self.flush()
+            self._check_versions()
+            _lib.check(lib.zrb_swap_average(self.ctx, C.byref(self._ps), self._stream()))
+            self._swapped = False
+
+    def average_state_dict(self):
+        """The average as a state dict under the model's own keys (tied: embed.W and fc.W both, as state_dict()
+        gives them): what AWD-LSTM saves as its final model.  Copies; pending updates are applied first."""
+        if getattr(self, "flat_avg", None) is None or self.averaged_steps == 0:
+            raise RuntimeError("no average: call start_averaging() and train at least one step")
+        self.flush()
+        base, n = self.flat_p.data_ptr(), self.flat_p.numel()
+        src = self.flat_p if getattr(self, "_swapped", False) else self.flat_avg
+        out = {}
+        for k, v in self.model.state_dict().items():
+            off = (v.data_ptr() - base) // 4
+            if v.dtype == torch.float32 and 0 <= off < n:
+                v = src[off:off + v.numel()].view_as(v)
+            out[k] = v.detach().clone()
+        return out
 
     # ---- dynamic evaluation (DESIGN.md section 14) -------------------------------------------------------------------
     def _single_replica(self, what):
