@@ -129,6 +129,30 @@ int  zrb_set_variational_dropout(zrb_ctx* ctx, int32_t on, float p_rec);
  * and zrb_lstm_layer_fwd / _bwd use the raw W_hh.  ZRB_E_INVALID for p outside [0, 1) or not finite.  A change of the
  * mode invalidates the saved forward, as zrb_set_variational_dropout does. */
 int  zrb_set_weight_drop(zrb_ctx* ctx, float p, uint64_t seed);
+/* Embedding dropout (Merity, Keskar & Socher 2018, AWD-LSTM's `embedded_dropout`; DESIGN.md section 17 states it bit
+ * for bit): whole word types are dropped in the gather of model.py:13-14 / :104, before the dropout of :105.  Opt-in; p = 0 (the default) changes nothing.  In a
+ * train-mode call with step s, vocabulary row v is gathered as fp32(fp32(W[v, j] * s_e(v)) * s_0) with s_e(v) = 0 or
+ * float32(1 / (1 - p)) from m = zrb_dropout_mask(seed, s, 3L + 1, V, p), element v = row v, and s_0 the site-0
+ * multiplier; each occurrence of v adds fp32(fp32(dA * s_0) * s_e(v)) to dE (dense scatter, rows-only update,
+ * zrb_set_embed_rows_out rows and the tied merge alike).  Tied: only the lookup is masked, the projection uses the raw
+ * E.  `seed` holds no rank: every data-parallel rank draws the same mask.  Eval mode (generation, beam search, the
+ * neural cache, dynamic evaluation) applies no mask.  ZRB_E_INVALID for p outside [0, 1) or not finite.  A change of
+ * (p, seed) invalidates the saved forward, as zrb_set_weight_drop does. */
+int  zrb_set_embed_dropout(zrb_ctx* ctx, float p, uint64_t seed);
+/* Activation regularization, AR and TAR (Merity, Keskar & Socher 2018, AWD-LSTM main.py's `alpha * dropped_rnn_hs
+ * .pow(2).mean()` and `beta * (rnn_hs[1:] - rnn_hs[:-1]).pow(2).mean()`; DESIGN.md section 17 states it bit for bit).
+ * Opt-in; alpha = beta = 0 (the default) changes nothing.  Every fused train step (zrb_train_step_grads / _begin /
+ * _host) differentiates NLL + R, in the unit of the loss of main.py:77-84 (B x the token mean):
+ *   R = alpha / (T*H) * sum_{t,b,j} y^2 + beta / ((T-1)*H) * sum_{t>=1,b,j} (h_t - h_{t-1})^2   (TAR = 0 when T = 1)
+ * with h the last layer's raw output and y = h * (its dropout multiplier, site L).  The gradient r_t = dR/dh_t enters
+ * the last layer's backward after the output mask: dh_t = fp32(m * s * dY_t) + r_t + the recurrent term.  The clip
+ * norm and the gradients include it.  The returned loss stays the NLL.  zrb_forward / zrb_backward, eval calls and the
+ * eval-mode gradient of dynamic evaluation ignore it.  ZRB_E_INVALID for negative or non-finite alpha, beta.  A change
+ * invalidates the saved forward. */
+int  zrb_set_activation_reg(zrb_ctx* ctx, float alpha, float beta);
+/* Enqueue on `stream` a copy of the last train step's alpha-weighted AR and beta-weighted TAR values into out2[0..1]
+ * (device memory; zeros before the first step with the mode on).  No host synchronisation. */
+int  zrb_activation_reg(zrb_ctx* ctx, float* out2, void* stream);
 
 /* Model.forward (model.py:103-110): embedding gather, dropout, L x (LSTM layer,
  * dropout), vocabulary projection.

@@ -56,6 +56,12 @@ ap.add_argument("--tied", action="store_true",
                 help="tie the embedding and softmax weights (Press & Wolf 2017): fc.W is embed.W")
 ap.add_argument("--weight_drop", type=float, default=0.0,
                 help="weight-dropped LSTM (Merity et al. 2018): DropConnect with this p on the hidden-to-hidden matrices")
+ap.add_argument("--embed_dropout", type=float, default=0.0,
+                help="embedding dropout (Merity et al. 2018): whole word types dropped with this p in each train step")
+ap.add_argument("--ar", type=float, default=0.0,
+                help="AR (Merity et al. 2018): alpha of the penalty on the last layer's dropped output (AWD: 2)")
+ap.add_argument("--tar", type=float, default=0.0,
+                help="TAR (Merity et al. 2018): beta of the penalty on the last layer's step-to-step change (AWD: 1)")
 ap.add_argument("--asgd", action="store_true",
                 help="NT-ASGD (Merity et al. 2018): start averaging the weights once validation stops improving "
                      "(AWD-LSTM's non-monotone trigger); validate, test and save with the average from then on")
@@ -108,8 +114,8 @@ torch.manual_seed(args.seed)
 if args.impl == "ours":
     model = zaremba_b200.Model(vocab, args.hidden_size, args.layer_num, args.dropout, args.winit,
                                variational=args.variational, recurrent_dropout=args.recurrent_dropout,
-                               tied=args.tied, weight_drop=args.weight_drop).to(dev)
-    tr = zaremba_b200.Trainer(model, B, T, lazy_update=args.lazy_update)
+                               tied=args.tied, weight_drop=args.weight_drop, embed_dropout=args.embed_dropout).to(dev)
+    tr = zaremba_b200.Trainer(model, B, T, lazy_update=args.lazy_update, ar=args.ar, tar=args.tar)
     # the corpus is staged on the device once (SURVEY 8f#2): 3 x [n_batches, T, B] int64
     trn_x = torch.stack([x for x, _ in trn_b]).contiguous().to(dev)
     trn_y = torch.stack([y for _, y in trn_b]).contiguous().to(dev)
@@ -148,6 +154,10 @@ else:
         raise SystemExit("--tied is a mode of --impl ours (the reference's cudnn path keeps embed.W and fc.W apart)")
     if args.weight_drop:
         raise SystemExit("--weight_drop is a mode of --impl ours")
+    if args.embed_dropout:
+        raise SystemExit("--embed_dropout is a mode of --impl ours")
+    if args.ar or args.tar:
+        raise SystemExit("--ar / --tar are modes of --impl ours")
     if args.asgd or args.asgd_from is not None:
         raise SystemExit("--asgd / --asgd_from are modes of --impl ours")
     from oracle import torch_port as P

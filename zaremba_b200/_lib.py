@@ -58,6 +58,9 @@ _SIGNATURES = {
     "zrb_set_explicit_masks": (C.c_int, [_vp, C.POINTER(_vp)]),
     "zrb_set_variational_dropout": (C.c_int, [_vp, C.c_int32, C.c_float]),
     "zrb_set_weight_drop": (C.c_int, [_vp, C.c_float, C.c_uint64]),
+    "zrb_set_embed_dropout": (C.c_int, [_vp, C.c_float, C.c_uint64]),
+    "zrb_set_activation_reg": (C.c_int, [_vp, C.c_float, C.c_float]),
+    "zrb_activation_reg": (C.c_int, [_vp, _vp, _vp]),
     "zrb_forward": (C.c_int, [_vp, C.POINTER(ZrbParams), _vp, C.c_int32, C.c_int32, C.POINTER(ZrbStates),
                               C.POINTER(ZrbStates), _vp, C.c_int32, C.c_uint64, C.c_uint64, _vp]),
     "zrb_backward": (C.c_int, [_vp, C.POINTER(ZrbParams), _vp, C.POINTER(ZrbParams), _vp]),

@@ -84,6 +84,20 @@ MaskSrc wd_mask(const zrb_ctx* c, int layer) {
     return make_mask_src(nullptr, c->wd_seed, c->step, 2 * c->cfg.layers + 1 + layer, c->p_wd, c->train);
 }
 
+bool reg_on(const zrb_ctx* c) { return c->ar_alpha > 0.f || c->tar_beta > 0.f; }
+
+int reg_compute(zrb_ctx* c, cudaStream_t s) {
+    const int L = c->cfg.layers;
+    ZRB_TRY(activation_reg(c->hraw[L - 1], c->reg_r, c->reg_part, c->reg_val, c->T, c->B, c->cfg.hidden, site_mask(c, L),
+                           c->ar_alpha, c->tar_beta, s));
+    c->reg_use = true;
+    return ZRB_OK;
+}
+
+MaskSrc ed_mask(const zrb_ctx* c) {
+    return make_mask_src(nullptr, c->ed_seed, c->step, 3 * c->cfg.layers + 1, c->p_ed, c->train);
+}
+
 static cudaEvent_t prof_event(zrb_ctx* c) {
     if (!c->prof_pool.empty()) {
         cudaEvent_t e = c->prof_pool.back();
@@ -277,6 +291,48 @@ int zrb_set_weight_drop(zrb_ctx* c, float p, uint64_t seed) {
     return ZRB_OK;
 }
 
+int zrb_set_embed_dropout(zrb_ctx* c, float p, uint64_t seed) {
+    ZRB_REQUIRE(c, "null ctx");
+    ZRB_REQUIRE(isfinite(p) && p >= 0.f && p < 1.f, "embedding-dropout p %f outside [0,1)", p);
+    if (p != c->p_ed || seed != c->ed_seed) {
+        c->have_fwd = false;        // a backward must not regenerate another mask than its forward used
+        c->bwd_next_layer = -1;
+    }
+    c->p_ed = p;
+    c->ed_seed = seed;
+    return ZRB_OK;
+}
+
+int zrb_set_activation_reg(zrb_ctx* c, float alpha, float beta) {
+    ZRB_REQUIRE(c, "null ctx");
+    ZRB_REQUIRE(isfinite(alpha) && alpha >= 0.f, "AR alpha %f must be finite and >= 0", alpha);
+    ZRB_REQUIRE(isfinite(beta) && beta >= 0.f, "TAR beta %f must be finite and >= 0", beta);
+    if ((alpha > 0.f || beta > 0.f) && !c->reg_r) {
+        ZRB_TRY(dalloc(c, &c->reg_r, (size_t)c->cfg.max_seq * c->cfg.max_batch * c->cfg.hidden));
+        ZRB_TRY(dalloc(c, &c->reg_part, (size_t)2 * kActRegBlocks));
+        ZRB_TRY(dalloc(c, &c->reg_val, 2));
+        ZRB_CUDA(cudaMemset(c->reg_val, 0, 2 * sizeof(float)));
+    }
+    if (alpha != c->ar_alpha || beta != c->tar_beta) {
+        c->have_fwd = false;        // a phased backward must not add another step's penalty gradient
+        c->bwd_next_layer = -1;
+    }
+    c->ar_alpha = alpha;
+    c->tar_beta = beta;
+    return ZRB_OK;
+}
+
+int zrb_activation_reg(zrb_ctx* c, float* out2, void* stream) {
+    ZRB_REQUIRE(c && out2, "null argument");
+    cudaStream_t s = (cudaStream_t)stream;
+    if (!c->reg_val) {
+        ZRB_CUDA(cudaMemsetAsync(out2, 0, 2 * sizeof(float), s));
+        return ZRB_OK;
+    }
+    ZRB_CUDA(cudaMemcpyAsync(out2, c->reg_val, 2 * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    return ZRB_OK;
+}
+
 int zrb_forward(zrb_ctx* c, const zrb_params* p, const int64_t* x, int32_t T, int32_t B, const zrb_states* in,
                 const zrb_states* out, float* scores, int32_t train, uint64_t seed, uint64_t step, void* stream) {
     ZRB_REQUIRE(c && p && x && in && out, "null argument");
@@ -285,6 +341,7 @@ int zrb_forward(zrb_ctx* c, const zrb_params* p, const int64_t* x, int32_t T, in
     cudaStream_t s = (cudaStream_t)stream;
     c->T = T; c->B = B; c->train = train ? 1 : 0; c->seed = seed; c->step = step;
     c->have_fwd = false;
+    c->reg_use = false;   // AR / TAR belongs to the fused train steps (DESIGN.md section 17)
     if (c->cfg.engine == ZRB_ENGINE_TC)
         ZRB_TRY(tc_forward(c, p, x, in, out, scores, s));
     else
@@ -436,6 +493,7 @@ int zrb_train_step_grads(zrb_ctx* c, const zrb_params* p, const zrb_params* g, c
         ProfScope ps(c, ZRB_PROF_SOFTMAX, s);
         ZRB_TRY(softmax_nll(c->scores, y, T * B, c->cfg.vocab, B, c->row_loss, loss, c->dscores, nullptr, s));
     }
+    if (reg_on(c)) ZRB_TRY(reg_compute(c, s));
     ZRB_TRY(zrb_backward(c, p, c->dscores, g, stream));
     return ZRB_OK;
 }

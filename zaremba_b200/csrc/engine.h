@@ -48,6 +48,13 @@ struct zrb_ctx {
     uint64_t wd_seed = 0;
     float* whh_wd[ZRB_MAX_LAYERS] = {};    // validation engine, weight drop: [4H, H] fp32(W_hh * mask * scale) of the
                                            // last train-mode forward; allocated when first switched on
+    float p_ed = 0.f;                      // zrb_set_embed_dropout: whole word types dropped (DESIGN.md section 17)
+    uint64_t ed_seed = 0;
+    float ar_alpha = 0.f, tar_beta = 0.f;  // zrb_set_activation_reg: AR / TAR on the last layer (DESIGN.md section 17)
+    bool reg_use = false;                  // this train step's backward adds reg_r (set by the fused train steps only)
+    float* reg_r = nullptr;                // [max_seq * max_batch, H] the penalties' gradient wrt h of the last layer
+    double* reg_part = nullptr;            // kActRegBlocks x 2 partial sums
+    float* reg_val = nullptr;              // [2] the last train step's alpha-weighted AR and beta-weighted TAR
     int64_t weights_version = 1;          // bumped whenever parameter values change
     bool avg_on = false;                   // zrb_set_average: iterate averaging into `avg` (DESIGN.md section 16)
     zrb_params avg{};
@@ -101,6 +108,11 @@ MaskSrc site_mask(const zrb_ctx* c, int site);   // dropout site 0..L (period B*
 MaskSrc rec_mask(const zrb_ctx* c, int layer);   // recurrent site L+1+layer of the variational mode (inactive otherwise)
 MaskSrc wd_mask(const zrb_ctx* c, int layer);    // weight-drop site 2L+1+layer over W_hh's 4H*H elements (inactive:
                                                  // eval mode or p_wd = 0)
+bool reg_on(const zrb_ctx* c);                   // AR / TAR is switched on (alpha > 0 or beta > 0)
+// AR / TAR of the last forward (train mode): r into reg_r and the two values into reg_val, then reg_use = true
+int reg_compute(zrb_ctx* c, cudaStream_t s);
+MaskSrc ed_mask(const zrb_ctx* c);               // embedding-dropout site 3L+1 over the V vocabulary rows (inactive:
+                                                 // eval mode or p_ed = 0)
 
 // RAII bracket: records an event pair around the launches of one kernel class
 struct ProfScope {

@@ -18,7 +18,7 @@ int simt_forward(zrb_ctx* c, const zrb_params* p, const int64_t* x, const zrb_st
     // model.py:104-105
     {
         ProfScope ps(c, ZRB_PROF_EMBED_FWD, s);
-        ZRB_TRY(embed_dropout_fwd(p->embed_w, x, c->act[0], nullptr, 0, N, H, V, site_mask(c, 0), s));
+        ZRB_TRY(embed_dropout_fwd(p->embed_w, x, c->act[0], nullptr, 0, N, H, V, site_mask(c, 0), ed_mask(c), s));
     }
     for (int l = 0; l < L; ++l) {  // model.py:106-108
         float* G = c->gates[l];
@@ -71,6 +71,7 @@ int simt_backward(zrb_ctx* c, const zrb_params* p, const float* dscores, const z
     for (int l = L - 1; l >= 0; --l) {
         MaskSrc m = site_mask(c, l + 1), rm = rec_mask(c, l), wm = wd_mask(c, l);
         const float* w_hh = wm.active ? c->whh_wd[l] : p->w_hh[l];
+        const float* r = (c->reg_use && l == L - 1) ? c->reg_r : nullptr;   // AR / TAR gradient (DESIGN.md section 17)
         ZRB_CUDA(cudaMemsetAsync(c->dc, 0, bh * sizeof(float), s));
         {
         ProfScope ps(c, ZRB_PROF_REC_BWD, s);
@@ -79,7 +80,7 @@ int simt_backward(zrb_ctx* c, const zrb_params* p, const float* dscores, const z
             float* dGt = c->dG + (size_t)t * B * 4 * H;
             ZRB_TRY(lstm_cell_bwd(dY + (size_t)t * bh, t == T - 1 ? nullptr : c->dh_rec, c->dc,
                                   c->gates[l] + (size_t)t * B * 4 * H, c->cst[l] + (size_t)t * bh, c_prev, dGt, B, H,
-                                  (int64_t)t * bh, (int64_t)N * H, m, rm, s));
+                                  (int64_t)t * bh, (int64_t)N * H, m, rm, s, r ? r + (size_t)t * bh : nullptr));
             if (t > 0) ZRB_TRY(gemm_f32(dGt, w_hh, c->dh_rec, B, H, 4 * H, 0, 0, 1.f, 0.f, s));
         }
         }
@@ -103,13 +104,14 @@ int simt_backward(zrb_ctx* c, const zrb_params* p, const float* dscores, const z
         float* tmp = dY; dY = dX; dX = tmp;
     }
     ProfScope ps(c, ZRB_PROF_EMBED_BWD, s);
-    if (c->embed_rows_out) return embed_rows(dY, c->embed_rows_out, N, H, site_mask(c, 0), s);
+    const MaskSrc m0 = site_mask(c, 0), em = ed_mask(c);
+    if (c->embed_rows_out) return embed_rows(dY, c->x_saved, c->embed_rows_out, N, H, V, m0, em, s);
     if (c->tied) {   // g->embed_w holds G_proj: add the row sums (the tensor-core engine's fixed-point merge)
-        ZRB_TRY(embed_rows(dY, dX, N, H, site_mask(c, 0), s));
+        ZRB_TRY(embed_rows(dY, c->x_saved, dX, N, H, V, m0, em, s));
         return embed_scatter_rows(c->x_saved, dX, g->embed_w, N, H, V, c->emb_first, c->emb_acc, s, true);
     }
     ZRB_CUDA(cudaMemsetAsync(g->embed_w, 0, (size_t)V * H * sizeof(float), s));
-    ZRB_TRY(embed_dropout_bwd(dY, c->x_saved, g->embed_w, N, H, V, site_mask(c, 0), s));
+    ZRB_TRY(embed_dropout_bwd(dY, c->x_saved, g->embed_w, N, H, V, m0, em, s));
     return ZRB_OK;
 }
 

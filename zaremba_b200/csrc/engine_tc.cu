@@ -314,7 +314,7 @@ int tc_forward(zrb_ctx* c, const zrb_params* p, const int64_t* x, const zrb_stat
         // tied: E's update (item L) is still deferred -> gather through it; the update itself rides beside the last
         // recurrence, before the projection reads fc_w_h
         const bool through = ride && c->tied && (t->upd_pending & (1u << L));
-        ZRB_TRY(embed_dropout_fwd(p->embed_w, x, nullptr, t->x_h[0], Hp, N, H, V, site_mask(c, 0), s,
+        ZRB_TRY(embed_dropout_fwd(p->embed_w, x, nullptr, t->x_h[0], Hp, N, H, V, site_mask(c, 0), ed_mask(c), s,
                                   through ? t->upd_tl.g[1 + 4 * L] : nullptr, t->upd_lr, c->scalars));
     }
     for (int l = 0; l < L; ++l) {
@@ -332,12 +332,14 @@ int tc_forward(zrb_ctx* c, const zrb_params* p, const int64_t* x, const zrb_stat
                                 p->b_hh[l]));
         }
         MaskSrc m = site_mask(c, l + 1), rm = rec_mask(c, l);
+        // AR / TAR (DESIGN.md section 17) reads the last layer's fp32 h (the per-timestep path always writes it)
+        const bool reg_h = t->in_train_step && reg_on(c) && l == L - 1;
         ProfScope ps(c, ZRB_PROF_REC_FWD, s);
         if (t->fplan.ok) {
             ZRB_TRY(t->fwd_bar.claim(T, t->fplan.nCTA, s, [&](unsigned int* word, unsigned int base) {
                 return lstm_rec_fwd(t->fplan, tc_watchdog(c), t->w_img_f[l], t->h0_img[l], t->h_img, G, c->c0s[l], c->cst[l],
                                     out->h[l], out->c[l], t->hprev_h[l], t->x_h[l + 1], word, base, T, B, H, Hp, m, rm, s,
-                                    t->trace);
+                                    t->trace, reg_h ? c->hraw[l] : nullptr);
             }));
             // deferred update of the NEXT layer's matrices (or of fc.W after the last layer): on the idle SMs, beside
             // this recurrence; their consumers (the next input GEMM / the projection) are enqueued behind them
@@ -461,6 +463,7 @@ static int tc_backward_layer(zrb_ctx* c, const zrb_params* p, const zrb_params* 
     float* dY = c->bwd_dy;
     float* dX = c->bwd_dx;
     __half* dG_h = (l & 1) ? t->dG_h_alt : t->dG_h;
+    const float* r = (c->reg_use && l == c->cfg.layers - 1) ? c->reg_r : nullptr;   // AR / TAR gradient (section 17)
     {
         MaskSrc m = site_mask(c, l + 1), rm = rec_mask(c, l);
         if (t->bplan.ok) {
@@ -469,7 +472,7 @@ static int tc_backward_layer(zrb_ctx* c, const zrb_params* p, const zrb_params* 
                 return lstm_rec_bwd(t->bplan, tc_watchdog(c), t->w_img_b[l], t->g_img, dY, c->gates[l], c->cst[l], c->c0s[l],
                                     dG_h, word, base, T, B, H, G4p, m, rm, s,
                                     t->trace ? t->trace + 8 + (size_t)c->cfg.max_seq * 8 : nullptr, g->b_ih[l], g->b_hh[l],
-                                    c->resident_flag, ++c->resident_seq, c->dG /* [N,4H] fp32, idle on this path */);
+                                    c->resident_flag, ++c->resident_seq, c->dG /* [N,4H] fp32, idle on this path */, r);
             }));
             ZRB_TRY(tc_issue_pending(c, g, s));   // runs on the SMs the cluster kernel leaves idle
         } else {
@@ -480,7 +483,7 @@ static int tc_backward_layer(zrb_ctx* c, const zrb_params* p, const zrb_params* 
                 ZRB_TRY(lstm_cell_bwd_tc(dY + (size_t)tt * bh, tt == T - 1 ? nullptr : c->dh_rec, c->dc,
                                          c->gates[l] + (size_t)tt * B * 4 * H, c->cst[l] + (size_t)tt * bh, c_prev,
                                          c->dG + (size_t)tt * B * 4 * H, dG_h + (size_t)tt * B * G4p, G4p, B, H,
-                                         (int64_t)tt * bh, (int64_t)N * H, m, rm, s));
+                                         (int64_t)tt * bh, (int64_t)N * H, m, rm, s, r ? r + (size_t)tt * bh : nullptr));
                 if (tt > 0)  // dh_{t-1}[B,H] = dG_t[B,4H] * W_hh[4H,H]
                     ZRB_TRY(gemm_f16_tc(dG_h + (size_t)tt * B * G4p, G4p, 0, t->w_hh_h[l], Hp, 1, c->dh_rec, H, B, H,
                                         4 * H, inv, nullptr, 0, s));
@@ -507,11 +510,12 @@ static int tc_backward_layer(zrb_ctx* c, const zrb_params* p, const zrb_params* 
     c->bwd_next_layer = l - 1;
     if (l > 0) return ZRB_OK;
     ProfScope ps(c, ZRB_PROF_EMBED_BWD, s);
-    if (c->embed_rows_out) return embed_rows(dY, c->embed_rows_out, N, H, site_mask(c, 0), s);
+    const MaskSrc m0 = site_mask(c, 0), em = ed_mask(c);
+    if (c->embed_rows_out) return embed_rows(dY, c->x_saved, c->embed_rows_out, N, H, V, m0, em, s);
     if (c->tied) {
         // g->embed_w holds G_proj (the projection's wgrad GEMM overwrote every row): add the fixed-point row sums, with
         // dX (free now) as the rows buffer; the fused norm's extra slots get the correction from G_proj^2 to dE^2
-        ZRB_TRY(embed_rows(dY, dX, N, H, site_mask(c, 0), s));
+        ZRB_TRY(embed_rows(dY, c->x_saved, dX, N, H, V, m0, em, s));
         return embed_scatter_rows(c->x_saved, dX, g->embed_w, N, H, V, c->emb_first, c->emb_acc, s, true,
                                   c->fused_norm ? c->partials + norm_partials_base() : nullptr, kNormExtra);
     }
@@ -520,7 +524,7 @@ static int tc_backward_layer(zrb_ctx* c, const zrb_params* p, const zrb_params* 
     } else {
         ZRB_CUDA(cudaMemsetAsync(g->embed_w, 0, (size_t)V * H * sizeof(float), s));
     }
-    ZRB_TRY(embed_dropout_bwd(dY, c->x_saved, g->embed_w, N, H, V, site_mask(c, 0), s));
+    ZRB_TRY(embed_dropout_bwd(dY, c->x_saved, g->embed_w, N, H, V, m0, em, s));
     if (c->emb_sparse) {
         ZRB_CUDA(cudaMemcpyAsync(c->emb_prev_ids, c->x_saved, (size_t)N * sizeof(int64_t), cudaMemcpyDeviceToDevice, s));
         c->emb_prev_n = N;
@@ -559,6 +563,8 @@ int tc_train_step_grads(zrb_ctx* c, const zrb_params* p, const zrb_params* g, co
         ZRB_TRY(softmax_nll(c->scores, y, T * B, c->cfg.vocab, B, c->row_loss, loss, nullptr, nullptr, s, c->tc->dS_h,
                             c->tc->Vp, kGradScale));
     }
+    c->reg_use = false;
+    if (reg_on(c)) ZRB_TRY(reg_compute(c, s));   // AR / TAR: between the softmax and the projection's backward
     return tc_backward_from_image(c, p, g, s);
 }
 
@@ -569,6 +575,7 @@ int tc_eval_grads(zrb_ctx* c, const zrb_params* p, const zrb_params* g, const in
                   const zrb_states* in, const zrb_states* out, float* loss, cudaStream_t s) {
     c->T = T; c->B = B; c->train = 0; c->seed = 0; c->step = 0;
     c->have_fwd = false;
+    c->reg_use = false;   // the eval-mode loss has no AR / TAR
     ZRB_TRY(tc_forward(c, p, x, in, out, c->scores, s));
     c->have_fwd = true;
     {
@@ -599,6 +606,8 @@ int tc_train_step_begin(zrb_ctx* c, const zrb_params* p, const zrb_params* g, co
         ZRB_TRY(softmax_nll(c->scores, y, T * B, c->cfg.vocab, B, c->row_loss, loss, nullptr, nullptr, s, c->tc->dS_h,
                             c->tc->Vp, kGradScale));
     }
+    c->reg_use = false;
+    if (reg_on(c)) ZRB_TRY(reg_compute(c, s));   // AR / TAR: between the softmax and the projection's backward
     c->tc->defer_wgrad = false;   // phased backward: every bucket is complete when its call returns
     return tc_backward_head(c, p, g, s);
 }

@@ -6,12 +6,13 @@ namespace zrb {
 
 // ---- pointwise.cu -----------------------------------------------------------------------
 // out[n, :] = W[idx[n], :] * dropout   (model.py:13-14 + :105)
+// em: embedding dropout (DESIGN.md section 17), stream element v = vocabulary row v; applied before m
 // pend_g (or null): gather sgd_elem(W, scalars[1] * pend_g, lr), W's deferred update (tied embedding, lazy update)
 int embed_dropout_fwd(const float* W, const int64_t* idx, float* out, __half* out_h, int64_t ld_h,
-                      int N, int H, int V, MaskSrc m, cudaStream_t s, const float* pend_g = nullptr, float lr = 0.f,
-                      const float* scalars = nullptr);
-// dW[idx[n], :] += dA[n, :] * dropout   (dW pre-zeroed)
-int embed_dropout_bwd(const float* dA, const int64_t* idx, float* dW, int N, int H, int V, MaskSrc m,
+                      int N, int H, int V, MaskSrc m, MaskSrc em, cudaStream_t s, const float* pend_g = nullptr,
+                      float lr = 0.f, const float* scalars = nullptr);
+// dW[idx[n], :] += dA[n, :] * dropout * embedding dropout   (dW pre-zeroed)
+int embed_dropout_bwd(const float* dA, const int64_t* idx, float* dW, int N, int H, int V, MaskSrc m, MaskSrc em,
                       cudaStream_t s);
 // pre [B,4H] holds x-part + h-part pre-activations (+bias already added); overwritten with
 // activated gates (i,f,g,o).  c_prev/c_out/h_raw/y_out [B,H]; y_out = dropout(h).
@@ -22,7 +23,13 @@ int lstm_cell_fwd(float* pre, const float* c_prev, float* c_out, float* h_raw, f
 // dy_post [B,H] upstream grad on the post-dropout output
 int lstm_cell_bwd(const float* dy_post, const float* dh_rec, float* dc, const float* gates, const float* c_t,
                   const float* c_prev, float* dG, int B, int H, int64_t elem_off, int64_t n_total, MaskSrc m,
-                  MaskSrc rm, cudaStream_t s);
+                  MaskSrc rm, cudaStream_t s, const float* r = nullptr);   // r: as lstm_cell_bwd_tc's
+// AR / TAR (DESIGN.md section 17) over the last layer's raw output h [T,B,H] with its output mask m: r [T,B,H] = the
+// penalties' gradient wrt h, out[0..1] = the alpha-weighted AR and beta-weighted TAR values (written on the device;
+// partial: >= 2 * 264 doubles of scratch).  Two launches, no float atomics.
+int activation_reg(const float* h, float* r, double* partial, float* out, int T, int B, int H, MaskSrc m, float alpha,
+                   float beta, cudaStream_t s);
+constexpr int kActRegBlocks = 264;
 // y[e] = x[e] * (mask multiplier of element e), e < n
 int dropout_copy(const float* x, float* y, int64_t n, MaskSrc m, cudaStream_t s);
 // weight drop (DESIGN.md section 15): y[e] = x[e] * (mask multiplier of element e), n % 4 == 0, x == y allowed (the
@@ -39,7 +46,9 @@ int colsum(const float* A, float* out, float* out2, int N, int M, cudaStream_t s
 int softmax_nll(const float* scores, const int64_t* y, int N, int V, int B, float* row_loss, float* loss,
                 float* dscores, float* tgt_prob, cudaStream_t s, __half* ds_h = nullptr, int64_t ld_s = 0,
                 float h_scale = 1.f);
-int embed_rows(const float* dA, float* rows, int N, int H, MaskSrc m, cudaStream_t s);
+// rows[n, :] = dA[n, :] * dropout * embedding dropout of token idx[n] (idx read only when em is active)
+int embed_rows(const float* dA, const int64_t* idx, float* rows, int N, int H, int V, MaskSrc m, MaskSrc em,
+               cudaStream_t s);
 // add: dW[id] += the id's sum instead of dW[id] = (tied embedding); sumsq: see embed_finish_add_kernel
 int embed_scatter_rows(const int64_t* ids, const float* rows, float* dW, int n_rows, int H, int V, int* first,
                        long long* acc, cudaStream_t s, bool add = false, float* sumsq = nullptr, int nblocks = 0);

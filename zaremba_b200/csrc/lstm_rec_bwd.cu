@@ -32,6 +32,7 @@ struct RecBwdArgs {
     const __half* w_img;      // [nCluster][4][Kc][G][8][8]
     __half* g_img;            // [2][4][Kc][GB][8][8] ring: slot (t & 1) holds kGradScale * dG_t per gate
     const float* dy;          // [N,H] grad wrt the layer's dropout'ed output
+    const float* r;           // [N,H] or null: AR/TAR gradient added after the mask (DESIGN.md section 17)
     const float* gates;       // [N,4H] activated (i,f,g,o)
     const float* cst;         // [N,H]
     const float* c0;          // [B,H]
@@ -291,6 +292,7 @@ __global__ void __launch_bounds__(kRecThreads, 1) lstm_rec_bwd_kernel(RecBwdArgs
                     // (variational mode: element b*H + j of the site's stream, the mask fixed over the window)
                     dyv[k] = __ldg(a.dy + n * H + j) *
                              mask_mul1_at(a.m, (uint64_t)(a.m.period ? b : (int)n) * H + j, n_total);
+                    if (a.r) dyv[k] += __ldg(a.r + n * H + j);
                 }
             }
             if (s > 0) {
@@ -505,11 +507,11 @@ int pack_whh_bwd(const float* W, __half* img, int H, const RecPlan& p, cudaStrea
 int lstm_rec_bwd(const RecPlan& p, const RecWatchdog& wd, const __half* w_img, __half* g_img, const float* dy, const float* gates,
                  const float* cst, const float* c0, __half* dG_h, unsigned int* counter, unsigned int counter_base, int T,
                  int B, int H, int G4p, MaskSrc m, MaskSrc rm, cudaStream_t s, long long* trace, float* db1, float* db2,
-                 unsigned int* resident_flag, unsigned int resident_value, float* db_scratch) {
+                 unsigned int* resident_flag, unsigned int resident_value, float* db_scratch, const float* r) {
     ZRB_REQUIRE(!db1 || db_scratch, "bias gradients need the scratch buffer");
     RecBwdArgs a;
     a.base = counter_base;
-    a.w_img = w_img; a.g_img = g_img; a.dy = dy; a.gates = gates; a.cst = cst; a.c0 = c0; a.dG_h = dG_h;
+    a.w_img = w_img; a.g_img = g_img; a.dy = dy; a.r = r; a.gates = gates; a.cst = cst; a.c0 = c0; a.dG_h = dG_h;
     static const bool pull = getenv("ZRB_BWD_PULL") != nullptr;   // A/B switch: the r01 staging + DSMEM-pull exchange (S = 1)
     a.push = pull ? 0 : 1;
     a.counter = counter; a.db1 = db1; a.db2 = db2; a.db_scratch = db_scratch; a.res_flag = resident_flag; a.res_value = resident_value;

@@ -12,11 +12,14 @@ namespace zrb {
 // Algorithmic bytes per token: H*4 read (table row) + H*4 written (+ H*2 fp16 image).
 // PENDING (tied embedding, lazy update): the SGD update of W is still deferred; every gathered element is
 // sgd_elem(W, coef * g, lr) with the coefficient of scalars[1], the value update_pack will store (g is only read).
+// em: embedding dropout (DESIGN.md section 17), one keep flag per vocabulary row; the row is multiplied by its
+// multiplier s_e before the site-0 mask: fp32(fp32(W * s_e) * s_0).  One Philox call per thread (the whole row
+// shares the flag), none when inactive.
 // ----------------------------------------------------------------------------------------
 template <bool PENDING>
 __global__ void embed_dropout_fwd_kernel(const float* __restrict__ W, const int64_t* __restrict__ idx,
                                          float* __restrict__ out, __half* __restrict__ out_h, int64_t ld_h, int N,
-                                         int H, int V, MaskSrc m, const float* __restrict__ pend_g, float lr,
+                                         int H, int V, MaskSrc m, MaskSrc em, const float* __restrict__ pend_g, float lr,
                                          const float* __restrict__ scalars) {
     int n = blockIdx.x;
     if (n >= N) return;
@@ -27,6 +30,7 @@ __global__ void embed_dropout_fwd_kernel(const float* __restrict__ W, const int6
     uint64_t n_total = (uint64_t)N * H;
     float coef = 0.f;
     if constexpr (PENDING) coef = scalars[1];
+    const float se = em.active ? mask_mul1_at(em, (uint64_t)row, (uint64_t)V) : 1.f;
     for (int g = threadIdx.x; g < groups; g += blockDim.x) {
         int j0 = g << 2;
         uint64_t e0 = (uint64_t)n * H + j0;
@@ -35,6 +39,10 @@ __global__ void embed_dropout_fwd_kernel(const float* __restrict__ W, const int6
         for (int i = 0; i < 4; ++i) {
             if constexpr (PENDING) v[i] = (j0 + i < H) ? sgd_elem(src[j0 + i], pend_g[row * (int64_t)H + j0 + i] * coef, lr) : 0.f;
             else v[i] = (j0 + i < H) ? src[j0 + i] : 0.f;
+        }
+        if (em.active) {
+#pragma unroll
+            for (int i = 0; i < 4; ++i) v[i] *= se;
         }
         if (m.active) {
             // rows are H long; H % 4 != 0 makes groups straddle Philox quads -> per-element path.  (A variational
@@ -59,34 +67,36 @@ __global__ void embed_dropout_fwd_kernel(const float* __restrict__ W, const int6
 }
 
 int embed_dropout_fwd(const float* W, const int64_t* idx, float* out, __half* out_h, int64_t ld_h, int N, int H,
-                      int V, MaskSrc m, cudaStream_t s, const float* pend_g, float lr, const float* scalars) {
+                      int V, MaskSrc m, MaskSrc em, cudaStream_t s, const float* pend_g, float lr, const float* scalars) {
     if (N == 0) return ZRB_OK;
     int threads = H >= 1024 ? 256 : 128;
-    if (pend_g) embed_dropout_fwd_kernel<true><<<N, threads, 0, s>>>(W, idx, out, out_h, ld_h, N, H, V, m, pend_g, lr, scalars);
-    else embed_dropout_fwd_kernel<false><<<N, threads, 0, s>>>(W, idx, out, out_h, ld_h, N, H, V, m, nullptr, 0.f, nullptr);
+    if (pend_g) embed_dropout_fwd_kernel<true><<<N, threads, 0, s>>>(W, idx, out, out_h, ld_h, N, H, V, m, em, pend_g, lr, scalars);
+    else embed_dropout_fwd_kernel<false><<<N, threads, 0, s>>>(W, idx, out, out_h, ld_h, N, H, V, m, em, nullptr, 0.f, nullptr);
     ZRB_KERNEL_CHECK();
     return ZRB_OK;
 }
 
 // Backward of the gather: scatter-add with fp32 atomics (duplicate tokens in a window hit
-// the same row).  dW must be zeroed by the caller.
+// the same row).  dW must be zeroed by the caller.  Each occurrence adds fp32(fp32(dA * s_0) * s_e).
 __global__ void embed_dropout_bwd_kernel(const float* __restrict__ dA, const int64_t* __restrict__ idx,
-                                         float* __restrict__ dW, int N, int H, int V, MaskSrc m) {
+                                         float* __restrict__ dW, int N, int H, int V, MaskSrc m, MaskSrc em) {
     int n = blockIdx.x;
     if (n >= N) return;
     int64_t row = idx[n];
     if (row < 0 || row >= V) return;
     uint64_t n_total = (uint64_t)N * H;
+    const float se = em.active ? mask_mul1_at(em, (uint64_t)row, (uint64_t)V) : 1.f;
     for (int j = threadIdx.x; j < H; j += blockDim.x) {
         float g = dA[(int64_t)n * H + j] * mask_mul1(m, (uint64_t)n * H + j, n_total);
+        if (em.active) g *= se;
         if (g != 0.f) atomicAdd(dW + row * (int64_t)H + j, g);
     }
 }
 
-int embed_dropout_bwd(const float* dA, const int64_t* idx, float* dW, int N, int H, int V, MaskSrc m,
+int embed_dropout_bwd(const float* dA, const int64_t* idx, float* dW, int N, int H, int V, MaskSrc m, MaskSrc em,
                       cudaStream_t s) {
     if (N == 0) return ZRB_OK;
-    embed_dropout_bwd_kernel<<<N, 256, 0, s>>>(dA, idx, dW, N, H, V, m);
+    embed_dropout_bwd_kernel<<<N, 256, 0, s>>>(dA, idx, dW, N, H, V, m, em);
     ZRB_KERNEL_CHECK();
     return ZRB_OK;
 }
@@ -129,13 +139,14 @@ __global__ void lstm_cell_bwd_kernel(const float* __restrict__ dy_post, const fl
                                      float* __restrict__ dc, const float* __restrict__ gates,
                                      const float* __restrict__ c_t, const float* __restrict__ c_prev,
                                      float* __restrict__ dG, int B, int H, int64_t elem_off, int64_t n_total,
-                                     MaskSrc m, MaskSrc rm) {
+                                     MaskSrc m, MaskSrc rm, const float* __restrict__ r) {
     int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (tid >= (int64_t)B * H) return;
     int b = (int)(tid / H), j = (int)(tid % H);
     const float* row = gates + (int64_t)b * 4 * H;
     float i = row[j], f = row[H + j], g = row[2 * H + j], o = row[3 * H + j];
     float dh = dy_post[tid] * mask_mul1(m, (uint64_t)(elem_off + tid), (uint64_t)n_total);
+    if (r) dh += r[tid];
     if (dh_rec) dh += dh_rec[tid] * mask_mul1_at(rm, (uint64_t)tid, (uint64_t)B * H);
     float tc = tanhf(c_t[tid]);
     float d_o = dh * tc;
@@ -153,10 +164,69 @@ __global__ void lstm_cell_bwd_kernel(const float* __restrict__ dy_post, const fl
 
 int lstm_cell_bwd(const float* dy_post, const float* dh_rec, float* dc, const float* gates, const float* c_t,
                   const float* c_prev, float* dG, int B, int H, int64_t elem_off, int64_t n_total, MaskSrc m,
-                  MaskSrc rm, cudaStream_t s) {
+                  MaskSrc rm, cudaStream_t s, const float* r) {
     int64_t n = (int64_t)B * H;
     lstm_cell_bwd_kernel<<<cdiv(n, 256), 256, 0, s>>>(dy_post, dh_rec, dc, gates, c_t, c_prev, dG, B, H, elem_off,
-                                                      n_total, m, rm);
+                                                      n_total, m, rm, r);
+    ZRB_KERNEL_CHECK();
+    return ZRB_OK;
+}
+
+// ---- AR / TAR (DESIGN.md section 17) ------------------------------------------------------------------------------
+// Over the last layer's raw output h [T, B*H] (bh = B*H), with s = the output site's multiplier of element e:
+//   y = fp32(h * s);  dp = h_t - h_{t-1} (t >= 1, else 0);  dn = h_{t+1} - h_t (t <= T-2, else 0)
+//   r = fp32(fp32(ca * y) * s) + fp32(cb * fp32(dp - dn))
+// and, per block (fixed grid, fixed block size, fixed tree: a step stays reproducible), the fp64 sums of y^2 and dp^2.
+__global__ void __launch_bounds__(256) act_reg_kernel(const float* __restrict__ h, float* __restrict__ r,
+                                                      double* __restrict__ partial, int T, int64_t bh, MaskSrc m,
+                                                      float ca, float cb) {
+    const int64_t n = (int64_t)T * bh;
+    double sy = 0.0, sd = 0.0;
+    for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < n; e += (int64_t)gridDim.x * blockDim.x) {
+        const int t = (int)(e / bh);
+        const float hv = h[e];
+        const float s = mask_mul1(m, (uint64_t)e, (uint64_t)n);
+        const float y = __fmul_rn(hv, s);
+        const float dp = t > 0 ? __fsub_rn(hv, h[e - bh]) : 0.f;
+        const float dn = t < T - 1 ? __fsub_rn(h[e + bh], hv) : 0.f;
+        r[e] = __fadd_rn(__fmul_rn(__fmul_rn(ca, y), s), __fmul_rn(cb, __fsub_rn(dp, dn)));   // (no contraction)
+        sy += (double)y * y;
+        sd += (double)dp * dp;
+    }
+    __shared__ double red[2][8];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        sy += __shfl_xor_sync(0xffffffffu, sy, o);
+        sd += __shfl_xor_sync(0xffffffffu, sd, o);
+    }
+    if ((threadIdx.x & 31) == 0) { red[0][threadIdx.x >> 5] = sy; red[1][threadIdx.x >> 5] = sd; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double a = 0.0, b = 0.0;
+        for (int w = 0; w < 8; ++w) { a += red[0][w]; b += red[1][w]; }
+        partial[2 * blockIdx.x] = a;
+        partial[2 * blockIdx.x + 1] = b;
+    }
+}
+
+// out[0] = fp32(wa * sum y^2), out[1] = fp32(wb * sum dp^2), the partials added in block order
+__global__ void act_reg_finish_kernel(const double* __restrict__ partial, int nblocks, double wa, double wb,
+                                      float* __restrict__ out) {
+    if (threadIdx.x != 0) return;
+    double a = 0.0, b = 0.0;
+    for (int i = 0; i < nblocks; ++i) { a += partial[2 * i]; b += partial[2 * i + 1]; }
+    out[0] = (float)(wa * a);
+    out[1] = (float)(wb * b);
+}
+
+int activation_reg(const float* h, float* r, double* partial, float* out, int T, int B, int H, MaskSrc m, float alpha,
+                   float beta, cudaStream_t s) {
+    const int64_t bh = (int64_t)B * H;
+    const double wa = (double)alpha / ((double)T * H);
+    const double wb = T > 1 ? (double)beta / ((double)(T - 1) * H) : 0.0;
+    act_reg_kernel<<<kActRegBlocks, 256, 0, s>>>(h, r, partial, T, bh, m, (float)(2.0 * wa), (float)(2.0 * wb));
+    ZRB_KERNEL_CHECK();
+    act_reg_finish_kernel<<<1, 32, 0, s>>>(partial, kActRegBlocks, wa, wb, out);
     ZRB_KERNEL_CHECK();
     return ZRB_OK;
 }
@@ -461,16 +531,27 @@ int softmax_nll(const float* scores, const int64_t* y, int N, int V, int B, floa
 
 // ---- sparse form of the embedding gradient (data parallel) ------------------------------------------------
 // rows[n, :] = dropout-masked dA[n, :]: what embed_dropout_bwd would scatter, kept as N rows so that ranks can
-// exchange 4 MB of rows instead of all-reducing the dense 60 MB table gradient.
-__global__ void embed_rows_kernel(const float* __restrict__ dA, float* __restrict__ rows, int N, int H, MaskSrc m) {
+// exchange 4 MB of rows instead of all-reducing the dense 60 MB table gradient.  Embedding dropout (em active): row n
+// is fp32(fp32(dA * s_0) * s_e) with the flag of its token idx[n], so the rows leave the library already masked.
+__global__ void embed_rows_kernel(const float* __restrict__ dA, const int64_t* __restrict__ idx, float* __restrict__ rows,
+                                  int N, int H, int V, MaskSrc m, MaskSrc em) {
     int n = blockIdx.x;
     uint64_t n_total = (uint64_t)N * H;
-    for (int j = threadIdx.x; j < H; j += blockDim.x)
-        rows[(int64_t)n * H + j] = dA[(int64_t)n * H + j] * mask_mul1(m, (uint64_t)n * H + j, n_total);
+    float se = 1.f;
+    if (em.active) {
+        const int64_t row = idx[n];
+        se = (row >= 0 && row < V) ? mask_mul1_at(em, (uint64_t)row, (uint64_t)V) : 0.f;   // (the scatter skips it)
+    }
+    for (int j = threadIdx.x; j < H; j += blockDim.x) {
+        float g = dA[(int64_t)n * H + j] * mask_mul1(m, (uint64_t)n * H + j, n_total);
+        if (em.active) g *= se;
+        rows[(int64_t)n * H + j] = g;
+    }
 }
-int embed_rows(const float* dA, float* rows, int N, int H, MaskSrc m, cudaStream_t s) {
+int embed_rows(const float* dA, const int64_t* idx, float* rows, int N, int H, int V, MaskSrc m, MaskSrc em,
+               cudaStream_t s) {
     if (!N) return ZRB_OK;
-    embed_rows_kernel<<<N, 256, 0, s>>>(dA, rows, N, H, m);
+    embed_rows_kernel<<<N, 256, 0, s>>>(dA, idx, rows, N, H, V, m, em);
     ZRB_KERNEL_CHECK();
     return ZRB_OK;
 }

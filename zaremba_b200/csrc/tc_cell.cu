@@ -45,13 +45,15 @@ __global__ void lstm_cell_bwd_tc_kernel(const float* __restrict__ dy_post, const
                                         float* __restrict__ dc, const float* __restrict__ gates,
                                         const float* __restrict__ c_t, const float* __restrict__ c_prev,
                                         float* __restrict__ dG, __half* __restrict__ dG_h, int64_t ld_g, int B, int H,
-                                        int64_t elem_off, int64_t n_total, MaskSrc m, MaskSrc rm) {
+                                        int64_t elem_off, int64_t n_total, MaskSrc m, MaskSrc rm,
+                                        const float* __restrict__ r) {
     int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (tid >= (int64_t)B * H) return;
     int b = (int)(tid / H), j = (int)(tid % H);
     const float* row = gates + (int64_t)b * 4 * H;
     float i = row[j], f = row[H + j], g = row[2 * H + j], o = row[3 * H + j];
     float dh = dy_post[tid] * mask_mul1(m, (uint64_t)(elem_off + tid), (uint64_t)n_total);
+    if (r) dh += r[tid];
     if (dh_rec) dh += dh_rec[tid] * mask_mul1_at(rm, (uint64_t)tid, (uint64_t)B * H);
     float tc = tanhf(c_t[tid]);
     float d_o = dh * tc;
@@ -68,10 +70,10 @@ __global__ void lstm_cell_bwd_tc_kernel(const float* __restrict__ dy_post, const
 
 int lstm_cell_bwd_tc(const float* dy_post, const float* dh_rec, float* dc, const float* gates, const float* c_t,
                      const float* c_prev, float* dG, __half* dG_h, int64_t ld_g, int B, int H, int64_t elem_off,
-                     int64_t n_total, MaskSrc m, MaskSrc rm, cudaStream_t s) {
+                     int64_t n_total, MaskSrc m, MaskSrc rm, cudaStream_t s, const float* r) {
     int64_t n = (int64_t)B * H;
     lstm_cell_bwd_tc_kernel<<<cdiv(n, 256), 256, 0, s>>>(dy_post, dh_rec, dc, gates, c_t, c_prev, dG, dG_h, ld_g, B, H,
-                                                         elem_off, n_total, m, rm);
+                                                         elem_off, n_total, m, rm, r);
     ZRB_KERNEL_CHECK();
     return ZRB_OK;
 }

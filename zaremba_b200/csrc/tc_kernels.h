@@ -20,7 +20,8 @@ int lstm_cell_fwd_tc(float* pre, const float* c_prev, float* c_out, float* h_raw
                      int64_t ld_h, int B, int H, int64_t elem_off, int64_t n_total, MaskSrc m, MaskSrc rm, cudaStream_t s);
 int lstm_cell_bwd_tc(const float* dy_post, const float* dh_rec, float* dc, const float* gates, const float* c_t,
                      const float* c_prev, float* dG, __half* dG_h, int64_t ld_g, int B, int H, int64_t elem_off,
-                     int64_t n_total, MaskSrc m, MaskSrc rm, cudaStream_t s);
+                     int64_t n_total, MaskSrc m, MaskSrc rm, cudaStream_t s, const float* r = nullptr);
+// r [B,H] (or null): the AR/TAR gradient of this step (DESIGN.md section 17), added to dh after the output mask
 
 // ---- persistent recurrence (lstm_rec_fwd.cu / lstm_rec_bwd.cu) ---------------------------------------
 struct RecPlan {
@@ -106,7 +107,8 @@ int lstm_rec_bwd(const RecPlan& p, const RecWatchdog& wd, const __half* w_img, _
                  const float* cst, const float* c0, __half* dG_h, unsigned int* counter, unsigned int counter_base, int T,
                  int B, int H, int G4p, MaskSrc m, MaskSrc rm, cudaStream_t s, long long* trace = nullptr, float* db1 = nullptr,
                  float* db2 = nullptr,    // db1 / db2: bias gradients sum_{t,b} dG [4H] written by the kernel (or null)
-                 unsigned int* resident_flag = nullptr, unsigned int resident_value = 0, float* db_scratch = nullptr);
+                 unsigned int* resident_flag = nullptr, unsigned int resident_value = 0, float* db_scratch = nullptr,
+                 const float* r = nullptr);   // r [N,H] or null: the AR/TAR gradient, added to dh after the output mask
 // resident_flag: CTA 0 stores resident_value there once every CTA of the grid has arrived at the first grid barrier,
 // i.e. the whole persistent grid holds its SMs: a stream gated on it (cuStreamWaitValue32) can then start work that
 // must only take the SMs this kernel leaves free (the data-parallel bucket all-reduce).

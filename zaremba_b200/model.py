@@ -138,16 +138,25 @@ class Model(nn.Module):
     W_hh * mask / (1 - p) at every time step; the gradient reaching `weight_hh_l0` is masked alike.  Eval mode uses the
     raw W_hh.  The masks are seeded by `torch.initial_seed()` when the library context is created (no rank in it: every
     data-parallel rank draws the same mask).  Not with lstm_type "custom".
+
+    Extra keyword `embed_dropout`: embedding dropout (Merity et al. 2018; DESIGN.md section 17), whole word types
+    dropped with this p.  In train mode each forward draws one keep flag per vocabulary row and gathers the kept rows
+    of `embed.W` scaled by 1 / (1 - p), before the dropout after the embedding; the gradient reaching `embed.W` is
+    masked alike.  Tied: only the lookup is masked, the projection uses the raw matrix.  Eval mode, `generate` and
+    `beam_search` use the raw rows.  Seeded like `weight_drop` (no rank in it).
     """
 
     def __init__(self, vocab_size, hidden_size, layer_num, dropout, winit, lstm_type="pytorch", engine="tc",
-                 variational=False, recurrent_dropout=None, *, tied=False, weight_drop=0.0):
+                 variational=False, recurrent_dropout=None, *, tied=False, weight_drop=0.0, embed_dropout=0.0):
         super().__init__()
         if lstm_type not in ("pytorch", "custom"):
             raise ValueError(f"lstm_type must be 'pytorch' or 'custom', got {lstm_type!r}")
         if isinstance(weight_drop, bool) or not isinstance(weight_drop, (int, float)) or \
                 not 0.0 <= float(weight_drop) < 1.0:
             raise ValueError(f"weight_drop must be a number in [0, 1), got {weight_drop!r}")
+        if isinstance(embed_dropout, bool) or not isinstance(embed_dropout, (int, float)) or \
+                not 0.0 <= float(embed_dropout) < 1.0:
+            raise ValueError(f"embed_dropout must be a number in [0, 1), got {embed_dropout!r}")
         if weight_drop and lstm_type == "custom":
             raise ValueError("weight_drop applies to lstm_type 'pytorch' only")
         if variational not in (False, True):
@@ -172,6 +181,7 @@ class Model(nn.Module):
         self.p_rec = p_rec
         self.tied = tied
         self.weight_drop = float(weight_drop)
+        self.embed_dropout = float(embed_dropout)
         self.embed = Embed(vocab_size, hidden_size)
         self.rnns = nn.ModuleList(LSTM(hidden_size, hidden_size, lstm_type) for _ in range(layer_num))
         self.fc = Linear(hidden_size, vocab_size)
@@ -397,6 +407,8 @@ class Model(nn.Module):
             _lib.check(lib.zrb_set_variational_dropout(h, 1, self.p_rec))
         if self.weight_drop:
             _lib.check(lib.zrb_set_weight_drop(h, self.weight_drop, int(torch.initial_seed()) & 0xFFFFFFFFFFFFFFFF))
+        if self.embed_dropout:
+            _lib.check(lib.zrb_set_embed_dropout(h, self.embed_dropout, int(torch.initial_seed()) & 0xFFFFFFFFFFFFFFFF))
         if self._explicit_masks is not None:
             self._push_masks()
         return self._ctx

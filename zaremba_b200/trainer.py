@@ -65,7 +65,8 @@ class _SideStream:
 
 class Trainer:
     def __init__(self, model: Model, batch_size: int, seq_length: int, process_group=None,
-                 keep_clipped_grads: bool = False, data_parallel: bool = True, lazy_update: bool = False):
+                 keep_clipped_grads: bool = False, data_parallel: bool = True, lazy_update: bool = False, *,
+                 ar: float = 0.0, tar: float = 0.0):
         """lazy_update: let the SGD update of the upper layers' matrices and of fc.W (HBM-bound, no consumer until the
         next forward reaches them) run beside the NEXT step's forward recurrence kernels instead of at the end of this
         step (zrb_set_lazy_update).  Same arithmetic; every Trainer entry point that reads parameters applies what is
@@ -77,7 +78,16 @@ class Trainer:
         BASELINE configs[4]: one model per GPU, no gradient exchange).
         keep_clipped_grads: after a step `.grad` holds coef * g as clip_grad_norm_ (main.py:115) leaves it.  The
         default skips that store (the values are dead: the next step overwrites them) and `.grad` keeps the raw
-        gradients of the step; weights, loss and norm are the same either way."""
+        gradients of the step; weights, loss and norm are the same either way.
+        ar / tar (keyword only): AWD-LSTM's activation regularization (Merity et al. 2018; DESIGN.md section 17), alpha
+        and beta >= 0.  Every fused train step adds alpha/(T*H) * sum(y^2) over the last layer's dropped output y and
+        beta/((T-1)*H) * sum((h_t - h_{t-1})^2) over its raw output h (AWD's main.py terms, times B) to the loss it
+        differentiates; the clip norm and `.grad` include their gradient.  The returned loss stays the NLL;
+        `activation_reg` holds the two penalty values of the last step.  Eval calls ignore them."""
+        for name, v in (("ar", ar), ("tar", tar)):
+            if isinstance(v, bool) or not isinstance(v, (int, float)) or not math.isfinite(v) or v < 0:
+                raise ValueError(f"{name} must be a finite number >= 0, got {v!r}")
+        self._ar, self._tar = float(ar), float(tar)
         if model.lstm_type != "pytorch":
             raise ValueError("Trainer drives the --lstm_type pytorch layout")
         dev = model.embed.W.device
@@ -129,6 +139,7 @@ class Trainer:
         self._st, self._keep_s = model._states_struct(self.states)
         self.loss = torch.zeros((), device=dev)
         self.norm = torch.zeros((), device=dev)
+        self._reg = torch.zeros(2, device=dev)
         self.tgt_prob = torch.zeros(batch_size * seq_length, device=dev)
         self._hx = torch.empty(seq_length, batch_size, dtype=torch.int64).pin_memory()
         self._hy = torch.empty(seq_length, batch_size, dtype=torch.int64).pin_memory()
@@ -250,8 +261,16 @@ class Trainer:
             _lib.check(_lib.load().zrb_set_embed_sparse(c, int(getattr(self, "_embed_sparse", 0))))
             _lib.check(_lib.load().zrb_set_keep_clipped_grads(c, 1 if self._keep_clipped else 0))
             _lib.check(_lib.load().zrb_set_lazy_update(c, 1 if getattr(self, "_lazy", False) else 0))
+            _lib.check(_lib.load().zrb_set_activation_reg(c, self._ar, self._tar))
             self._ctx_cached = c.value
         return c
+
+    @property
+    def activation_reg(self):
+        """CUDA tensor [2]: the alpha-weighted AR and beta-weighted TAR values of the last train step (zeros while both
+        are off), copied on the Trainer's stream without a host synchronisation."""
+        _lib.check(_lib.load().zrb_activation_reg(self.ctx, _lib.ptr(self._reg), self._stream()))
+        return self._reg
 
     def flush(self):
         """Apply weight updates deferred by `lazy_update` now (no-op otherwise).  Call before reading parameter tensors
