@@ -49,17 +49,15 @@ struct SwapRule : NoTileRule {
 };
 
 int update_pack_avg(float* p, float* g, float* a, float mu, bool first, int rows, int cols, float lr,
-                    const float* scalars, __half* row_img, int64_t ld, __half* fwd_img, const RecPlan* fp,
-                    __half* bwd_img, const RecPlan* bp, bool write_g, cudaStream_t s, bool pdl) {
+                    const float* scalars, const WeightImages& img, bool write_g, cudaStream_t s, bool pdl) {
     AvgRule rule;
     rule.lr = lr; rule.scalars = scalars; rule.coef = 0.f;
     rule.a = a; rule.mu = mu; rule.first = first ? 1 : 0;
-    return update_pack_rule(p, g, rows, cols, rule, (uintptr_t)a, row_img, ld, fwd_img, fp, bwd_img, bp, write_g, s, pdl);
+    return update_pack_rule(p, g, rows, cols, rule, (uintptr_t)a, img, write_g, s, pdl);
 }
 
-int swap_pack(float* p, float* a, int rows, int cols, __half* row_img, int64_t ld, __half* fwd_img, const RecPlan* fp,
-              __half* bwd_img, const RecPlan* bp, cudaStream_t s) {
-    return update_pack_rule(p, a, rows, cols, SwapRule{}, 0, row_img, ld, fwd_img, fp, bwd_img, bp, true, s, false);
+int swap_pack(float* p, float* a, int rows, int cols, const WeightImages& img, cudaStream_t s) {
+    return update_pack_rule(p, a, rows, cols, SwapRule{}, 0, img, true, s, false);
 }
 
 // ---- tensors without an fp16 image (and every tensor on the validation engine / the unaligned fallback) ------------

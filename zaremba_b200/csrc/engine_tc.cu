@@ -89,6 +89,30 @@ struct zrb_tc_state {
         uint64_t seed = 0, step = 0;
         float p = 0.f;
     } whh_img[ZRB_MAX_LAYERS];
+
+    // ---- which fp16 images each weight matrix has: what a pack or a fused update of it must write -------------------
+    zrb::WeightImages row_image(__half* img) const {
+        zrb::WeightImages w;
+        w.row = img; w.ld = Hp;
+        return w;
+    }
+    zrb::WeightImages w_ih_images(int l) const { return row_image(w_ih_h[l]); }
+    zrb::WeightImages fc_w_images() const { return row_image(fc_w_h); }
+    // both recurrences run in the persistent kernels: fplan.ok && bplan.ok, and bplan.ok implies fplan.ok (tc_ctx_init
+    // clears bplan.ok when the forward plan is off)
+    bool persistent() const { return bplan.ok; }
+    // W_hh of layer l, recording what its images will hold.  kWhhStale asks for no image: the caller changes p and leaves
+    // the images behind it.  Otherwise the slices of each persistent kernel in use, and the row image only where it is
+    // read, on the per-timestep path.  row_too: the row image regardless.
+    zrb::WeightImages w_hh_images(int l, const WhhImage& holds, bool row_too = false) {
+        whh_img[l] = holds;
+        zrb::WeightImages w = row_image(nullptr);
+        if (holds.kind == kWhhStale) return w;
+        if (row_too || !persistent()) w.row = w_hh_h[l];
+        w.fwd = fplan.ok ? w_img_f[l] : nullptr; w.fplan = &fplan;
+        w.bwd = bplan.ok ? w_img_b[l] : nullptr; w.bplan = &bplan;
+        return w;
+    }
 };
 
 namespace zrb {
@@ -203,13 +227,12 @@ static bool whh_current(const zrb_ctx* c, int l) {
 // build layer l's W_hh images from W with the mask the call needs; row_image: also the row image w_hh_h when the
 // persistent kernels do not need it (it is read only on the per-timestep path)
 static int tc_pack_whh(zrb_ctx* c, const float* W, int l, bool row_image, cudaStream_t s) {
-    zrb_tc_state* t = c->tc;
     const int H = c->cfg.hidden;
     const MaskSrc m = wd_mask(c, l);
-    if (row_image || !t->bplan.ok) ZRB_TRY(convert_pad_f16(W, H, t->w_hh_h[l], t->Hp, 4 * H, H, 1.f, s, m));
-    if (t->fplan.ok) ZRB_TRY(pack_whh_fwd(W, t->w_img_f[l], H, t->fplan, s, m));
-    if (t->bplan.ok) ZRB_TRY(pack_whh_bwd(W, t->w_img_b[l], H, t->bplan, s, m));
-    t->whh_img[l] = whh_wanted(c, l);
+    const WeightImages w = c->tc->w_hh_images(l, whh_wanted(c, l), row_image);
+    if (w.row) ZRB_TRY(convert_pad_f16(W, H, w.row, w.ld, 4 * H, H, 1.f, s, m));
+    if (w.fwd) ZRB_TRY(pack_whh_fwd(W, w.fwd, H, *w.fplan, s, m));
+    if (w.bwd) ZRB_TRY(pack_whh_bwd(W, w.bwd, H, *w.bplan, s, m));
     return ZRB_OK;
 }
 
@@ -229,55 +252,86 @@ static int tc_pack_weights(zrb_ctx* c, const zrb_params* p, cudaStream_t s) {
     return ZRB_OK;
 }
 
-// the train step's update of one matrix: update_pack, or with iterate averaging on (avg non-null) update_pack_avg,
-// which also averages the new p into a (DESIGN.md section 16)
-static int tc_update_pack(zrb_ctx* c, const AvgStep* avg, float* a, float* p, float* g, int rows, int cols, float lr,
-                          __half* row_img, __half* fwd_img, const RecPlan* fp, __half* bwd_img, const RecPlan* bp,
-                          bool pdl, cudaStream_t s) {
-    const int64_t ld = c->tc->Hp;
-    if (!avg)
-        return update_pack(p, g, rows, cols, lr, c->scalars, row_img, ld, fwd_img, fp, bwd_img, bp, c->keep_clipped, s,
-                           pdl);
-    return update_pack_avg(p, g, a, avg->mu, avg->first, rows, cols, lr, c->scalars, row_img, ld, fwd_img, fp, bwd_img,
-                           bp, c->keep_clipped, s, pdl);
+// One weight matrix of a param_list()-ordered TensorList: its index there, its shape, and the lazy-update item it belongs
+// to (layer l, or L for fc.W; see zrb_tc_state::upd_pending).
+struct WeightMatrix {
+    int i, rows, cols, item;
+    enum { kWih, kWhh, kFcW } kind;
+};
+struct WeightMatrices {
+    WeightMatrix m[2 * ZRB_MAX_LAYERS + 1];
+    int n = 0;
+    const WeightMatrix* begin() const { return m; }
+    const WeightMatrix* end() const { return m + n; }
+    const WeightMatrix& fc_w() const { return m[n - 1]; }
+};
+// The matrices in the order the update launches them: W_ih then W_hh per layer, then fc.W.  This is the one place that
+// knows where param_list() (api.cu) puts them: embed, (w_ih, w_hh, b_ih, b_hh) x L, fc_w, fc_b (tied: embed has n = 0,
+// E is fc_w).
+static WeightMatrices tc_matrices(const zrb_ctx* c) {
+    const int H = c->cfg.hidden, L = c->cfg.layers, V = c->cfg.vocab;
+    WeightMatrices ms;
+    for (int l = 0; l < L; ++l) {
+        ms.m[ms.n++] = {1 + 4 * l, 4 * H, H, l, WeightMatrix::kWih};
+        ms.m[ms.n++] = {2 + 4 * l, 4 * H, H, l, WeightMatrix::kWhh};
+    }
+    ms.m[ms.n++] = {1 + 4 * L, V, H, L, WeightMatrix::kFcW};
+    return ms;
+}
+// the images a fused update of m writes; whh: what W_hh's will hold afterwards (zrb_tc_state::w_hh_images)
+static WeightImages tc_images(zrb_ctx* c, const WeightMatrix& m, const zrb_tc_state::WhhImage& whh) {
+    if (m.kind == WeightMatrix::kWhh) return c->tc->w_hh_images(m.item, whh);
+    return m.kind == WeightMatrix::kWih ? c->tc->w_ih_images(m.item) : c->tc->fc_w_images();
+}
+// tl for the list kernels once the tile kernels have taken the matrices: their lengths set to 0, which every list
+// kernel skips
+static TensorList tc_without_matrices(const zrb_ctx* c, const TensorList& tl) {
+    TensorList rest = tl;
+    for (const WeightMatrix& m : tc_matrices(c)) rest.n[m.i] = 0;
+    return rest;
+}
+// every pointer the tile kernels would stream is 4-byte aligned (they pick 16 / 8 / 4-byte accesses from the matrix
+// width and the alignment); x1, x2: further per-tensor streams in tl's order, or null
+static bool tc_streams_aligned(const TensorList& tl, float* const* x1 = nullptr, float* const* x2 = nullptr) {
+    uintptr_t all = 0;
+    for (int i = 0; i < tl.count; ++i)
+        all |= (uintptr_t)tl.p[i] | (uintptr_t)tl.g[i] | (x1 ? (uintptr_t)x1[i] : 0) | (x2 ? (uintptr_t)x2[i] : 0);
+    return (all & 3) == 0;
+}
+// after a fused update of every matrix (applied or pending): the images are current, the next forward needs no pack
+static void tc_images_current(zrb_ctx* c, const zrb_params* p) {
+    zrb_tc_state* t = c->tc;
+    t->wg_ok = false;
+    c->weights_version++;
+    t->packed_version = c->weights_version;
+    t->packed_params = *p;
 }
 
-// the SGD update of layer l's W_hh.  Outside the weight-drop mode it rebuilds the layer's fp16 images from registers (the
-// next forward needs no pack); in it, it updates p (and g) only, and the next forward packs the images with its own mask.
-static int tc_update_whh(zrb_ctx* c, int l, float* p, float* g, float lr, const AvgStep* avg, float* a, bool pdl,
-                         cudaStream_t s) {
-    zrb_tc_state* t = c->tc;
-    const int H = c->cfg.hidden;
-    if (c->p_wd > 0.f) {
-        t->whh_img[l].kind = zrb_tc_state::kWhhStale;
-        return tc_update_pack(c, avg, a, p, g, 4 * H, H, lr, nullptr, nullptr, &t->fplan, nullptr, &t->bplan, pdl, s);
-    }
-    const bool persistent = t->fplan.ok && t->bplan.ok;
-    t->whh_img[l] = zrb_tc_state::WhhImage{};
-    return tc_update_pack(c, avg, a, p, g, 4 * H, H, lr, persistent ? nullptr : t->w_hh_h[l],
-                          t->fplan.ok ? t->w_img_f[l] : nullptr, &t->fplan, t->bplan.ok ? t->w_img_b[l] : nullptr,
-                          &t->bplan, pdl, s);
+// The train step's update of one matrix: update_pack, or with iterate averaging on (avg non-null) update_pack_avg,
+// which also averages the new p into a (DESIGN.md section 16).  Both rebuild the matrix's fp16 images from registers, so
+// the next forward needs no pack.  The exception is W_hh in the weight-drop mode: p (and g) only, and the next forward
+// packs the images with its own mask.
+static int tc_update_matrix(zrb_ctx* c, const WeightMatrix& m, const TensorList& tl, float lr, const AvgStep* avg,
+                            bool pdl, cudaStream_t s) {
+    zrb_tc_state::WhhImage whh;
+    if (c->p_wd > 0.f) whh.kind = zrb_tc_state::kWhhStale;
+    const WeightImages img = tc_images(c, m, whh);
+    float *p = tl.p[m.i], *g = tl.g[m.i];
+    if (!avg) return update_pack(p, g, m.rows, m.cols, lr, c->scalars, img, c->keep_clipped, s, pdl);
+    return update_pack_avg(p, g, avg->a[m.i], avg->mu, avg->first, m.rows, m.cols, lr, c->scalars, img, c->keep_clipped,
+                           s, pdl);
 }
 
 // apply deferred update item `item` (see zrb_tc_state::upd_pending); pdl: as a programmatic dependent of the forward
 // recurrence kernel just enqueued on `s`
 static int tc_issue_update(zrb_ctx* c, int item, bool pdl, cudaStream_t s) {
     zrb_tc_state* t = c->tc;
-    const int H = c->cfg.hidden, L = c->cfg.layers, V = c->cfg.vocab;
     if (!(t->upd_pending & (1u << item))) return ZRB_OK;
     t->upd_pending &= ~(1u << item);
-    const TensorList& tl = t->upd_tl;
     const AvgStep* avg = t->upd_avg_on ? &t->upd_avg : nullptr;
-    float* const* a = t->upd_avg.a;
-    if (item < L) {
-        const int l = item, b = 1 + 4 * l;
-        ZRB_TRY(tc_update_pack(c, avg, a[b], tl.p[b], tl.g[b], 4 * H, H, t->upd_lr, t->w_ih_h[l], nullptr, nullptr,
-                               nullptr, nullptr, pdl, s));
-        return tc_update_whh(c, l, tl.p[b + 1], tl.g[b + 1], t->upd_lr, avg, a[b + 1], pdl, s);
-    }
-    const int f = 1 + 4 * L;
-    return tc_update_pack(c, avg, a[f], tl.p[f], tl.g[f], V, H, t->upd_lr, t->fc_w_h, nullptr, nullptr, nullptr, nullptr,
-                          pdl, s);
+    for (const WeightMatrix& m : tc_matrices(c))
+        if (m.item == item) ZRB_TRY(tc_update_matrix(c, m, t->upd_tl, t->upd_lr, avg, pdl, s));
+    return ZRB_OK;
 }
 
 int tc_flush_updates(zrb_ctx* c, cudaStream_t s) {
@@ -315,7 +369,7 @@ int tc_forward(zrb_ctx* c, const zrb_params* p, const int64_t* x, const zrb_stat
         // recurrence, before the projection reads fc_w_h
         const bool through = ride && c->tied && (t->upd_pending & (1u << L));
         ZRB_TRY(embed_dropout_fwd(p->embed_w, x, nullptr, t->x_h[0], Hp, N, H, V, site_mask(c, 0), ed_mask(c), s,
-                                  through ? t->upd_tl.g[1 + 4 * L] : nullptr, t->upd_lr, c->scalars));
+                                  through ? t->upd_tl.g[tc_matrices(c).fc_w().i] : nullptr, t->upd_lr, c->scalars));
     }
     for (int l = 0; l < L; ++l) {
         float* G = c->gates[l];
@@ -548,14 +602,18 @@ int tc_backward(zrb_ctx* c, const zrb_params* p, const float* dscores, const zrb
     return tc_backward_from_image(c, p, g, s);
 }
 
-int tc_train_step_grads(zrb_ctx* c, const zrb_params* p, const zrb_params* g, const int64_t* x, const int64_t* y,
-                        int T, int B, const zrb_states* in, const zrb_states* out, uint64_t seed, uint64_t step,
-                        float* loss, cudaStream_t s) {
-    c->T = T; c->B = B; c->train = 1; c->seed = seed; c->step = step;
+// The first half of a fused gradient step: the forward over the window, the loss, and the scaled fp16 image of dscores
+// in dS_h.  train = 1: dropout on with the masks of (seed, step), pending lazy updates ride beside the forward
+// recurrences, and AR / TAR is computed when it is on; train = 0: the eval-mode loss.
+static int tc_step_forward(zrb_ctx* c, const zrb_params* p, const int64_t* x, const int64_t* y, int T, int B,
+                           const zrb_states* in, const zrb_states* out, int train, uint64_t seed, uint64_t step,
+                           float* loss, cudaStream_t s) {
+    c->T = T; c->B = B; c->train = train; c->seed = seed; c->step = step;
     c->have_fwd = false;
-    c->tc->in_train_step = true;
+    c->reg_use = false;
+    c->tc->in_train_step = train != 0;
     const int frc = tc_forward(c, p, x, in, out, c->scores, s);
-    c->tc->in_train_step = false;
+    c->tc->in_train_step = false;   // before the return code is tested: a failed forward must not leave it set
     ZRB_TRY(frc);
     c->have_fwd = true;
     {
@@ -563,26 +621,24 @@ int tc_train_step_grads(zrb_ctx* c, const zrb_params* p, const zrb_params* g, co
         ZRB_TRY(softmax_nll(c->scores, y, T * B, c->cfg.vocab, B, c->row_loss, loss, nullptr, nullptr, s, c->tc->dS_h,
                             c->tc->Vp, kGradScale));
     }
-    c->reg_use = false;
-    if (reg_on(c)) ZRB_TRY(reg_compute(c, s));   // AR / TAR: between the softmax and the projection's backward
+    if (train && reg_on(c)) ZRB_TRY(reg_compute(c, s));   // AR / TAR: between the softmax and the projection's backward
+    return ZRB_OK;
+}
+
+int tc_train_step_grads(zrb_ctx* c, const zrb_params* p, const zrb_params* g, const int64_t* x, const int64_t* y,
+                        int T, int B, const zrb_states* in, const zrb_states* out, uint64_t seed, uint64_t step,
+                        float* loss, cudaStream_t s) {
+    ZRB_TRY(tc_step_forward(c, p, x, y, T, B, in, out, 1, seed, step, loss, s));
     return tc_backward_from_image(c, p, g, s);
 }
 
 // the gradient of the eval-mode loss (DESIGN.md section 14): the fused gradient path with c->train = 0, so that every
 // site_mask / rec_mask is off while tc_forward still keeps the activations; pending lazy updates are applied first (the
-// forward runs outside a train step).  No clip norm follows, so the wgrad epilogues write no sum-of-squares slots.
+// forward runs outside a train step), and the loss has no AR / TAR.  No clip norm follows, so the wgrad epilogues write
+// no sum-of-squares slots.
 int tc_eval_grads(zrb_ctx* c, const zrb_params* p, const zrb_params* g, const int64_t* x, const int64_t* y, int T, int B,
                   const zrb_states* in, const zrb_states* out, float* loss, cudaStream_t s) {
-    c->T = T; c->B = B; c->train = 0; c->seed = 0; c->step = 0;
-    c->have_fwd = false;
-    c->reg_use = false;   // the eval-mode loss has no AR / TAR
-    ZRB_TRY(tc_forward(c, p, x, in, out, c->scores, s));
-    c->have_fwd = true;
-    {
-        ProfScope ps(c, ZRB_PROF_SOFTMAX, s);
-        ZRB_TRY(softmax_nll(c->scores, y, T * B, c->cfg.vocab, B, c->row_loss, loss, nullptr, nullptr, s, c->tc->dS_h,
-                            c->tc->Vp, kGradScale));
-    }
+    ZRB_TRY(tc_step_forward(c, p, x, y, T, B, in, out, 0, 0, 0, loss, s));
     const bool fused = c->fused_norm;
     c->fused_norm = false;
     const int rc = tc_backward_from_image(c, p, g, s);
@@ -594,20 +650,7 @@ int tc_eval_grads(zrb_ctx* c, const zrb_params* p, const zrb_params* g, const in
 int tc_train_step_begin(zrb_ctx* c, const zrb_params* p, const zrb_params* g, const int64_t* x, const int64_t* y,
                         int T, int B, const zrb_states* in, const zrb_states* out, uint64_t seed, uint64_t step,
                         float* loss, cudaStream_t s) {
-    c->T = T; c->B = B; c->train = 1; c->seed = seed; c->step = step;
-    c->have_fwd = false;
-    c->tc->in_train_step = true;
-    const int frc = tc_forward(c, p, x, in, out, c->scores, s);
-    c->tc->in_train_step = false;
-    ZRB_TRY(frc);
-    c->have_fwd = true;
-    {
-        ProfScope ps(c, ZRB_PROF_SOFTMAX, s);
-        ZRB_TRY(softmax_nll(c->scores, y, T * B, c->cfg.vocab, B, c->row_loss, loss, nullptr, nullptr, s, c->tc->dS_h,
-                            c->tc->Vp, kGradScale));
-    }
-    c->reg_use = false;
-    if (reg_on(c)) ZRB_TRY(reg_compute(c, s));   // AR / TAR: between the softmax and the projection's backward
+    ZRB_TRY(tc_step_forward(c, p, x, y, T, B, in, out, 1, seed, step, loss, s));
     c->tc->defer_wgrad = false;   // phased backward: every bucket is complete when its call returns
     return tc_backward_head(c, p, g, s);
 }
@@ -701,13 +744,10 @@ int tc_rec_trace(zrb_ctx* c, long long* h_out, int max_entries) {
 int tc_update(zrb_ctx* c, const zrb_params* p, const TensorList& tl, float lr, float max_norm, float* norm_out,
               const AvgStep* avg, cudaStream_t s) {
     zrb_tc_state* t = c->tc;
-    const int H = c->cfg.hidden, L = c->cfg.layers, V = c->cfg.vocab;
+    const int H = c->cfg.hidden, V = c->cfg.vocab;
     ZRB_TRY(tc_flush_updates(c, s));   // (a second update without a forward in between)
-    bool fuse = true;   // update_pack picks 16 / 8 / 4-byte accesses from the matrix width and alignment
-    for (int i = 0; i < tl.count && fuse; ++i)
-        fuse = ((((uintptr_t)tl.p[i]) | ((uintptr_t)tl.g[i]) | (avg ? (uintptr_t)avg->a[i] : 0)) & 3) == 0;
     ProfScope ps(c, ZRB_PROF_CLIP_SGD, s);
-    if (!fuse) {
+    if (!tc_streams_aligned(tl, avg ? avg->a : nullptr)) {   // images rebuilt by the next forward's pack
         if (avg) {
             ZRB_TRY(grad_norm(tl, max_norm, c->partials, c->scalars, norm_out, s));
             ZRB_TRY(sgd_avg_apply(tl, avg->a, lr, c->scalars, c->keep_clipped, avg->mu, avg->first, s));
@@ -717,25 +757,18 @@ int tc_update(zrb_ctx* c, const zrb_params* p, const TensorList& tl, float lr, f
         c->weights_version++;
         return ZRB_OK;
     }
-    // tensor order of param_list(): embed, (w_ih, w_hh, b_ih, b_hh) x L, fc_w, fc_b (tied: embed has n = 0, E is fc_w)
+    // rows_only: only the embedding rows of the last window can be non-zero -> norm and update over those rows
     const bool rows_only = !c->tied && c->emb_sparse && c->emb_prev_grad == tl.g[0] && c->emb_prev_n > 0;
-    const bool tied_gemm_norm = c->tied && t->wg_ok && t->wg_key == tl.g[1 + 4 * L];
-    if (tied_gemm_norm) {
-        // matrices from the wgrad epilogue slots (E's describe G_proj); the extra slots hold the merge's correction
-        // to dE (tc_backward_layer): no read of the matrices' gradients
-        TensorList dense = tl;
-        for (int l = 0; l < L; ++l) dense.n[1 + 4 * l] = dense.n[2 + 4 * l] = 0;
-        dense.n[1 + 4 * L] = 0;
+    // gemm_norm: the matrices' sums of squares are in the wgrad epilogue slots: no read of their gradients
+    const bool gemm_norm = t->wg_ok && t->wg_key == tl.g[tc_matrices(c).fc_w().i];
+    TensorList rest = tc_without_matrices(c, tl);   // what the list kernel updates ...
+    if (rows_only) rest.n[0] = 0;
+    TensorList dense = gemm_norm ? rest : tl;       // ... and what the norm reads
+    if (rows_only) dense.n[0] = 0;
+    if (c->tied && gemm_norm) {
+        // E's slots describe G_proj; the extra slots hold the merge's correction to dE (tc_backward_layer)
         ZRB_TRY(grad_norm(dense, max_norm, c->partials, c->scalars, norm_out, s, true, t->wg_slots));
     } else if (rows_only) {
-        // embedding: only the rows of the last window can be non-zero -> norm and update over those rows
-        TensorList dense = tl;
-        dense.n[0] = 0;
-        const bool gemm_norm = t->wg_ok && t->wg_key == tl.g[1 + 4 * L];   // matrices: summed by the wgrad GEMMs
-        if (gemm_norm) {
-            for (int l = 0; l < L; ++l) dense.n[1 + 4 * l] = dense.n[2 + 4 * l] = 0;
-            dense.n[1 + 4 * L] = 0;
-        }
         ZRB_TRY(embed_first_table(c->emb_prev_ids, c->emb_first, c->emb_prev_n, V, s));
         ZRB_TRY(embed_rows_sumsq(tl.g[0], c->emb_prev_ids, c->emb_first, c->emb_prev_n, H, V,
                                  c->partials + norm_partials_base(), kNormExtra, s));   // one token per block
@@ -750,128 +783,58 @@ int tc_update(zrb_ctx* c, const zrb_params* p, const TensorList& tl, float lr, f
     } else {
         ZRB_TRY(grad_norm(tl, max_norm, c->partials, c->scalars, norm_out, s));
     }
-    TensorList rest;
-    rest.count = 0;
-    float* rest_a[16] = {};   // the averages of rest's tensors
-    auto push = [&](int i) {
-        rest.p[rest.count] = tl.p[i]; rest.g[rest.count] = tl.g[i]; rest.n[rest.count] = tl.n[i];
-        rest_a[rest.count] = avg ? avg->a[i] : nullptr;
-        rest.count++;
-    };
-    if (!rows_only) push(0);
-    const bool persistent = t->fplan.ok && t->bplan.ok;
     // lazy update: layer 0 (needed by the very next kernels) now; layers >= 1 and fc.W beside the forward recurrences of
     // the next step (tc_forward), or at the next call that is not a fused train step (tc_flush_updates)
-    const bool lazy = c->lazy_update && persistent && pdl_beside_rec(c);
+    const bool lazy = c->lazy_update && t->persistent() && pdl_beside_rec(c);
     if (lazy) {
         t->upd_tl = tl;
         t->upd_lr = lr;
         t->upd_avg_on = avg != nullptr;
         if (avg) t->upd_avg = *avg;
     }
-    for (int l = 0; l < L; ++l) {
-        const int b = 1 + 4 * l;
-        push(b + 2);
-        push(b + 3);
-        if (lazy && l >= 1) {
-            t->upd_pending |= 1u << l;
-            continue;
-        }
-        float* const a0 = avg ? avg->a[b] : nullptr;
-        float* const a1 = avg ? avg->a[b + 1] : nullptr;
-        ZRB_TRY(tc_update_pack(c, avg, a0, tl.p[b], tl.g[b], 4 * H, H, lr, t->w_ih_h[l], nullptr, nullptr, nullptr, nullptr,
-                               false, s));
-        ZRB_TRY(tc_update_whh(c, l, tl.p[b + 1], tl.g[b + 1], lr, avg, a1, false, s));
+    for (const WeightMatrix& m : tc_matrices(c)) {
+        if (lazy && m.item >= 1) t->upd_pending |= 1u << m.item;
+        else ZRB_TRY(tc_update_matrix(c, m, tl, lr, avg, false, s));
     }
-    const int f = 1 + 4 * L;
-    if (lazy) t->upd_pending |= 1u << L;
-    else ZRB_TRY(tc_update_pack(c, avg, avg ? avg->a[f] : nullptr, tl.p[f], tl.g[f], V, H, lr, t->fc_w_h, nullptr, nullptr,
-                                nullptr, nullptr, false, s));
-    push(f + 1);
-    if (avg) ZRB_TRY(sgd_avg_apply(rest, rest_a, lr, c->scalars, c->keep_clipped, avg->mu, avg->first, s));
+    if (avg) ZRB_TRY(sgd_avg_apply(rest, avg->a, lr, c->scalars, c->keep_clipped, avg->mu, avg->first, s));
     else ZRB_TRY(sgd_apply(rest, lr, c->scalars, c->keep_clipped, s));
-    t->wg_ok = false;
-    c->weights_version++;
-    t->packed_version = c->weights_version;      // images are current
-    t->packed_params = *p;
+    tc_images_current(c, p);
     return ZRB_OK;
 }
 
 // The dynamic-evaluation update (DESIGN.md section 14): tc_update's schedule with the dynamic rule, no norm and no lazy
-// deferral.  The matrices go through update_pack's kernels, which rebuild their fp16 images from registers; the rest
-// through the list kernel.  tg / r: theta_g and the RMS statistic in param_list() order (r null: the SGD rule).
+// deferral.  tg / r: theta_g and the RMS statistic in param_list() order (r null: the SGD rule).  The W_hh images then
+// hold the raw weights: evaluation applies no weight drop.
 int tc_dyneval_update(zrb_ctx* c, const zrb_params* p, const TensorList& tl, float* const* tg, float* const* r,
                       const DynArgs& a, cudaStream_t s) {
-    zrb_tc_state* t = c->tc;
-    const int H = c->cfg.hidden, L = c->cfg.layers, V = c->cfg.vocab;
     ZRB_TRY(tc_flush_updates(c, s));
     ProfScope ps(c, ZRB_PROF_CLIP_SGD, s);
-    bool fuse = true;
-    for (int i = 0; i < tl.count && fuse; ++i)
-        fuse = ((((uintptr_t)tl.p[i]) | ((uintptr_t)tl.g[i]) | ((uintptr_t)tg[i]) | (r ? (uintptr_t)r[i] : 0)) & 3) == 0;
-    if (!fuse) {   // images rebuilt by the next forward's pack
+    if (!tc_streams_aligned(tl, tg, r)) {   // images rebuilt by the next forward's pack
         ZRB_TRY(dyneval_apply(tl, tg, r, a, s));
         c->weights_version++;
         return ZRB_OK;
     }
-    TensorList rest = tl;   // entries with an image get length 0 here (skipped by the list kernel)
-    const bool persistent = t->fplan.ok && t->bplan.ok;
-    for (int l = 0; l < L; ++l) {
-        const int b = 1 + 4 * l;
-        ZRB_TRY(update_pack_dyn(tl.p[b], tl.g[b], tg[b], r ? r[b] : nullptr, 4 * H, H, a, t->w_ih_h[l], t->Hp, nullptr,
-                                nullptr, nullptr, nullptr, s));
-        ZRB_TRY(update_pack_dyn(tl.p[b + 1], tl.g[b + 1], tg[b + 1], r ? r[b + 1] : nullptr, 4 * H, H, a,
-                                persistent ? nullptr : t->w_hh_h[l], t->Hp, t->fplan.ok ? t->w_img_f[l] : nullptr,
-                                &t->fplan, t->bplan.ok ? t->w_img_b[l] : nullptr, &t->bplan, s));
-        t->whh_img[l] = zrb_tc_state::WhhImage{};   // the raw weights: evaluation applies no weight drop
-        rest.n[b] = rest.n[b + 1] = 0;
-    }
-    const int f = 1 + 4 * L;
-    ZRB_TRY(update_pack_dyn(tl.p[f], tl.g[f], tg[f], r ? r[f] : nullptr, V, H, a, t->fc_w_h, t->Hp, nullptr, nullptr,
-                            nullptr, nullptr, s));
-    rest.n[f] = 0;
-    ZRB_TRY(dyneval_apply(rest, tg, r, a, s));
-    t->wg_ok = false;
-    c->weights_version++;
-    t->packed_version = c->weights_version;      // images are current
-    t->packed_params = *p;
+    for (const WeightMatrix& m : tc_matrices(c))
+        ZRB_TRY(update_pack_dyn(tl.p[m.i], tl.g[m.i], tg[m.i], r ? r[m.i] : nullptr, m.rows, m.cols, a,
+                                tc_images(c, m, {}), s));
+    ZRB_TRY(dyneval_apply(tc_without_matrices(c, tl), tg, r, a, s));
+    tc_images_current(c, p);
     return ZRB_OK;
 }
 
 // Exchange the weights with their average (DESIGN.md section 16), tl = param_list() over p, a = the averages in its
-// order.  The matrices go through update_pack's kernels, which write the fp16 images of the weights now in p; the rest
-// through the list kernel.  The W_hh images then hold the raw weights, as after the dynamic-evaluation update.
+// order.  The W_hh images then hold the raw weights, as after the dynamic-evaluation update.
 int tc_swap_average(zrb_ctx* c, const zrb_params* p, const TensorList& tl, float* const* a, cudaStream_t s) {
-    zrb_tc_state* t = c->tc;
-    const int H = c->cfg.hidden, L = c->cfg.layers, V = c->cfg.vocab;
     ZRB_TRY(tc_flush_updates(c, s));
     ProfScope ps(c, ZRB_PROF_PACK, s);
-    bool fuse = true;
-    for (int i = 0; i < tl.count && fuse; ++i) fuse = ((((uintptr_t)tl.p[i]) | ((uintptr_t)a[i])) & 3) == 0;
-    if (!fuse) {   // images rebuilt by the next forward's pack
+    if (!tc_streams_aligned(tl, a)) {   // images rebuilt by the next forward's pack
         ZRB_TRY(swap_apply(tl, a, s));
         c->weights_version++;
         return ZRB_OK;
     }
-    TensorList rest = tl;   // entries with an image get length 0 here (skipped by the list kernel)
-    const bool persistent = t->fplan.ok && t->bplan.ok;
-    for (int l = 0; l < L; ++l) {
-        const int b = 1 + 4 * l;
-        ZRB_TRY(swap_pack(tl.p[b], a[b], 4 * H, H, t->w_ih_h[l], t->Hp, nullptr, nullptr, nullptr, nullptr, s));
-        ZRB_TRY(swap_pack(tl.p[b + 1], a[b + 1], 4 * H, H, persistent ? nullptr : t->w_hh_h[l], t->Hp,
-                          t->fplan.ok ? t->w_img_f[l] : nullptr, &t->fplan, t->bplan.ok ? t->w_img_b[l] : nullptr,
-                          &t->bplan, s));
-        t->whh_img[l] = zrb_tc_state::WhhImage{};
-        rest.n[b] = rest.n[b + 1] = 0;
-    }
-    const int f = 1 + 4 * L;
-    ZRB_TRY(swap_pack(tl.p[f], a[f], V, H, t->fc_w_h, t->Hp, nullptr, nullptr, nullptr, nullptr, s));
-    rest.n[f] = 0;
-    ZRB_TRY(swap_apply(rest, a, s));
-    t->wg_ok = false;
-    c->weights_version++;
-    t->packed_version = c->weights_version;      // images are current
-    t->packed_params = *p;
+    for (const WeightMatrix& m : tc_matrices(c)) ZRB_TRY(swap_pack(tl.p[m.i], a[m.i], m.rows, m.cols, tc_images(c, m, {}), s));
+    ZRB_TRY(swap_apply(tc_without_matrices(c, tl), a, s));
+    tc_images_current(c, p);
     return ZRB_OK;
 }
 

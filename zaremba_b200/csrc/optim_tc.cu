@@ -30,24 +30,22 @@ struct DynRule : NoTileRule {
     }
 };
 
-int update_pack(float* p, float* g, int rows, int cols, float lr, const float* scalars, __half* row_img, int64_t ld,
-                __half* fwd_img, const RecPlan* fp, __half* bwd_img, const RecPlan* bp, bool write_g, cudaStream_t s,
-                bool pdl) {
+int update_pack(float* p, float* g, int rows, int cols, float lr, const float* scalars, const WeightImages& img,
+                bool write_g, cudaStream_t s, bool pdl) {
     SgdRule rule;
     rule.lr = lr; rule.scalars = scalars; rule.coef = 0.f;
-    return update_pack_rule(p, g, rows, cols, rule, 0, row_img, ld, fwd_img, fp, bwd_img, bp, write_g, s, pdl);
+    return update_pack_rule(p, g, rows, cols, rule, 0, img, write_g, s, pdl);
 }
 
 int update_pack_dyn(float* p, float* g, const float* tg, const float* r, int rows, int cols, const DynArgs& a,
-                    __half* row_img, int64_t ld, __half* fwd_img, const RecPlan* fp, __half* bwd_img, const RecPlan* bp,
-                    cudaStream_t s) {
+                    const WeightImages& img, cudaStream_t s) {
     const uintptr_t align = ((uintptr_t)tg) | ((uintptr_t)r);
     if (a.rbar) {
         DynRule<true> rule{{}, tg, r, a, 0.f};
-        return update_pack_rule(p, g, rows, cols, rule, align, row_img, ld, fwd_img, fp, bwd_img, bp, false, s, false);
+        return update_pack_rule(p, g, rows, cols, rule, align, img, false, s, false);
     }
     DynRule<false> rule{{}, tg, nullptr, a, 0.f};
-    return update_pack_rule(p, g, rows, cols, rule, align, row_img, ld, fwd_img, fp, bwd_img, bp, false, s, false);
+    return update_pack_rule(p, g, rows, cols, rule, align, img, false, s, false);
 }
 
 }  // namespace zrb

@@ -84,23 +84,29 @@ struct FwdPrep {
     int L, B, H, Hp, GB, Kc, N;
 };
 int fwd_prep(const FwdPrep& a, cudaStream_t s);
+// The fp16 operand images of one weight matrix, as the fused update rewrites them from registers.  Default: no image.
+struct WeightImages {
+    __half* row = nullptr;           // [rows, ld] row-major image
+    int64_t ld = 0;
+    __half* fwd = nullptr;           // forward recurrent slices (pack_whh_fwd's layout) under fplan
+    const RecPlan* fplan = nullptr;
+    __half* bwd = nullptr;           // backward recurrent slices (pack_whh_bwd's layout) under bplan
+    const RecPlan* bplan = nullptr;
+};
 // SGD update of one matrix fused with its fp16 image rebuild (optim_tc.cu)
-int update_pack(float* p, float* g, int rows, int cols, float lr, const float* scalars, __half* row_img, int64_t ld,
-                __half* fwd_img, const RecPlan* fp, __half* bwd_img, const RecPlan* bp, bool write_g, cudaStream_t s,
+int update_pack(float* p, float* g, int rows, int cols, float lr, const float* scalars, const WeightImages& img,
+                bool write_g, cudaStream_t s,
                 bool pdl = false);   // pdl: programmatic dependent of the (forward recurrence) kernel enqueued before it
 // the same kernels with the dynamic-evaluation rule (dyneval_elem): theta_g tg and r at p's offsets (r unused under the
 // SGD rule, a.rbar null); g is read, never written; the same images
 int update_pack_dyn(float* p, float* g, const float* tg, const float* r, int rows, int cols, const DynArgs& a,
-                    __half* row_img, int64_t ld, __half* fwd_img, const RecPlan* fp, __half* bwd_img, const RecPlan* bp,
-                    cudaStream_t s);
+                    const WeightImages& img, cudaStream_t s);
 // iterate averaging (average_tc.cu, DESIGN.md section 16): update_pack's update, then a = first ? p : a + (p - a) * mu
 // over the new p in the same pass; the same images
 int update_pack_avg(float* p, float* g, float* a, float mu, bool first, int rows, int cols, float lr,
-                    const float* scalars, __half* row_img, int64_t ld, __half* fwd_img, const RecPlan* fp,
-                    __half* bwd_img, const RecPlan* bp, bool write_g, cudaStream_t s, bool pdl = false);
+                    const float* scalars, const WeightImages& img, bool write_g, cudaStream_t s, bool pdl = false);
 // exchange p and a, and write the images of the new p (update_pack's image stores)
-int swap_pack(float* p, float* a, int rows, int cols, __half* row_img, int64_t ld, __half* fwd_img, const RecPlan* fp,
-              __half* bwd_img, const RecPlan* bp, cudaStream_t s);
+int swap_pack(float* p, float* a, int rows, int cols, const WeightImages& img, cudaStream_t s);
 int rec_bwd_plan(int H, int B, RecPlan* plan);   // U = units per CTA, nCTA = 4 * clusters
 int pack_whh_bwd(const float* W, __half* img, int H, const RecPlan& p, cudaStream_t s, MaskSrc m = MaskSrc{});
 int lstm_rec_bwd(const RecPlan& p, const RecWatchdog& wd, const __half* w_img, __half* g_img, const float* dy, const float* gates,

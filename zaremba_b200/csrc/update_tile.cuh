@@ -321,18 +321,18 @@ static int update_pack_launch(float* p, float* g, int rows, int cols, const Rule
 
 // align: OR of every pointer the rule streams besides p and g (their alignment picks the access width too)
 template <class Rule>
-static int update_pack_rule(float* p, float* g, int rows, int cols, const Rule& rule, uintptr_t align, __half* row_img,
-                            int64_t ld, __half* fwd_img, const RecPlan* fp, __half* bwd_img, const RecPlan* bp,
-                            bool write_g, cudaStream_t s, bool pdl) {
+static int update_pack_rule(float* p, float* g, int rows, int cols, const Rule& rule, uintptr_t align,
+                            const WeightImages& img, bool write_g, cudaStream_t s, bool pdl) {
+    const RecPlan *fp = img.fplan, *bp = img.bplan;
     PackSpec sp;
     sp.write_g = write_g ? 1 : 0;
     sp.pdl = pdl ? 1 : 0;
-    sp.row_img = row_img; sp.ld = ld;
-    sp.fwd_img = fwd_img; sp.fKS = fp ? fp->KS : 1; sp.fU = fp ? fp->KS * fp->U : 1; sp.fG = fp ? fp->G : 1;
+    sp.row_img = img.row; sp.ld = img.ld;
+    sp.fwd_img = img.fwd; sp.fKS = fp ? fp->KS : 1; sp.fU = fp ? fp->KS * fp->U : 1; sp.fG = fp ? fp->G : 1;
     sp.fKc = fp ? fp->KcS : 1;
-    sp.bwd_img = bwd_img; sp.bS = bp ? bp->KS : 1; sp.bUC = bp ? 4 * bp->KS * bp->U : 4; sp.bG = bp ? bp->G : 1;
+    sp.bwd_img = img.bwd; sp.bS = bp ? bp->KS : 1; sp.bUC = bp ? 4 * bp->KS * bp->U : 4; sp.bG = bp ? bp->G : 1;
     sp.bKc = bp ? bp->KcS : 1;
-    const bool whh = (fwd_img || bwd_img) && rows == 4 * cols;
+    const bool whh = (img.fwd || img.bwd) && rows == 4 * cols;
     const uintptr_t all = ((uintptr_t)p) | ((uintptr_t)g) | align;
     const bool al16 = (all & 15) == 0, al8 = (all & 7) == 0;
     if (cols % 4 == 0 && al16) return update_pack_launch<4>(p, g, rows, cols, rule, sp, whh, s);
