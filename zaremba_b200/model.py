@@ -191,6 +191,8 @@ class Model(nn.Module):
         self.reset_parameters()
         self._ctx = None
         self._ctx_key = None
+        self._ctx_serial = 0           # contexts created so far
+        self._ctx_pinned = None        # what a re-created context would lose (a Trainer's average), or None
         self._fwd_id = 0
         self._drop_step = 0
         self._seed = None
@@ -221,6 +223,7 @@ class Model(nn.Module):
         if dev.type != "cuda":
             raise RuntimeError("zaremba_b200.Model runs on a CUDA device only (no CPU fallback): call .to('cuda')")
         x_dev = x.to(device=dev, dtype=torch.int64).contiguous()   # main.py hands CPU non-contiguous views
+        self._context(*x_dev.shape)    # a window the model cannot take raises before it consumes a dropout step
         weights = self._lib_weights()
         seed, step = self._next_dropout_key()
         need_grad = torch.is_grad_enabled() and any(w.requires_grad for w in weights)
@@ -245,8 +248,8 @@ class Model(nn.Module):
 
         Returns (tokens [n_new,B] int64, logprobs [n_new,B] fp32, states).  The returned states are those BEFORE the
         last token is consumed, so `generate(tokens[-1:], m, states, ..., seed=seed, pos=pos + n_new)` continues the
-        same stream.  The model's library context is reused, never replaced (that would drop a Trainer's pending
-        lazy updates): a B above its max_batch raises; a model without one gets a context for (min(T0, 64), B).
+        same stream.  The model's library context is reused, never replaced (a Trainer's context keeps the recurrence
+        plans of its own batch): a B above its max_batch raises; a model without one gets a context for (min(T0, 64), B).
         """
         dev = self.embed.W.device
         if dev.type != "cuda":
@@ -393,6 +396,14 @@ class Model(nn.Module):
             ok = self._ctx_key[2] == key[2] and self._ctx_key[0] >= T and self._ctx_key[1] >= B
             if ok:
                 return self._ctx
+            if self._ctx_pinned:
+                raise RuntimeError(f"a [T={T}, B={B}] window needs a larger library context than the model's "
+                                   f"[{self._ctx_key[0]}, {self._ctx_key[1]}], and re-creating it would lose "
+                                   f"{self._ctx_pinned}")
+            # the context holds a lazy Trainer's deferred weight updates: apply them before it goes
+            dev = self._ctx_key[2]
+            with torch.cuda.device(dev):
+                _lib.check(_lib.load().zrb_flush_updates(self._ctx, torch.cuda.current_stream(dev).cuda_stream))
             self._destroy_ctx()
         lib = _lib.load()
         cfg = _lib.ZrbConfig(self.vocab_size, self.hidden_size, self.layer_num, key[0], key[1],
@@ -402,6 +413,7 @@ class Model(nn.Module):
         with torch.cuda.device(self.embed.W.device):
             _lib.check(lib.zrb_ctx_create(C.byref(cfg), C.byref(h)))
         self._ctx, self._ctx_key = h, key
+        self._ctx_serial += 1          # a new context may reuse the old one's address: this tells them apart
         self._versions = None
         if self.variational:
             _lib.check(lib.zrb_set_variational_dropout(h, 1, self.p_rec))

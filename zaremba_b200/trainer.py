@@ -254,16 +254,28 @@ class Trainer:
     @property
     def ctx(self):
         """The model's library context (re-fetched every call: the model re-creates it when a larger window is
-        requested, and a fresh context must be told that the weights are new to it)."""
+        requested, and a fresh context must be told that the weights are new to it and get the Trainer's modes).  A
+        fresh context holds no average: one found while averaging is on stops the averaging and raises RuntimeError
+        (the model refuses to re-create its context while a Trainer averages, so only a context dropped some other
+        way gets here)."""
         c = self.model._context(self.T, self.B)
-        if self._ctx_cached is None or c.value != self._ctx_cached:
+        if self._ctx_cached != self.model._ctx_serial:
             _lib.check(_lib.load().zrb_params_changed(c))
             _lib.check(_lib.load().zrb_set_embed_sparse(c, int(getattr(self, "_embed_sparse", 0))))
             _lib.check(_lib.load().zrb_set_keep_clipped_grads(c, 1 if self._keep_clipped else 0))
             _lib.check(_lib.load().zrb_set_lazy_update(c, 1 if getattr(self, "_lazy", False) else 0))
             _lib.check(_lib.load().zrb_set_activation_reg(c, self._ar, self._tar))
-            self._ctx_cached = c.value
+            self._ctx_cached = self.model._ctx_serial
+            if getattr(self, "_averaging", False):
+                self._set_averaging(False)
+                raise RuntimeError("the model's library context was re-created while averaging was on: the average "
+                                   "stops here (flat_avg holds it as it was); call start_averaging() to restart")
         return c
+
+    def _set_averaging(self, on):
+        """Whether averaging is on; while it is, the model keeps its library context (the average's count lives there)."""
+        self._averaging = on
+        self.model._ctx_pinned = "the Trainer's running average (start_averaging)" if on else None
 
     @property
     def activation_reg(self):
@@ -486,12 +498,14 @@ class Trainer:
         self._avg_s = self._flat_params_struct(self.flat_avg)
         self.flush()
         _lib.check(_lib.load().zrb_set_average(self.ctx, C.byref(self._avg_s)))
+        self._set_averaging(True)
 
     def stop_averaging(self):
         """Stop averaging; `flat_avg` keeps the average so far."""
         self._check_not_swapped()
         self.flush()
         _lib.check(_lib.load().zrb_set_average(self.ctx, None))
+        self._set_averaging(False)
 
     @property
     def averaged_steps(self):
@@ -511,14 +525,25 @@ class Trainer:
         self.flush()
         self._check_versions()
         _lib.check(lib.zrb_swap_average(self.ctx, C.byref(self._ps), self._stream()))
+        serial = self.model._ctx_serial
         self._swapped = True
         try:
             yield self
         finally:
-            self.flush()
-            self._check_versions()
-            _lib.check(lib.zrb_swap_average(self.ctx, C.byref(self._ps), self._stream()))
-            self._swapped = False
+            if self.model._ctx is not None and self.model._ctx_serial == serial:
+                self.flush()
+                self._check_versions()
+                _lib.check(lib.zrb_swap_average(self.ctx, C.byref(self._ps), self._stream()))
+                self._swapped = False
+            else:
+                # the context was dropped inside the block and its successor holds no average to swap back: exchange
+                # the two buffers with copies, then have the weights repacked (which reports the lost average)
+                with torch.no_grad():
+                    trained = self.flat_avg.clone()
+                    self.flat_avg.copy_(self.flat_p)
+                    self.flat_p.copy_(trained)
+                self._swapped = False
+                self.params_changed()
 
     def average_state_dict(self):
         """The average as a state dict under the model's own keys (tied: embed.W and fc.W both, as state_dict()
@@ -561,7 +586,8 @@ class Trainer:
         the model re-create its context for the larger shape, and the Trainer then keeps running in that context, whose
         recurrence plans were chosen for the larger batch.  To keep the Trainer's own plans, compute such statistics on
         a Trainer of their shape: a `GradStats` serves every Trainer of the same model configuration (the flat layout
-        depends only on the model).  Returns a `GradStats`."""
+        depends only on the model).  While averaging is on (or inside averaged_weights()) larger windows raise
+        ValueError before anything changes: the average lives in the context.  Returns a `GradStats`."""
         from .dyneval import GradStats
         self._single_replica("gradient_stats")
         batches = list(batches)
@@ -572,6 +598,11 @@ class Trainer:
             raise ValueError(f"all statistics windows must have one batch size (got {sorted(Bs)})")
         B = Bs.pop()
         T = max(x.shape[0] for x, _ in batches)
+        T_ctx, B_ctx = self.model._ctx_key[:2]
+        if (T > T_ctx or B > B_ctx) and getattr(self, "_averaging", False):
+            raise ValueError(f"[T={T}, B={B}] windows need a larger library context than [{T_ctx}, {B_ctx}], and "
+                             "re-creating it would lose the running average: compute the statistics on a Trainer of "
+                             "their shape")
         lib = _lib.load()
         self.flush()
         self._check_versions()
