@@ -65,7 +65,9 @@ typedef struct {
 #define ZRB_TIED_EMBEDDING 1
 
 /* The 11 (= 3 + 4L) parameter tensors in the reference's registration order
- * (model.py:83-86; SURVEY 8b): fp32, row-major, contiguous. */
+ * (model.py:83-86; SURVEY 8b): fp32, row-major, contiguous.  Shapes for one width H; a context of per-layer widths
+ * (zrb_ctx_create_widths: embedding E, layer l of width H_l and input width In_l = E for l = 0, H_{l-1} after) takes
+ * embed_w [V,E], w_ih[l] [4H_l,In_l], w_hh[l] [4H_l,H_l], b_ih[l] / b_hh[l] [4H_l], fc_w [V,H_{L-1}]. */
 typedef struct {
     float* embed_w;                       /* [V,H]   embed.W              model.py:11 */
     float* w_ih[ZRB_MAX_LAYERS];          /* [4H,H]  rnns.l.weight_ih_l0  model.py:84 */
@@ -77,7 +79,7 @@ typedef struct {
 } zrb_params;
 
 /* (h, c) entering / leaving the BPTT window: model.py:94-98.  [B,H] fp32 each (the
- * pytorch path's [1,B,H] has the same bytes). */
+ * pytorch path's [1,B,H] has the same bytes); [B,H_l] for layer l of a context of per-layer widths. */
 typedef struct {
     float* h[ZRB_MAX_LAYERS];
     float* c[ZRB_MAX_LAYERS];
@@ -89,6 +91,16 @@ const char* zrb_version(void);
 int64_t     zrb_launch_count(void);
 
 int  zrb_ctx_create(const zrb_config* cfg, zrb_ctx** out);
+/* Layers of unequal width (AWD-LSTM's 400-1150-1150-400 model; DESIGN.md section 18): widths[0] = E, the embedding
+ * width, and widths[1 + l] = H_l, the width of layer l, for l < cfg->layers; cfg->hidden must be 0.  Layer l's input
+ * width is E (l = 0) or H_{l-1}; the projection reads H_{L-1}.  Every per-site rule takes its site's width: dropout
+ * site 0 is over E and site l+1 over H_l (element t*B*W + b*W + j; variational: b*W + j), recurrent site L+1+l over
+ * B*H_l, weight drop of layer l over 4*H_l*H_l, AR / TAR normalised by H_{L-1}, explicit masks [T*B*W] per site.  With
+ * every width equal to H this is zrb_ctx_create with cfg->hidden = H, bit for bit.  ZRB_E_INVALID for a width < 1,
+ * cfg->hidden != 0, a tied context with E != H_{L-1}, and ZRB_ENGINE_SIMT with unequal widths; zrb_lstm_layer_fwd /
+ * _bwd return ZRB_E_INVALID on a context of unequal widths.  The neural cache takes H = H_{L-1}.  zrb_ctx_create's
+ * other rules apply. */
+int  zrb_ctx_create_widths(const zrb_config* cfg, const int32_t* widths, zrb_ctx** out);
 void zrb_ctx_destroy(zrb_ctx* ctx);
 /* bytes of device memory the context holds */
 int64_t zrb_ctx_workspace_bytes(const zrb_ctx* ctx);
@@ -311,8 +323,11 @@ int  zrb_resident_flag(zrb_ctx* ctx, uint32_t** d_flag, uint32_t* next_value);
  * seven are then 0); KS = CTAs sharing one set of gate rows, each holding 1/KS of the contraction (K-split); U = hidden
  * units per CTA; G = 8-row groups of a CTA's weight slice; nCTA = grid size; GBi = 8-row batch groups of the operand
  * images (the MMA's N is 8 * GBi); Kc = 8-element chunks of the contraction; KcS = Kc / KS.  ZRB_E_INVALID for a
- * validation-engine context.  Host only, no synchronisation. */
+ * validation-engine context.  Host only, no synchronisation.  A context of per-layer widths plans every layer for its
+ * own width and reports layer 0 here; either direction runs persistent only when every layer's plan fits. */
 int  zrb_rec_plans(const zrb_ctx* ctx, int32_t* h_out);
+/* zrb_rec_plans for layer `layer` (0 <= layer < L, else ZRB_E_INVALID). */
+int  zrb_rec_plans_layer(const zrb_ctx* ctx, int32_t layer, int32_t* h_out);
 int  zrb_stream_wait_value32(void* stream, const uint32_t* d_flag, uint32_t value);
 
 /* perplexity's inner step (main.py:91-94) without materialising scores for the caller:

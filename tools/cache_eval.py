@@ -91,7 +91,7 @@ out = {"checkpoint": os.path.basename(args.checkpoint), "hidden": H, "layers": L
        "engine": args.engine, "no_cache": {"valid": base_v, "test": base_t}, "cache": [],
        "gpu": torch.cuda.get_device_name(0)}
 for W in [int(v) for v in args.size.split(",")]:
-    cache = zaremba_b200.NeuralCache(H, EB, W, T)
+    cache = zaremba_b200.NeuralCache(model.layer_sizes[-1], EB, W, T)   # keys: the last layer's output
     best = (float("inf"), 0.0, 0.0)
     for theta in thetas:
         pm, pc = probs_pass(vld_b, cache, theta)

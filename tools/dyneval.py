@@ -62,7 +62,8 @@ tied = bool(torch.equal(src.embed.W, src.fc.W))
 def fresh_model():
     """The checkpoint as a pytorch-layout model (the Trainer drives that layout; a custom-layout checkpoint's gate
     blocks are permuted as the library permutes them), tied when its embed.W and fc.W are equal."""
-    m = zaremba_b200.Model(V, H, L, 0.0, 0.0, engine=args.engine, tied=tied)
+    m = zaremba_b200.Model(V, H, L, 0.0, 0.0, engine=args.engine, tied=tied, embed_size=src.embed_size,
+                           layer_sizes=src.layer_sizes)
     ws = src._lib_weights()
     if tied:
         ws = ws[:-2] + ws[-1:]          # E once: drop fc.W, keep fc.b

@@ -41,19 +41,24 @@ SHAPES = {"small": 200, "medium": 650, "large": 1500}   # hidden sizes of the RE
 def load_model(path, engine):
     import zaremba_b200
     sd = torch.load(path, map_location="cpu")
+    if not any(k.endswith(".W_x") for k in sd):   # pytorch layout: V, E and the layer widths from the shapes
+        return zaremba_b200.model_from_state_dict(sd, tied=False, engine=engine)
     V, H = sd["embed.W"].shape
-    custom = any(k.endswith(".W_x") for k in sd)
-    L = sum(1 for k in sd if k.endswith(".W_x" if custom else ".weight_ih_l0"))
-    m = zaremba_b200.Model(V, H, L, 0.0, 0.0, "custom" if custom else "pytorch", engine=engine)
+    L = sum(1 for k in sd if k.endswith(".W_x"))
+    m = zaremba_b200.Model(V, H, L, 0.0, 0.0, "custom", engine=engine)
     m.load_state_dict(sd)
     return m
 
 
-def weight_image_bytes(V, H, L):
-    """fp16 bytes a decode step reads from the weight images: per layer W_ih and W_hh [4H, Hp], and fc.W [V, Hp]
-    (Hp = H padded to 64 columns); fp32 biases besides."""
-    Hp = (H + 63) // 64 * 64
-    return 2 * (L * 2 * 4 * H * Hp + V * Hp) + 4 * (L * 2 * 4 * H + V)
+def weight_image_bytes(model):
+    """fp16 bytes a decode step reads from the weight images: per layer W_ih [4H_l, pad(In_l)] and W_hh [4H_l, pad(H_l)],
+    and fc.W [V, pad(H_{L-1})] (pad: to 64 columns); fp32 biases besides."""
+    pad = lambda n: (n + 63) // 64 * 64
+    ins = [model.embed_size, *model.layer_sizes[:-1]]
+    V, nb = model.vocab_size, 0
+    for In, H in zip(ins, model.layer_sizes):
+        nb += 2 * 4 * H * (pad(In) + pad(H)) + 4 * 2 * 4 * H
+    return nb + 2 * V * pad(model.layer_sizes[-1]) + 4 * V
 
 
 def power_limit():
@@ -151,7 +156,7 @@ def main():
     scores = torch.randn(B, V, device=dev) * 2
     sample(scores, pos=1, **kw)
     sample_ms = event_ms(lambda: sample(scores, pos=1, **kw), 200, hold=True)
-    nbytes = weight_image_bytes(V, H, L)
+    nbytes = weight_image_bytes(model)
     out = {"device": torch.cuda.get_device_name(dev), "power_limit": power_limit(), "engine": args.engine,
            "V": V, "H": H, "L": L, "B": B, "decode_steps": n, "ms_per_step": round(step_ms, 4),
            "device_ms_per_step": round(device_step_ms, 4),
@@ -205,7 +210,7 @@ def beams(model, prompt, ids, args, show):
            "ms_per_step": round(step_ms, 4), "device_ms_per_step": round(device_step_ms, 4),
            "beam_row_ms": round(kern["row"], 4), "beam_merge_ms": round(kern["merge"], 4),
            "beam_share": round((kern["row"] + kern["merge"]) / device_step_ms, 4),
-           "step_bytes": weight_image_bytes(V, H, L) + B * K * V * 4}
+           "step_bytes": weight_image_bytes(model) + B * K * V * 4}
     print(json.dumps(out))
     if args.json:
         os.makedirs(os.path.dirname(os.path.abspath(args.json)), exist_ok=True)

@@ -8,7 +8,7 @@ ahmetumutdurmus/zaremba behind the reference's `model.Model` interface.
     from zaremba_b200 import NeuralCache      # neural-cache evaluation (Trainer.perplexity(cache=...))
     from zaremba_b200 import GradStats        # dynamic evaluation's statistics (Trainer.dynamic_perplexity)
 """
-from .model import Model, Embed, LSTM, Linear  # noqa: F401
+from .model import Model, Embed, LSTM, Linear, model_from_state_dict  # noqa: F401
 from .trainer import Trainer, minibatch  # noqa: F401
 from .sampling import sample, beam_step  # noqa: F401
 from .cache import NeuralCache, cache_step  # noqa: F401

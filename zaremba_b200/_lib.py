@@ -51,6 +51,7 @@ _SIGNATURES = {
     "zrb_version": (C.c_char_p, []),
     "zrb_launch_count": (C.c_int64, []),
     "zrb_ctx_create": (C.c_int, [C.POINTER(ZrbConfig), C.POINTER(_vp)]),
+    "zrb_ctx_create_widths": (C.c_int, [C.POINTER(ZrbConfig), C.POINTER(C.c_int32), C.POINTER(_vp)]),
     "zrb_ctx_destroy": (None, [_vp]),
     "zrb_ctx_workspace_bytes": (C.c_int64, [_vp]),
     "zrb_params_changed": (C.c_int, [_vp]),
@@ -113,6 +114,7 @@ _SIGNATURES = {
     "zrb_resident_flag": (C.c_int, [_vp, C.POINTER(_vp), C.POINTER(C.c_uint32)]),
     "zrb_stream_wait_value32": (C.c_int, [_vp, _vp, C.c_uint32]),
     "zrb_rec_plans": (C.c_int, [_vp, _vp]),
+    "zrb_rec_plans_layer": (C.c_int, [_vp, C.c_int32, _vp]),
     "zrb_dp_create": (C.c_int, [C.c_int32, C.c_int32, C.c_int64, C.POINTER(_vp)]),
     "zrb_dp_destroy": (None, [_vp]),
     "zrb_dp_grad_buffer": (_vp, [_vp]),
@@ -176,8 +178,12 @@ def ptr(t):
     return None if t is None else C.c_void_p(t.data_ptr())
 
 
-def rec_plans(ctx):
-    """zrb_rec_plans: {"fwd": {field: value}, "bwd": {...}} for a tensor-core context (fields: REC_PLAN_FIELDS)."""
+def rec_plans(ctx, layer=None):
+    """zrb_rec_plans (layer None) or zrb_rec_plans_layer: {"fwd": {field: value}, "bwd": {...}} for a tensor-core
+    context (fields: REC_PLAN_FIELDS)."""
     out = (C.c_int32 * 16)()
-    check(load().zrb_rec_plans(ctx, out))
+    if layer is None:
+        check(load().zrb_rec_plans(ctx, out))
+    else:
+        check(load().zrb_rec_plans_layer(ctx, int(layer), out))
     return {d: dict(zip(REC_PLAN_FIELDS, out[8 * i:8 * i + 8])) for i, d in enumerate(("fwd", "bwd"))}

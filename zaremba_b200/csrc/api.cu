@@ -72,7 +72,7 @@ static int check_tied(const zrb_ctx* c, const zrb_params* p) {
 MaskSrc site_mask(const zrb_ctx* c, int site) {
     const uint8_t* ex = c->explicit_masks_set ? c->explicit_masks[site] : nullptr;
     MaskSrc m = make_mask_src(ex, c->seed, c->step, site, c->cfg.dropout, c->train);
-    if (c->variational) m.period = (uint32_t)c->B * (uint32_t)c->cfg.hidden;   // element (t, b, j) reads b*H + j
+    if (c->variational) m.period = (uint32_t)c->B * (uint32_t)c->width[site];   // element (t, b, j) reads b*W + j
     return m;
 }
 
@@ -88,7 +88,7 @@ bool reg_on(const zrb_ctx* c) { return c->ar_alpha > 0.f || c->tar_beta > 0.f; }
 
 int reg_compute(zrb_ctx* c, cudaStream_t s) {
     const int L = c->cfg.layers;
-    ZRB_TRY(activation_reg(c->hraw[L - 1], c->reg_r, c->reg_part, c->reg_val, c->T, c->B, c->cfg.hidden, site_mask(c, L),
+    ZRB_TRY(activation_reg(c->hraw[L - 1], c->reg_r, c->reg_part, c->reg_val, c->T, c->B, c->width[L], site_mask(c, L),
                            c->ar_alpha, c->tar_beta, s));
     c->reg_use = true;
     return ZRB_OK;
@@ -130,10 +130,8 @@ const char* zrb_last_error(void) { return t_err; }
 const char* zrb_version(void) { return "zaremba_b200 0.1 (sm_90a)"; }
 int64_t zrb_launch_count(void) { return g_launches.load(); }
 
-int zrb_ctx_create(const zrb_config* cfg, zrb_ctx** out) {
-    ZRB_REQUIRE(cfg && out, "null argument");
-    ZRB_REQUIRE(cfg->vocab > 0 && cfg->hidden > 0 && cfg->layers > 0 && cfg->layers <= ZRB_MAX_LAYERS,
-                "bad model shape V=%d H=%d L=%d", cfg->vocab, cfg->hidden, cfg->layers);
+// zrb_ctx_create and zrb_ctx_create_widths: widths[0] = E, widths[1 + l] = H_l (already checked)
+static int ctx_create(const zrb_config* cfg, const int* widths, zrb_ctx** out) {
     ZRB_REQUIRE(cfg->max_seq > 0 && cfg->max_batch > 0, "bad window T=%d B=%d", cfg->max_seq, cfg->max_batch);
     ZRB_REQUIRE(cfg->dropout >= 0.f && cfg->dropout < 1.f, "dropout %f outside [0,1)", cfg->dropout);
     ZRB_REQUIRE(cfg->engine == ZRB_ENGINE_SIMT || cfg->engine == ZRB_ENGINE_TC, "unknown engine %d", cfg->engine);
@@ -146,22 +144,31 @@ int zrb_ctx_create(const zrb_config* cfg, zrb_ctx** out) {
     zrb_ctx* c = new zrb_ctx();
     c->cfg = *cfg;
     c->tied = (cfg->flags & ZRB_TIED_EMBEDDING) != 0;
-    const int H = cfg->hidden, L = cfg->layers, V = cfg->vocab;
-    const size_t N = (size_t)cfg->max_seq * cfg->max_batch, BH = (size_t)cfg->max_batch * H;
+    const int L = cfg->layers, V = cfg->vocab;
+    bool equal = true;
+    for (int s = 0; s <= L; ++s) {
+        c->width[s] = widths[s];
+        equal = equal && widths[s] == widths[0];
+        if (widths[s] > c->max_width) c->max_width = widths[s];
+    }
+    c->cfg.hidden = equal ? widths[0] : 0;
+    const int Hm = c->max_width;
+    const size_t N = (size_t)cfg->max_seq * cfg->max_batch, B = cfg->max_batch;
     int rc = ZRB_OK;
-    for (int l = 0; l <= L && rc == ZRB_OK; ++l) rc = dalloc(c, &c->act[l], N * H);
+    for (int l = 0; l <= L && rc == ZRB_OK; ++l) rc = dalloc(c, &c->act[l], N * c->width[l]);
     for (int l = 0; l < L && rc == ZRB_OK; ++l) {
+        const size_t H = c->width[l + 1];
         rc = dalloc(c, &c->gates[l], N * 4 * H);
         if (rc == ZRB_OK) rc = dalloc(c, &c->cst[l], N * H);
         if (rc == ZRB_OK) rc = dalloc(c, &c->hraw[l], N * H);
-        if (rc == ZRB_OK) rc = dalloc(c, &c->h0s[l], BH);
-        if (rc == ZRB_OK) rc = dalloc(c, &c->c0s[l], BH);
+        if (rc == ZRB_OK) rc = dalloc(c, &c->h0s[l], B * H);
+        if (rc == ZRB_OK) rc = dalloc(c, &c->c0s[l], B * H);
     }
-    if (rc == ZRB_OK) rc = dalloc(c, &c->dy, N * H);
-    if (rc == ZRB_OK) rc = dalloc(c, &c->dx, N * H);
-    if (rc == ZRB_OK) rc = dalloc(c, &c->dG, N * 4 * H);
-    if (rc == ZRB_OK) rc = dalloc(c, &c->dh_rec, BH);
-    if (rc == ZRB_OK) rc = dalloc(c, &c->dc, BH);
+    if (rc == ZRB_OK) rc = dalloc(c, &c->dy, N * Hm);
+    if (rc == ZRB_OK) rc = dalloc(c, &c->dx, N * Hm);
+    if (rc == ZRB_OK) rc = dalloc(c, &c->dG, N * 4 * Hm);
+    if (rc == ZRB_OK) rc = dalloc(c, &c->dh_rec, B * Hm);
+    if (rc == ZRB_OK) rc = dalloc(c, &c->dc, B * Hm);
     if (rc == ZRB_OK) rc = dalloc(c, &c->row_loss, N);
     if (rc == ZRB_OK) rc = dalloc(c, &c->partials, 4096 + kNormGemm);
     if (rc == ZRB_OK) rc = dalloc(c, &c->scalars, 16);
@@ -183,7 +190,7 @@ int zrb_ctx_create(const zrb_config* cfg, zrb_ctx** out) {
     }
     if (rc == ZRB_OK) rc = dalloc(c, &c->emb_first, (size_t)V);
     if (rc == ZRB_OK && c->tied) {   // fixed-point sums of the embedding rows, every backward
-        rc = dalloc(c, &c->emb_acc, N * H);
+        rc = dalloc(c, &c->emb_acc, N * c->width[0]);
         c->emb_cap_rows = (int64_t)N;
     }
     if (rc == ZRB_OK) rc = dalloc(c, &c->y_dev, N);
@@ -197,6 +204,34 @@ int zrb_ctx_create(const zrb_config* cfg, zrb_ctx** out) {
     }
     *out = c;
     return ZRB_OK;
+}
+
+int zrb_ctx_create(const zrb_config* cfg, zrb_ctx** out) {
+    ZRB_REQUIRE(cfg && out, "null argument");
+    ZRB_REQUIRE(cfg->vocab > 0 && cfg->hidden > 0 && cfg->layers > 0 && cfg->layers <= ZRB_MAX_LAYERS,
+                "bad model shape V=%d H=%d L=%d", cfg->vocab, cfg->hidden, cfg->layers);
+    int widths[ZRB_MAX_LAYERS + 1];
+    for (int s = 0; s <= cfg->layers; ++s) widths[s] = cfg->hidden;
+    return ctx_create(cfg, widths, out);
+}
+
+int zrb_ctx_create_widths(const zrb_config* cfg, const int32_t* widths, zrb_ctx** out) {
+    ZRB_REQUIRE(cfg && widths && out, "null argument");
+    ZRB_REQUIRE(cfg->vocab > 0 && cfg->layers > 0 && cfg->layers <= ZRB_MAX_LAYERS, "bad model shape V=%d L=%d",
+                cfg->vocab, cfg->layers);
+    ZRB_REQUIRE(cfg->hidden == 0, "cfg->hidden must be 0 when the widths are given (got %d)", cfg->hidden);
+    const int L = cfg->layers;
+    bool equal = true;
+    for (int s = 0; s <= L; ++s) {
+        ZRB_REQUIRE(widths[s] > 0, "width %d of site %d must be >= 1", widths[s], s);
+        equal = equal && widths[s] == widths[0];
+    }
+    ZRB_REQUIRE(!(cfg->flags & ZRB_TIED_EMBEDDING) || widths[0] == widths[L],
+                "a tied context needs E = H_{L-1} (E = %d, H_{L-1} = %d)", widths[0], widths[L]);
+    ZRB_REQUIRE(equal || cfg->engine != ZRB_ENGINE_SIMT, "the validation engine takes one width only");
+    int w[ZRB_MAX_LAYERS + 1];
+    for (int s = 0; s <= L; ++s) w[s] = widths[s];
+    return ctx_create(cfg, w, out);
 }
 
 void zrb_ctx_destroy(zrb_ctx* c) {
@@ -308,7 +343,7 @@ int zrb_set_activation_reg(zrb_ctx* c, float alpha, float beta) {
     ZRB_REQUIRE(isfinite(alpha) && alpha >= 0.f, "AR alpha %f must be finite and >= 0", alpha);
     ZRB_REQUIRE(isfinite(beta) && beta >= 0.f, "TAR beta %f must be finite and >= 0", beta);
     if ((alpha > 0.f || beta > 0.f) && !c->reg_r) {
-        ZRB_TRY(dalloc(c, &c->reg_r, (size_t)c->cfg.max_seq * c->cfg.max_batch * c->cfg.hidden));
+        ZRB_TRY(dalloc(c, &c->reg_r, (size_t)c->cfg.max_seq * c->cfg.max_batch * c->width[c->cfg.layers]));
         ZRB_TRY(dalloc(c, &c->reg_part, (size_t)2 * kActRegBlocks));
         ZRB_TRY(dalloc(c, &c->reg_val, 2));
         ZRB_CUDA(cudaMemset(c->reg_val, 0, 2 * sizeof(float)));
@@ -461,16 +496,17 @@ int zrb_swap_average(zrb_ctx* c, const zrb_params* p, void* stream) {
 
 static TensorList param_list(const zrb_ctx* c, const zrb_params* p, const zrb_params* g) {
     TensorList tl;
-    const int64_t H = c->cfg.hidden, V = c->cfg.vocab;
+    const int64_t V = c->cfg.vocab;
     int k = 0;
-    tl.p[k] = p->embed_w; tl.g[k] = g->embed_w; tl.n[k++] = V * H;
+    tl.p[k] = p->embed_w; tl.g[k] = g->embed_w; tl.n[k++] = V * c->width[0];
     for (int l = 0; l < c->cfg.layers; ++l) {
-        tl.p[k] = p->w_ih[l]; tl.g[k] = g->w_ih[l]; tl.n[k++] = 4 * H * H;
+        const int64_t In = c->width[l], H = c->width[l + 1];
+        tl.p[k] = p->w_ih[l]; tl.g[k] = g->w_ih[l]; tl.n[k++] = 4 * H * In;
         tl.p[k] = p->w_hh[l]; tl.g[k] = g->w_hh[l]; tl.n[k++] = 4 * H * H;
         tl.p[k] = p->b_ih[l]; tl.g[k] = g->b_ih[l]; tl.n[k++] = 4 * H;
         tl.p[k] = p->b_hh[l]; tl.g[k] = g->b_hh[l]; tl.n[k++] = 4 * H;
     }
-    tl.p[k] = p->fc_w; tl.g[k] = g->fc_w; tl.n[k++] = V * H;
+    tl.p[k] = p->fc_w; tl.g[k] = g->fc_w; tl.n[k++] = V * c->width[c->cfg.layers];
     if (c->tied) tl.n[0] = 0;   // E once, at fc.W's slot (zero-length entries are skipped by the norm and the update)
     tl.p[k] = p->fc_b; tl.g[k] = g->fc_b; tl.n[k++] = V;
     tl.count = k;
@@ -554,7 +590,15 @@ int zrb_resident_flag(zrb_ctx* c, uint32_t** flag, uint32_t* next_value) {
 int zrb_rec_plans(const zrb_ctx* c, int32_t* h_out) {
     ZRB_REQUIRE(c && h_out, "null argument");
     ZRB_REQUIRE(c->cfg.engine == ZRB_ENGINE_TC && c->tc, "recurrence plans exist only in tensor-core contexts");
-    tc_rec_plans(c, h_out);
+    tc_rec_plans(c, 0, h_out);
+    return ZRB_OK;
+}
+
+int zrb_rec_plans_layer(const zrb_ctx* c, int32_t layer, int32_t* h_out) {
+    ZRB_REQUIRE(c && h_out, "null argument");
+    ZRB_REQUIRE(c->cfg.engine == ZRB_ENGINE_TC && c->tc, "recurrence plans exist only in tensor-core contexts");
+    ZRB_REQUIRE(layer >= 0 && layer < c->cfg.layers, "layer %d outside [0, %d)", layer, c->cfg.layers);
+    tc_rec_plans(c, layer, h_out);
     return ZRB_OK;
 }
 
@@ -569,11 +613,11 @@ int zrb_embed_scatter_rows(zrb_ctx* c, float* grad_embed, const int64_t* ids, co
     ZRB_REQUIRE(c && grad_embed && ids && rows && n_rows >= 0, "bad arguments");
     cudaStream_t s = (cudaStream_t)stream;
     if (n_rows > c->emb_cap_rows) {
-        ZRB_TRY(dalloc(c, &c->emb_acc, (size_t)n_rows * c->cfg.hidden));   // (a previous, smaller one is kept until destroy)
+        ZRB_TRY(dalloc(c, &c->emb_acc, (size_t)n_rows * c->width[0]));   // (a previous, smaller one is kept until destroy)
         c->emb_cap_rows = n_rows;
     }
     ProfScope ps(c, ZRB_PROF_EMBED_BWD, s);
-    const int H = c->cfg.hidden, V = c->cfg.vocab;
+    const int H = c->width[0], V = c->cfg.vocab;
     // tied: grad_embed holds the reduced projection gradient, every row of it non-zero and updated densely
     if (c->tied) return embed_scatter_rows(ids, rows, grad_embed, (int)n_rows, H, V, c->emb_first, c->emb_acc, s, true);
     if (c->emb_sparse && c->emb_prev_grad == grad_embed) {
@@ -760,7 +804,7 @@ int zrb_beam_step(const float* scores, int64_t ld, int32_t B, int32_t K_in, int3
     BeamCand* cands = nullptr;   // stream-ordered scratch: no context here, and no synchronisation
     ZRB_CUDA(cudaMallocAsync((void**)&cands, (size_t)B * K_in * K * sizeof(BeamCand), s));
     const int rc = beam_step(scores, ld, B, K_in, K, V, cum_in, tok_in, eos, cands, tokens, parents, cum_out, logprobs,
-                             nullptr, nullptr, 0, 0, s);
+                             nullptr, nullptr, 0, LayerWidths{}, s);
     ZRB_CUDA(cudaFreeAsync(cands, s));
     return rc;
 }
@@ -768,14 +812,18 @@ int zrb_beam_step(const float* scores, int64_t ld, int32_t B, int32_t K_in, int3
 // zrb_beam_search's scratch (engine.h): the fixed part once, the per-step arrays grown to `entries`
 static int beam_scratch(zrb_ctx* c, int64_t entries) {
     if (!c->beam_cand) {
-        const size_t BH = (size_t)c->cfg.max_batch * c->cfg.hidden;
+        size_t total = 0;
+        for (int l = 0; l < c->cfg.layers; ++l) total += 4 * (size_t)c->cfg.max_batch * c->width[l + 1];
         float* st = nullptr;
-        ZRB_TRY(dalloc(c, &st, 4 * (size_t)c->cfg.layers * BH));
-        for (int l = 0; l < c->cfg.layers; ++l)
+        ZRB_TRY(dalloc(c, &st, total));
+        for (int l = 0; l < c->cfg.layers; ++l) {
+            const size_t BH = (size_t)c->cfg.max_batch * c->width[l + 1];
             for (int k = 0; k < 2; ++k) {
-                c->beam_st[k].h[l] = st + (4 * l + 2 * k) * BH;
-                c->beam_st[k].c[l] = st + (4 * l + 2 * k + 1) * BH;
+                c->beam_st[k].h[l] = st + 2 * k * BH;
+                c->beam_st[k].c[l] = st + (2 * k + 1) * BH;
             }
+            st += 4 * BH;
+        }
         ZRB_TRY(dalloc(c, &c->beam_cum, (size_t)c->cfg.max_batch));
         ZRB_TRY(dalloc(c, &c->beam_cand, (size_t)c->cfg.max_batch * ZRB_MAX_BEAMS));
     }
@@ -799,7 +847,9 @@ int zrb_beam_search(zrb_ctx* c, const zrb_params* p, const int64_t* prompt, int3
     ZRB_TRY(check_shapes(c, 1, B * K));
     ZRB_TRY(check_tied(c, p));
     cudaStream_t s = (cudaStream_t)stream;
-    const int V = c->cfg.vocab, S = c->cfg.max_seq, L = c->cfg.layers, H = c->cfg.hidden, BK = B * K;
+    const int V = c->cfg.vocab, S = c->cfg.max_seq, L = c->cfg.layers, BK = B * K;
+    LayerWidths hw{};
+    for (int l = 0; l < L; ++l) hw.h[l] = c->width[l + 1];
     ZRB_TRY(beam_scratch(c, (int64_t)n_new * BK));
     const zrb_states* fwd_out = &c->beam_st[0];   // the forward's output rows: B after the prefill, then B*K
     const zrb_states* gathered = &c->beam_st[1];  // rows reordered by parent, the next forward's input
@@ -821,7 +871,7 @@ int zrb_beam_search(zrb_ctx* c, const zrb_params* p, const int64_t* prompt, int3
         const bool last = k + 1 == n_new;
         ZRB_TRY(beam_step(c->scores, V, B, K_in, K, V, k ? c->beam_cum : nullptr, k ? c->beam_tok + at - BK : nullptr, eos,
                           c->beam_cand, c->beam_tok + at, c->beam_par + at, c->beam_cum, c->beam_lp + at, fwd_out,
-                          last ? out : gathered, L, H, s));
+                          last ? out : gathered, L, hw, s));
         if (!last) ZRB_TRY(forward_last_rows(c, p, c->beam_tok + at, gathered, fwd_out, c->scores, s));
     }
     return beam_backtrack(c->beam_tok, c->beam_par, c->beam_lp, c->beam_cum, n_new, BK, K, tokens, logprobs, scores, s);
@@ -855,6 +905,7 @@ int zrb_lstm_layer_fwd(zrb_ctx* c, const float* w_ih, const float* w_hh, const f
     ZRB_REQUIRE(c && w_ih && w_hh && b_ih && b_hh && x && h0 && c0 && y, "null argument");
     ZRB_TRY(check_shapes(c, T, B));
     ZRB_REQUIRE(c->cfg.engine == ZRB_ENGINE_TC, "zrb_lstm_layer_fwd is an entry point of the tensor-core engine");
+    ZRB_REQUIRE(c->cfg.hidden > 0, "zrb_lstm_layer_fwd needs a context of one width");
     ZRB_REQUIRE(h0 != hT && c0 != cT, "the unit-level entry point does not alias states");
     return tc_layer_fwd(c, w_ih, w_hh, b_ih, b_hh, x, T, B, h0, c0, y, hT, cT, (cudaStream_t)stream);
 }
@@ -863,6 +914,7 @@ int zrb_lstm_layer_bwd(zrb_ctx* c, const float* dy, float* dx, float* dw_ih, flo
                        void* stream) {
     ZRB_REQUIRE(c && dy && dw_ih && dw_hh && db_ih && db_hh, "null argument");
     ZRB_REQUIRE(c->cfg.engine == ZRB_ENGINE_TC, "zrb_lstm_layer_bwd is an entry point of the tensor-core engine");
+    ZRB_REQUIRE(c->cfg.hidden > 0, "zrb_lstm_layer_bwd needs a context of one width");
     return tc_layer_bwd(c, dy, dx, dw_ih, dw_hh, db_ih, db_hh, (cudaStream_t)stream);
 }
 

@@ -98,16 +98,18 @@ __global__ void __launch_bounds__(kMergeThreads) beam_merge_kernel(const BeamCan
                                                                    int V, int64_t* __restrict__ tokens,
                                                                    int32_t* __restrict__ parents, float* cum_out,
                                                                    float* __restrict__ logprobs, zrb_states src,
-                                                                   zrb_states dst, int L, int H) {
+                                                                   zrb_states dst, int L, LayerWidths w) {
     __shared__ unsigned long long s_key[ZRB_MAX_BEAMS * ZRB_MAX_BEAMS];
     __shared__ int s_pick[ZRB_MAX_BEAMS];
     __shared__ const float* s_src[2 * ZRB_MAX_LAYERS];   // (h, c) of layer l at 2l, 2l+1: constant indices into the
     __shared__ float* s_dst[2 * ZRB_MAX_LAYERS];         // kernel parameters, so they stay out of local memory
+    __shared__ int s_h[ZRB_MAX_LAYERS];                  // (the width of layer l, likewise)
     if (threadIdx.x == 0) {
 #pragma unroll
         for (int l = 0; l < ZRB_MAX_LAYERS; ++l) {
             s_src[2 * l] = src.h[l]; s_src[2 * l + 1] = src.c[l];
             s_dst[2 * l] = dst.h[l]; s_dst[2 * l + 1] = dst.c[l];
+            s_h[l] = w.h[l];
         }
     }
     const int b = blockIdx.x, n = K_in * K;
@@ -137,7 +139,7 @@ __global__ void __launch_bounds__(kMergeThreads) beam_merge_kernel(const BeamCan
     }
     // row q = ((l, h or c), k'): dst row b*K + k' <- src row b*K_in + parent(k')
     for (int q = blockIdx.y; q < 2 * L * K; q += gridDim.y) {
-        const int lhc = q / K, k = q % K;
+        const int lhc = q / K, k = q % K, H = s_h[lhc >> 1];
         const int par = (int)(cb[s_pick[k]].flat / (uint32_t)V);
         const float* s = s_src[lhc] + ((size_t)b * K_in + par) * H;
         float* d = s_dst[lhc] + ((size_t)b * K + k) * H;
@@ -174,7 +176,7 @@ int beam_check(int B, int K, int V, int eos) {
 
 int beam_step(const float* scores, int64_t ld, int B, int K_in, int K, int V, const float* cum_in, const int64_t* tok_in,
               int eos, BeamCand* cands, int64_t* tokens, int32_t* parents, float* cum_out, float* logprobs,
-              const zrb_states* src, const zrb_states* dst, int L, int H, cudaStream_t s) {
+              const zrb_states* src, const zrb_states* dst, int L, const LayerWidths& w, cudaStream_t s) {
     ZRB_TRY(beam_check(B, K, V, eos));
     // a step-0 row is never finished, so every step has at least K candidates per prompt
     ZRB_REQUIRE(K_in == K || (K_in == 1 && !tok_in), "K_in=%d must be K=%d, or 1 without tok_in (step 0)", K_in, K);
@@ -197,7 +199,7 @@ int beam_step(const float* scores, int64_t ld, int B, int K_in, int K, int V, co
     const int gy = L ? std::max(1, std::min(2 * L * K, 128 / B)) : 1;
     const zrb_states none = {};
     beam_merge_kernel<<<dim3(B, gy), kMergeThreads, 0, s>>>(cands, K_in, K, V, tokens, parents, cum_out, logprobs,
-                                                            src ? *src : none, dst ? *dst : none, L, H);
+                                                            src ? *src : none, dst ? *dst : none, L, w);
     ZRB_KERNEL_CHECK();
     return ZRB_OK;
 }

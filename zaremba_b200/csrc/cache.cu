@@ -464,7 +464,8 @@ int zrb_eval_step_cache(zrb_ctx* c, const zrb_params* p, const int64_t* x, const
     ZRB_TRY(check_device(cache));
     ZRB_REQUIRE(lambda >= 0.f && lambda < 1.f, "lambda %f outside [0,1)", lambda);
     ZRB_REQUIRE(B == cache->B, "B=%d but the cache holds %d streams", B, cache->B);
-    ZRB_REQUIRE(c->cfg.hidden == cache->H, "the model's H=%d but the cache's %d", c->cfg.hidden, cache->H);
+    const int H = c->width[c->cfg.layers];   // the last layer's width
+    ZRB_REQUIRE(H == cache->H, "the model's last layer has H=%d but the cache %d", H, cache->H);
     ZRB_REQUIRE(T >= 1 && T <= cache->max_seq, "T=%d outside [1,%d] of the cache", T, cache->max_seq);
     cudaStream_t s = (cudaStream_t)stream;
     // zrb_eval_step's forward and softmax (the same row losses and tgt_prob), its loss reduction left to the combine
@@ -473,7 +474,7 @@ int zrb_eval_step_cache(zrb_ctx* c, const zrb_params* p, const int64_t* x, const
     ZRB_TRY(softmax_nll(c->scores, y, T * B, c->cfg.vocab, B, c->row_loss, nullptr, nullptr, tgt_prob, s));
     const __half* xh = nullptr;
     const float* xf = nullptr;
-    int64_t ld = c->cfg.hidden;
+    int64_t ld = H;
     if (c->cfg.engine == ZRB_ENGINE_TC) {
         xh = tc_last_layer_image(c);     // fp16 image of the last layer's output, pitch Hp: the projection's operand
         ld = cache->Hp;

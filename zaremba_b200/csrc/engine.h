@@ -7,7 +7,11 @@
 struct zrb_tc_state;  // tensor-core engine private data (engine_tc.cu)
 
 struct zrb_ctx {
-    zrb_config cfg{};
+    zrb_config cfg{};              // cfg.hidden = 0 when the layers' widths differ (zrb_ctx_create_widths)
+    // width of dropout site s (DESIGN.md section 18): width[0] = E, width[l + 1] = H_l; layer l reads width[l] and
+    // writes width[l + 1].  Every entry is cfg.hidden in a context of one width.
+    int width[ZRB_MAX_LAYERS + 1] = {};
+    int max_width = 0;
     std::vector<void*> allocs;
     int64_t bytes = 0;
 
@@ -141,8 +145,10 @@ int tc_train_step_layer(zrb_ctx* c, const zrb_params* p, const zrb_params* g, in
 int tc_rec_trace(zrb_ctx* c, long long* h_out, int max_entries);
 int tc_flush_updates(zrb_ctx* c, cudaStream_t s);   // apply deferred weight updates now (zrb_set_lazy_update)
 bool tc_persistent_bwd(const zrb_ctx* c);
-const __half* tc_last_layer_image(const zrb_ctx* c);   // x_h[L]: fp16 last-layer output of the last forward, pitch pad64(H)
-void tc_rec_plans(const zrb_ctx* c, int32_t* h_out);   // zrb_rec_plans: 2 x {ok, KS, U, G, nCTA, GBi, Kc, KcS}
+const __half* tc_last_layer_image(const zrb_ctx* c);   // x_h[L]: fp16 last-layer output of the last forward, pitch
+                                                       // pad64(H_{L-1})
+// zrb_rec_plans_layer: layer l's 2 x {ok, KS, U, G, nCTA, GBi, Kc, KcS}
+void tc_rec_plans(const zrb_ctx* c, int l, int32_t* h_out);
 int tc_layer_fwd(zrb_ctx* c, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh, const float* x,
                  int T, int B, const float* h0, const float* c0, float* y, float* hT, float* cT, cudaStream_t s);
 int tc_layer_bwd(zrb_ctx* c, const float* dy, float* dx, float* dw_ih, float* dw_hh, float* db_ih, float* db_hh,

@@ -1,13 +1,13 @@
 // ZRB_ENGINE_TC: every dense contraction of the path on wgmma tensor cores (fp16 operands,
 // fp32 accumulation), pointwise math and state in fp32.
 //
-// fp16 images (K = contraction index):
-//   w_ih_h[l], w_hh_h[l] [4H, Hp]   read K-major by the forward GEMMs (X*W^T, h*W^T) and MN-major
-//   fc_w_h               [V,  Hp]   by the dgrads (dG*W, dS*W): one image serves both
-//   x_h[l]      [N, Hp]  dropout'ed input of layer l (x_h[L] feeds the projection); MN-major B of wgrads
-//   hprev_h[l]  [N+B,Hp] rows 0..B-1 = h entering the window, rows B.. = h_t: row block t is h_{t-1}
-//                        (variational mode: times the layer's recurrent mask, so the dW_hh GEMM needs no change)
-//   dG_h        [N, G4p] kGradScale * dG;  dS_h [N, Vp] kGradScale * dscores
+// fp16 images (K = contraction index; Xp[s] = pad64(width of site s): Xp[l] = pad64(In_l), Xp[l+1] = pad64(H_l)):
+//   w_ih_h[l] [4H_l, Xp[l]], w_hh_h[l] [4H_l, Xp[l+1]]   read K-major by the forward GEMMs (X*W^T, h*W^T) and MN-major
+//   fc_w_h    [V,    Xp[L]]                             by the dgrads (dG*W, dS*W): one image serves both
+//   x_h[l]      [N, Xp[l]]     dropout'ed input of layer l (x_h[L] feeds the projection); MN-major B of wgrads
+//   hprev_h[l]  [N+B, Xp[l+1]] rows 0..B-1 = h entering the window, rows B.. = h_t: row block t is h_{t-1}
+//                              (variational mode: times the layer's recurrent mask, so the dW_hh GEMM needs no change)
+//   dG_h        [N, G4p[l]] kGradScale * dG;  dS_h [N, Vp] kGradScale * dscores
 // Gradient images are scaled by an exact power of two and unscaled by the consuming GEMM's alpha.
 #include "engine.h"
 #include <stdlib.h>
@@ -38,7 +38,7 @@ struct GridBarrier {
 };
 
 struct zrb_tc_state {
-    int Hp = 0, G4p = 0, Vp = 0;
+    int Xp[ZRB_MAX_LAYERS + 1] = {}, G4p[ZRB_MAX_LAYERS] = {}, Vp = 0;
     int device = 0;
     __half* w_ih_h[ZRB_MAX_LAYERS] = {};
     __half* w_hh_h[ZRB_MAX_LAYERS] = {};
@@ -65,13 +65,14 @@ struct zrb_tc_state {
     int64_t packed_version = 0;
     zrb_params packed_params{};
     std::vector<void*> allocs;
-    // persistent recurrence
-    zrb::RecPlan fplan{};
+    // persistent recurrence: one plan per layer and direction, each for the layer's width.  Either direction is on for
+    // every layer or for none (tc_ctx_init), so fplan[0].ok / bplan[0].ok say which path a step takes.
+    zrb::RecPlan fplan[ZRB_MAX_LAYERS] = {};
     __half* w_img_f[ZRB_MAX_LAYERS] = {};
     __half* h0_img[ZRB_MAX_LAYERS] = {};   // image of the state entering the window (step 0's B operand)
     __half* h_img = nullptr;
     GridBarrier fwd_bar, bwd_bar;          // words 0 and 32 of one allocation; shared by the model- and layer-level calls
-    zrb::RecPlan bplan{};
+    zrb::RecPlan bplan[ZRB_MAX_LAYERS] = {};
     __half* w_img_b[ZRB_MAX_LAYERS] = {};
     __half* g_img = nullptr;
     long long* trace = nullptr;   // [2][8 + T*8]: launch stamps + per-step clock stamps (zrb_prof_rec_trace)
@@ -91,26 +92,26 @@ struct zrb_tc_state {
     } whh_img[ZRB_MAX_LAYERS];
 
     // ---- which fp16 images each weight matrix has: what a pack or a fused update of it must write -------------------
-    zrb::WeightImages row_image(__half* img) const {
+    zrb::WeightImages row_image(__half* img, int ld) const {
         zrb::WeightImages w;
-        w.row = img; w.ld = Hp;
+        w.row = img; w.ld = ld;
         return w;
     }
-    zrb::WeightImages w_ih_images(int l) const { return row_image(w_ih_h[l]); }
-    zrb::WeightImages fc_w_images() const { return row_image(fc_w_h); }
+    zrb::WeightImages w_ih_images(int l) const { return row_image(w_ih_h[l], Xp[l]); }
+    zrb::WeightImages fc_w_images(int L) const { return row_image(fc_w_h, Xp[L]); }
     // both recurrences run in the persistent kernels: fplan.ok && bplan.ok, and bplan.ok implies fplan.ok (tc_ctx_init
     // clears bplan.ok when the forward plan is off)
-    bool persistent() const { return bplan.ok; }
+    bool persistent() const { return bplan[0].ok; }
     // W_hh of layer l, recording what its images will hold.  kWhhStale asks for no image: the caller changes p and leaves
     // the images behind it.  Otherwise the slices of each persistent kernel in use, and the row image only where it is
     // read, on the per-timestep path.  row_too: the row image regardless.
     zrb::WeightImages w_hh_images(int l, const WhhImage& holds, bool row_too = false) {
         whh_img[l] = holds;
-        zrb::WeightImages w = row_image(nullptr);
+        zrb::WeightImages w = row_image(nullptr, Xp[l + 1]);
         if (holds.kind == kWhhStale) return w;
         if (row_too || !persistent()) w.row = w_hh_h[l];
-        w.fwd = fplan.ok ? w_img_f[l] : nullptr; w.fplan = &fplan;
-        w.bwd = bplan.ok ? w_img_b[l] : nullptr; w.bplan = &bplan;
+        w.fwd = fplan[l].ok ? w_img_f[l] : nullptr; w.fplan = &fplan[l];
+        w.bwd = bplan[l].ok ? w_img_b[l] : nullptr; w.bplan = &bplan[l];
         return w;
     }
 };
@@ -160,42 +161,64 @@ int tc_ctx_init(zrb_ctx* c) {
     zrb_tc_state* t = c->tc;
     t->device = dev & 63;
     g_live_tc_ctx[t->device].fetch_add(1);
-    const int H = c->cfg.hidden, L = c->cfg.layers, V = c->cfg.vocab;
+    const int L = c->cfg.layers, V = c->cfg.vocab, Hm = c->max_width;
     const size_t N = (size_t)c->cfg.max_seq * c->cfg.max_batch, B = c->cfg.max_batch;
-    t->Hp = pad64(H); t->G4p = pad64(4 * H); t->Vp = pad64(V);
+    for (int s = 0; s <= L; ++s) t->Xp[s] = pad64(c->width[s]);
+    int G4m = 0;
     for (int l = 0; l < L; ++l) {
-        ZRB_TRY(tc_alloc(c, &t->w_ih_h[l], (size_t)4 * H * t->Hp));
-        ZRB_TRY(tc_alloc(c, &t->w_hh_h[l], (size_t)4 * H * t->Hp));
-        ZRB_TRY(tc_alloc(c, &t->hprev_h[l], (N + B) * t->Hp));
+        t->G4p[l] = pad64(4 * c->width[l + 1]);
+        if (t->G4p[l] > G4m) G4m = t->G4p[l];
     }
-    for (int l = 0; l <= L; ++l) ZRB_TRY(tc_alloc(c, &t->x_h[l], N * t->Hp));
-    ZRB_TRY(tc_alloc(c, &t->fc_w_h, (size_t)V * t->Hp));
-    ZRB_TRY(tc_alloc(c, &t->dG_h, N * t->G4p));
-    ZRB_TRY(tc_alloc(c, &t->dG_h_alt, N * t->G4p));
+    t->Vp = pad64(V);
+    for (int l = 0; l < L; ++l) {
+        const size_t H = c->width[l + 1];
+        ZRB_TRY(tc_alloc(c, &t->w_ih_h[l], 4 * H * t->Xp[l]));
+        ZRB_TRY(tc_alloc(c, &t->w_hh_h[l], 4 * H * t->Xp[l + 1]));
+        ZRB_TRY(tc_alloc(c, &t->hprev_h[l], (N + B) * t->Xp[l + 1]));
+    }
+    for (int l = 0; l <= L; ++l) ZRB_TRY(tc_alloc(c, &t->x_h[l], N * t->Xp[l]));
+    ZRB_TRY(tc_alloc(c, &t->fc_w_h, (size_t)V * t->Xp[L]));
+    ZRB_TRY(tc_alloc(c, &t->dG_h, N * G4m));
+    ZRB_TRY(tc_alloc(c, &t->dG_h_alt, N * G4m));
     ZRB_TRY(tc_alloc(c, &t->dS_h, N * t->Vp));
-    ZRB_TRY(tc_alloc(c, &t->colsum_scratch, (size_t)colsum_h_scratch_floats(V > 4 * H ? V : 4 * H)));
-    ZRB_TRY(rec_fwd_plan(H, c->cfg.max_batch, &t->fplan));
+    ZRB_TRY(tc_alloc(c, &t->colsum_scratch, (size_t)colsum_h_scratch_floats(V > 4 * Hm ? V : 4 * Hm)));
+    // one plan per layer; a direction is persistent only when every layer's plan fits (no mixed step)
     const char* force = getenv("ZRB_REC");
-    if (force && !strcmp(force, "steps")) t->fplan.ok = 0;   // A/B switch: per-timestep launches
-    if (t->fplan.ok) {
-        const RecPlan& fp = t->fplan;
+    bool fwd_ok = !(force && !strcmp(force, "steps")), bwd_ok = !(force && !strcmp(force, "fwdonly"));   // A/B switches
+    for (int l = 0; l < L; ++l) {
+        ZRB_TRY(rec_fwd_plan(c->width[l + 1], c->cfg.max_batch, &t->fplan[l]));
+        ZRB_TRY(rec_bwd_plan(c->width[l + 1], c->cfg.max_batch, &t->bplan[l]));
+        fwd_ok = fwd_ok && t->fplan[l].ok;
+        bwd_ok = bwd_ok && t->bplan[l].ok;
+    }
+    for (int l = 0; l < L; ++l) {
+        if (!fwd_ok) t->fplan[l].ok = 0;
+        if (!fwd_ok || !bwd_ok) t->bplan[l].ok = 0;
+    }
+    size_t h_img = 0, g_img = 0;   // the operand images the layers run one after another share, sized for the largest
+    if (fwd_ok) {
         for (int l = 0; l < L; ++l) {
+            const RecPlan& fp = t->fplan[l];
             ZRB_TRY(tc_alloc(c, &t->w_img_f[l], (size_t)fp.nCTA * fp.KcS * fp.G * 64 + 16 * 64 /* M=128 over-read */));
             ZRB_TRY(tc_alloc(c, &t->h0_img[l], (size_t)fp.Kc * fp.GBi * 64));
+            const size_t n = (size_t)(c->cfg.max_seq + 1) * fp.Kc * fp.GBi * 64;
+            if (n > h_img) h_img = n;
         }
-        ZRB_TRY(tc_alloc(c, &t->h_img, (size_t)(c->cfg.max_seq + 1) * fp.Kc * fp.GBi * 64));
+        ZRB_TRY(tc_alloc(c, &t->h_img, h_img));
         unsigned int* words = nullptr;
         ZRB_TRY(tc_alloc(c, &words, 64));
         t->fwd_bar.word = words;
         t->bwd_bar.word = words + 32;
     }
     if (getenv("ZRB_REC_TRACE")) ZRB_TRY(tc_alloc(c, &t->trace, (size_t)2 * (8 + c->cfg.max_seq * 8)));
-    ZRB_TRY(rec_bwd_plan(H, c->cfg.max_batch, &t->bplan));
-    if (!t->fplan.ok || (force && !strcmp(force, "fwdonly"))) t->bplan.ok = 0;
-    if (t->bplan.ok) {
-        const RecPlan& bp = t->bplan;
-        for (int l = 0; l < L; ++l) ZRB_TRY(tc_alloc(c, &t->w_img_b[l], (size_t)bp.nCTA * bp.KcS * bp.G * 64 + 16 * 64));
-        ZRB_TRY(tc_alloc(c, &t->g_img, (size_t)2 * 4 * bp.Kc * bp.GBi * 64));
+    if (t->bplan[0].ok) {
+        for (int l = 0; l < L; ++l) {
+            const RecPlan& bp = t->bplan[l];
+            ZRB_TRY(tc_alloc(c, &t->w_img_b[l], (size_t)bp.nCTA * bp.KcS * bp.G * 64 + 16 * 64));
+            const size_t n = (size_t)2 * 4 * bp.Kc * bp.GBi * 64;
+            if (n > g_img) g_img = n;
+        }
+        ZRB_TRY(tc_alloc(c, &t->g_img, g_img));
     }
     return ZRB_OK;
 }
@@ -227,7 +250,7 @@ static bool whh_current(const zrb_ctx* c, int l) {
 // build layer l's W_hh images from W with the mask the call needs; row_image: also the row image w_hh_h when the
 // persistent kernels do not need it (it is read only on the per-timestep path)
 static int tc_pack_whh(zrb_ctx* c, const float* W, int l, bool row_image, cudaStream_t s) {
-    const int H = c->cfg.hidden;
+    const int H = c->width[l + 1];
     const MaskSrc m = wd_mask(c, l);
     const WeightImages w = c->tc->w_hh_images(l, whh_wanted(c, l), row_image);
     if (w.row) ZRB_TRY(convert_pad_f16(W, H, w.row, w.ld, 4 * H, H, 1.f, s, m));
@@ -241,12 +264,13 @@ static int tc_pack_weights(zrb_ctx* c, const zrb_params* p, cudaStream_t s) {
     zrb_tc_state* t = c->tc;
     if (t->packed_version == c->weights_version && !memcmp(&t->packed_params, p, sizeof(*p))) return ZRB_OK;
     ProfScope ps(c, ZRB_PROF_PACK, s);
-    const int H = c->cfg.hidden, L = c->cfg.layers, V = c->cfg.vocab;
+    const int L = c->cfg.layers, V = c->cfg.vocab;
     for (int l = 0; l < L; ++l) {
-        ZRB_TRY(convert_pad_f16(p->w_ih[l], H, t->w_ih_h[l], t->Hp, 4 * H, H, 1.f, s));
+        const int In = c->width[l], H = c->width[l + 1];
+        ZRB_TRY(convert_pad_f16(p->w_ih[l], In, t->w_ih_h[l], t->Xp[l], 4 * H, In, 1.f, s));
         ZRB_TRY(tc_pack_whh(c, p->w_hh[l], l, true, s));
     }
-    ZRB_TRY(convert_pad_f16(p->fc_w, H, t->fc_w_h, t->Hp, V, H, 1.f, s));
+    ZRB_TRY(convert_pad_f16(p->fc_w, c->width[L], t->fc_w_h, t->Xp[L], V, c->width[L], 1.f, s));
     t->packed_version = c->weights_version;
     t->packed_params = *p;
     return ZRB_OK;
@@ -267,21 +291,23 @@ struct WeightMatrices {
 };
 // The matrices in the order the update launches them: W_ih then W_hh per layer, then fc.W.  This is the one place that
 // knows where param_list() (api.cu) puts them: embed, (w_ih, w_hh, b_ih, b_hh) x L, fc_w, fc_b (tied: embed has n = 0,
-// E is fc_w).
+// E is fc_w), and the one place of the update path that knows their shapes: W_ih [4H_l, In_l], W_hh [4H_l, H_l],
+// fc.W [V, H_{L-1}].
 static WeightMatrices tc_matrices(const zrb_ctx* c) {
-    const int H = c->cfg.hidden, L = c->cfg.layers, V = c->cfg.vocab;
+    const int L = c->cfg.layers, V = c->cfg.vocab;
     WeightMatrices ms;
     for (int l = 0; l < L; ++l) {
-        ms.m[ms.n++] = {1 + 4 * l, 4 * H, H, l, WeightMatrix::kWih};
+        const int In = c->width[l], H = c->width[l + 1];
+        ms.m[ms.n++] = {1 + 4 * l, 4 * H, In, l, WeightMatrix::kWih};
         ms.m[ms.n++] = {2 + 4 * l, 4 * H, H, l, WeightMatrix::kWhh};
     }
-    ms.m[ms.n++] = {1 + 4 * L, V, H, L, WeightMatrix::kFcW};
+    ms.m[ms.n++] = {1 + 4 * L, V, c->width[L], L, WeightMatrix::kFcW};
     return ms;
 }
 // the images a fused update of m writes; whh: what W_hh's will hold afterwards (zrb_tc_state::w_hh_images)
 static WeightImages tc_images(zrb_ctx* c, const WeightMatrix& m, const zrb_tc_state::WhhImage& whh) {
     if (m.kind == WeightMatrix::kWhh) return c->tc->w_hh_images(m.item, whh);
-    return m.kind == WeightMatrix::kWih ? c->tc->w_ih_images(m.item) : c->tc->fc_w_images();
+    return m.kind == WeightMatrix::kWih ? c->tc->w_ih_images(m.item) : c->tc->fc_w_images(m.item);
 }
 // tl for the list kernels once the tile kernels have taken the matrices: their lengths set to 0, which every list
 // kernel skips
@@ -345,22 +371,21 @@ int tc_flush_updates(zrb_ctx* c, cudaStream_t s) {
 int tc_forward(zrb_ctx* c, const zrb_params* p, const int64_t* x, const zrb_states* in, const zrb_states* out,
                float* scores, cudaStream_t s, bool last_only) {
     zrb_tc_state* t = c->tc;
-    const int H = c->cfg.hidden, L = c->cfg.layers, V = c->cfg.vocab, T = c->T, B = c->B, N = T * B;
-    const int Hp = t->Hp;
-    const size_t bh = (size_t)B * H * sizeof(float);
+    const int L = c->cfg.layers, V = c->cfg.vocab, T = c->T, B = c->B, N = T * B;
     // deferred updates ride beside the forward recurrences of a fused train step; any other forward applies them first
-    const bool ride = t->upd_pending && t->in_train_step && t->fplan.ok && pdl_beside_rec(c);
+    const bool ride = t->upd_pending && t->in_train_step && t->fplan[0].ok && pdl_beside_rec(c);
     if (t->upd_pending && !ride) ZRB_TRY(tc_flush_updates(c, s));
     ZRB_TRY(tc_pack_weights(c, p, s));
     {   // state copies (in / out may be the same buffers), fp16 h0 rows and images, saved tokens: one launch
         FwdPrep fp = {};
         for (int l = 0; l < L; ++l) {
             fp.in_h[l] = in->h[l]; fp.in_c[l] = in->c[l]; fp.h0s[l] = c->h0s[l]; fp.c0s[l] = c->c0s[l];
-            fp.hprev_h[l] = t->hprev_h[l]; fp.h0_img[l] = t->fplan.ok ? t->h0_img[l] : nullptr;
+            fp.hprev_h[l] = t->hprev_h[l]; fp.h0_img[l] = t->fplan[l].ok ? t->h0_img[l] : nullptr;
             fp.rm[l] = rec_mask(c, l);
+            fp.H[l] = c->width[l + 1]; fp.Hp[l] = t->Xp[l + 1]; fp.GB[l] = t->fplan[l].GBi; fp.Kc[l] = t->fplan[l].Kc;
         }
         fp.x = x; fp.x_saved = c->x_saved;
-        fp.L = L; fp.B = B; fp.H = H; fp.Hp = Hp; fp.GB = t->fplan.GBi; fp.Kc = t->fplan.Kc; fp.N = N;
+        fp.L = L; fp.B = B; fp.N = N;
         ZRB_TRY(fwd_prep(fp, s));
     }
     {
@@ -368,10 +393,13 @@ int tc_forward(zrb_ctx* c, const zrb_params* p, const int64_t* x, const zrb_stat
         // tied: E's update (item L) is still deferred -> gather through it; the update itself rides beside the last
         // recurrence, before the projection reads fc_w_h
         const bool through = ride && c->tied && (t->upd_pending & (1u << L));
-        ZRB_TRY(embed_dropout_fwd(p->embed_w, x, nullptr, t->x_h[0], Hp, N, H, V, site_mask(c, 0), ed_mask(c), s,
+        ZRB_TRY(embed_dropout_fwd(p->embed_w, x, nullptr, t->x_h[0], t->Xp[0], N, c->width[0], V, site_mask(c, 0), ed_mask(c), s,
                                   through ? t->upd_tl.g[tc_matrices(c).fc_w().i] : nullptr, t->upd_lr, c->scalars));
     }
     for (int l = 0; l < L; ++l) {
+        const int In = c->width[l], H = c->width[l + 1], Xi = t->Xp[l], Hp = t->Xp[l + 1];
+        const size_t bh = (size_t)B * H * sizeof(float);
+        const RecPlan& fplan = t->fplan[l];
         float* G = c->gates[l];
         if (!whh_current(c, l)) {
             // weight drop (DESIGN.md section 15): this step's masked images, or the raw ones after a masked step.  After
@@ -382,16 +410,16 @@ int tc_forward(zrb_ctx* c, const zrb_params* p, const int64_t* x, const zrb_stat
         }
         {
             ProfScope ps(c, ZRB_PROF_GEMM_IN, s);
-            ZRB_TRY(gemm_f16_tc(t->x_h[l], Hp, 0, t->w_ih_h[l], Hp, 0, G, 4 * H, N, 4 * H, H, 1.f, p->b_ih[l], 0, s, nullptr,
+            ZRB_TRY(gemm_f16_tc(t->x_h[l], Xi, 0, t->w_ih_h[l], Xi, 0, G, 4 * H, N, 4 * H, In, 1.f, p->b_ih[l], 0, s, nullptr,
                                 p->b_hh[l]));
         }
         MaskSrc m = site_mask(c, l + 1), rm = rec_mask(c, l);
         // AR / TAR (DESIGN.md section 17) reads the last layer's fp32 h (the per-timestep path always writes it)
         const bool reg_h = t->in_train_step && reg_on(c) && l == L - 1;
         ProfScope ps(c, ZRB_PROF_REC_FWD, s);
-        if (t->fplan.ok) {
-            ZRB_TRY(t->fwd_bar.claim(T, t->fplan.nCTA, s, [&](unsigned int* word, unsigned int base) {
-                return lstm_rec_fwd(t->fplan, tc_watchdog(c), t->w_img_f[l], t->h0_img[l], t->h_img, G, c->c0s[l], c->cst[l],
+        if (fplan.ok) {
+            ZRB_TRY(t->fwd_bar.claim(T, fplan.nCTA, s, [&](unsigned int* word, unsigned int base) {
+                return lstm_rec_fwd(fplan, tc_watchdog(c), t->w_img_f[l], t->h0_img[l], t->h_img, G, c->c0s[l], c->cst[l],
                                     out->h[l], out->c[l], t->hprev_h[l], t->x_h[l + 1], word, base, T, B, H, Hp, m, rm, s,
                                     t->trace, reg_h ? c->hraw[l] : nullptr);
             }));
@@ -415,8 +443,9 @@ int tc_forward(zrb_ctx* c, const zrb_params* p, const int64_t* x, const zrb_stat
     if (scores) {
         ProfScope ps(c, ZRB_PROF_PROJ_FWD, s);
         const int rows = last_only ? B : N;
-        ZRB_TRY(gemm_f16_tc(t->x_h[L] + (size_t)(N - rows) * Hp, Hp, 0, t->fc_w_h, Hp, 0, scores, V, rows, V, H, 1.f,
-                            p->fc_b, 0, s));
+        const int Xl = t->Xp[L];
+        ZRB_TRY(gemm_f16_tc(t->x_h[L] + (size_t)(N - rows) * Xl, Xl, 0, t->fc_w_h, Xl, 0, scores, V, rows, V, c->width[L],
+                            1.f, p->fc_b, 0, s));
     }
     return ZRB_OK;
 }
@@ -442,8 +471,8 @@ static float* wgrad_sumsq(zrb_ctx* c, int M, int N, int K) { return wgrad_slots(
 // projection backward: afterwards fc.W / fc.b gradients are complete and c->bwd_dy holds d loss / d act[L]
 static int tc_backward_head(zrb_ctx* c, const zrb_params* p, const zrb_params* g, cudaStream_t s) {
     zrb_tc_state* t = c->tc;
-    const int H = c->cfg.hidden, L = c->cfg.layers, V = c->cfg.vocab, N = c->T * c->B;
-    const int Hp = t->Hp, Vp = t->Vp;
+    const int L = c->cfg.layers, V = c->cfg.vocab, N = c->T * c->B, H = c->width[L];
+    const int Hp = t->Xp[L], Vp = t->Vp;
     const float inv = 1.f / kGradScale;
     float* dY = c->dy;
     c->bwd_dy = c->dy;
@@ -460,7 +489,7 @@ static int tc_backward_head(zrb_ctx* c, const zrb_params* p, const zrb_params* g
         // dW[V,H] = dS^T[V,N] * A[N,H]     (both operands MN-major: contraction over tokens).  Nothing downstream in
         // backward reads it: with deferral on it runs underneath the first backward recurrence instead of before it.
         t->pending = 0;
-        if (t->defer_wgrad && t->bplan.ok && pdl_beside_rec(c)) t->pending = 1;
+        if (t->defer_wgrad && t->persistent() && pdl_beside_rec(c)) t->pending = 1;
         else ZRB_TRY(gemm_f16_tc(t->dS_h, Vp, 1, t->x_h[L], Hp, 1, g->fc_w, H, V, H, N, inv, nullptr, 0, s,
                                  wgrad_sumsq(c, V, H, N)));
     }
@@ -472,12 +501,15 @@ static int tc_backward_head(zrb_ctx* c, const zrb_params* p, const zrb_params* g
 // order makes it scale * m * dW_eff in place and writes its sums of squares into the norm slots instead of the GEMM.
 static int tc_layer_wgrads(zrb_ctx* c, const zrb_params* g, int l, const __half* dG_h, bool pdl, cudaStream_t s) {
     zrb_tc_state* t = c->tc;
-    const int H = c->cfg.hidden, N = c->T * c->B;
+    const int In = c->width[l], H = c->width[l + 1], N = c->T * c->B;
     const MaskSrc wm = wd_mask(c, l);
-    float* ss1 = wgrad_sumsq(c, 4 * H, H, N);
-    float* ss2 = wm.active ? nullptr : wgrad_sumsq(c, 4 * H, H, N);
-    ZRB_TRY(gemm_f16_tc(dG_h, t->G4p, 1, t->x_h[l], t->Hp, 1, g->w_ih[l], H, 4 * H, H, N, 1.f / kGradScale, nullptr, 0, s,
-                        ss1, nullptr, pdl, t->hprev_h[l], g->w_hh[l], ss2));
+    int n1 = 0, n2 = 0;
+    gemm_f16_tc_dual_sumsq_slots(4 * H, In, H, N, &n1, &n2);
+    float* ss1 = wgrad_slots(c, n1);
+    float* ss2 = wm.active ? nullptr : wgrad_slots(c, n2);
+    ZRB_TRY(gemm_f16_tc(dG_h, t->G4p[l], 1, t->x_h[l], t->Xp[l], 1, g->w_ih[l], In, 4 * H, In, N, 1.f / kGradScale, nullptr,
+                        0, s, ss1, nullptr, pdl, t->hprev_h[l], g->w_hh[l], ss2, nullptr, 0, nullptr, 0,
+                        DualB{H, t->Xp[l + 1], H}));
     if (!wm.active) return ZRB_OK;
     return weight_drop(g->w_hh[l], g->w_hh[l], (int64_t)4 * H * H, wm, wgrad_slots(c, kWeightDropBlocks), s);
 }
@@ -486,13 +518,13 @@ static int tc_layer_wgrads(zrb_ctx* c, const zrb_params* g, int l, const __half*
 // that was just enqueued on `s`
 static int tc_issue_pending(zrb_ctx* c, const zrb_params* g, cudaStream_t s) {
     zrb_tc_state* t = c->tc;
-    const int H = c->cfg.hidden, L = c->cfg.layers, V = c->cfg.vocab, N = c->T * c->B;
+    const int L = c->cfg.layers, V = c->cfg.vocab, N = c->T * c->B, H = c->width[L];
     const int kind = t->pending;
     t->pending = 0;
     // (no event bracket here: an event record between the recurrence kernel and its programmatic dependent would sit
     // between the two launches; while profiling with ZRB_PROF_KEEP_PDL=1 the time lands in the enclosing REC_BWD class)
     if (kind == 1) {
-        return gemm_f16_tc(t->dS_h, t->Vp, 1, t->x_h[L], t->Hp, 1, g->fc_w, H, V, H, N, 1.f / kGradScale, nullptr, 0, s,
+        return gemm_f16_tc(t->dS_h, t->Vp, 1, t->x_h[L], t->Xp[L], 1, g->fc_w, H, V, H, N, 1.f / kGradScale, nullptr, 0, s,
                            wgrad_sumsq(c, V, H, N), nullptr, true);
     }
     if (kind == 2) {
@@ -506,9 +538,10 @@ static int tc_issue_pending(zrb_ctx* c, const zrb_params* g, cudaStream_t s) {
 // gradients are complete; l == 0 also finishes the embedding gradient
 static int tc_backward_layer(zrb_ctx* c, const zrb_params* p, const zrb_params* g, int l, cudaStream_t s) {
     zrb_tc_state* t = c->tc;
-    const int H = c->cfg.hidden, V = c->cfg.vocab, T = c->T, B = c->B, N = T * B;
-    const int Hp = t->Hp, G4p = t->G4p;
+    const int In = c->width[l], H = c->width[l + 1], V = c->cfg.vocab, T = c->T, B = c->B, N = T * B;
+    const int Xi = t->Xp[l], Hp = t->Xp[l + 1], G4p = t->G4p[l];
     const size_t bh = (size_t)B * H;
+    const RecPlan& bplan = t->bplan[l];
     const float inv = 1.f / kGradScale;
     if (l != c->bwd_next_layer) {
         set_error("backward layers must be visited in order L-1..0 (expected %d, got %d)", c->bwd_next_layer, l);
@@ -520,10 +553,10 @@ static int tc_backward_layer(zrb_ctx* c, const zrb_params* p, const zrb_params* 
     const float* r = (c->reg_use && l == c->cfg.layers - 1) ? c->reg_r : nullptr;   // AR / TAR gradient (section 17)
     {
         MaskSrc m = site_mask(c, l + 1), rm = rec_mask(c, l);
-        if (t->bplan.ok) {
+        if (bplan.ok) {
             ProfScope ps(c, ZRB_PROF_REC_BWD, s);
-            ZRB_TRY(t->bwd_bar.claim(T, t->bplan.nCTA, s, [&](unsigned int* word, unsigned int base) {
-                return lstm_rec_bwd(t->bplan, tc_watchdog(c), t->w_img_b[l], t->g_img, dY, c->gates[l], c->cst[l], c->c0s[l],
+            ZRB_TRY(t->bwd_bar.claim(T, bplan.nCTA, s, [&](unsigned int* word, unsigned int base) {
+                return lstm_rec_bwd(bplan, tc_watchdog(c), t->w_img_b[l], t->g_img, dY, c->gates[l], c->cst[l], c->c0s[l],
                                     dG_h, word, base, T, B, H, G4p, m, rm, s,
                                     t->trace ? t->trace + 8 + (size_t)c->cfg.max_seq * 8 : nullptr, g->b_ih[l], g->b_hh[l],
                                     c->resident_flag, ++c->resident_seq, c->dG /* [N,4H] fp32, idle on this path */, r);
@@ -545,18 +578,18 @@ static int tc_backward_layer(zrb_ctx* c, const zrb_params* p, const zrb_params* 
         }
         {
             ProfScope ps(c, ZRB_PROF_GEMM_DX, s);
-            ZRB_TRY(gemm_f16_tc(dG_h, G4p, 0, t->w_ih_h[l], Hp, 1, dX, H, N, H, 4 * H, inv, nullptr, 0, s));
+            ZRB_TRY(gemm_f16_tc(dG_h, G4p, 0, t->w_ih_h[l], Xi, 1, dX, In, N, In, 4 * H, inv, nullptr, 0, s));
         }
         // dW_ih, dW_hh: nothing downstream in backward reads them -> for l > 0 they run underneath the next layer's
         // recurrence (which writes the other dG buffer); the bias gradients come out of the recurrence kernel itself
-        if (t->defer_wgrad && t->bplan.ok && l > 0 && pdl_beside_rec(c)) {
+        if (t->defer_wgrad && bplan.ok && l > 0 && pdl_beside_rec(c)) {
             t->pending = 2;
             t->pending_layer = l;
         } else {
             ProfScope ps(c, ZRB_PROF_GEMM_WGRAD, s);
             ZRB_TRY(tc_layer_wgrads(c, g, l, dG_h, false, s));
         }
-        if (!t->bplan.ok) ZRB_TRY(colsum(c->dG, g->b_ih[l], g->b_hh[l], N, 4 * H, s));
+        if (!bplan.ok) ZRB_TRY(colsum(c->dG, g->b_ih[l], g->b_hh[l], N, 4 * H, s));
         float* tmp = dY; dY = dX; dX = tmp;
     }
     c->bwd_dy = dY;
@@ -564,21 +597,22 @@ static int tc_backward_layer(zrb_ctx* c, const zrb_params* p, const zrb_params* 
     c->bwd_next_layer = l - 1;
     if (l > 0) return ZRB_OK;
     ProfScope ps(c, ZRB_PROF_EMBED_BWD, s);
+    const int E = In;   // dY now holds d loss / d act[0], [N, E]
     const MaskSrc m0 = site_mask(c, 0), em = ed_mask(c);
-    if (c->embed_rows_out) return embed_rows(dY, c->x_saved, c->embed_rows_out, N, H, V, m0, em, s);
+    if (c->embed_rows_out) return embed_rows(dY, c->x_saved, c->embed_rows_out, N, E, V, m0, em, s);
     if (c->tied) {
         // g->embed_w holds G_proj (the projection's wgrad GEMM overwrote every row): add the fixed-point row sums, with
         // dX (free now) as the rows buffer; the fused norm's extra slots get the correction from G_proj^2 to dE^2
-        ZRB_TRY(embed_rows(dY, c->x_saved, dX, N, H, V, m0, em, s));
-        return embed_scatter_rows(c->x_saved, dX, g->embed_w, N, H, V, c->emb_first, c->emb_acc, s, true,
+        ZRB_TRY(embed_rows(dY, c->x_saved, dX, N, E, V, m0, em, s));
+        return embed_scatter_rows(c->x_saved, dX, g->embed_w, N, E, V, c->emb_first, c->emb_acc, s, true,
                                   c->fused_norm ? c->partials + norm_partials_base() : nullptr, kNormExtra);
     }
     if (c->emb_sparse && c->emb_prev_grad == g->embed_w) {
-        ZRB_TRY(embed_zero_rows(g->embed_w, c->emb_prev_ids, c->emb_prev_n, H, V, s));   // only last window's rows are non-zero
+        ZRB_TRY(embed_zero_rows(g->embed_w, c->emb_prev_ids, c->emb_prev_n, E, V, s));   // only last window's rows are non-zero
     } else {
-        ZRB_CUDA(cudaMemsetAsync(g->embed_w, 0, (size_t)V * H * sizeof(float), s));
+        ZRB_CUDA(cudaMemsetAsync(g->embed_w, 0, (size_t)V * E * sizeof(float), s));
     }
-    ZRB_TRY(embed_dropout_bwd(dY, c->x_saved, g->embed_w, N, H, V, m0, em, s));
+    ZRB_TRY(embed_dropout_bwd(dY, c->x_saved, g->embed_w, N, E, V, m0, em, s));
     if (c->emb_sparse) {
         ZRB_CUDA(cudaMemcpyAsync(c->emb_prev_ids, c->x_saved, (size_t)N * sizeof(int64_t), cudaMemcpyDeviceToDevice, s));
         c->emb_prev_n = N;
@@ -659,10 +693,10 @@ int tc_train_step_layer(zrb_ctx* c, const zrb_params* p, const zrb_params* g, in
     return tc_backward_layer(c, p, g, l, s);
 }
 
-bool tc_persistent_bwd(const zrb_ctx* c) { return c->tc && c->tc->bplan.ok; }
+bool tc_persistent_bwd(const zrb_ctx* c) { return c->tc && c->tc->persistent(); }
 
-void tc_rec_plans(const zrb_ctx* c, int32_t* h_out) {
-    const RecPlan* plans[2] = {&c->tc->fplan, &c->tc->bplan};
+void tc_rec_plans(const zrb_ctx* c, int l, int32_t* h_out) {
+    const RecPlan* plans[2] = {&c->tc->fplan[l], &c->tc->bplan[l]};
     for (int d = 0; d < 2; ++d) {
         const RecPlan& p = *plans[d];
         int32_t* o = h_out + 8 * d;
@@ -678,8 +712,9 @@ void tc_rec_plans(const zrb_ctx* c, int32_t* h_out) {
 int tc_layer_fwd(zrb_ctx* c, const float* w_ih, const float* w_hh, const float* b_ih, const float* b_hh, const float* x,
                  int T, int B, const float* h0, const float* c0, float* y, float* hT, float* cT, cudaStream_t s) {
     zrb_tc_state* t = c->tc;
-    const int H = c->cfg.hidden, N = T * B, Hp = t->Hp;
-    if (!t->fplan.ok || !t->bplan.ok) {
+    const int H = c->cfg.hidden, N = T * B, Hp = t->Xp[0];   // (a context of one width: every pitch is Hp)
+    const RecPlan &fplan = t->fplan[0], &bplan = t->bplan[0];
+    if (!fplan.ok || !bplan.ok) {
         set_error("zrb_lstm_layer_fwd needs the persistent recurrence kernels (shape H=%d B=%d does not fit them)", H, B);
         return ZRB_E_INVALID;
     }
@@ -688,19 +723,19 @@ int tc_layer_fwd(zrb_ctx* c, const float* w_ih, const float* w_hh, const float* 
     t->packed_version = 0;                       // slot 0 is about to hold this call's weights
     t->whh_img[0].kind = zrb_tc_state::kWhhStale;
     ZRB_TRY(convert_pad_f16(w_ih, H, t->w_ih_h[0], Hp, 4 * H, H, 1.f, s));
-    ZRB_TRY(pack_whh_fwd(w_hh, t->w_img_f[0], H, t->fplan, s));
-    ZRB_TRY(pack_whh_bwd(w_hh, t->w_img_b[0], H, t->bplan, s));
+    ZRB_TRY(pack_whh_fwd(w_hh, t->w_img_f[0], H, fplan, s));
+    ZRB_TRY(pack_whh_bwd(w_hh, t->w_img_b[0], H, bplan, s));
     ZRB_TRY(convert_pad_f16(x, H, t->x_h[0], Hp, N, H, 1.f, s));
     FwdPrep fp = {};
     fp.in_h[0] = h0; fp.in_c[0] = c0; fp.h0s[0] = c->h0s[0]; fp.c0s[0] = c->c0s[0];
     fp.hprev_h[0] = t->hprev_h[0]; fp.h0_img[0] = t->h0_img[0];
     fp.x = nullptr; fp.x_saved = nullptr;
-    fp.L = 1; fp.B = B; fp.H = H; fp.Hp = Hp; fp.GB = t->fplan.GBi; fp.Kc = t->fplan.Kc; fp.N = 0;
+    fp.L = 1; fp.B = B; fp.H[0] = H; fp.Hp[0] = Hp; fp.GB[0] = fplan.GBi; fp.Kc[0] = fplan.Kc; fp.N = 0;
     ZRB_TRY(fwd_prep(fp, s));
     ZRB_TRY(gemm_f16_tc(t->x_h[0], Hp, 0, t->w_ih_h[0], Hp, 0, c->gates[0], 4 * H, N, 4 * H, H, 1.f, b_ih, 0, s, nullptr, b_hh));
     MaskSrc m = make_mask_src(nullptr, 0, 0, 0, 0.f, 0);    // no dropout at this level: the caller applies it (model.py:105,108)
-    ZRB_TRY(t->fwd_bar.claim(T, t->fplan.nCTA, s, [&](unsigned int* word, unsigned int base) {
-        return lstm_rec_fwd(t->fplan, tc_watchdog(c), t->w_img_f[0], t->h0_img[0], t->h_img, c->gates[0], c->c0s[0], c->cst[0],
+    ZRB_TRY(t->fwd_bar.claim(T, fplan.nCTA, s, [&](unsigned int* word, unsigned int base) {
+        return lstm_rec_fwd(fplan, tc_watchdog(c), t->w_img_f[0], t->h0_img[0], t->h_img, c->gates[0], c->c0s[0], c->cst[0],
                             hT, cT, t->hprev_h[0], t->x_h[1], word, base, T, B, H, Hp, m, m, s, nullptr, y);
     }));
     c->have_fwd = false;                         // a model-level backward must not follow this
@@ -711,14 +746,15 @@ int tc_layer_fwd(zrb_ctx* c, const float* w_ih, const float* w_hh, const float* 
 int tc_layer_bwd(zrb_ctx* c, const float* dy, float* dx, float* dw_ih, float* dw_hh, float* db_ih, float* db_hh,
                  cudaStream_t s) {
     zrb_tc_state* t = c->tc;
-    const int H = c->cfg.hidden, T = c->T, B = c->B, N = T * B, Hp = t->Hp, G4p = t->G4p;
+    const int H = c->cfg.hidden, T = c->T, B = c->B, N = T * B, Hp = t->Xp[0], G4p = t->G4p[0];
+    const RecPlan& bplan = t->bplan[0];
     if (!c->layer_fwd_ok) {
         set_error("zrb_lstm_layer_bwd without a preceding zrb_lstm_layer_fwd");
         return ZRB_E_STATE;
     }
     MaskSrc m = make_mask_src(nullptr, 0, 0, 0, 0.f, 0);
-    ZRB_TRY(t->bwd_bar.claim(T, t->bplan.nCTA, s, [&](unsigned int* word, unsigned int base) {
-        return lstm_rec_bwd(t->bplan, tc_watchdog(c), t->w_img_b[0], t->g_img, dy, c->gates[0], c->cst[0], c->c0s[0], t->dG_h,
+    ZRB_TRY(t->bwd_bar.claim(T, bplan.nCTA, s, [&](unsigned int* word, unsigned int base) {
+        return lstm_rec_bwd(bplan, tc_watchdog(c), t->w_img_b[0], t->g_img, dy, c->gates[0], c->cst[0], c->c0s[0], t->dG_h,
                             word, base, T, B, H, G4p, m, m, s, nullptr, db_ih, db_hh, c->resident_flag, ++c->resident_seq, c->dG);
     }));
     const float inv = 1.f / kGradScale;
@@ -744,7 +780,7 @@ int tc_rec_trace(zrb_ctx* c, long long* h_out, int max_entries) {
 int tc_update(zrb_ctx* c, const zrb_params* p, const TensorList& tl, float lr, float max_norm, float* norm_out,
               const AvgStep* avg, cudaStream_t s) {
     zrb_tc_state* t = c->tc;
-    const int H = c->cfg.hidden, V = c->cfg.vocab;
+    const int E = c->width[0], V = c->cfg.vocab;
     ZRB_TRY(tc_flush_updates(c, s));   // (a second update without a forward in between)
     ProfScope ps(c, ZRB_PROF_CLIP_SGD, s);
     if (!tc_streams_aligned(tl, avg ? avg->a : nullptr)) {   // images rebuilt by the next forward's pack
@@ -770,10 +806,10 @@ int tc_update(zrb_ctx* c, const zrb_params* p, const TensorList& tl, float lr, f
         ZRB_TRY(grad_norm(dense, max_norm, c->partials, c->scalars, norm_out, s, true, t->wg_slots));
     } else if (rows_only) {
         ZRB_TRY(embed_first_table(c->emb_prev_ids, c->emb_first, c->emb_prev_n, V, s));
-        ZRB_TRY(embed_rows_sumsq(tl.g[0], c->emb_prev_ids, c->emb_first, c->emb_prev_n, H, V,
+        ZRB_TRY(embed_rows_sumsq(tl.g[0], c->emb_prev_ids, c->emb_first, c->emb_prev_n, E, V,
                                  c->partials + norm_partials_base(), kNormExtra, s));   // one token per block
         ZRB_TRY(grad_norm(dense, max_norm, c->partials, c->scalars, norm_out, s, true, gemm_norm ? t->wg_slots : 0));
-        ZRB_TRY(embed_rows_update(tl.p[0], tl.g[0], c->emb_prev_ids, c->emb_first, c->emb_prev_n, H, V, lr, c->scalars,
+        ZRB_TRY(embed_rows_update(tl.p[0], tl.g[0], c->emb_prev_ids, c->emb_first, c->emb_prev_n, E, V, lr, c->scalars,
                                   c->keep_clipped, s));
         if (avg) {   // the average is dense: every row moves toward the new embedding
             TensorList e{};

@@ -50,8 +50,10 @@ struct GemmArgs {
     int splits;      // split-K factor (1 or 2); with 2 the epilogue adds atomically into a zeroed C
     float* sumsq_out; // or null: slot [tile * 8 + w] = sum of squares of the outputs consumer warp w stored for `tile`
                       // (the wgrads feed clip_grad_norm_ from here instead of re-reading 200 MB of gradients)
-    float* C2;        // dual launch (or null): a second problem with the same A, shapes and pitches but its own B (tma_b2),
-    float* sumsq_out2;  // output and sum-of-squares slots; work items [num_tiles, 2*num_tiles) belong to it (splits == 1)
+    float* C2;        // dual launch (or null): a second problem with the same A, M and K but its own B (tma_b2), N2, C2
+    float* sumsq_out2;  // pitch, output and sum-of-squares slots; work items [num_tiles, num_tiles + tiles_m * tiles_n2)
+    int N2, tiles_n2;   // belong to it, tile w - num_tiles (splits == 1)
+    int64_t ldc2;
     const __half* a_tiled;   // EXPERIMENT (zrb_gemm_f16_tiled): pre-tiled, pre-swizzled K-major images ([K block][128-row
     const __half* b_tiled;   // tile][128][64] halves, chunk c of row r stored at c ^ (r % 8)): operand tiles are fetched with
     int a_nt128, b_nt128;    // 1-D bulk copies instead of 2-D tensor loads
@@ -91,8 +93,10 @@ gemm_f16_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_const
     const int num_tiles = p.tiles_m * p.tiles_n;
     const int num_kb = (p.K + GBK - 1) / GBK;
     const bool dual = p.C2 != nullptr;
-    const int num_work = dual ? 2 * num_tiles : num_tiles * p.splits;   // work item w: tile = w % num_tiles; w / num_tiles =
-    const int kb_per = (num_kb + p.splits - 1) / p.splits;              //   K range (split-K) or problem (dual launch)
+    // work item w: tile = w % num_tiles and K range w / num_tiles (split-K), or tile w - num_tiles of the second problem
+    // once w >= num_tiles (dual launch)
+    const int num_work = dual ? num_tiles + p.tiles_m * p.tiles_n2 : num_tiles * p.splits;
+    const int kb_per = (num_kb + p.splits - 1) / p.splits;
 
     if (threadIdx.x == 0) {
         if (p.pdl_trigger) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
@@ -110,9 +114,10 @@ gemm_f16_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_const
         if (warp == 0 && lane == 0) {
             int s = 0; uint32_t ph = 0;
             for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
-                const int tile = w % num_tiles, sp = dual ? 0 : w / num_tiles;
+                const bool second = dual && w >= num_tiles;
+                const int tile = second ? w - num_tiles : w % num_tiles, sp = dual ? 0 : w / num_tiles;
                 const int kb0 = sp * kb_per, kb1 = min(num_kb, kb0 + kb_per);
-                const CUtensorMap* tmb = (dual && w >= num_tiles) ? &tma_b2 : &tma_b;
+                const CUtensorMap* tmb = second ? &tma_b2 : &tma_b;
                 const int m0 = (tile % p.tiles_m) * GBM, n0 = (tile / p.tiles_m) * GBN;
                 for (int kb = kb0; kb < kb1; ++kb) {
                     mbar_wait(&empty[s], ph ^ 1);
@@ -152,13 +157,16 @@ gemm_f16_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_const
         if (!p.epi_direct && wg == 1) asm volatile("bar.sync %0, 256;" :: "n"(kStaggerBar) : "memory");
         int kb_issued = 0;
         // float2 stores (and float2 atomics for split-K): a quad of lanes writes one whole 32-byte sector of a row
-        const bool pair_store = !p.epi_direct && !p.accumulate && (p.ldc & 1) == 0 && ((uintptr_t)p.C & 7) == 0 &&
-                                ((uintptr_t)p.C2 & 7) == 0;
+        const bool pair_store = !p.epi_direct && !p.accumulate && (p.ldc & 1) == 0 && (p.ldc2 & 1) == 0 &&
+                                ((uintptr_t)p.C & 7) == 0 && ((uintptr_t)p.C2 & 7) == 0;
         for (int w = blockIdx.x; w < num_work; w += gridDim.x) {
-            const int tile = w % num_tiles, split = dual ? 0 : w / num_tiles;
+            const bool second = dual && w >= num_tiles;
+            const int tile = second ? w - num_tiles : w % num_tiles, split = dual ? 0 : w / num_tiles;
             const int kb0 = split * kb_per, kb1 = min(num_kb, kb0 + kb_per);
-            float* const Cout = (dual && w >= num_tiles) ? p.C2 : p.C;
-            float* const ssq = (dual && w >= num_tiles) ? p.sumsq_out2 : p.sumsq_out;
+            float* const Cout = second ? p.C2 : p.C;
+            float* const ssq = second ? p.sumsq_out2 : p.sumsq_out;
+            const int Nw = second ? p.N2 : p.N;
+            const int64_t ldcw = second ? p.ldc2 : p.ldc;
             const int m0 = (tile % p.tiles_m) * GBM + 64 * wg, n0 = (tile / p.tiles_m) * GBN;
 #pragma unroll
             for (int i = 0; i < GBN / 2; ++i) acc[i] = 0.f;
@@ -212,11 +220,11 @@ gemm_f16_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_const
             for (int h = 0; h < 2; ++h) {
                 const int row = m0 + wgmma_row(t, h);
                 if (row >= p.M) continue;
-                float* const crow = Cout + (int64_t)row * p.ldc;
+                float* const crow = Cout + (int64_t)row * ldcw;
 #pragma unroll
                 for (int c8 = 0; c8 < GBN / 8; ++c8) {
                     const int col0 = n0 + wgmma_col(t, c8);   // even
-                    if (pair_store && col0 + 1 < p.N) {
+                    if (pair_store && col0 + 1 < Nw) {
                         // the same two elements, values and sum-of-squares order as the per-element loop below
                         const float bv0 = add_bias ? p.bias[col0] + (p.bias2 ? p.bias2[col0] : 0.f) : 0.f;
                         const float bv1 = add_bias ? p.bias[col0 + 1] + (p.bias2 ? p.bias2[col0 + 1] : 0.f) : 0.f;
@@ -234,7 +242,7 @@ gemm_f16_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_const
 #pragma unroll
                     for (int e = 0; e < 2; ++e) {
                         const int col = n0 + wgmma_col(t, c8) + e;
-                        if (col >= p.N) continue;
+                        if (col >= Nw) continue;
                         const float bv = add_bias ? p.bias[col] + (p.bias2 ? p.bias2[col] : 0.f) : 0.f;
                         const float o = p.alpha * acc[4 * c8 + 2 * h + e] + bv;
                         if (p.splits > 1) {
@@ -332,7 +340,8 @@ static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const CUten
         ZRB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmCfg<GBN>::kSmem));
         g_attr_set[dev][idx] = true;
     }
-    int grid = a.tiles_m * a.tiles_n * (a.C2 ? 2 : a.splits);
+    const int work = a.C2 ? a.tiles_m * (a.tiles_n + a.tiles_n2) : a.tiles_m * a.tiles_n * a.splits;
+    int grid = work;
     if (grid > tc_num_sms()) grid = tc_num_sms();
     if (a.pdl_tail) {
         // programmatic dependent launch: the grid may start as soon as every CTA of the preceding kernel has executed
@@ -341,7 +350,7 @@ static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const CUten
         // here (not the persistent one-CTA-per-SM grid): the hardware block scheduler then hands tiles to whichever
         // SMs are free, so the idle SMs work through most of the tiles while the recurrence runs, instead of each
         // late CTA still owning a full static share of them.
-        grid = a.tiles_m * a.tiles_n * (a.C2 ? 2 : a.splits);
+        grid = work;
         cudaLaunchConfig_t cfg = {};
         cfg.gridDim = dim3(grid); cfg.blockDim = dim3(kGemmThreads);
         cfg.dynamicSmemBytes = GemmCfg<GBN>::kSmem; cfg.stream = s;
@@ -405,12 +414,24 @@ int gemm_f16_tc_sumsq_slots(int M, int N, int K) {
     return c.tiles_m * c.tiles_n * kEpiWarps;
 }
 
+// A dual launch takes the tile width of its wider problem; both problems are cut into tiles of that width
+static TileChoice choose_dual_tiles(int M, int N1, int N2, int K) {
+    return choose_tiles(M, N1 > N2 ? N1 : N2, cdiv(K, GBK), false);
+}
+void gemm_f16_tc_dual_sumsq_slots(int M, int N1, int N2, int K, int* n1, int* n2) {
+    const TileChoice c = choose_dual_tiles(M, N1, N2, K);
+    *n1 = c.tiles_m * cdiv(N1, c.bn) * kEpiWarps;
+    *n2 = c.tiles_m * cdiv(N2, c.bn) * kEpiWarps;
+}
+
 int gemm_f16_tc(const __half* A, int64_t lda, int a_mn, const __half* B, int64_t ldb, int b_mn, float* C, int64_t ldc,
                 int M, int N, int K, float alpha, const float* bias, int accumulate, cudaStream_t s, float* sumsq_out,
                 const float* bias2, bool pdl, const __half* B2, float* C2, float* sumsq_out2, const __half* A_tiled,
-                int a_nt128, const __half* B_tiled, int b_nt128) {
+                int a_nt128, const __half* B_tiled, int b_nt128, DualB d2) {
     if (M <= 0 || N <= 0) return ZRB_OK;
     ZRB_REQUIRE(!B2 == !C2, "dual launch needs both B2 and C2");
+    if (d2.N == 0) d2 = DualB{N, ldb, ldc};
+    ZRB_REQUIRE(!C2 || (d2.N > 0 && !bias && !accumulate), "dual launch: N2 > 0, no bias, no accumulate");
     ZRB_REQUIRE(!bias2 || bias, "bias2 needs bias");
     ZRB_REQUIRE(!sumsq_out || !accumulate, "sumsq_out needs a plain store epilogue");
     ZRB_REQUIRE(K > 0, "gemm_f16_tc needs K > 0");
@@ -418,8 +439,9 @@ int gemm_f16_tc(const __half* A, int64_t lda, int a_mn, const __half* B, int64_t
     // comparisons, bit for bit and in time); read at every launch so that one process can run both
     const char* epi = getenv("ZRB_GEMM_EPI");
     const bool direct = epi && strcmp(epi, "direct") == 0;
-    const TileChoice tc = choose_tiles(M, N, cdiv(K, GBK), !sumsq_out && ldc == N && !C2 && !accumulate,
-                                       !direct && !sumsq_out && !C2 && !accumulate);
+    const TileChoice tc = C2 ? choose_dual_tiles(M, N, d2.N, K)
+                             : choose_tiles(M, N, cdiv(K, GBK), !sumsq_out && ldc == N && !accumulate,
+                                            !direct && !sumsq_out && !accumulate);
     const int bn = tc.bn;
     CUtensorMap ta, tb;
     if (!a_mn) ZRB_TRY(tc_make_tmap_f16(&ta, A, K, M, lda, GBK, GBM, 1));
@@ -428,16 +450,17 @@ int gemm_f16_tc(const __half* A, int64_t lda, int a_mn, const __half* B, int64_t
     else       ZRB_TRY(tc_make_tmap_f16(&tb, B, N, K, ldb, 64, GBK, 1));
     CUtensorMap tb2 = tb;
     if (B2) {
-        if (!b_mn) ZRB_TRY(tc_make_tmap_f16(&tb2, B2, K, N, ldb, GBK, bn, 1));
-        else       ZRB_TRY(tc_make_tmap_f16(&tb2, B2, N, K, ldb, 64, GBK, 1));
+        if (!b_mn) ZRB_TRY(tc_make_tmap_f16(&tb2, B2, K, d2.N, d2.ldb, GBK, bn, 1));
+        else       ZRB_TRY(tc_make_tmap_f16(&tb2, B2, d2.N, K, d2.ldb, 64, GBK, 1));
     }
     GemmArgs a;
     a.M = M; a.N = N; a.K = K; a.alpha = alpha; a.bias = bias; a.C = C; a.ldc = ldc; a.accumulate = accumulate;
-    a.tiles_m = tc.tiles_m; a.tiles_n = tc.tiles_n;
+    a.tiles_m = tc.tiles_m; a.tiles_n = cdiv(N, bn);   // (a dual plan's tile width comes from the wider problem)
     a.splits = tc.splits;
     a.sumsq_out = sumsq_out;
     a.bias2 = bias2;
     a.C2 = C2; a.sumsq_out2 = sumsq_out2;
+    a.N2 = d2.N; a.ldc2 = d2.ldc; a.tiles_n2 = cdiv(d2.N, bn);
     a.a_tiled = a_mn ? nullptr : A_tiled; a.a_nt128 = a_nt128; a.b_tiled = b_mn ? nullptr : B_tiled; a.b_nt128 = b_nt128;
     a.pdl_tail = (pdl && a.splits == 1) ? 1 : 0;    // (a split launch is preceded by a memset: nothing to chain to)
     a.pdl_trigger = (rec_pdl_enabled() && !a.pdl_tail) ? 1 : 0;

@@ -117,15 +117,19 @@ struct BeamCand {
     float cand, logp;
     uint32_t flat;
 };
+// the state width of each layer (the states of layer l are [rows, h[l]])
+struct LayerWidths {
+    int h[ZRB_MAX_LAYERS];
+};
 // ZRB_E_INVALID for the arguments zrb_beam_step / zrb_beam_search reject (B, beam width K, vocabulary V, eos)
 int beam_check(int B, int K, int V, int eos);
 // One selection step (DESIGN.md section 10) over B prompts of K_in rows of scores [B*K_in, ld]: cum_in [B*K_in] (NULL:
 // all 0), tok_in [B*K_in] (NULL: no row finished); outputs [B*K].  cands: B*K_in*K entries of scratch.  With L > 0 the
-// (h, c) rows of every layer are gathered from src (row b*K_in + parent) to dst (row b*K + k); src and dst must not
+// (h, c) rows of every layer (widths w) are gathered from src (row b*K_in + parent) to dst (row b*K + k); src and dst must not
 // alias.  Two launches.
 int beam_step(const float* scores, int64_t ld, int B, int K_in, int K, int V, const float* cum_in, const int64_t* tok_in,
               int eos, BeamCand* cands, int64_t* tokens, int32_t* parents, float* cum_out, float* logprobs,
-              const zrb_states* src, const zrb_states* dst, int L, int H, cudaStream_t s);
+              const zrb_states* src, const zrb_states* dst, int L, const LayerWidths& w, cudaStream_t s);
 // per-step [n_new, BK] tokens / parents / logprobs -> the hypotheses [n_new, B, K] of each final slot; scores = cum
 int beam_backtrack(const int64_t* step_tok, const int32_t* step_par, const float* step_lp, const float* cum, int n_new,
                    int BK, int K, int64_t* tokens, float* logprobs, float* scores, cudaStream_t s);

@@ -47,8 +47,9 @@ int convert_pad_f16(const float* src, int64_t ld_src, __half* dst, int64_t ld_ds
 
 __global__ void fwd_prep_kernel(FwdPrep a) {
     const int tid = blockIdx.x * blockDim.x + threadIdx.x, nth = gridDim.x * blockDim.x;
-    const int bh = a.B * a.H, bhp = a.B * a.Hp, img_n = a.Kc * a.GB * 64;
     for (int l = 0; l < a.L; ++l) {
+        const int H = a.H[l], Hp = a.Hp[l], GB = a.GB[l];
+        const int bh = a.B * H, bhp = a.B * Hp, img_n = a.Kc[l] * GB * 64;
         const float* __restrict__ h = a.in_h[l];
         const float* __restrict__ c = a.in_c[l];
         const MaskSrc rm = a.rm[l];   // variational mode: the recurrent operand of step 0 is h0 * rm
@@ -57,23 +58,24 @@ __global__ void fwd_prep_kernel(FwdPrep a) {
             a.c0s[l][i] = c[i];
         }
         for (int i = tid; i < bhp; i += nth) {
-            const int r = i / a.Hp, col = i % a.Hp;
+            const int r = i / Hp, col = i % Hp;
             a.hprev_h[l][i] = __float2half_rn(
-                col < a.H ? h[(size_t)r * a.H + col] * mask_mul1_at(rm, (uint64_t)r * a.H + col, (uint64_t)bh) : 0.f);
+                col < H ? h[(size_t)r * H + col] * mask_mul1_at(rm, (uint64_t)r * H + col, (uint64_t)bh) : 0.f);
         }
         if (a.h0_img[l]) {
             for (int i = tid; i < img_n; i += nth) {
-                const int e = i & 7, r = (i >> 3) & 7, g = (i >> 6) % a.GB, kc = (i >> 6) / a.GB;
+                const int e = i & 7, r = (i >> 3) & 7, g = (i >> 6) % GB, kc = (i >> 6) / GB;
                 const int b = g * 8 + r, k = kc * 8 + e;
                 a.h0_img[l][i] = __float2half_rn(
-                    (b < a.B && k < a.H) ? h[(size_t)b * a.H + k] * mask_mul1_at(rm, (uint64_t)b * a.H + k, (uint64_t)bh) : 0.f);
+                    (b < a.B && k < H) ? h[(size_t)b * H + k] * mask_mul1_at(rm, (uint64_t)b * H + k, (uint64_t)bh) : 0.f);
             }
         }
     }
     for (int i = tid; i < a.N; i += nth) a.x_saved[i] = a.x[i];
 }
 int fwd_prep(const FwdPrep& a, cudaStream_t s) {
-    const int work = max(max(a.B * a.Hp, a.Kc * a.GB * 64), a.N);
+    int work = a.N;
+    for (int l = 0; l < a.L; ++l) work = max(work, max(a.B * a.Hp[l], a.Kc[l] * a.GB[l] * 64));
     int blocks = cdiv(work, 256);
     if (blocks > 132 * 2) blocks = 132 * 2;
     if (blocks < 1) blocks = 1;

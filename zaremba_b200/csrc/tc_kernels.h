@@ -81,7 +81,9 @@ struct FwdPrep {
     MaskSrc rm[ZRB_MAX_LAYERS];
     const int64_t* x;
     int64_t* x_saved;
-    int L, B, H, Hp, GB, Kc, N;
+    int H[ZRB_MAX_LAYERS], Hp[ZRB_MAX_LAYERS];   // layer l's width and the pitch of its hprev_h rows
+    int GB[ZRB_MAX_LAYERS], Kc[ZRB_MAX_LAYERS];  // ... and the shape of its h0_img (layer l's forward plan)
+    int L, B, N;
 };
 int fwd_prep(const FwdPrep& a, cudaStream_t s);
 // The fp16 operand images of one weight matrix, as the fused update rewrites them from registers.  Default: no image.

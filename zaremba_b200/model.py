@@ -17,6 +17,7 @@ from __future__ import annotations
 
 import ctypes as C
 import math
+import operator
 
 import torch
 from torch import nn
@@ -25,7 +26,7 @@ from . import _lib
 
 
 class Embed(nn.Module):
-    """Parameter holder for `embed.W` [V,H] (model.py:6-17)."""
+    """Parameter holder for `embed.W` [V,E] (model.py:6-17; E = H unless `Model(embed_size=E)`)."""
 
     def __init__(self, vocab_size, embed_size):
         super().__init__()
@@ -40,17 +41,18 @@ class LSTM(nn.Module):
     """Parameter holder for one recurrent layer.
 
     lstm_type "pytorch": torch.nn.LSTM names and gate order (i,f,g,o) (model.py:84);
-    constructing it consumes the global RNG exactly like nn.LSTM.__init__ does (four
-    U(-1/sqrt(H), 1/sqrt(H)) draws), so that a seeded `Model(...)` gets the reference's
-    weights.  lstm_type "custom": the reference's own cell (model.py:20-31): names
-    W_x/W_h/b_x/b_h, row blocks (i,f,o,n), no RNG consumption.
+    constructing it consumes the global RNG exactly like nn.LSTM(input_size, hidden_size).__init__
+    does (four U(-1/sqrt(H), 1/sqrt(H)) draws: [4H,In], [4H,H], [4H], [4H]), so that a seeded
+    `Model(...)` gets the reference's weights.  lstm_type "custom": the reference's own cell
+    (model.py:20-31): names W_x/W_h/b_x/b_h, row blocks (i,f,o,n), no RNG consumption, H->H only.
     """
 
     def __init__(self, input_size, hidden_size, lstm_type="pytorch"):
         super().__init__()
-        assert input_size == hidden_size, "the reference only builds H->H layers"
+        if lstm_type == "custom" and input_size != hidden_size:
+            raise ValueError("lstm_type 'custom' builds H->H layers only")
         self.input_size, self.hidden_size, self.lstm_type = input_size, hidden_size, lstm_type
-        H = hidden_size
+        H, In = hidden_size, input_size
         if lstm_type == "custom":
             self.W_x = nn.Parameter(torch.empty(4 * H, H))
             self.W_h = nn.Parameter(torch.empty(4 * H, H))
@@ -58,7 +60,7 @@ class LSTM(nn.Module):
             self.b_h = nn.Parameter(torch.empty(4 * H))
         else:
             stdv = 1.0 / math.sqrt(H)
-            self.weight_ih_l0 = nn.Parameter(torch.empty(4 * H, H).uniform_(-stdv, stdv))
+            self.weight_ih_l0 = nn.Parameter(torch.empty(4 * H, In).uniform_(-stdv, stdv))
             self.weight_hh_l0 = nn.Parameter(torch.empty(4 * H, H).uniform_(-stdv, stdv))
             self.bias_ih_l0 = nn.Parameter(torch.empty(4 * H).uniform_(-stdv, stdv))
             self.bias_hh_l0 = nn.Parameter(torch.empty(4 * H).uniform_(-stdv, stdv))
@@ -73,7 +75,7 @@ class LSTM(nn.Module):
 
 
 class Linear(nn.Module):
-    """Parameter holder for `fc.W` [V,H], `fc.b` [V] (model.py:57-71)."""
+    """Parameter holder for `fc.W` [V,H_{L-1}], `fc.b` [V] (model.py:57-71)."""
 
     def __init__(self, input_size, hidden_size):
         super().__init__()
@@ -83,6 +85,48 @@ class Linear(nn.Module):
 
     def extra_repr(self):
         return f"input: {self.input_size}, output: {self.hidden_size}"
+
+
+def _check_widths(hidden_size, layer_num, embed_size, layer_sizes):
+    """(E, layer widths) of a Model, or ValueError"""
+    def width(v, what):
+        try:
+            n = operator.index(v)
+        except TypeError:
+            n = 0
+        if isinstance(v, bool) or n < 1:
+            raise ValueError(f"{what} must be a positive int, got {v!r}")
+        return n
+    H = width(hidden_size, "hidden_size")
+    E = H if embed_size is None else width(embed_size, "embed_size")
+    if layer_sizes is None:
+        return E, (H,) * layer_num
+    sizes = tuple(width(v, "every entry of layer_sizes") for v in layer_sizes)
+    if len(sizes) != layer_num:
+        raise ValueError(f"layer_sizes has {len(sizes)} entries for {layer_num} layers")
+    if sizes[0] != H:
+        raise ValueError(f"hidden_size ({H}) must equal layer_sizes[0] ({sizes[0]})")
+    return E, sizes
+
+
+def model_from_state_dict(state_dict, dropout=0.0, winit=0.0, tied=None, **kwargs):
+    """A `Model` shaped like `state_dict` (pytorch layout) with its values loaded: V and E from `embed.W`, the layer
+    widths from each `rnns.l.weight_hh_l0`, tied (None) when `fc.W` equals `embed.W`.  kwargs go to `Model`."""
+    E_w = torch.as_tensor(state_dict["embed.W"])
+    V, E = E_w.shape
+    sizes, l = [], 0
+    while f"rnns.{l}.weight_hh_l0" in state_dict:
+        sizes.append(int(torch.as_tensor(state_dict[f"rnns.{l}.weight_hh_l0"]).shape[1]))
+        l += 1
+    if not sizes:
+        raise ValueError("state_dict has no rnns.<l>.weight_hh_l0 (lstm_type 'pytorch' layout expected)")
+    fc_w = torch.as_tensor(state_dict["fc.W"])
+    if tied is None:
+        tied = fc_w.shape == E_w.shape and torch.equal(fc_w.cpu(), E_w.cpu())
+    m = Model(int(V), sizes[0], len(sizes), dropout, winit, tied=tied, embed_size=int(E), layer_sizes=tuple(sizes),
+              **kwargs)
+    m.load_state_dict(state_dict)
+    return m
 
 
 def _ifon_to_ifgo(t):
@@ -144,11 +188,27 @@ class Model(nn.Module):
     of `embed.W` scaled by 1 / (1 - p), before the dropout after the embedding; the gradient reaching `embed.W` is
     masked alike.  Tied: only the lookup is masked, the projection uses the raw matrix.  Eval mode, `generate` and
     `beam_search` use the raw rows.  Seeded like `weight_drop` (no rank in it).
+
+    Extra keywords `embed_size` / `layer_sizes`: layers of unequal width (DESIGN.md section 18), e.g. AWD-LSTM's PTB
+    model `Model(10000, 1150, 3, p, winit, tied=True, embed_size=400, layer_sizes=(1150, 1150, 400))`.  `embed.W` is
+    [V,E], layer l is an nn.LSTM(In_l, H_l) with In_0 = E and In_l = H_{l-1}, `fc.W` is [V,H_{L-1}], and the states of
+    layer l are [1,B,H_l].  `embed_size` defaults to `hidden_size`, `layer_sizes` to (hidden_size,) * layer_num; given,
+    it has layer_num entries and the first is `hidden_size`.  `tied=True` needs E = H_{L-1}.  Unequal widths take the
+    tensor-core engine and lstm_type "pytorch".  With every width equal this is the model above, bit for bit.
     """
 
     def __init__(self, vocab_size, hidden_size, layer_num, dropout, winit, lstm_type="pytorch", engine="tc",
-                 variational=False, recurrent_dropout=None, *, tied=False, weight_drop=0.0, embed_dropout=0.0):
+                 variational=False, recurrent_dropout=None, *, tied=False, weight_drop=0.0, embed_dropout=0.0,
+                 embed_size=None, layer_sizes=None):
         super().__init__()
+        E, sizes = _check_widths(hidden_size, layer_num, embed_size, layer_sizes)
+        equal = all(w == E for w in sizes)
+        if not equal and lstm_type == "custom":
+            raise ValueError("layers of unequal width need lstm_type 'pytorch'")
+        if not equal and engine == "simt":
+            raise ValueError("layers of unequal width need the tensor-core engine (engine='tc')")
+        if tied and E != sizes[-1]:
+            raise ValueError(f"tied=True needs embed_size = layer_sizes[-1] (got {E} and {sizes[-1]})")
         if lstm_type not in ("pytorch", "custom"):
             raise ValueError(f"lstm_type must be 'pytorch' or 'custom', got {lstm_type!r}")
         if isinstance(weight_drop, bool) or not isinstance(weight_drop, (int, float)) or \
@@ -182,9 +242,12 @@ class Model(nn.Module):
         self.tied = tied
         self.weight_drop = float(weight_drop)
         self.embed_dropout = float(embed_dropout)
-        self.embed = Embed(vocab_size, hidden_size)
-        self.rnns = nn.ModuleList(LSTM(hidden_size, hidden_size, lstm_type) for _ in range(layer_num))
-        self.fc = Linear(hidden_size, vocab_size)
+        self.embed_size = E
+        self.layer_sizes = sizes
+        self._widths_given = embed_size is not None or layer_sizes is not None
+        self.embed = Embed(vocab_size, E)
+        self.rnns = nn.ModuleList(LSTM(([E] + list(sizes))[l], sizes[l], lstm_type) for l in range(layer_num))
+        self.fc = Linear(sizes[-1], vocab_size)
         if tied:
             self.fc.W = self.embed.W
         self.dropout = nn.Dropout(p=dropout)     # kept for repr / state parity; masks come from the library
@@ -206,8 +269,13 @@ class Model(nn.Module):
 
     def state_init(self, batch_size):
         dev = next(self.parameters()).device
-        shape = (batch_size, self.hidden_size) if self.lstm_type == "custom" else (1, batch_size, self.hidden_size)
-        return [(torch.zeros(shape, device=dev), torch.zeros(shape, device=dev)) for _ in self.rnns]
+        return [(torch.zeros(s, device=dev), torch.zeros(s, device=dev)) for s in self._state_shapes(batch_size)]
+
+    def _state_shapes(self, batch_size):
+        """the (h, c) shape of every layer for `batch_size` rows"""
+        if self.lstm_type == "custom":
+            return [(batch_size, H) for H in self.layer_sizes]
+        return [(1, batch_size, H) for H in self.layer_sizes]
 
     def detach(self, states):
         return [(h.detach(), c.detach()) for (h, c) in states]
@@ -280,8 +348,7 @@ class Model(nn.Module):
             self._note_param_versions()
             ps, keep_w = self._params_struct(self._lib_weights())   # custom layout: permuted once per call
             st_in, keep_in = self._states_struct(states)
-            shape = (B, self.hidden_size) if self.lstm_type == "custom" else (1, B, self.hidden_size)
-            out_states = [(torch.empty(shape, device=dev), torch.empty(shape, device=dev)) for _ in range(self.layer_num)]
+            out_states = [(torch.empty(s, device=dev), torch.empty(s, device=dev)) for s in self._state_shapes(B)]
             st_out, keep_out = self._states_struct(out_states)
             tokens = torch.empty(int(n_new), B, dtype=torch.int64, device=dev)
             logprobs = torch.empty(int(n_new), B, dtype=torch.float32, device=dev)
@@ -332,8 +399,7 @@ class Model(nn.Module):
             self._note_param_versions()
             ps, keep_w = self._params_struct(self._lib_weights())   # custom layout: permuted once per call
             st_in, keep_in = self._states_struct(states)
-            shape = (B * K, self.hidden_size) if self.lstm_type == "custom" else (1, B * K, self.hidden_size)
-            out_states = [(torch.empty(shape, device=dev), torch.empty(shape, device=dev)) for _ in range(self.layer_num)]
+            out_states = [(torch.empty(s, device=dev), torch.empty(s, device=dev)) for s in self._state_shapes(B * K)]
             st_out, keep_out = self._states_struct(out_states)
             tokens = torch.empty(int(n_new), B, K, dtype=torch.int64, device=dev)
             logprobs = torch.empty(int(n_new), B, K, dtype=torch.float32, device=dev)
@@ -373,7 +439,7 @@ class Model(nn.Module):
         return self._seed, step
 
     def set_explicit_dropout_masks(self, masks):
-        """Replay given keep-masks (list of L+1 uint8/bool CUDA tensors [T,B,H]) instead of
+        """Replay given keep-masks (list of L+1 uint8/bool CUDA tensors [T,B,W], W = the site's width) instead of
         Philox; None restores Philox.  Used by parity tests with the reference's masks.  They are Zaremba's per-step
         masks: a model in the variational mode refuses them."""
         if masks is not None and self.variational:
@@ -406,12 +472,18 @@ class Model(nn.Module):
                 _lib.check(_lib.load().zrb_flush_updates(self._ctx, torch.cuda.current_stream(dev).cuda_stream))
             self._destroy_ctx()
         lib = _lib.load()
-        cfg = _lib.ZrbConfig(self.vocab_size, self.hidden_size, self.layer_num, key[0], key[1],
+        # a model given its widths takes zrb_ctx_create_widths, which equals zrb_ctx_create at equal widths
+        widths = [self.embed_size, *self.layer_sizes]
+        equal = not self._widths_given
+        cfg = _lib.ZrbConfig(self.vocab_size, self.hidden_size if equal else 0, self.layer_num, key[0], key[1],
                              _lib.ENGINE_TC if self.engine == "tc" else _lib.ENGINE_SIMT, self.p_drop,
                              _lib.TIED_EMBEDDING if self.tied else 0)
         h = C.c_void_p()
         with torch.cuda.device(self.embed.W.device):
-            _lib.check(lib.zrb_ctx_create(C.byref(cfg), C.byref(h)))
+            if equal:
+                _lib.check(lib.zrb_ctx_create(C.byref(cfg), C.byref(h)))
+            else:
+                _lib.check(lib.zrb_ctx_create_widths(C.byref(cfg), (C.c_int32 * len(widths))(*widths), C.byref(h)))
         self._ctx, self._ctx_key = h, key
         self._ctx_serial += 1          # a new context may reuse the old one's address: this tells them apart
         self._versions = None

@@ -178,9 +178,9 @@ class Trainer:
         _lib.check(_lib.load().zrb_set_keep_clipped_grads(self.ctx, 1 if self._keep_clipped else 0))
         _lib.check(_lib.load().zrb_set_lazy_update(self.ctx, 1 if self._lazy else 0))
         if self.world > 1 and self._embed_sparse == 2:
-            H, N = model.hidden_size, batch_size * seq_length
-            self._rows = torch.zeros(N, H, device=dev)
-            self._rows_all = torch.zeros(self.world * N, H, device=dev)
+            E, N = model.embed_size, batch_size * seq_length    # embedding rows are E wide
+            self._rows = torch.zeros(N, E, device=dev)
+            self._rows_all = torch.zeros(self.world * N, E, device=dev)
             self._ids_all = torch.zeros(self.world * N, dtype=torch.int64, device=dev)
             # (the rows buffer is handed to the context only for the duration of a DP step, see _grads_ce)
 
