@@ -78,6 +78,25 @@ typedef struct {
     float* fc_b;                          /* [V]     fc.b                 model.py:63 */
 } zrb_params;
 
+/* Mixture of Softmaxes (Yang, Dai, Salakhutdinov & Cohen, "Breaking the Softmax Bottleneck", ICLR 2018; DESIGN.md
+ * section 19 states it bit for bit).  A context created by zrb_ctx_create_mos with K = experts takes, wherever an entry
+ * point takes a `const zrb_params*`, a pointer to the `base` of a zrb_mos_params (parameters, gradients and averages
+ * alike): the three head tensors follow the 3 + 4L of zrb_params, which keeps its size for every other context.
+ * With h [N, H_{L-1}] the last layer's output after its dropout (site L), E the embedding width and W = fc_w [V,E]:
+ *   u = h latent_w^T + latent_b [N, K*E];  c = tanh(u);  c^ = c * m / (1 - p_l), m = latent dropout, Philox site 3L + 2,
+ *       element (t, b, j) = stream element t*B*K*E + b*K*E + j (variational mode: b*K*E + j), the other sites' seed
+ *       and step, no mask in eval mode;
+ *   a = h prior_w^T [N, K] (no bias), pi = softmax(a);  z_k = c^_k W^T + fc_b [V], q_k = softmax(z_k);
+ *   p = sum_k pi_k q_k, and log p[y] = logsumexp_k(log pi_k + z_k[y] - LSE(z_k)).
+ * The loss is zrb_softmax_nll's unit, B/N * sum_n -log p_n[y_n]. */
+#define ZRB_MAX_EXPERTS  32
+typedef struct {
+    zrb_params base;
+    float* prior_w;                       /* [K, H_{L-1}]    prior.W  */
+    float* latent_w;                      /* [K*E, H_{L-1}]  latent.W */
+    float* latent_b;                      /* [K*E]           latent.b */
+} zrb_mos_params;
+
 /* (h, c) entering / leaving the BPTT window: model.py:94-98.  [B,H] fp32 each (the
  * pytorch path's [1,B,H] has the same bytes); [B,H_l] for layer l of a context of per-layer widths. */
 typedef struct {
@@ -101,6 +120,20 @@ int  zrb_ctx_create(const zrb_config* cfg, zrb_ctx** out);
  * _bwd return ZRB_E_INVALID on a context of unequal widths.  The neural cache takes H = H_{L-1}.  zrb_ctx_create's
  * other rules apply. */
 int  zrb_ctx_create_widths(const zrb_config* cfg, const int32_t* widths, zrb_ctx** out);
+/* A Mixture-of-Softmaxes context (zrb_mos_params above) of K = experts softmaxes, 1 <= K <= ZRB_MAX_EXPERTS.  widths as
+ * zrb_ctx_create_widths (cfg->hidden = 0), or NULL for one width cfg->hidden.  fc_w is [V,E]; a tied context needs
+ * nothing beyond that (E = H_{L-1} is not required).  In such a context zrb_forward writes log p into scores [N,V] and
+ * zrb_backward takes dL / d log p; the fused train steps (_grads / _begin / _layer / _host / _update, the lazy update),
+ * zrb_eval_step, averaging and swapping, zrb_generate, zrb_beam_step and zrb_beam_search work as documented, and the
+ * variational mode, weight drop, embedding dropout and AR / TAR act below the head.  Its score workspace holds N*K
+ * logits rows (zrb_ctx_workspace_bytes reports it).  ZRB_E_INVALID, before anything is launched, for K outside
+ * [1, ZRB_MAX_EXPERTS], ZRB_ENGINE_SIMT, more layers than the fused step's tensor list holds (L <= 3), and -- follow-ups
+ * not built yet -- zrb_eval_step_cache, zrb_grad_stats_step / _finish, zrb_dyneval_step and zrb_set_embed_rows_out
+ * (data parallel) on such a context. */
+int  zrb_ctx_create_mos(const zrb_config* cfg, const int32_t* widths, int32_t experts, zrb_ctx** out);
+/* Latent dropout p_l of a Mixture-of-Softmaxes context (0 by default; train mode only).  ZRB_E_INVALID for p outside
+ * [0, 1) or not finite and for a context without experts.  A change invalidates the saved forward. */
+int  zrb_set_mos_dropout(zrb_ctx* ctx, float p);
 void zrb_ctx_destroy(zrb_ctx* ctx);
 /* bytes of device memory the context holds */
 int64_t zrb_ctx_workspace_bytes(const zrb_ctx* ctx);

@@ -42,6 +42,10 @@ ap.add_argument("--embed_size", type=int, default=None,
                 help="embedding width E (default: --hidden_size); with --tied it must equal the last layer's width")
 ap.add_argument("--layer_sizes", type=lambda s: tuple(int(v) for v in s.split(",")), default=None,
                 help="one width per layer, e.g. AWD-LSTM's 1150,1150,400; sets --hidden_size and --layer_num")
+ap.add_argument("--experts", type=int, default=None,
+                help="a Mixture-of-Softmaxes head of this many softmaxes (Yang et al. 2018; e.g. 15 with --embed_size 280 "
+                     "--layer_sizes 960,960,620 --tied)")
+ap.add_argument("--mos_dropout", type=float, default=0.0, help="latent dropout of the --experts head")
 ap.add_argument("--dropout", type=float, default=0.5)
 ap.add_argument("--winit", type=float, default=0.05)
 ap.add_argument("--batch_size", type=int, default=20)
@@ -89,13 +93,17 @@ if args.layer_sizes is not None:
     args.hidden_size, args.layer_num = args.layer_sizes[0], len(args.layer_sizes)
 if args.impl == "cudnn" and (args.embed_size is not None or args.layer_sizes is not None):
     raise SystemExit("--embed_size / --layer_sizes are modes of --impl ours")
+if args.impl == "cudnn" and (args.experts is not None or args.mos_dropout):
+    raise SystemExit("--experts / --mos_dropout are modes of --impl ours")
+if args.mos_dropout and args.experts is None:
+    raise SystemExit("--mos_dropout needs --experts")
 if args.embed_size is not None or args.layer_sizes is not None:
     from zaremba_b200.model import _check_widths
     try:
         _E, _sizes = _check_widths(args.hidden_size, args.layer_num, args.embed_size, args.layer_sizes)
     except ValueError as e:
         raise SystemExit(f"--embed_size / --layer_sizes: {e}")
-    if args.tied and _E != _sizes[-1]:
+    if args.tied and _E != _sizes[-1] and args.experts is None:
         raise SystemExit(f"--tied needs --embed_size equal to the last layer's width ({_E} != {_sizes[-1]})")
 
 
@@ -131,7 +139,8 @@ if args.impl == "ours":
     model = zaremba_b200.Model(vocab, args.hidden_size, args.layer_num, args.dropout, args.winit,
                                variational=args.variational, recurrent_dropout=args.recurrent_dropout,
                                tied=args.tied, weight_drop=args.weight_drop, embed_dropout=args.embed_dropout,
-                               embed_size=args.embed_size, layer_sizes=args.layer_sizes).to(dev)
+                               embed_size=args.embed_size, layer_sizes=args.layer_sizes, experts=args.experts,
+                               mos_dropout=args.mos_dropout).to(dev)
     tr = zaremba_b200.Trainer(model, B, T, lazy_update=args.lazy_update, ar=args.ar, tar=args.tar)
     # the corpus is staged on the device once (SURVEY 8f#2): 3 x [n_batches, T, B] int64
     trn_x = torch.stack([x for x, _ in trn_b]).contiguous().to(dev)

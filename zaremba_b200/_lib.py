@@ -12,6 +12,7 @@ from . import build as _build
 
 MAX_LAYERS = 8
 MAX_BEAMS = 32
+MAX_EXPERTS = 32
 ENGINE_SIMT = 0
 ENGINE_TC = 1
 TIED_EMBEDDING = 1   # zrb_config.flags bit ZRB_TIED_EMBEDDING
@@ -33,6 +34,12 @@ class ZrbParams(C.Structure):
                 ("fc_w", _vp), ("fc_b", _vp)]
 
 
+class ZrbMosParams(ZrbParams):
+    """zrb_mos_params: a ZrbParams (its `base`) followed by the Mixture-of-Softmaxes head; passes wherever a
+    POINTER(ZrbParams) is expected"""
+    _fields_ = [("prior_w", _vp), ("latent_w", _vp), ("latent_b", _vp)]
+
+
 class ZrbStates(C.Structure):
     _fields_ = [("h", _vp * MAX_LAYERS), ("c", _vp * MAX_LAYERS)]
 
@@ -52,6 +59,8 @@ _SIGNATURES = {
     "zrb_launch_count": (C.c_int64, []),
     "zrb_ctx_create": (C.c_int, [C.POINTER(ZrbConfig), C.POINTER(_vp)]),
     "zrb_ctx_create_widths": (C.c_int, [C.POINTER(ZrbConfig), C.POINTER(C.c_int32), C.POINTER(_vp)]),
+    "zrb_ctx_create_mos": (C.c_int, [C.POINTER(ZrbConfig), C.POINTER(C.c_int32), C.c_int32, C.POINTER(_vp)]),
+    "zrb_set_mos_dropout": (C.c_int, [_vp, C.c_float]),
     "zrb_ctx_destroy": (None, [_vp]),
     "zrb_ctx_workspace_bytes": (C.c_int64, [_vp]),
     "zrb_params_changed": (C.c_int, [_vp]),

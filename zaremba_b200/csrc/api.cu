@@ -98,6 +98,21 @@ MaskSrc ed_mask(const zrb_ctx* c) {
     return make_mask_src(nullptr, c->ed_seed, c->step, 3 * c->cfg.layers + 1, c->p_ed, c->train);
 }
 
+MaskSrc mos_mask(const zrb_ctx* c) {
+    MaskSrc m = make_mask_src(nullptr, c->seed, c->step, 3 * c->cfg.layers + 2, c->p_mos, c->train);
+    if (c->variational) m.period = (uint32_t)c->B * (uint32_t)(c->experts * c->width[0]);   // element (t, b, j): b*K*E + j
+    return m;
+}
+
+// the tensors of param_list(): 3 + 4L, and the head's three with experts
+static int tensor_count(const zrb_ctx* c) { return 4 * c->cfg.layers + 3 + (c->experts ? 3 : 0); }
+
+// ZRB_E_INVALID for an entry point a Mixture-of-Softmaxes context does not support yet
+static int refuse_experts(const zrb_ctx* c, const char* what) {
+    ZRB_REQUIRE(!c->experts, "%s does not support a Mixture-of-Softmaxes context (experts = %d)", what, c->experts);
+    return ZRB_OK;
+}
+
 static cudaEvent_t prof_event(zrb_ctx* c) {
     if (!c->prof_pool.empty()) {
         cudaEvent_t e = c->prof_pool.back();
@@ -130,8 +145,8 @@ const char* zrb_last_error(void) { return t_err; }
 const char* zrb_version(void) { return "zaremba_b200 0.1 (sm_90a)"; }
 int64_t zrb_launch_count(void) { return g_launches.load(); }
 
-// zrb_ctx_create and zrb_ctx_create_widths: widths[0] = E, widths[1 + l] = H_l (already checked)
-static int ctx_create(const zrb_config* cfg, const int* widths, zrb_ctx** out) {
+// zrb_ctx_create, zrb_ctx_create_widths and zrb_ctx_create_mos: widths[0] = E, widths[1 + l] = H_l (already checked)
+static int ctx_create(const zrb_config* cfg, const int* widths, zrb_ctx** out, int experts = 0) {
     ZRB_REQUIRE(cfg->max_seq > 0 && cfg->max_batch > 0, "bad window T=%d B=%d", cfg->max_seq, cfg->max_batch);
     ZRB_REQUIRE(cfg->dropout >= 0.f && cfg->dropout < 1.f, "dropout %f outside [0,1)", cfg->dropout);
     ZRB_REQUIRE(cfg->engine == ZRB_ENGINE_SIMT || cfg->engine == ZRB_ENGINE_TC, "unknown engine %d", cfg->engine);
@@ -144,6 +159,7 @@ static int ctx_create(const zrb_config* cfg, const int* widths, zrb_ctx** out) {
     zrb_ctx* c = new zrb_ctx();
     c->cfg = *cfg;
     c->tied = (cfg->flags & ZRB_TIED_EMBEDDING) != 0;
+    c->experts = experts;
     const int L = cfg->layers, V = cfg->vocab;
     bool equal = true;
     for (int s = 0; s <= L; ++s) {
@@ -232,6 +248,40 @@ int zrb_ctx_create_widths(const zrb_config* cfg, const int32_t* widths, zrb_ctx*
     int w[ZRB_MAX_LAYERS + 1];
     for (int s = 0; s <= L; ++s) w[s] = widths[s];
     return ctx_create(cfg, w, out);
+}
+
+int zrb_ctx_create_mos(const zrb_config* cfg, const int32_t* widths, int32_t experts, zrb_ctx** out) {
+    ZRB_REQUIRE(cfg && out, "null argument");
+    ZRB_REQUIRE(experts >= 1 && experts <= ZRB_MAX_EXPERTS, "experts=%d outside [1, %d]", experts, ZRB_MAX_EXPERTS);
+    ZRB_REQUIRE(cfg->engine == ZRB_ENGINE_TC, "a Mixture-of-Softmaxes context needs the tensor-core engine");
+    ZRB_REQUIRE(cfg->vocab > 0 && cfg->layers > 0 && 4 * cfg->layers + 6 <= kMaxTensors,
+                "bad model shape V=%d L=%d (a Mixture-of-Softmaxes context takes at most 3 layers)", cfg->vocab,
+                cfg->layers);
+    const int L = cfg->layers;
+    int w[ZRB_MAX_LAYERS + 1];
+    if (widths) {
+        ZRB_REQUIRE(cfg->hidden == 0, "cfg->hidden must be 0 when the widths are given (got %d)", cfg->hidden);
+        for (int s = 0; s <= L; ++s) {
+            ZRB_REQUIRE(widths[s] > 0, "width %d of site %d must be >= 1", widths[s], s);
+            w[s] = widths[s];
+        }
+    } else {
+        ZRB_REQUIRE(cfg->hidden > 0, "bad model shape H=%d", cfg->hidden);
+        for (int s = 0; s <= L; ++s) w[s] = cfg->hidden;
+    }
+    return ctx_create(cfg, w, out, experts);
+}
+
+int zrb_set_mos_dropout(zrb_ctx* c, float p) {
+    ZRB_REQUIRE(c, "null ctx");
+    ZRB_REQUIRE(c->experts > 0, "latent dropout needs a Mixture-of-Softmaxes context");
+    ZRB_REQUIRE(isfinite(p) && p >= 0.f && p < 1.f, "latent-dropout p %f outside [0,1)", p);
+    if (p != c->p_mos) {
+        c->have_fwd = false;        // a backward must not regenerate another mask than its forward used
+        c->bwd_next_layer = -1;
+    }
+    c->p_mos = p;
+    return ZRB_OK;
 }
 
 void zrb_ctx_destroy(zrb_ctx* c) {
@@ -453,6 +503,8 @@ int zrb_set_average(zrb_ctx* c, const zrb_params* avg) {
     ZRB_REQUIRE(!c->avg_swapped, "the parameters hold the average (zrb_swap_average): swap back first");
     if (avg) {
         ZRB_REQUIRE(avg->embed_w && avg->fc_w && avg->fc_b, "null average tensor");
+        ZRB_REQUIRE(!c->experts || (mos_of(avg)->prior_w && mos_of(avg)->latent_w && mos_of(avg)->latent_b),
+                    "null average tensor of the Mixture-of-Softmaxes head");
         for (int l = 0; l < c->cfg.layers; ++l)
             ZRB_REQUIRE(avg->w_ih[l] && avg->w_hh[l] && avg->b_ih[l] && avg->b_hh[l], "null average tensor of layer %d", l);
         ZRB_TRY(check_tied(c, avg));
@@ -464,7 +516,7 @@ int zrb_set_average(zrb_ctx* c, const zrb_params* avg) {
     // deferred updates belong to the steps before: they average (or not) with the n they were issued with
     if (c->cfg.engine == ZRB_ENGINE_TC) ZRB_TRY(tc_flush_updates(c, nullptr));
     c->avg_on = avg != nullptr;
-    if (avg) c->avg = *avg;
+    if (avg) memcpy(&c->avg, avg, c->experts ? sizeof(zrb_mos_params) : sizeof(zrb_params));
     c->avg_n = 0;
     return ZRB_OK;
 }
@@ -480,7 +532,7 @@ int zrb_swap_average(zrb_ctx* c, const zrb_params* p, void* stream) {
     ZRB_TRY(watchdog_check(c));
     ZRB_TRY(check_tied(c, p));
     ZRB_REQUIRE(c->avg_on && c->avg_n > 0, "no average to swap in: no train step has been averaged since zrb_set_average");
-    const TensorList tl = param_list(c, p, p), ta = param_list(c, &c->avg, &c->avg);
+    const TensorList tl = param_list(c, p, p), ta = param_list(c, &c->avg.base, &c->avg.base);
     ZRB_TRY(check_avg_alias(ta, tl, false));
     cudaStream_t s = (cudaStream_t)stream;
     if (c->cfg.engine == ZRB_ENGINE_TC) {
@@ -506,9 +558,16 @@ static TensorList param_list(const zrb_ctx* c, const zrb_params* p, const zrb_pa
         tl.p[k] = p->b_ih[l]; tl.g[k] = g->b_ih[l]; tl.n[k++] = 4 * H;
         tl.p[k] = p->b_hh[l]; tl.g[k] = g->b_hh[l]; tl.n[k++] = 4 * H;
     }
-    tl.p[k] = p->fc_w; tl.g[k] = g->fc_w; tl.n[k++] = V * c->width[c->cfg.layers];
+    const int64_t H = c->width[c->cfg.layers], E = c->width[0], K = c->experts;
+    tl.p[k] = p->fc_w; tl.g[k] = g->fc_w; tl.n[k++] = V * (K ? E : H);
     if (c->tied) tl.n[0] = 0;   // E once, at fc.W's slot (zero-length entries are skipped by the norm and the update)
     tl.p[k] = p->fc_b; tl.g[k] = g->fc_b; tl.n[k++] = V;
+    if (K) {   // the Mixture-of-Softmaxes head (zrb_mos_params)
+        const zrb_mos_params *pm = mos_of(p), *gm = mos_of(g);
+        tl.p[k] = pm->prior_w; tl.g[k] = gm->prior_w; tl.n[k++] = K * H;
+        tl.p[k] = pm->latent_w; tl.g[k] = gm->latent_w; tl.n[k++] = K * E * H;
+        tl.p[k] = pm->latent_b; tl.g[k] = gm->latent_b; tl.n[k++] = K * E;
+    }
     tl.count = k;
     return tl;
 }
@@ -517,7 +576,7 @@ int zrb_train_step_grads(zrb_ctx* c, const zrb_params* p, const zrb_params* g, c
                          int32_t T, int32_t B, const zrb_states* in, const zrb_states* out, uint64_t seed,
                          uint64_t step, float* loss, void* stream) {
     ZRB_REQUIRE(c && p && g && x && y && in && out, "null argument");
-    ZRB_REQUIRE(c->cfg.layers * 4 + 3 <= 16, "fused step supports at most 3 layers");
+    ZRB_REQUIRE(tensor_count(c) <= kMaxTensors, "fused step supports at most 3 layers");
     ZRB_TRY(check_not_swapped(c));
     cudaStream_t s = (cudaStream_t)stream;
     ZRB_TRY(check_shapes(c, T, B));
@@ -604,6 +663,7 @@ int zrb_rec_plans_layer(const zrb_ctx* c, int32_t layer, int32_t* h_out) {
 
 int zrb_set_embed_rows_out(zrb_ctx* c, float* rows) {
     ZRB_REQUIRE(c, "null ctx");
+    ZRB_TRY(refuse_experts(c, "zrb_set_embed_rows_out (data parallel)"));
     c->embed_rows_out = rows;
     return ZRB_OK;
 }
@@ -642,7 +702,7 @@ int zrb_train_step_update(zrb_ctx* c, const zrb_params* p, const zrb_params* g, 
                           float* norm_out, void* stream) {
     ZRB_REQUIRE(c && p && g, "null argument");
     ZRB_TRY(watchdog_check(c));
-    ZRB_REQUIRE(c->cfg.layers * 4 + 3 <= 16, "fused step supports at most 3 layers");
+    ZRB_REQUIRE(tensor_count(c) <= kMaxTensors, "fused step supports at most 3 layers");
     ZRB_TRY(check_tied(c, p));
     ZRB_TRY(check_tied(c, g));
     ZRB_TRY(check_not_swapped(c));
@@ -652,7 +712,7 @@ int zrb_train_step_update(zrb_ctx* c, const zrb_params* p, const zrb_params* g, 
     AvgStep as{};
     const AvgStep* avg = nullptr;
     if (c->avg_on) {
-        const TensorList ta = param_list(c, &c->avg, &c->avg);
+        const TensorList ta = param_list(c, &c->avg.base, &c->avg.base);
         ZRB_TRY(check_avg_alias(ta, tl, true));
         for (int i = 0; i < ta.count; ++i) as.a[i] = ta.p[i];
         as.mu = (float)(1.0 / (double)(c->avg_n + 1));
@@ -680,6 +740,12 @@ int zrb_eval_step(zrb_ctx* c, const zrb_params* p, const int64_t* x, const int64
     ZRB_REQUIRE(c && p && x && y && in && out, "null argument");
     ZRB_TRY(check_shapes(c, T, B));
     ZRB_TRY(check_tied(c, p));
+    if (c->experts) {
+        c->T = T; c->B = B; c->train = 0; c->seed = 0; c->step = 0;
+        c->have_fwd = false;  // eval keeps nothing for backward
+        c->reg_use = false;
+        return tc_mos_eval_step(c, p, x, y, in, out, loss, tgt_prob, (cudaStream_t)stream);
+    }
     ZRB_TRY(zrb_forward(c, p, x, T, B, in, out, c->scores, 0, 0, 0, stream));
     c->have_fwd = false;  // eval keeps nothing for backward
     return softmax_nll(c->scores, y, T * B, c->cfg.vocab, B, c->row_loss, loss, nullptr, tgt_prob,
@@ -703,7 +769,8 @@ int zrb_grad_stats_step(zrb_ctx* c, const zrb_params* p, const zrb_params* g, co
                         const int64_t* y, int32_t T, int32_t B, const zrb_states* in, const zrb_states* out, float* loss,
                         void* stream) {
     ZRB_REQUIRE(c && p && g && ms && x && y && in && out, "null argument");
-    ZRB_REQUIRE(c->cfg.layers * 4 + 3 <= 16, "gradient statistics support at most 3 layers");
+    ZRB_REQUIRE(tensor_count(c) <= kMaxTensors, "gradient statistics support at most 3 layers");
+    ZRB_TRY(refuse_experts(c, "gradient statistics"));
     ZRB_TRY(check_shapes(c, T, B));
     ZRB_TRY(check_tied(c, p));
     ZRB_TRY(check_tied(c, g));
@@ -716,7 +783,8 @@ int zrb_grad_stats_step(zrb_ctx* c, const zrb_params* p, const zrb_params* g, co
 int zrb_grad_stats_finish(zrb_ctx* c, const zrb_params* ms, int64_t windows, float* rms_mean, void* stream) {
     ZRB_REQUIRE(c && ms && rms_mean, "null argument");
     ZRB_REQUIRE(windows >= 1, "windows=%lld must be >= 1", (long long)windows);
-    ZRB_REQUIRE(c->cfg.layers * 4 + 3 <= 16, "gradient statistics support at most 3 layers");
+    ZRB_REQUIRE(tensor_count(c) <= kMaxTensors, "gradient statistics support at most 3 layers");
+    ZRB_TRY(refuse_experts(c, "gradient statistics"));
     ZRB_TRY(check_tied(c, ms));
     if (!c->stats_partials) ZRB_TRY(dalloc(c, &c->stats_partials, kStatsPartials));
     return stats_finish(param_list(c, ms, ms), windows, c->stats_partials, rms_mean, (cudaStream_t)stream);
@@ -727,7 +795,8 @@ int zrb_dyneval_step(zrb_ctx* c, const zrb_params* p, const zrb_params* g, const
                      int32_t B, const zrb_states* in, const zrb_states* out, float lr, float lambda, float eps,
                      float* loss, void* stream) {
     ZRB_REQUIRE(c && p && g && global && x && y && in && out, "null argument");
-    ZRB_REQUIRE(c->cfg.layers * 4 + 3 <= 16, "dynamic evaluation supports at most 3 layers");
+    ZRB_REQUIRE(tensor_count(c) <= kMaxTensors, "dynamic evaluation supports at most 3 layers");
+    ZRB_TRY(refuse_experts(c, "dynamic evaluation"));
     ZRB_REQUIRE(isfinite(lr) && lr >= 0.f, "lr %f must be finite and >= 0", lr);
     ZRB_REQUIRE(isfinite(lambda) && lambda >= 0.f, "lambda %f must be finite and >= 0", lambda);
     ZRB_REQUIRE(!rms || rms_mean, "the RMS rule needs rms_mean");

@@ -66,10 +66,10 @@ constexpr int kListThreads = 256;
 constexpr int kListBlocks = 148 * 16;
 
 struct AvgRuns {
-    float* p[16];
-    float* g[16];
-    float* a[16];
-    int64_t n[16];
+    float* p[kMaxTensors];
+    float* g[kMaxTensors];
+    float* a[kMaxTensors];
+    int64_t n[kMaxTensors];
 };
 
 static int avg_runs(const TensorList& tl, float* const* a, AvgRuns* d, int* bx) {

@@ -460,6 +460,7 @@ int zrb_eval_step_cache(zrb_ctx* c, const zrb_params* p, const int64_t* x, const
                         const zrb_states* in, const zrb_states* out, zrb_cache* cache, float theta, float lambda,
                         float* loss, float* tgt_prob, float* cache_prob, void* stream) {
     ZRB_REQUIRE(c && p && x && y && in && out && cache, "null argument");
+    ZRB_REQUIRE(!c->experts, "the neural cache does not support a Mixture-of-Softmaxes context (experts = %d)", c->experts);
     ZRB_TRY(check_theta(theta));
     ZRB_TRY(check_device(cache));
     ZRB_REQUIRE(lambda >= 0.f && lambda < 1.f, "lambda %f outside [0,1)", lambda);

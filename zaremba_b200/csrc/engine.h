@@ -12,6 +12,8 @@ struct zrb_ctx {
     // writes width[l + 1].  Every entry is cfg.hidden in a context of one width.
     int width[ZRB_MAX_LAYERS + 1] = {};
     int max_width = 0;
+    int experts = 0;                       // zrb_ctx_create_mos: K softmaxes in the head (DESIGN.md section 19), 0 = plain
+    float p_mos = 0.f;                     // zrb_set_mos_dropout: latent dropout of the head
     std::vector<void*> allocs;
     int64_t bytes = 0;
 
@@ -61,7 +63,7 @@ struct zrb_ctx {
     float* reg_val = nullptr;              // [2] the last train step's alpha-weighted AR and beta-weighted TAR
     int64_t weights_version = 1;          // bumped whenever parameter values change
     bool avg_on = false;                   // zrb_set_average: iterate averaging into `avg` (DESIGN.md section 16)
-    zrb_params avg{};
+    zrb_mos_params avg{};                  // (the head tensors only in a context with experts)
     int64_t avg_n = 0;                     // train-step updates averaged so far
     bool avg_swapped = false;              // zrb_swap_average: the parameters hold the average
     float* bwd_dy = nullptr;               // phased backward: grad wrt the next layer's output / scratch
@@ -117,6 +119,10 @@ bool reg_on(const zrb_ctx* c);                   // AR / TAR is switched on (alp
 int reg_compute(zrb_ctx* c, cudaStream_t s);
 MaskSrc ed_mask(const zrb_ctx* c);               // embedding-dropout site 3L+1 over the V vocabulary rows (inactive:
                                                  // eval mode or p_ed = 0)
+MaskSrc mos_mask(const zrb_ctx* c);              // latent-dropout site 3L+2 over N*K*E (period B*K*E in the variational
+                                                 // mode; inactive: eval mode or p_mos = 0)
+// the head tensors of a zrb_params that a context with experts was given (zrb_mos_params, its base first)
+inline const zrb_mos_params* mos_of(const zrb_params* p) { return reinterpret_cast<const zrb_mos_params*>(p); }
 
 // RAII bracket: records an event pair around the launches of one kernel class
 struct ProfScope {
@@ -138,6 +144,8 @@ int tc_backward(zrb_ctx* c, const zrb_params* p, const float* dscores, const zrb
 int tc_train_step_grads(zrb_ctx* c, const zrb_params* p, const zrb_params* g, const int64_t* x, const int64_t* y,
                         int T, int B, const zrb_states* in, const zrb_states* out, uint64_t seed, uint64_t step,
                         float* loss, cudaStream_t s);
+int tc_mos_eval_step(zrb_ctx* c, const zrb_params* p, const int64_t* x, const int64_t* y, const zrb_states* in,
+                     const zrb_states* out, float* loss, float* tgt_prob, cudaStream_t s);
 int tc_train_step_begin(zrb_ctx* c, const zrb_params* p, const zrb_params* g, const int64_t* x, const int64_t* y,
                         int T, int B, const zrb_states* in, const zrb_states* out, uint64_t seed, uint64_t step,
                         float* loss, cudaStream_t s);

@@ -39,6 +39,7 @@ struct GridBarrier {
 
 struct zrb_tc_state {
     int Xp[ZRB_MAX_LAYERS + 1] = {}, G4p[ZRB_MAX_LAYERS] = {}, Vp = 0;
+    int Fp = 0;                        // pitch of fc_w_h: pad64 of fc.W's width (H_{L-1}; E in a Mixture-of-Softmaxes head)
     int device = 0;
     __half* w_ih_h[ZRB_MAX_LAYERS] = {};
     __half* w_hh_h[ZRB_MAX_LAYERS] = {};
@@ -63,7 +64,23 @@ struct zrb_tc_state {
     bool in_train_step = false;   // tc_forward is running as the first half of a fused train step
     float* colsum_scratch = nullptr;   // row-split partials of the bias-gradient column sums
     int64_t packed_version = 0;
-    zrb_params packed_params{};
+    zrb_mos_params packed_params{};    // (the head tensors only with experts)
+    // Mixture-of-Softmaxes head (DESIGN.md section 19), with K = c->experts, E = width[0], H = H_{L-1}, Ua = pad64(K*E),
+    // HW = Ua + pad64(K): head_w_h [HW, Xp[L]] = latent.W in rows [0, K*E) and prior.W in rows [Ua, Ua + K), zero rows
+    // between; ua [N, HW] fp32 the head GEMM's output (u, then c = tanh(u); a); lat_h [N*K, pad64(E)] the dropped latent
+    // rows; logits [N*K, V] and lse [N*K]; dua_h [N, HW] the scaled fp16 [du | da]; dlat [N*K, E] fp32 dc^; headg
+    // [Ua + K, H] the head's weight gradients before they are copied out; vjp_s [N*K] the drop-in backward's s.
+    int Ua = 0, HW = 0;
+    __half* head_w_h = nullptr;
+    float* ua = nullptr;
+    __half* lat_h = nullptr;
+    float* logits = nullptr;
+    float* lse = nullptr;
+    __half* dua_h = nullptr;
+    float* dlat = nullptr;
+    float* headg = nullptr;
+    float* vjp_s = nullptr;
+    bool head_loss_only = false;       // tc_forward of a fused step or eval step: the head stops at the LSEs (no log p)
     std::vector<void*> allocs;
     // persistent recurrence: one plan per layer and direction, each for the layer's width.  Either direction is on for
     // every layer or for none (tc_ctx_init), so fplan[0].ok / bplan[0].ok say which path a step takes.
@@ -98,7 +115,7 @@ struct zrb_tc_state {
         return w;
     }
     zrb::WeightImages w_ih_images(int l) const { return row_image(w_ih_h[l], Xp[l]); }
-    zrb::WeightImages fc_w_images(int L) const { return row_image(fc_w_h, Xp[L]); }
+    zrb::WeightImages fc_w_images() const { return row_image(fc_w_h, Fp); }
     // both recurrences run in the persistent kernels: fplan.ok && bplan.ok, and bplan.ok implies fplan.ok (tc_ctx_init
     // clears bplan.ok when the forward plan is off)
     bool persistent() const { return bplan[0].ok; }
@@ -170,6 +187,8 @@ int tc_ctx_init(zrb_ctx* c) {
         if (t->G4p[l] > G4m) G4m = t->G4p[l];
     }
     t->Vp = pad64(V);
+    const int K = c->experts, E = c->width[0], H = c->width[L];
+    t->Fp = pad64(K ? E : H);
     for (int l = 0; l < L; ++l) {
         const size_t H = c->width[l + 1];
         ZRB_TRY(tc_alloc(c, &t->w_ih_h[l], 4 * H * t->Xp[l]));
@@ -177,11 +196,27 @@ int tc_ctx_init(zrb_ctx* c) {
         ZRB_TRY(tc_alloc(c, &t->hprev_h[l], (N + B) * t->Xp[l + 1]));
     }
     for (int l = 0; l <= L; ++l) ZRB_TRY(tc_alloc(c, &t->x_h[l], N * t->Xp[l]));
-    ZRB_TRY(tc_alloc(c, &t->fc_w_h, (size_t)V * t->Xp[L]));
+    ZRB_TRY(tc_alloc(c, &t->fc_w_h, (size_t)V * t->Fp));
     ZRB_TRY(tc_alloc(c, &t->dG_h, N * G4m));
     ZRB_TRY(tc_alloc(c, &t->dG_h_alt, N * G4m));
-    ZRB_TRY(tc_alloc(c, &t->dS_h, N * t->Vp));
-    ZRB_TRY(tc_alloc(c, &t->colsum_scratch, (size_t)colsum_h_scratch_floats(V > 4 * Hm ? V : 4 * Hm)));
+    ZRB_TRY(tc_alloc(c, &t->dS_h, N * (K ? K : 1) * t->Vp));
+    int colsum_cols = V > 4 * Hm ? V : 4 * Hm;
+    if (K) {
+        t->Ua = pad64(K * E);
+        t->HW = t->Ua + pad64(K);
+        const size_t NK = N * K;
+        if (K * E > colsum_cols) colsum_cols = K * E;
+        ZRB_TRY(tc_alloc(c, &t->head_w_h, (size_t)t->HW * t->Xp[L]));
+        ZRB_TRY(tc_alloc(c, &t->ua, N * t->HW));
+        ZRB_TRY(tc_alloc(c, &t->lat_h, NK * pad64(E)));
+        ZRB_TRY(tc_alloc(c, &t->logits, NK * V));
+        ZRB_TRY(tc_alloc(c, &t->lse, NK));
+        ZRB_TRY(tc_alloc(c, &t->dua_h, N * t->HW));
+        ZRB_TRY(tc_alloc(c, &t->dlat, NK * E));
+        ZRB_TRY(tc_alloc(c, &t->headg, (size_t)(t->Ua + K) * H));
+        ZRB_TRY(tc_alloc(c, &t->vjp_s, NK));
+    }
+    ZRB_TRY(tc_alloc(c, &t->colsum_scratch, (size_t)colsum_h_scratch_floats(colsum_cols)));
     // one plan per layer; a direction is persistent only when every layer's plan fits (no mixed step)
     const char* force = getenv("ZRB_REC");
     bool fwd_ok = !(force && !strcmp(force, "steps")), bwd_ok = !(force && !strcmp(force, "fwdonly"));   // A/B switches
@@ -260,9 +295,17 @@ static int tc_pack_whh(zrb_ctx* c, const float* W, int l, bool row_image, cudaSt
 }
 
 // rebuild the fp16 weight images when parameter values changed (main.py:116-117 / zrb_clip_sgd)
+// the zrb_params a context reads: zrb_mos_params with experts (DESIGN.md section 19)
+static size_t params_bytes(const zrb_ctx* c) { return c->experts ? sizeof(zrb_mos_params) : sizeof(zrb_params); }
+static void note_packed(zrb_ctx* c, const zrb_params* p) {
+    zrb_tc_state* t = c->tc;
+    t->packed_version = c->weights_version;
+    memcpy(&t->packed_params, p, params_bytes(c));
+}
+
 static int tc_pack_weights(zrb_ctx* c, const zrb_params* p, cudaStream_t s) {
     zrb_tc_state* t = c->tc;
-    if (t->packed_version == c->weights_version && !memcmp(&t->packed_params, p, sizeof(*p))) return ZRB_OK;
+    if (t->packed_version == c->weights_version && !memcmp(&t->packed_params, p, params_bytes(c))) return ZRB_OK;
     ProfScope ps(c, ZRB_PROF_PACK, s);
     const int L = c->cfg.layers, V = c->cfg.vocab;
     for (int l = 0; l < L; ++l) {
@@ -270,9 +313,15 @@ static int tc_pack_weights(zrb_ctx* c, const zrb_params* p, cudaStream_t s) {
         ZRB_TRY(convert_pad_f16(p->w_ih[l], In, t->w_ih_h[l], t->Xp[l], 4 * H, In, 1.f, s));
         ZRB_TRY(tc_pack_whh(c, p->w_hh[l], l, true, s));
     }
-    ZRB_TRY(convert_pad_f16(p->fc_w, c->width[L], t->fc_w_h, t->Xp[L], V, c->width[L], 1.f, s));
-    t->packed_version = c->weights_version;
-    t->packed_params = *p;
+    const int F = c->experts ? c->width[0] : c->width[L];
+    ZRB_TRY(convert_pad_f16(p->fc_w, F, t->fc_w_h, t->Fp, V, F, 1.f, s));
+    if (c->experts) {
+        const int K = c->experts, H = c->width[L];
+        const zrb_mos_params* mp = mos_of(p);
+        ZRB_TRY(convert_pad_f16(mp->latent_w, H, t->head_w_h, t->Xp[L], K * c->width[0], H, 1.f, s));
+        ZRB_TRY(convert_pad_f16(mp->prior_w, H, t->head_w_h + (size_t)t->Ua * t->Xp[L], t->Xp[L], K, H, 1.f, s));
+    }
+    note_packed(c, p);
     return ZRB_OK;
 }
 
@@ -280,34 +329,45 @@ static int tc_pack_weights(zrb_ctx* c, const zrb_params* p, cudaStream_t s) {
 // to (layer l, or L for fc.W; see zrb_tc_state::upd_pending).
 struct WeightMatrix {
     int i, rows, cols, item;
-    enum { kWih, kWhh, kFcW } kind;
+    enum { kWih, kWhh, kFcW, kPrior, kLatent } kind;
 };
 struct WeightMatrices {
-    WeightMatrix m[2 * ZRB_MAX_LAYERS + 1];
+    WeightMatrix m[2 * ZRB_MAX_LAYERS + 3];
     int n = 0;
     const WeightMatrix* begin() const { return m; }
     const WeightMatrix* end() const { return m + n; }
     const WeightMatrix& fc_w() const { return m[n - 1]; }
 };
-// The matrices in the order the update launches them: W_ih then W_hh per layer, then fc.W.  This is the one place that
-// knows where param_list() (api.cu) puts them: embed, (w_ih, w_hh, b_ih, b_hh) x L, fc_w, fc_b (tied: embed has n = 0,
-// E is fc_w), and the one place of the update path that knows their shapes: W_ih [4H_l, In_l], W_hh [4H_l, H_l],
-// fc.W [V, H_{L-1}].
+// The matrices in the order the update launches them: W_ih then W_hh per layer, the head's prior.W and latent.W, then
+// fc.W.  This is the one place that knows where param_list() (api.cu) puts them: embed, (w_ih, w_hh, b_ih, b_hh) x L,
+// fc_w, fc_b (tied: embed has n = 0, E is fc_w), then with experts prior_w, latent_w, latent_b; and the one place of the
+// update path that knows their shapes: W_ih [4H_l, In_l], W_hh [4H_l, H_l], fc.W [V, H_{L-1}] ([V, E] with experts),
+// prior.W [K, H_{L-1}], latent.W [K*E, H_{L-1}].  The head's matrices belong to lazy item L with fc.W.
 static WeightMatrices tc_matrices(const zrb_ctx* c) {
-    const int L = c->cfg.layers, V = c->cfg.vocab;
+    const int L = c->cfg.layers, V = c->cfg.vocab, K = c->experts;
     WeightMatrices ms;
     for (int l = 0; l < L; ++l) {
         const int In = c->width[l], H = c->width[l + 1];
         ms.m[ms.n++] = {1 + 4 * l, 4 * H, In, l, WeightMatrix::kWih};
         ms.m[ms.n++] = {2 + 4 * l, 4 * H, H, l, WeightMatrix::kWhh};
     }
-    ms.m[ms.n++] = {1 + 4 * L, V, c->width[L], L, WeightMatrix::kFcW};
+    if (K) {
+        ms.m[ms.n++] = {3 + 4 * L, K, c->width[L], L, WeightMatrix::kPrior};
+        ms.m[ms.n++] = {4 + 4 * L, K * c->width[0], c->width[L], L, WeightMatrix::kLatent};
+    }
+    ms.m[ms.n++] = {1 + 4 * L, V, K ? c->width[0] : c->width[L], L, WeightMatrix::kFcW};
     return ms;
 }
 // the images a fused update of m writes; whh: what W_hh's will hold afterwards (zrb_tc_state::w_hh_images)
 static WeightImages tc_images(zrb_ctx* c, const WeightMatrix& m, const zrb_tc_state::WhhImage& whh) {
-    if (m.kind == WeightMatrix::kWhh) return c->tc->w_hh_images(m.item, whh);
-    return m.kind == WeightMatrix::kWih ? c->tc->w_ih_images(m.item) : c->tc->fc_w_images(m.item);
+    zrb_tc_state* t = c->tc;
+    switch (m.kind) {
+        case WeightMatrix::kWhh: return t->w_hh_images(m.item, whh);
+        case WeightMatrix::kWih: return t->w_ih_images(m.item);
+        case WeightMatrix::kFcW: return t->fc_w_images();
+        case WeightMatrix::kPrior: return t->row_image(t->head_w_h + (size_t)t->Ua * t->Xp[m.item], t->Xp[m.item]);
+        default: return t->row_image(t->head_w_h, t->Xp[m.item]);
+    }
 }
 // tl for the list kernels once the tile kernels have taken the matrices: their lengths set to 0, which every list
 // kernel skips
@@ -329,8 +389,7 @@ static void tc_images_current(zrb_ctx* c, const zrb_params* p) {
     zrb_tc_state* t = c->tc;
     t->wg_ok = false;
     c->weights_version++;
-    t->packed_version = c->weights_version;
-    t->packed_params = *p;
+    note_packed(c, p);
 }
 
 // The train step's update of one matrix: update_pack, or with iterate averaging on (avg non-null) update_pack_avg,
@@ -365,6 +424,22 @@ int tc_flush_updates(zrb_ctx* c, cudaStream_t s) {
     if (!t || !t->upd_pending) return ZRB_OK;
     ProfScope ps(c, ZRB_PROF_CLIP_SGD, s);
     for (int item = 1; item <= c->cfg.layers; ++item) ZRB_TRY(tc_issue_update(c, item, false, s));
+    return ZRB_OK;
+}
+
+// The Mixture-of-Softmaxes head (DESIGN.md section 19) over the last `rows` tokens of the window: [u | a] in one GEMM,
+// c and the dropped latent image, the N*K logits rows with fc.b, their LSEs, and (logp non-null) log p [rows, V].
+static int tc_mos_head(zrb_ctx* c, const zrb_params* p, int rows, float* logp, cudaStream_t s) {
+    zrb_tc_state* t = c->tc;
+    const int L = c->cfg.layers, V = c->cfg.vocab, K = c->experts, E = c->width[0], H = c->width[L];
+    const int N = c->T * c->B, Xl = t->Xp[L], Ep = pad64(E);
+    ProfScope ps(c, ZRB_PROF_PROJ_FWD, s);
+    ZRB_TRY(gemm_f16_tc(t->x_h[L] + (size_t)(N - rows) * Xl, Xl, 0, t->head_w_h, Xl, 0, t->ua, t->HW, rows, t->Ua + K, H,
+                        1.f, nullptr, 0, s));
+    ZRB_TRY(mos_latent_fwd(t->ua, t->HW, mos_of(p)->latent_b, t->lat_h, Ep, rows, K, E, N - rows, mos_mask(c), s));
+    ZRB_TRY(gemm_f16_tc(t->lat_h, Ep, 0, t->fc_w_h, t->Fp, 0, t->logits, V, rows * K, V, E, 1.f, p->fc_b, 0, s));
+    ZRB_TRY(mos_lse(t->logits, rows * K, V, t->lse, s));
+    if (logp) ZRB_TRY(mos_logp(t->logits, t->lse, t->ua, t->HW, t->Ua, rows, K, V, logp, V, s));
     return ZRB_OK;
 }
 
@@ -440,6 +515,7 @@ int tc_forward(zrb_ctx* c, const zrb_params* p, const int64_t* x, const zrb_stat
         ZRB_CUDA(cudaMemcpyAsync(out->h[l], c->hraw[l] + (size_t)(T - 1) * B * H, bh, cudaMemcpyDeviceToDevice, s));
         ZRB_CUDA(cudaMemcpyAsync(out->c[l], c->cst[l] + (size_t)(T - 1) * B * H, bh, cudaMemcpyDeviceToDevice, s));
     }
+    if (scores && c->experts) return tc_mos_head(c, p, last_only ? B : N, t->head_loss_only ? nullptr : scores, s);
     if (scores) {
         ProfScope ps(c, ZRB_PROF_PROJ_FWD, s);
         const int rows = last_only ? B : N;
@@ -467,6 +543,35 @@ static float* wgrad_slots(zrb_ctx* c, int n) {
 // ... for an [M,N] weight gradient written by gemm_f16_tc
 static float* wgrad_sumsq(zrb_ctx* c, int M, int N, int K) { return wgrad_slots(c, gemm_f16_tc_sumsq_slots(M, N, K)); }
 
+// Mixture-of-Softmaxes head backward from dS_h (N*K rows) and the da columns of dua_h: fc.W / fc.b over the N*K rows,
+// dc^ -> du, then dh = [du | da] [latent.W; prior.W] into dY and the head's weight gradients in one GEMM
+static int tc_mos_backward(zrb_ctx* c, const zrb_params* g, float* dY, cudaStream_t s) {
+    zrb_tc_state* t = c->tc;
+    const int L = c->cfg.layers, V = c->cfg.vocab, N = c->T * c->B, H = c->width[L], K = c->experts, E = c->width[0];
+    const int NK = N * K, Xl = t->Xp[L], Vp = t->Vp, Ep = pad64(E);
+    const float inv = 1.f / kGradScale;
+    ProfScope ps(c, ZRB_PROF_PROJ_BWD, s);
+    t->wg_ok = c->fused_norm;
+    t->wg_slots = 0;
+    t->wg_key = g->fc_w;
+    t->pending = 0;
+    // dc^[NK,E] = dS[NK,V] * W[V,E]; dW[V,E] = dS^T * c^ (contraction over the N*K rows); fc.b = column sums
+    ZRB_TRY(gemm_f16_tc(t->dS_h, Vp, 0, t->fc_w_h, t->Fp, 1, t->dlat, E, NK, E, V, inv, nullptr, 0, s));
+    ZRB_TRY(colsum_h(t->dS_h, Vp, g->fc_b, nullptr, NK, V, inv, t->colsum_scratch, s));
+    ZRB_TRY(gemm_f16_tc(t->dS_h, Vp, 1, t->lat_h, Ep, 1, g->fc_w, E, V, E, NK, inv, nullptr, 0, s,
+                        wgrad_sumsq(c, V, E, NK)));
+    ZRB_TRY(mos_latent_bwd(t->dlat, t->ua, t->HW, t->dua_h, t->HW, N, K, E, mos_mask(c), s));
+    const int M = t->Ua + K;   // [du | da] columns, zero between K*E and Ua
+    ZRB_TRY(gemm_f16_tc(t->dua_h, t->HW, 0, t->head_w_h, Xl, 1, dY, H, N, H, M, inv, nullptr, 0, s));
+    ZRB_TRY(gemm_f16_tc(t->dua_h, t->HW, 1, t->x_h[L], Xl, 1, t->headg, H, M, H, N, inv, nullptr, 0, s,
+                        wgrad_sumsq(c, M, H, N)));   // the rows between K*E and Ua are zero: the slots sum both tensors
+    const zrb_mos_params* gm = mos_of(g);
+    ZRB_CUDA(cudaMemcpyAsync(gm->latent_w, t->headg, (size_t)K * E * H * sizeof(float), cudaMemcpyDeviceToDevice, s));
+    ZRB_CUDA(cudaMemcpyAsync(gm->prior_w, t->headg + (size_t)t->Ua * H, (size_t)K * H * sizeof(float),
+                             cudaMemcpyDeviceToDevice, s));
+    return colsum_h(t->dua_h, t->HW, gm->latent_b, nullptr, N, K * E, inv, t->colsum_scratch, s);
+}
+
 // backward from the scaled fp16 image dS_h already in place
 // projection backward: afterwards fc.W / fc.b gradients are complete and c->bwd_dy holds d loss / d act[L]
 static int tc_backward_head(zrb_ctx* c, const zrb_params* p, const zrb_params* g, cudaStream_t s) {
@@ -478,6 +583,7 @@ static int tc_backward_head(zrb_ctx* c, const zrb_params* p, const zrb_params* g
     c->bwd_dy = c->dy;
     c->bwd_dx = c->dx;
     c->bwd_next_layer = L - 1;
+    if (c->experts) return tc_mos_backward(c, g, dY, s);
     {
         ProfScope ps(c, ZRB_PROF_PROJ_BWD, s);
         // dA[N,H] = dS[N,V] * W[V,H]       (W image read MN-major)
@@ -632,7 +738,13 @@ static int tc_backward_from_image(zrb_ctx* c, const zrb_params* p, const zrb_par
 int tc_backward(zrb_ctx* c, const zrb_params* p, const float* dscores, const zrb_params* g, cudaStream_t s) {
     zrb_tc_state* t = c->tc;
     const int N = c->T * c->B, V = c->cfg.vocab;
-    ZRB_TRY(convert_pad_f16(dscores, V, t->dS_h, t->Vp, N, V, kGradScale, s));
+    if (c->experts) {   // dscores = dL / d log p: the mixture's VJP (log p itself goes to the scratch c->dscores)
+        ProfScope ps(c, ZRB_PROF_SOFTMAX, s);
+        ZRB_TRY(mos_vjp(t->logits, t->lse, t->ua, t->HW, t->Ua, N, c->experts, V, dscores, c->dscores, t->vjp_s, t->dS_h,
+                        t->Vp, t->dua_h, t->HW, s));
+    } else {
+        ZRB_TRY(convert_pad_f16(dscores, V, t->dS_h, t->Vp, N, V, kGradScale, s));
+    }
     return tc_backward_from_image(c, p, g, s);
 }
 
@@ -645,15 +757,22 @@ static int tc_step_forward(zrb_ctx* c, const zrb_params* p, const int64_t* x, co
     c->T = T; c->B = B; c->train = train; c->seed = seed; c->step = step;
     c->have_fwd = false;
     c->reg_use = false;
-    c->tc->in_train_step = train != 0;
+    zrb_tc_state* t = c->tc;
+    t->in_train_step = train != 0;
+    t->head_loss_only = true;
     const int frc = tc_forward(c, p, x, in, out, c->scores, s);
-    c->tc->in_train_step = false;   // before the return code is tested: a failed forward must not leave it set
+    t->in_train_step = false;   // before the return code is tested: a failed forward must not leave it set
+    t->head_loss_only = false;
     ZRB_TRY(frc);
     c->have_fwd = true;
     {
         ProfScope ps(c, ZRB_PROF_SOFTMAX, s);
-        ZRB_TRY(softmax_nll(c->scores, y, T * B, c->cfg.vocab, B, c->row_loss, loss, nullptr, nullptr, s, c->tc->dS_h,
-                            c->tc->Vp, kGradScale));
+        if (c->experts)
+            ZRB_TRY(mos_nll_grad(t->logits, t->lse, t->ua, t->HW, t->Ua, y, T * B, c->experts, c->cfg.vocab, B,
+                                 c->row_loss, loss, t->dS_h, t->Vp, t->dua_h, t->HW, s));
+        else
+            ZRB_TRY(softmax_nll(c->scores, y, T * B, c->cfg.vocab, B, c->row_loss, loss, nullptr, nullptr, s, t->dS_h,
+                                t->Vp, kGradScale));
     }
     if (train && reg_on(c)) ZRB_TRY(reg_compute(c, s));   // AR / TAR: between the softmax and the projection's backward
     return ZRB_OK;
@@ -679,6 +798,18 @@ int tc_eval_grads(zrb_ctx* c, const zrb_params* p, const zrb_params* g, const in
     c->fused_norm = fused;
     c->tc->wg_ok = false;
     return rc;
+}
+
+// zrb_eval_step of a Mixture-of-Softmaxes context: the eval-mode forward through the LSEs, then the mixture's row losses
+int tc_mos_eval_step(zrb_ctx* c, const zrb_params* p, const int64_t* x, const int64_t* y, const zrb_states* in,
+                     const zrb_states* out, float* loss, float* tgt_prob, cudaStream_t s) {
+    zrb_tc_state* t = c->tc;
+    t->head_loss_only = true;
+    const int frc = tc_forward(c, p, x, in, out, c->scores, s);
+    t->head_loss_only = false;
+    ZRB_TRY(frc);
+    return mos_nll_eval(t->logits, t->lse, t->ua, t->HW, t->Ua, y, c->T * c->B, c->experts, c->cfg.vocab, c->B,
+                        c->row_loss, loss, tgt_prob, s);
 }
 
 int tc_train_step_begin(zrb_ctx* c, const zrb_params* p, const zrb_params* g, const int64_t* x, const int64_t* y,

@@ -59,12 +59,16 @@ int embed_rows_sumsq(const float* dW, const int64_t* ids, const int* first, int 
 int embed_rows_update(float* W, float* dW, const int64_t* ids, const int* first, int n, int H, int V, float lr,
                       const float* scalars, bool write_g, cudaStream_t s);
 int dropout_mask_bytes(MaskSrc m, int64_t n, uint8_t* out, cudaStream_t s);
+// loss = scale * sum_n row_loss[n] (fixed-order tree: deterministic); softmax_nll's reduction
+int loss_reduce(const float* row_loss, int N, float scale, float* loss, cudaStream_t s);
 
 // ---- optim.cu ----------------------------------------------------------------------------
+// the most tensors one list holds: embed, 4 per layer, fc.W, fc.b and a Mixture-of-Softmaxes head's three at L = 3
+constexpr int kMaxTensors = 18;
 struct TensorList {
-    float* p[16];
-    float* g[16];
-    int64_t n[16];
+    float* p[kMaxTensors];
+    float* g[kMaxTensors];
+    int64_t n[kMaxTensors];
     int count;
 };
 // partials: >= 1024 floats scratch; scalars: >= 4 floats (norm, coef)
@@ -92,7 +96,7 @@ int stats_finish(const TensorList& tl, int64_t windows, double* partials, float*
 // ---- average_tc.cu: iterate averaging (DESIGN.md section 16) ------------------------------------------------------
 // The average of one train-step update: a[i] averages tl.p[i] (param_list() order); mu = fp32(1 / n), first: n = 1
 struct AvgStep {
-    float* a[16];
+    float* a[kMaxTensors];
     float mu;
     bool first;
 };

@@ -54,9 +54,9 @@ __device__ __forceinline__ float block_sumsq(const float* __restrict__ g, int64_
 // runs of contiguous floats (the tensor list after merging neighbours); block (x, y) takes share x of run y and owns
 // partial slot y * gridDim.x + x, so one launch covers the whole list and no slot is written twice
 struct Runs {
-    float* p[16];
-    float* g[16];
-    int64_t n[16];
+    float* p[kMaxTensors];
+    float* g[kMaxTensors];
+    int64_t n[kMaxTensors];
 };
 __global__ void sumsq_kernel(Runs r, float* __restrict__ partials) {
     __shared__ float sh[kThreads / 32];
@@ -141,7 +141,7 @@ static int coalesce(const TensorList& tl, Runs* r, int* blocks_per_run) {
             ++runs;
         }
     }
-    for (int i = runs; i < 16; ++i) { r->p[i] = nullptr; r->g[i] = nullptr; r->n[i] = 0; }
+    for (int i = runs; i < kMaxTensors; ++i) { r->p[i] = nullptr; r->g[i] = nullptr; r->n[i] = 0; }
     for (int i = 0; i < runs; ++i) longest = r->n[i] > longest ? r->n[i] : longest;
     int64_t b = (longest / 4 + kThreads - 1) / kThreads;
     if (b < 1) b = 1;
@@ -194,11 +194,11 @@ int clip_sgd(const TensorList& tl, float lr, float max_norm, float* partials, fl
 // Tensors without an fp16 image (biases, fc.b, the untied embedding; every tensor on the validation engine).  Block
 // (x, y) streams share x of tensor y; no coalescing, so theta_g and r need not be laid out like p.
 struct DynRuns {
-    float* p[16];
-    const float* g[16];
-    const float* tg[16];
-    const float* r[16];
-    int64_t n[16];
+    float* p[kMaxTensors];
+    const float* g[kMaxTensors];
+    const float* tg[kMaxTensors];
+    const float* r[kMaxTensors];
+    int64_t n[kMaxTensors];
 };
 
 // the non-empty entries of the list; returns their count and sets *bx to the blocks per tensor (cap: no more in all)

@@ -522,10 +522,13 @@ int softmax_nll(const float* scores, const int64_t* y, int N, int V, int B, floa
     else softmax_nll_kernel<<<N, 512, 0, s>>>(scores, y, N, V, gscale, row_loss, dscores, tgt_prob, ds_h, ld_s, h_scale);
 #undef ZRB_SM_LAUNCH
     ZRB_KERNEL_CHECK();
-    if (loss) {
-        loss_reduce_kernel<<<1, 256, 0, s>>>(row_loss, N, gscale, loss);
-        ZRB_KERNEL_CHECK();
-    }
+    if (loss) ZRB_TRY(loss_reduce(row_loss, N, gscale, loss, s));
+    return ZRB_OK;
+}
+
+int loss_reduce(const float* row_loss, int N, float scale, float* loss, cudaStream_t s) {
+    loss_reduce_kernel<<<1, 256, 0, s>>>(row_loss, N, scale, loss);
+    ZRB_KERNEL_CHECK();
     return ZRB_OK;
 }
 

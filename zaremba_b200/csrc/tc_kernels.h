@@ -14,6 +14,31 @@ int colsum_h_scratch_floats(int M);
 int colsum_h(const __half* A, int64_t ld, float* out, float* out2, int N, int M, float inv_scale, float* scratch,
              cudaStream_t s);
 
+// ---- Mixture-of-Softmaxes head (mos.cu; DESIGN.md section 19) ----------------------------------------------------
+// ua [rows, ldu]: the head GEMM's output, latent u in columns [0, K*E), prior a in [Ua, Ua + K).  Logits Z [rows*K, V],
+// row r*K + k = expert k of token r; lse [rows*K].  K <= ZRB_MAX_EXPERTS (one warp holds a token's K statistics).
+// c = tanh(u + b) back into ua, and lat_h row r*K + k = half(c * the latent mask of element (row0 + r)*K*E + j)
+int mos_latent_fwd(float* ua, int64_t ldu, const float* b, __half* lat_h, int64_t ld_l, int rows, int K, int E,
+                   int64_t row0, MaskSrc m, cudaStream_t s);
+// dua_h columns [0, K*E) = kGradScale * dlat * mask * (1 - c^2), c from ua; dlat [N*K, E] fp32
+int mos_latent_bwd(const float* dlat, const float* ua, int64_t ldu, __half* dua_h, int64_t ld_d, int N, int K, int E,
+                   MaskSrc m, cudaStream_t s);
+int mos_lse(const float* Z, int rows, int V, float* lse, cudaStream_t s);
+// the mixture NLL of the train step: row_loss, loss = B/N sum, the scaled fp16 dz rows into ds_h and da into the
+// columns [Ua, Ua + K) of dua_h
+int mos_nll_grad(const float* Z, const float* lse, const float* ua, int64_t ldu, int Ua, const int64_t* y, int N, int K,
+                 int V, int B, float* row_loss, float* loss, __half* ds_h, int64_t ld_s, __half* dua_h, int64_t ld_d,
+                 cudaStream_t s);
+// eval mode: row_loss, loss (or null) and tgt_prob = p[y] (or null)
+int mos_nll_eval(const float* Z, const float* lse, const float* ua, int64_t ldu, int Ua, const int64_t* y, int N, int K,
+                 int V, int B, float* row_loss, float* loss, float* tgt_prob, cudaStream_t s);
+// out [rows, ldo] = log p
+int mos_logp(const float* Z, const float* lse, const float* ua, int64_t ldu, int Ua, int rows, int K, int V, float* out,
+             int64_t ldo, cudaStream_t s);
+// the drop-in backward from G = dL / d log p [N, V]: dz into ds_h and da into dua_h.  Scratch: P [N, V], s_buf [N*K]
+int mos_vjp(const float* Z, const float* lse, const float* ua, int64_t ldu, int Ua, int N, int K, int V, const float* G,
+            float* P, float* s_buf, __half* ds_h, int64_t ld_s, __half* dua_h, int64_t ld_d, cudaStream_t s);
+
 // cell pointwise with fp16 side outputs (tc_cell.cu).  rm: recurrent mask of element b*H + j (variational mode), applied
 // to h_raw_h (the next step's operand) forward and to dh_rec backward
 int lstm_cell_fwd_tc(float* pre, const float* c_prev, float* c_out, float* h_raw, __half* h_raw_h, __half* y_h,

@@ -87,6 +87,18 @@ class Linear(nn.Module):
         return f"input: {self.input_size}, output: {self.hidden_size}"
 
 
+class Prior(nn.Module):
+    """Parameter holder for `prior.W` [K,H_{L-1}] of a Mixture-of-Softmaxes head (no bias)."""
+
+    def __init__(self, input_size, experts):
+        super().__init__()
+        self.input_size, self.experts = input_size, experts
+        self.W = nn.Parameter(torch.empty(experts, input_size))
+
+    def extra_repr(self):
+        return f"input: {self.input_size}, experts: {self.experts}"
+
+
 def _check_widths(hidden_size, layer_num, embed_size, layer_sizes):
     """(E, layer widths) of a Model, or ValueError"""
     def width(v, what):
@@ -123,6 +135,8 @@ def model_from_state_dict(state_dict, dropout=0.0, winit=0.0, tied=None, **kwarg
     fc_w = torch.as_tensor(state_dict["fc.W"])
     if tied is None:
         tied = fc_w.shape == E_w.shape and torch.equal(fc_w.cpu(), E_w.cpu())
+    if "prior.W" in state_dict:   # a Mixture-of-Softmaxes head: K from prior.W
+        kwargs.setdefault("experts", int(torch.as_tensor(state_dict["prior.W"]).shape[0]))
     m = Model(int(V), sizes[0], len(sizes), dropout, winit, tied=tied, embed_size=int(E), layer_sizes=tuple(sizes),
               **kwargs)
     m.load_state_dict(state_dict)
@@ -195,19 +209,43 @@ class Model(nn.Module):
     layer l are [1,B,H_l].  `embed_size` defaults to `hidden_size`, `layer_sizes` to (hidden_size,) * layer_num; given,
     it has layer_num entries and the first is `hidden_size`.  `tied=True` needs E = H_{L-1}.  Unequal widths take the
     tensor-core engine and lstm_type "pytorch".  With every width equal this is the model above, bit for bit.
+
+    Extra keywords `experts` / `mos_dropout`: a Mixture-of-Softmaxes head (Yang et al. 2018; DESIGN.md section 19),
+    e.g. the PTB model `Model(10000, 960, 3, p, winit, tied=True, embed_size=280, layer_sizes=(960, 960, 620),
+    experts=15)`.  With h the last layer's output after its dropout, `latent.W` [K*E,H_{L-1}] and `latent.b` [K*E] give K
+    latent vectors c_k = tanh(latent(h))_k (dropped with p = `mos_dropout` in train mode), `prior.W` [K,H_{L-1}] (no bias)
+    the mixture weights pi = softmax(h prior.W^T), and `fc` [V,E] each expert's softmax; forward returns
+    log(sum_k pi_k softmax(fc(c_k))) [T*B,V], so nn.CrossEntropyLoss on it is the exact NLL, and `generate` /
+    `beam_search` sample from the mixture.  The three head tensors are registered after `fc`, so with the same seed the
+    other tensors equal the plain model's.  `tied=True` needs nothing beyond E.  Not with engine "simt", lstm_type
+    "custom", data parallel, the neural cache or dynamic evaluation (ValueError).
     """
 
     def __init__(self, vocab_size, hidden_size, layer_num, dropout, winit, lstm_type="pytorch", engine="tc",
                  variational=False, recurrent_dropout=None, *, tied=False, weight_drop=0.0, embed_dropout=0.0,
-                 embed_size=None, layer_sizes=None):
+                 embed_size=None, layer_sizes=None, experts=None, mos_dropout=0.0):
         super().__init__()
         E, sizes = _check_widths(hidden_size, layer_num, embed_size, layer_sizes)
         equal = all(w == E for w in sizes)
+        if experts is not None:
+            if isinstance(experts, bool) or not isinstance(experts, int) or not 1 <= experts <= _lib.MAX_EXPERTS:
+                raise ValueError(f"experts must be an int in [1, {_lib.MAX_EXPERTS}], got {experts!r}")
+            if engine == "simt":
+                raise ValueError("a Mixture-of-Softmaxes head needs the tensor-core engine (engine='tc')")
+            if lstm_type == "custom":
+                raise ValueError("a Mixture-of-Softmaxes head needs lstm_type 'pytorch'")
+            if layer_num > 3:
+                raise ValueError("a Mixture-of-Softmaxes model takes at most 3 layers")
+        if isinstance(mos_dropout, bool) or not isinstance(mos_dropout, (int, float)) or \
+                not 0.0 <= float(mos_dropout) < 1.0:
+            raise ValueError(f"mos_dropout must be a number in [0, 1), got {mos_dropout!r}")
+        if mos_dropout and experts is None:
+            raise ValueError("mos_dropout needs experts")
         if not equal and lstm_type == "custom":
             raise ValueError("layers of unequal width need lstm_type 'pytorch'")
         if not equal and engine == "simt":
             raise ValueError("layers of unequal width need the tensor-core engine (engine='tc')")
-        if tied and E != sizes[-1]:
+        if tied and E != sizes[-1] and experts is None:
             raise ValueError(f"tied=True needs embed_size = layer_sizes[-1] (got {E} and {sizes[-1]})")
         if lstm_type not in ("pytorch", "custom"):
             raise ValueError(f"lstm_type must be 'pytorch' or 'custom', got {lstm_type!r}")
@@ -245,11 +283,16 @@ class Model(nn.Module):
         self.embed_size = E
         self.layer_sizes = sizes
         self._widths_given = embed_size is not None or layer_sizes is not None
+        self.experts = experts
+        self.mos_dropout = float(mos_dropout)
         self.embed = Embed(vocab_size, E)
         self.rnns = nn.ModuleList(LSTM(([E] + list(sizes))[l], sizes[l], lstm_type) for l in range(layer_num))
-        self.fc = Linear(sizes[-1], vocab_size)
+        self.fc = Linear(E if experts else sizes[-1], vocab_size)
         if tied:
             self.fc.W = self.embed.W
+        if experts:   # after fc: a seeded model's other tensors equal the plain model's
+            self.prior = Prior(sizes[-1], experts)
+            self.latent = Linear(sizes[-1], experts * E)
         self.dropout = nn.Dropout(p=dropout)     # kept for repr / state parity; masks come from the library
         self.reset_parameters()
         self._ctx = None
@@ -415,11 +458,13 @@ class Model(nn.Module):
     def ordered_parameters(self):
         """The 3+4L tensors in registration order, as the library's zrb_params expects them
         (pytorch names / gate order; the custom layout is permuted by `_lib_weights`).  Tied: the 2+4L distinct
-        tensors, E once (no fc.W entry)."""
+        tensors, E once (no fc.W entry).  With experts, prior.W, latent.W and latent.b follow (zrb_mos_params)."""
         out = [self.embed.W]
         for r in self.rnns:
             out += list(r.tensors())
         out += [self.fc.b] if self.tied else [self.fc.W, self.fc.b]
+        if self.experts:
+            out += [self.prior.W, self.latent.W, self.latent.b]
         return out
 
     def _lib_weights(self):
@@ -480,7 +525,10 @@ class Model(nn.Module):
                              _lib.TIED_EMBEDDING if self.tied else 0)
         h = C.c_void_p()
         with torch.cuda.device(self.embed.W.device):
-            if equal:
+            if self.experts:
+                ws = None if equal else (C.c_int32 * len(widths))(*widths)
+                _lib.check(lib.zrb_ctx_create_mos(C.byref(cfg), ws, self.experts, C.byref(h)))
+            elif equal:
                 _lib.check(lib.zrb_ctx_create(C.byref(cfg), C.byref(h)))
             else:
                 _lib.check(lib.zrb_ctx_create_widths(C.byref(cfg), (C.c_int32 * len(widths))(*widths), C.byref(h)))
@@ -493,6 +541,8 @@ class Model(nn.Module):
             _lib.check(lib.zrb_set_weight_drop(h, self.weight_drop, int(torch.initial_seed()) & 0xFFFFFFFFFFFFFFFF))
         if self.embed_dropout:
             _lib.check(lib.zrb_set_embed_dropout(h, self.embed_dropout, int(torch.initial_seed()) & 0xFFFFFFFFFFFFFFFF))
+        if self.mos_dropout:
+            _lib.check(lib.zrb_set_mos_dropout(h, self.mos_dropout))
         if self._explicit_masks is not None:
             self._push_masks()
         return self._ctx
@@ -510,7 +560,7 @@ class Model(nn.Module):
 
     def _params_struct(self, tensors):
         L = self.layer_num
-        ps = _lib.ZrbParams()
+        ps = _lib.ZrbMosParams() if self.experts else _lib.ZrbParams()
         for t in tensors:
             if t.dtype != torch.float32 or not t.is_cuda:
                 raise RuntimeError("parameters must be fp32 CUDA tensors")
@@ -522,7 +572,11 @@ class Model(nn.Module):
             ps.b_ih[l] = ts[3 + 4 * l].data_ptr()
             ps.b_hh[l] = ts[4 + 4 * l].data_ptr()
         ps.fc_w = ts[0].data_ptr() if self.tied else ts[1 + 4 * L].data_ptr()   # tied: E is fc.W too
-        ps.fc_b = ts[-1].data_ptr()
+        if self.experts:
+            ps.prior_w, ps.latent_w, ps.latent_b = (t.data_ptr() for t in ts[-3:])
+            ps.fc_b = ts[-4].data_ptr()
+        else:
+            ps.fc_b = ts[-1].data_ptr()
         return ps, ts
 
     def _states_struct(self, states):

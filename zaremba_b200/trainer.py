@@ -100,10 +100,15 @@ class Trainer:
         self._pending = False          # lazy mode: a train step has run since the last flush
         self.world = (dist.get_world_size(process_group)
                       if data_parallel and dist.is_available() and dist.is_initialized() else 1)
+        if model.experts and self.world > 1:
+            raise ValueError("a Mixture-of-Softmaxes model does not train data parallel yet: "
+                             "create the Trainer with data_parallel=False")
         params = model.ordered_parameters()
+        head = params[len(params) - 3:] if model.experts else []   # the Mixture-of-Softmaxes head, laid out last
+        base = params[:len(params) - len(head)]
         # flat layout: the library's order, except that a tied E sits next to fc.b, so that the bucket the projection
         # backward completes (E's G_proj part, fc.b) is one range
-        layout = params[1:-1] + [params[0], params[-1]] if model.tied else params
+        layout = (base[1:-1] + [base[0], base[-1]] if model.tied else base) + head
         sizes = [p.numel() for p in layout]
         # one flat parameter buffer and one flat gradient buffer; the nn.Parameters become views
         self.flat_p = torch.empty(sum(sizes), device=dev, dtype=torch.float32)
@@ -449,6 +454,7 @@ class Trainer:
         self._check_versions()
         self._pending = False          # zrb_eval_step applies what is pending before it reads the weights
         if cache is not None:
+            self._no_experts("the neural cache")
             return self._eval_step_cache(lib, x, y, T, B, want_probs, cache, theta, lam)
         _lib.check(lib.zrb_eval_step(self.ctx, C.byref(self._ps), _lib.ptr(x), _lib.ptr(y), T, B,
                                      C.byref(self._st), C.byref(self._st), _lib.ptr(self.loss),
@@ -470,6 +476,8 @@ class Trainer:
         """main.py:86-95 with the per-batch `.item()` sync removed: losses accumulate on the
         device and are read once.  cache: a `NeuralCache`, reset together with the states, through which every window
         is evaluated (eval_step(cache=, theta=, lam=))."""
+        if cache is not None:
+            self._no_experts("the neural cache")
         self.reset_states()
         if cache is not None:
             cache.reset()
@@ -562,7 +570,12 @@ class Trainer:
         return out
 
     # ---- dynamic evaluation (DESIGN.md section 14) -------------------------------------------------------------------
+    def _no_experts(self, what):
+        if self.model.experts:
+            raise ValueError(f"{what} does not support a Mixture-of-Softmaxes model (experts={self.model.experts}) yet")
+
     def _single_replica(self, what):
+        self._no_experts(what)
         if self.world > 1:
             raise ValueError(f"{what} adapts one replica: create the Trainer with data_parallel=False")
 
