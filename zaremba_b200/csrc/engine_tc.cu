@@ -434,10 +434,15 @@ static int tc_mos_head(zrb_ctx* c, const zrb_params* p, int rows, float* logp, c
     const int L = c->cfg.layers, V = c->cfg.vocab, K = c->experts, E = c->width[0], H = c->width[L];
     const int N = c->T * c->B, Xl = t->Xp[L], Ep = pad64(E);
     ProfScope ps(c, ZRB_PROF_PROJ_FWD, s);
-    ZRB_TRY(gemm_f16_tc(t->x_h[L] + (size_t)(N - rows) * Xl, Xl, 0, t->head_w_h, Xl, 0, t->ua, t->HW, rows, t->Ua + K, H,
-                        1.f, nullptr, 0, s));
+    Gemm head;
+    head.A = {t->x_h[L] + (size_t)(N - rows) * Xl, Xl}; head.B = {t->head_w_h, Xl};
+    head.C = t->ua; head.ldc = t->HW; head.M = rows; head.N = t->Ua + K; head.K = H;
+    ZRB_TRY(gemm_f16_tc(head, s));
     ZRB_TRY(mos_latent_fwd(t->ua, t->HW, mos_of(p)->latent_b, t->lat_h, Ep, rows, K, E, N - rows, mos_mask(c), s));
-    ZRB_TRY(gemm_f16_tc(t->lat_h, Ep, 0, t->fc_w_h, t->Fp, 0, t->logits, V, rows * K, V, E, 1.f, p->fc_b, 0, s));
+    Gemm logits;
+    logits.A = {t->lat_h, Ep}; logits.B = {t->fc_w_h, t->Fp};
+    logits.C = t->logits; logits.ldc = V; logits.M = rows * K; logits.N = V; logits.K = E; logits.bias = p->fc_b;
+    ZRB_TRY(gemm_f16_tc(logits, s));
     ZRB_TRY(mos_lse(t->logits, rows * K, V, t->lse, s));
     if (logp) ZRB_TRY(mos_logp(t->logits, t->lse, t->ua, t->HW, t->Ua, rows, K, V, logp, V, s));
     return ZRB_OK;
@@ -485,8 +490,10 @@ int tc_forward(zrb_ctx* c, const zrb_params* p, const int64_t* x, const zrb_stat
         }
         {
             ProfScope ps(c, ZRB_PROF_GEMM_IN, s);
-            ZRB_TRY(gemm_f16_tc(t->x_h[l], Xi, 0, t->w_ih_h[l], Xi, 0, G, 4 * H, N, 4 * H, In, 1.f, p->b_ih[l], 0, s, nullptr,
-                                p->b_hh[l]));
+            Gemm xw;
+            xw.A = {t->x_h[l], Xi}; xw.B = {t->w_ih_h[l], Xi};
+            xw.C = G; xw.ldc = 4 * H; xw.M = N; xw.N = 4 * H; xw.K = In; xw.bias = p->b_ih[l]; xw.bias2 = p->b_hh[l];
+            ZRB_TRY(gemm_f16_tc(xw, s));
         }
         MaskSrc m = site_mask(c, l + 1), rm = rec_mask(c, l);
         // AR / TAR (DESIGN.md section 17) reads the last layer's fp32 h (the per-timestep path always writes it)
@@ -494,9 +501,12 @@ int tc_forward(zrb_ctx* c, const zrb_params* p, const int64_t* x, const zrb_stat
         ProfScope ps(c, ZRB_PROF_REC_FWD, s);
         if (fplan.ok) {
             ZRB_TRY(t->fwd_bar.claim(T, fplan.nCTA, s, [&](unsigned int* word, unsigned int base) {
-                return lstm_rec_fwd(fplan, tc_watchdog(c), t->w_img_f[l], t->h0_img[l], t->h_img, G, c->c0s[l], c->cst[l],
-                                    out->h[l], out->c[l], t->hprev_h[l], t->x_h[l + 1], word, base, T, B, H, Hp, m, rm, s,
-                                    t->trace, reg_h ? c->hraw[l] : nullptr);
+                RecFwdArgs a = {};
+                a.w_img = t->w_img_f[l]; a.h0_img = t->h0_img[l]; a.h_img = t->h_img; a.gates = G; a.c0 = c->c0s[l];
+                a.cst = c->cst[l]; a.h_last = out->h[l]; a.c_last = out->c[l]; a.hprev_h = t->hprev_h[l];
+                a.y_h = t->x_h[l + 1]; a.h_f32 = reg_h ? c->hraw[l] : nullptr; a.counter = word; a.base = base;
+                a.T = T; a.B = B; a.H = H; a.Hp = Hp; a.m = m; a.rm = rm; a.trace = t->trace;
+                return lstm_rec_fwd(fplan, tc_watchdog(c), a, s);
             }));
             // deferred update of the NEXT layer's matrices (or of fc.W after the last layer): on the idle SMs, beside
             // this recurrence; their consumers (the next input GEMM / the projection) are enqueued behind them
@@ -506,8 +516,10 @@ int tc_forward(zrb_ctx* c, const zrb_params* p, const int64_t* x, const zrb_stat
         for (int tt = 0; tt < T; ++tt) {
             const float* c_prev = tt ? c->cst[l] + (size_t)(tt - 1) * B * H : c->c0s[l];
             float* Gt = G + (size_t)tt * B * 4 * H;
-            ZRB_TRY(gemm_f16_tc(t->hprev_h[l] + (size_t)tt * B * Hp, Hp, 0, t->w_hh_h[l], Hp, 0, Gt, 4 * H, B, 4 * H, H,
-                                1.f, nullptr, 1, s));
+            Gemm hw;
+            hw.A = {t->hprev_h[l] + (size_t)tt * B * Hp, Hp}; hw.B = {t->w_hh_h[l], Hp};
+            hw.C = Gt; hw.ldc = 4 * H; hw.M = B; hw.N = 4 * H; hw.K = H; hw.accumulate = true;
+            ZRB_TRY(gemm_f16_tc(hw, s));
             ZRB_TRY(lstm_cell_fwd_tc(Gt, c_prev, c->cst[l] + (size_t)tt * B * H, c->hraw[l] + (size_t)tt * B * H,
                                      t->hprev_h[l] + (size_t)(tt + 1) * B * Hp, t->x_h[l + 1] + (size_t)tt * B * Hp, Hp, B,
                                      H, (int64_t)tt * B * H, (int64_t)N * H, m, rm, s));
@@ -520,8 +532,10 @@ int tc_forward(zrb_ctx* c, const zrb_params* p, const int64_t* x, const zrb_stat
         ProfScope ps(c, ZRB_PROF_PROJ_FWD, s);
         const int rows = last_only ? B : N;
         const int Xl = t->Xp[L];
-        ZRB_TRY(gemm_f16_tc(t->x_h[L] + (size_t)(N - rows) * Xl, Xl, 0, t->fc_w_h, Xl, 0, scores, V, rows, V, c->width[L],
-                            1.f, p->fc_b, 0, s));
+        Gemm proj;
+        proj.A = {t->x_h[L] + (size_t)(N - rows) * Xl, Xl}; proj.B = {t->fc_w_h, Xl};
+        proj.C = scores; proj.ldc = V; proj.M = rows; proj.N = V; proj.K = c->width[L]; proj.bias = p->fc_b;
+        ZRB_TRY(gemm_f16_tc(proj, s));
     }
     return ZRB_OK;
 }
@@ -540,8 +554,8 @@ static float* wgrad_slots(zrb_ctx* c, int n) {
     t->wg_slots += n;
     return out;
 }
-// ... for an [M,N] weight gradient written by gemm_f16_tc
-static float* wgrad_sumsq(zrb_ctx* c, int M, int N, int K) { return wgrad_slots(c, gemm_f16_tc_sumsq_slots(M, N, K)); }
+// ... for the weight gradient the GEMM d writes
+static float* wgrad_sumsq(zrb_ctx* c, const Gemm& d) { return wgrad_slots(c, gemm_f16_tc_sumsq_slots(d).first); }
 
 // Mixture-of-Softmaxes head backward from dS_h (N*K rows) and the da columns of dua_h: fc.W / fc.b over the N*K rows,
 // dc^ -> du, then dh = [du | da] [latent.W; prior.W] into dY and the head's weight gradients in one GEMM
@@ -556,20 +570,44 @@ static int tc_mos_backward(zrb_ctx* c, const zrb_params* g, float* dY, cudaStrea
     t->wg_key = g->fc_w;
     t->pending = 0;
     // dc^[NK,E] = dS[NK,V] * W[V,E]; dW[V,E] = dS^T * c^ (contraction over the N*K rows); fc.b = column sums
-    ZRB_TRY(gemm_f16_tc(t->dS_h, Vp, 0, t->fc_w_h, t->Fp, 1, t->dlat, E, NK, E, V, inv, nullptr, 0, s));
+    Gemm dlat;
+    dlat.A = {t->dS_h, Vp}; dlat.B = {t->fc_w_h, t->Fp, true};
+    dlat.C = t->dlat; dlat.ldc = E; dlat.M = NK; dlat.N = E; dlat.K = V; dlat.alpha = inv;
+    ZRB_TRY(gemm_f16_tc(dlat, s));
     ZRB_TRY(colsum_h(t->dS_h, Vp, g->fc_b, nullptr, NK, V, inv, t->colsum_scratch, s));
-    ZRB_TRY(gemm_f16_tc(t->dS_h, Vp, 1, t->lat_h, Ep, 1, g->fc_w, E, V, E, NK, inv, nullptr, 0, s,
-                        wgrad_sumsq(c, V, E, NK)));
+    Gemm dfc;
+    dfc.A = {t->dS_h, Vp, true}; dfc.B = {t->lat_h, Ep, true};
+    dfc.C = g->fc_w; dfc.ldc = E; dfc.M = V; dfc.N = E; dfc.K = NK; dfc.alpha = inv;
+    dfc.sumsq = wgrad_sumsq(c, dfc);
+    ZRB_TRY(gemm_f16_tc(dfc, s));
     ZRB_TRY(mos_latent_bwd(t->dlat, t->ua, t->HW, t->dua_h, t->HW, N, K, E, mos_mask(c), s));
     const int M = t->Ua + K;   // [du | da] columns, zero between K*E and Ua
-    ZRB_TRY(gemm_f16_tc(t->dua_h, t->HW, 0, t->head_w_h, Xl, 1, dY, H, N, H, M, inv, nullptr, 0, s));
-    ZRB_TRY(gemm_f16_tc(t->dua_h, t->HW, 1, t->x_h[L], Xl, 1, t->headg, H, M, H, N, inv, nullptr, 0, s,
-                        wgrad_sumsq(c, M, H, N)));   // the rows between K*E and Ua are zero: the slots sum both tensors
+    Gemm dh;
+    dh.A = {t->dua_h, t->HW}; dh.B = {t->head_w_h, Xl, true};
+    dh.C = dY; dh.ldc = H; dh.M = N; dh.N = H; dh.K = M; dh.alpha = inv;
+    ZRB_TRY(gemm_f16_tc(dh, s));
+    Gemm dhead;
+    dhead.A = {t->dua_h, t->HW, true}; dhead.B = {t->x_h[L], Xl, true};
+    dhead.C = t->headg; dhead.ldc = H; dhead.M = M; dhead.N = H; dhead.K = N; dhead.alpha = inv;
+    dhead.sumsq = wgrad_sumsq(c, dhead);   // the rows between K*E and Ua are zero: the slots sum both tensors
+    ZRB_TRY(gemm_f16_tc(dhead, s));
     const zrb_mos_params* gm = mos_of(g);
     ZRB_CUDA(cudaMemcpyAsync(gm->latent_w, t->headg, (size_t)K * E * H * sizeof(float), cudaMemcpyDeviceToDevice, s));
     ZRB_CUDA(cudaMemcpyAsync(gm->prior_w, t->headg + (size_t)t->Ua * H, (size_t)K * H * sizeof(float),
                              cudaMemcpyDeviceToDevice, s));
     return colsum_h(t->dua_h, t->HW, gm->latent_b, nullptr, N, K * E, inv, t->colsum_scratch, s);
+}
+
+// fc.W's weight gradient dW[V,H] = dS^T[V,N] * A[N,H] (both operands MN-major: contraction over tokens), with its norm
+// slots: claimed here, so call it where the GEMM is launched
+static Gemm fc_w_wgrad(zrb_ctx* c, const zrb_params* g) {
+    const zrb_tc_state* t = c->tc;
+    const int L = c->cfg.layers, H = c->width[L];
+    Gemm d;
+    d.A = {t->dS_h, t->Vp, true}; d.B = {t->x_h[L], t->Xp[L], true};
+    d.C = g->fc_w; d.ldc = H; d.M = c->cfg.vocab; d.N = H; d.K = c->T * c->B; d.alpha = 1.f / kGradScale;
+    d.sumsq = wgrad_sumsq(c, d);
+    return d;
 }
 
 // backward from the scaled fp16 image dS_h already in place
@@ -587,17 +625,19 @@ static int tc_backward_head(zrb_ctx* c, const zrb_params* p, const zrb_params* g
     {
         ProfScope ps(c, ZRB_PROF_PROJ_BWD, s);
         // dA[N,H] = dS[N,V] * W[V,H]       (W image read MN-major)
-        ZRB_TRY(gemm_f16_tc(t->dS_h, Vp, 0, t->fc_w_h, Hp, 1, dY, H, N, H, V, inv, nullptr, 0, s));
+        Gemm dA;
+        dA.A = {t->dS_h, Vp}; dA.B = {t->fc_w_h, Hp, true};
+        dA.C = dY; dA.ldc = H; dA.M = N; dA.N = H; dA.K = V; dA.alpha = inv;
+        ZRB_TRY(gemm_f16_tc(dA, s));
         t->wg_ok = c->fused_norm;
         t->wg_slots = 0;
         t->wg_key = g->fc_w;
         ZRB_TRY(colsum_h(t->dS_h, Vp, g->fc_b, nullptr, N, V, inv, t->colsum_scratch, s));
-        // dW[V,H] = dS^T[V,N] * A[N,H]     (both operands MN-major: contraction over tokens).  Nothing downstream in
-        // backward reads it: with deferral on it runs underneath the first backward recurrence instead of before it.
+        // dW: nothing downstream in backward reads it: with deferral on it runs underneath the first backward
+        // recurrence instead of before it.
         t->pending = 0;
         if (t->defer_wgrad && t->persistent() && pdl_beside_rec(c)) t->pending = 1;
-        else ZRB_TRY(gemm_f16_tc(t->dS_h, Vp, 1, t->x_h[L], Hp, 1, g->fc_w, H, V, H, N, inv, nullptr, 0, s,
-                                 wgrad_sumsq(c, V, H, N)));
+        else ZRB_TRY(gemm_f16_tc(fc_w_wgrad(c, g), s));
     }
     return ZRB_OK;
 }
@@ -609,13 +649,14 @@ static int tc_layer_wgrads(zrb_ctx* c, const zrb_params* g, int l, const __half*
     zrb_tc_state* t = c->tc;
     const int In = c->width[l], H = c->width[l + 1], N = c->T * c->B;
     const MaskSrc wm = wd_mask(c, l);
-    int n1 = 0, n2 = 0;
-    gemm_f16_tc_dual_sumsq_slots(4 * H, In, H, N, &n1, &n2);
-    float* ss1 = wgrad_slots(c, n1);
-    float* ss2 = wm.active ? nullptr : wgrad_slots(c, n2);
-    ZRB_TRY(gemm_f16_tc(dG_h, t->G4p[l], 1, t->x_h[l], t->Xp[l], 1, g->w_ih[l], In, 4 * H, In, N, 1.f / kGradScale, nullptr,
-                        0, s, ss1, nullptr, pdl, t->hprev_h[l], g->w_hh[l], ss2, nullptr, 0, nullptr, 0,
-                        DualB{H, t->Xp[l + 1], H}));
+    Gemm dw;   // dW_ih[4H,In] = dG^T * x_l, and as the dual problem dW_hh[4H,H] = dG^T * h_prev
+    dw.A = {dG_h, t->G4p[l], true}; dw.B = {t->x_h[l], t->Xp[l], true};
+    dw.C = g->w_ih[l]; dw.ldc = In; dw.M = 4 * H; dw.N = In; dw.K = N; dw.alpha = 1.f / kGradScale; dw.pdl = pdl;
+    dw.dual.B = t->hprev_h[l]; dw.dual.C = g->w_hh[l]; dw.dual.N = H; dw.dual.ldb = t->Xp[l + 1]; dw.dual.ldc = H;
+    const GemmSlots n = gemm_f16_tc_sumsq_slots(dw);
+    dw.sumsq = wgrad_slots(c, n.first);
+    if (!wm.active) dw.dual.sumsq = wgrad_slots(c, n.dual);
+    ZRB_TRY(gemm_f16_tc(dw, s));
     if (!wm.active) return ZRB_OK;
     return weight_drop(g->w_hh[l], g->w_hh[l], (int64_t)4 * H * H, wm, wgrad_slots(c, kWeightDropBlocks), s);
 }
@@ -624,14 +665,14 @@ static int tc_layer_wgrads(zrb_ctx* c, const zrb_params* g, int l, const __half*
 // that was just enqueued on `s`
 static int tc_issue_pending(zrb_ctx* c, const zrb_params* g, cudaStream_t s) {
     zrb_tc_state* t = c->tc;
-    const int L = c->cfg.layers, V = c->cfg.vocab, N = c->T * c->B, H = c->width[L];
     const int kind = t->pending;
     t->pending = 0;
     // (no event bracket here: an event record between the recurrence kernel and its programmatic dependent would sit
     // between the two launches; while profiling with ZRB_PROF_KEEP_PDL=1 the time lands in the enclosing REC_BWD class)
     if (kind == 1) {
-        return gemm_f16_tc(t->dS_h, t->Vp, 1, t->x_h[L], t->Xp[L], 1, g->fc_w, H, V, H, N, 1.f / kGradScale, nullptr, 0, s,
-                           wgrad_sumsq(c, V, H, N), nullptr, true);
+        Gemm dw = fc_w_wgrad(c, g);
+        dw.pdl = true;
+        return gemm_f16_tc(dw, s);
     }
     if (kind == 2) {
         const int l = t->pending_layer;
@@ -662,10 +703,14 @@ static int tc_backward_layer(zrb_ctx* c, const zrb_params* p, const zrb_params* 
         if (bplan.ok) {
             ProfScope ps(c, ZRB_PROF_REC_BWD, s);
             ZRB_TRY(t->bwd_bar.claim(T, bplan.nCTA, s, [&](unsigned int* word, unsigned int base) {
-                return lstm_rec_bwd(bplan, tc_watchdog(c), t->w_img_b[l], t->g_img, dY, c->gates[l], c->cst[l], c->c0s[l],
-                                    dG_h, word, base, T, B, H, G4p, m, rm, s,
-                                    t->trace ? t->trace + 8 + (size_t)c->cfg.max_seq * 8 : nullptr, g->b_ih[l], g->b_hh[l],
-                                    c->resident_flag, ++c->resident_seq, c->dG /* [N,4H] fp32, idle on this path */, r);
+                RecBwdArgs a = {};
+                a.w_img = t->w_img_b[l]; a.g_img = t->g_img; a.dy = dY; a.r = r; a.gates = c->gates[l];
+                a.cst = c->cst[l]; a.c0 = c->c0s[l]; a.dG_h = dG_h; a.db1 = g->b_ih[l]; a.db2 = g->b_hh[l];
+                a.db_scratch = c->dG;   // [N,4H] fp32, idle on this path
+                a.res_flag = c->resident_flag; a.res_value = ++c->resident_seq; a.counter = word; a.base = base;
+                a.T = T; a.B = B; a.H = H; a.G4p = G4p; a.m = m; a.rm = rm;
+                a.trace = t->trace ? t->trace + 8 + (size_t)c->cfg.max_seq * 8 : nullptr;
+                return lstm_rec_bwd(bplan, tc_watchdog(c), a, s);
             }));
             ZRB_TRY(tc_issue_pending(c, g, s));   // runs on the SMs the cluster kernel leaves idle
         } else {
@@ -677,14 +722,19 @@ static int tc_backward_layer(zrb_ctx* c, const zrb_params* p, const zrb_params* 
                                          c->gates[l] + (size_t)tt * B * 4 * H, c->cst[l] + (size_t)tt * bh, c_prev,
                                          c->dG + (size_t)tt * B * 4 * H, dG_h + (size_t)tt * B * G4p, G4p, B, H,
                                          (int64_t)tt * bh, (int64_t)N * H, m, rm, s, r ? r + (size_t)tt * bh : nullptr));
-                if (tt > 0)  // dh_{t-1}[B,H] = dG_t[B,4H] * W_hh[4H,H]
-                    ZRB_TRY(gemm_f16_tc(dG_h + (size_t)tt * B * G4p, G4p, 0, t->w_hh_h[l], Hp, 1, c->dh_rec, H, B, H,
-                                        4 * H, inv, nullptr, 0, s));
+                if (tt == 0) continue;
+                Gemm dh;   // dh_{t-1}[B,H] = dG_t[B,4H] * W_hh[4H,H]
+                dh.A = {dG_h + (size_t)tt * B * G4p, G4p}; dh.B = {t->w_hh_h[l], Hp, true};
+                dh.C = c->dh_rec; dh.ldc = H; dh.M = B; dh.N = H; dh.K = 4 * H; dh.alpha = inv;
+                ZRB_TRY(gemm_f16_tc(dh, s));
             }
         }
         {
             ProfScope ps(c, ZRB_PROF_GEMM_DX, s);
-            ZRB_TRY(gemm_f16_tc(dG_h, G4p, 0, t->w_ih_h[l], Xi, 1, dX, In, N, In, 4 * H, inv, nullptr, 0, s));
+            Gemm dx;
+            dx.A = {dG_h, G4p}; dx.B = {t->w_ih_h[l], Xi, true};
+            dx.C = dX; dx.ldc = In; dx.M = N; dx.N = In; dx.K = 4 * H; dx.alpha = inv;
+            ZRB_TRY(gemm_f16_tc(dx, s));
         }
         // dW_ih, dW_hh: nothing downstream in backward reads them -> for l > 0 they run underneath the next layer's
         // recurrence (which writes the other dG buffer); the bias gradients come out of the recurrence kernel itself
@@ -863,11 +913,17 @@ int tc_layer_fwd(zrb_ctx* c, const float* w_ih, const float* w_hh, const float* 
     fp.x = nullptr; fp.x_saved = nullptr;
     fp.L = 1; fp.B = B; fp.H[0] = H; fp.Hp[0] = Hp; fp.GB[0] = fplan.GBi; fp.Kc[0] = fplan.Kc; fp.N = 0;
     ZRB_TRY(fwd_prep(fp, s));
-    ZRB_TRY(gemm_f16_tc(t->x_h[0], Hp, 0, t->w_ih_h[0], Hp, 0, c->gates[0], 4 * H, N, 4 * H, H, 1.f, b_ih, 0, s, nullptr, b_hh));
+    Gemm xw;
+    xw.A = {t->x_h[0], Hp}; xw.B = {t->w_ih_h[0], Hp};
+    xw.C = c->gates[0]; xw.ldc = 4 * H; xw.M = N; xw.N = 4 * H; xw.K = H; xw.bias = b_ih; xw.bias2 = b_hh;
+    ZRB_TRY(gemm_f16_tc(xw, s));
     MaskSrc m = make_mask_src(nullptr, 0, 0, 0, 0.f, 0);    // no dropout at this level: the caller applies it (model.py:105,108)
     ZRB_TRY(t->fwd_bar.claim(T, fplan.nCTA, s, [&](unsigned int* word, unsigned int base) {
-        return lstm_rec_fwd(fplan, tc_watchdog(c), t->w_img_f[0], t->h0_img[0], t->h_img, c->gates[0], c->c0s[0], c->cst[0],
-                            hT, cT, t->hprev_h[0], t->x_h[1], word, base, T, B, H, Hp, m, m, s, nullptr, y);
+        RecFwdArgs a = {};
+        a.w_img = t->w_img_f[0]; a.h0_img = t->h0_img[0]; a.h_img = t->h_img; a.gates = c->gates[0]; a.c0 = c->c0s[0];
+        a.cst = c->cst[0]; a.h_last = hT; a.c_last = cT; a.hprev_h = t->hprev_h[0]; a.y_h = t->x_h[1]; a.h_f32 = y;
+        a.counter = word; a.base = base; a.T = T; a.B = B; a.H = H; a.Hp = Hp; a.m = m; a.rm = m;
+        return lstm_rec_fwd(fplan, tc_watchdog(c), a, s);
     }));
     c->have_fwd = false;                         // a model-level backward must not follow this
     c->layer_fwd_ok = true;
@@ -885,13 +941,25 @@ int tc_layer_bwd(zrb_ctx* c, const float* dy, float* dx, float* dw_ih, float* dw
     }
     MaskSrc m = make_mask_src(nullptr, 0, 0, 0, 0.f, 0);
     ZRB_TRY(t->bwd_bar.claim(T, bplan.nCTA, s, [&](unsigned int* word, unsigned int base) {
-        return lstm_rec_bwd(bplan, tc_watchdog(c), t->w_img_b[0], t->g_img, dy, c->gates[0], c->cst[0], c->c0s[0], t->dG_h,
-                            word, base, T, B, H, G4p, m, m, s, nullptr, db_ih, db_hh, c->resident_flag, ++c->resident_seq, c->dG);
+        RecBwdArgs a = {};
+        a.w_img = t->w_img_b[0]; a.g_img = t->g_img; a.dy = dy; a.gates = c->gates[0]; a.cst = c->cst[0];
+        a.c0 = c->c0s[0]; a.dG_h = t->dG_h; a.db1 = db_ih; a.db2 = db_hh; a.db_scratch = c->dG;
+        a.res_flag = c->resident_flag; a.res_value = ++c->resident_seq; a.counter = word; a.base = base;
+        a.T = T; a.B = B; a.H = H; a.G4p = G4p; a.m = m; a.rm = m;
+        return lstm_rec_bwd(bplan, tc_watchdog(c), a, s);
     }));
     const float inv = 1.f / kGradScale;
-    if (dx) ZRB_TRY(gemm_f16_tc(t->dG_h, G4p, 0, t->w_ih_h[0], Hp, 1, dx, H, N, H, 4 * H, inv, nullptr, 0, s));
-    ZRB_TRY(gemm_f16_tc(t->dG_h, G4p, 1, t->x_h[0], Hp, 1, dw_ih, H, 4 * H, H, N, inv, nullptr, 0, s, nullptr, nullptr, false,
-                        t->hprev_h[0], dw_hh, nullptr));
+    if (dx) {
+        Gemm dX;
+        dX.A = {t->dG_h, G4p}; dX.B = {t->w_ih_h[0], Hp, true};
+        dX.C = dx; dX.ldc = H; dX.M = N; dX.N = H; dX.K = 4 * H; dX.alpha = inv;
+        ZRB_TRY(gemm_f16_tc(dX, s));
+    }
+    Gemm dw;   // dW_ih and, as the dual problem, dW_hh; never norm slots: those belong to the model-level step
+    dw.A = {t->dG_h, G4p, true}; dw.B = {t->x_h[0], Hp, true};
+    dw.C = dw_ih; dw.ldc = H; dw.M = 4 * H; dw.N = H; dw.K = N; dw.alpha = inv;
+    dw.dual.B = t->hprev_h[0]; dw.dual.C = dw_hh; dw.dual.N = H; dw.dual.ldb = Hp; dw.dual.ldc = H;
+    ZRB_TRY(gemm_f16_tc(dw, s));
     c->layer_fwd_ok = false;
     return ZRB_OK;
 }

@@ -408,65 +408,64 @@ static TileChoice choose_tiles(int M, int N, int num_kb, bool can_split, bool re
     return c;
 }
 
-// number of sumsq_out slots gemm_f16_tc writes for an [M,N] output with contraction length K
-int gemm_f16_tc_sumsq_slots(int M, int N, int K) {
-    TileChoice c = choose_tiles(M, N, cdiv(K, GBK), false);
-    return c.tiles_m * c.tiles_n * kEpiWarps;
+// The tile plan of g's launch.  sumsq: it writes sum-of-squares slots.  A dual launch takes the tile width of its
+// wider problem; both problems are cut into tiles of that width.
+static TileChoice gemm_tiles(const Gemm& g, bool sumsq, bool direct) {
+    if (g.dual.C) return choose_tiles(g.M, g.N > g.dual.N ? g.N : g.dual.N, cdiv(g.K, GBK), false);
+    const bool plain = !sumsq && !g.accumulate;
+    return choose_tiles(g.M, g.N, cdiv(g.K, GBK), plain && g.ldc == g.N, plain && !direct);
 }
 
-// A dual launch takes the tile width of its wider problem; both problems are cut into tiles of that width
-static TileChoice choose_dual_tiles(int M, int N1, int N2, int K) {
-    return choose_tiles(M, N1 > N2 ? N1 : N2, cdiv(K, GBK), false);
-}
-void gemm_f16_tc_dual_sumsq_slots(int M, int N1, int N2, int K, int* n1, int* n2) {
-    const TileChoice c = choose_dual_tiles(M, N1, N2, K);
-    *n1 = c.tiles_m * cdiv(N1, c.bn) * kEpiWarps;
-    *n2 = c.tiles_m * cdiv(N2, c.bn) * kEpiWarps;
+GemmSlots gemm_f16_tc_sumsq_slots(const Gemm& g) {
+    const TileChoice c = gemm_tiles(g, true, false);
+    GemmSlots n;
+    n.first = c.tiles_m * cdiv(g.N, c.bn) * kEpiWarps;
+    n.dual = g.dual.C ? c.tiles_m * cdiv(g.dual.N, c.bn) * kEpiWarps : 0;
+    return n;
 }
 
-int gemm_f16_tc(const __half* A, int64_t lda, int a_mn, const __half* B, int64_t ldb, int b_mn, float* C, int64_t ldc,
-                int M, int N, int K, float alpha, const float* bias, int accumulate, cudaStream_t s, float* sumsq_out,
-                const float* bias2, bool pdl, const __half* B2, float* C2, float* sumsq_out2, const __half* A_tiled,
-                int a_nt128, const __half* B_tiled, int b_nt128, DualB d2) {
+int gemm_f16_tc(const Gemm& g, cudaStream_t s) {
+    const int M = g.M, N = g.N, K = g.K;
+    const Gemm::Dual& d2 = g.dual;
     if (M <= 0 || N <= 0) return ZRB_OK;
-    ZRB_REQUIRE(!B2 == !C2, "dual launch needs both B2 and C2");
-    if (d2.N == 0) d2 = DualB{N, ldb, ldc};
-    ZRB_REQUIRE(!C2 || (d2.N > 0 && !bias && !accumulate), "dual launch: N2 > 0, no bias, no accumulate");
-    ZRB_REQUIRE(!bias2 || bias, "bias2 needs bias");
-    ZRB_REQUIRE(!sumsq_out || !accumulate, "sumsq_out needs a plain store epilogue");
+    ZRB_REQUIRE(!d2.B == !d2.C, "dual launch needs both B2 and C2");
+    ZRB_REQUIRE(!d2.C || (d2.N > 0 && !g.bias && !g.accumulate), "dual launch: N2 > 0, no bias, no accumulate");
+    ZRB_REQUIRE(!g.bias2 || g.bias, "bias2 needs bias");
+    ZRB_REQUIRE(!g.sumsq || !g.accumulate, "sumsq_out needs a plain store epilogue");
     ZRB_REQUIRE(K > 0, "gemm_f16_tc needs K > 0");
     // ZRB_GEMM_EPI=direct: the lockstep consumers with per-element stores and the tile plan they were tuned with (A/B
     // comparisons, bit for bit and in time); read at every launch so that one process can run both
     const char* epi = getenv("ZRB_GEMM_EPI");
     const bool direct = epi && strcmp(epi, "direct") == 0;
-    const TileChoice tc = C2 ? choose_dual_tiles(M, N, d2.N, K)
-                             : choose_tiles(M, N, cdiv(K, GBK), !sumsq_out && ldc == N && !accumulate,
-                                            !direct && !sumsq_out && !accumulate);
+    const TileChoice tc = gemm_tiles(g, g.sumsq != nullptr, direct);
     const int bn = tc.bn;
+    const bool a_mn = g.A.mn_major, b_mn = g.B.mn_major;
     CUtensorMap ta, tb;
-    if (!a_mn) ZRB_TRY(tc_make_tmap_f16(&ta, A, K, M, lda, GBK, GBM, 1));
-    else       ZRB_TRY(tc_make_tmap_f16(&ta, A, M, K, lda, 64, GBK, 1));
-    if (!b_mn) ZRB_TRY(tc_make_tmap_f16(&tb, B, K, N, ldb, GBK, bn, 1));
-    else       ZRB_TRY(tc_make_tmap_f16(&tb, B, N, K, ldb, 64, GBK, 1));
+    if (!a_mn) ZRB_TRY(tc_make_tmap_f16(&ta, g.A.ptr, K, M, g.A.ld, GBK, GBM, 1));
+    else       ZRB_TRY(tc_make_tmap_f16(&ta, g.A.ptr, M, K, g.A.ld, 64, GBK, 1));
+    if (!b_mn) ZRB_TRY(tc_make_tmap_f16(&tb, g.B.ptr, K, N, g.B.ld, GBK, bn, 1));
+    else       ZRB_TRY(tc_make_tmap_f16(&tb, g.B.ptr, N, K, g.B.ld, 64, GBK, 1));
     CUtensorMap tb2 = tb;
-    if (B2) {
-        if (!b_mn) ZRB_TRY(tc_make_tmap_f16(&tb2, B2, K, d2.N, d2.ldb, GBK, bn, 1));
-        else       ZRB_TRY(tc_make_tmap_f16(&tb2, B2, d2.N, K, d2.ldb, 64, GBK, 1));
+    if (d2.B) {
+        if (!b_mn) ZRB_TRY(tc_make_tmap_f16(&tb2, d2.B, K, d2.N, d2.ldb, GBK, bn, 1));
+        else       ZRB_TRY(tc_make_tmap_f16(&tb2, d2.B, d2.N, K, d2.ldb, 64, GBK, 1));
     }
     GemmArgs a;
-    a.M = M; a.N = N; a.K = K; a.alpha = alpha; a.bias = bias; a.C = C; a.ldc = ldc; a.accumulate = accumulate;
+    a.M = M; a.N = N; a.K = K; a.alpha = g.alpha; a.bias = g.bias; a.C = g.C; a.ldc = g.ldc;
+    a.accumulate = g.accumulate;
     a.tiles_m = tc.tiles_m; a.tiles_n = cdiv(N, bn);   // (a dual plan's tile width comes from the wider problem)
     a.splits = tc.splits;
-    a.sumsq_out = sumsq_out;
-    a.bias2 = bias2;
-    a.C2 = C2; a.sumsq_out2 = sumsq_out2;
+    a.sumsq_out = g.sumsq;
+    a.bias2 = g.bias2;
+    a.C2 = d2.C; a.sumsq_out2 = d2.sumsq;
     a.N2 = d2.N; a.ldc2 = d2.ldc; a.tiles_n2 = cdiv(d2.N, bn);
-    a.a_tiled = a_mn ? nullptr : A_tiled; a.a_nt128 = a_nt128; a.b_tiled = b_mn ? nullptr : B_tiled; a.b_nt128 = b_nt128;
-    a.pdl_tail = (pdl && a.splits == 1) ? 1 : 0;    // (a split launch is preceded by a memset: nothing to chain to)
+    a.a_tiled = a_mn ? nullptr : g.a_tiled; a.a_nt128 = g.a_nt128; a.b_tiled = b_mn ? nullptr : g.b_tiled;
+    a.b_nt128 = g.b_nt128;
+    a.pdl_tail = (g.pdl && a.splits == 1) ? 1 : 0;    // (a split launch is preceded by a memset: nothing to chain to)
     a.pdl_trigger = (rec_pdl_enabled() && !a.pdl_tail) ? 1 : 0;
     a.epi_direct = direct ? 1 : 0;
     // split partials are added into a zeroed C: order-independent for two (a+b == b+a)
-    if (a.splits > 1 && !accumulate) ZRB_CUDA(cudaMemsetAsync(C, 0, (size_t)M * N * sizeof(float), s));
+    if (a.splits > 1 && !g.accumulate) ZRB_CUDA(cudaMemsetAsync(g.C, 0, (size_t)M * N * sizeof(float), s));
     return bn == 256 ? dispatch_gemm<256>(ta, tb, tb2, a, a_mn, b_mn, s) : dispatch_gemm<128>(ta, tb, tb2, a, a_mn, b_mn, s);
 }
 
@@ -478,15 +477,19 @@ extern "C" int zrb_gemm_f16_tiled(const void* A, int64_t lda, const void* B, int
                                   const void* B_tiled, int32_t b_nt128, float* C, int64_t ldc, int32_t M, int32_t N, int32_t K,
                                   float alpha, void* stream) {
     ZRB_REQUIRE(A && B && C, "null argument");
-    return zrb::gemm_f16_tc((const __half*)A, lda, 0, (const __half*)B, ldb, 0, C, ldc, M, N, K, alpha, nullptr, 0,
-                            (cudaStream_t)stream, nullptr, nullptr, false, nullptr, nullptr, nullptr, (const __half*)A_tiled,
-                            a_nt128, (const __half*)B_tiled, b_nt128);
+    zrb::Gemm g;
+    g.A = {(const __half*)A, lda}; g.B = {(const __half*)B, ldb};
+    g.C = C; g.ldc = ldc; g.M = M; g.N = N; g.K = K; g.alpha = alpha;
+    g.a_tiled = (const __half*)A_tiled; g.a_nt128 = a_nt128; g.b_tiled = (const __half*)B_tiled; g.b_nt128 = b_nt128;
+    return zrb::gemm_f16_tc(g, (cudaStream_t)stream);
 }
 
 extern "C" int zrb_gemm_f16(const void* A, int64_t lda, int32_t a_mn_major, const void* B, int64_t ldb,
                             int32_t b_mn_major, float* C, int64_t ldc, int32_t M, int32_t N, int32_t K, float alpha,
                             const float* bias, int32_t accumulate, void* stream) {
     ZRB_REQUIRE(A && B && C, "null argument");
-    return zrb::gemm_f16_tc((const __half*)A, lda, a_mn_major, (const __half*)B, ldb, b_mn_major, C, ldc, M, N, K,
-                            alpha, bias, accumulate, (cudaStream_t)stream, nullptr, nullptr, false, nullptr, nullptr, nullptr, nullptr, 0, nullptr, 0);
+    zrb::Gemm g;
+    g.A = {(const __half*)A, lda, a_mn_major != 0}; g.B = {(const __half*)B, ldb, b_mn_major != 0};
+    g.C = C; g.ldc = ldc; g.M = M; g.N = N; g.K = K; g.alpha = alpha; g.bias = bias; g.accumulate = accumulate != 0;
+    return zrb::gemm_f16_tc(g, (cudaStream_t)stream);
 }

@@ -28,32 +28,6 @@
 
 namespace zrb {
 
-struct RecBwdArgs {
-    const __half* w_img;      // [nCluster][4][Kc][G][8][8]
-    __half* g_img;            // [2][4][Kc][GB][8][8] ring: slot (t & 1) holds kGradScale * dG_t per gate
-    const float* dy;          // [N,H] grad wrt the layer's dropout'ed output
-    const float* r;           // [N,H] or null: AR/TAR gradient added after the mask (DESIGN.md section 17)
-    const float* gates;       // [N,4H] activated (i,f,g,o)
-    const float* cst;         // [N,H]
-    const float* c0;          // [B,H]
-    __half* dG_h;             // [N,G4p] row-major, kGradScale * dG
-    float* db1;               // [4H] or null: bias gradient sum_{t,b} dG (model.py:35-36: b_ih and b_hh get the same
-    float* db2;               //      gradient), accumulated in registers over the window and reduced over the batch here
-    float* db_scratch;        // [4][B][H] fp32 scratch of that reduction (needed when db1 is set)
-    int push;                 // exchange of the cluster's partial products: 1 = st.async pushes into the owners' shared
-                              // memory (complete_tx on their mbarrier), 0 = stage + remote arrive + DSMEM pulls
-    unsigned int* res_flag;   // or null: CTA 0 publishes res_value here when the whole grid is resident
-    unsigned int res_value;
-    unsigned int* counter;    // grid barrier: never reset, `base` is its value when this launch starts
-    unsigned int base;
-    int T, B, H, G4p, U, G, GB, Kc, nCTA;
-    int KcS, GBi;             // K chunks per CTA (Kc / S); 8-row batch groups of the dG images (GB, or 4 when N = 32)
-    MaskSrc m;                // the output site's dropout (period B*H: variational mode, fixed over the window)
-    MaskSrc rm;               // variational mode: recurrent mask of element b*H + j; scales the recurrent gradient
-    RecWatch w;               // watchdog (rec_common.cuh)
-    long long* trace;         // optional (profiling): [8] launch stamps (rec_launch_stamps) + [T][8] clock64 stamps of CTA 0
-};
-
 __device__ __forceinline__ uint32_t cluster_ctarank() {
     uint32_t r;
     asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
@@ -504,26 +478,18 @@ int pack_whh_bwd(const float* W, __half* img, int H, const RecPlan& p, cudaStrea
     return ZRB_OK;
 }
 
-int lstm_rec_bwd(const RecPlan& p, const RecWatchdog& wd, const __half* w_img, __half* g_img, const float* dy, const float* gates,
-                 const float* cst, const float* c0, __half* dG_h, unsigned int* counter, unsigned int counter_base, int T,
-                 int B, int H, int G4p, MaskSrc m, MaskSrc rm, cudaStream_t s, long long* trace, float* db1, float* db2,
-                 unsigned int* resident_flag, unsigned int resident_value, float* db_scratch, const float* r) {
-    ZRB_REQUIRE(!db1 || db_scratch, "bias gradients need the scratch buffer");
-    RecBwdArgs a;
-    a.base = counter_base;
-    a.w_img = w_img; a.g_img = g_img; a.dy = dy; a.r = r; a.gates = gates; a.cst = cst; a.c0 = c0; a.dG_h = dG_h;
+int lstm_rec_bwd(const RecPlan& p, const RecWatchdog& wd, RecBwdArgs a, cudaStream_t s) {
+    ZRB_REQUIRE(!a.db1 || a.db_scratch, "bias gradients need the scratch buffer");
     static const bool pull = getenv("ZRB_BWD_PULL") != nullptr;   // A/B switch: the r01 staging + DSMEM-pull exchange (S = 1)
     a.push = pull ? 0 : 1;
-    a.counter = counter; a.db1 = db1; a.db2 = db2; a.db_scratch = db_scratch; a.res_flag = resident_flag; a.res_value = resident_value;
-    a.T = T; a.B = B; a.H = H; a.G4p = G4p; a.U = p.U; a.G = p.G; a.GB = p.GB; a.Kc = p.Kc; a.nCTA = p.nCTA; a.m = m; a.rm = rm; a.trace = trace;
-    if (!rm.active) a.rm.scale = 1.f;   // (the epilogue multiplies by it unconditionally)
-    a.KcS = p.KcS; a.GBi = p.GBi;
+    a.U = p.U; a.G = p.G; a.GB = p.GB; a.Kc = p.Kc; a.nCTA = p.nCTA; a.KcS = p.KcS; a.GBi = p.GBi;
+    if (!a.rm.active) a.rm.scale = 1.f;   // (the epilogue multiplies by it unconditionally)
     ZRB_REQUIRE(wd.flag && wd.host, "lstm_rec_bwd needs the context's watchdog words");
     a.w = rec_watch_args(wd);
     a.base += rec_fault_base("bwd");   // (tests only)
-    if (trace) ZRB_CUDA(cudaMemsetAsync(trace + 4, 0x80, 2 * sizeof(long long), s));
+    if (a.trace) ZRB_CUDA(cudaMemsetAsync(a.trace + 4, 0x80, 2 * sizeof(long long), s));
     void* args[] = {&a};
-    return rec_launch(p, args, trace != nullptr, s, "lstm_rec_bwd");
+    return rec_launch(p, args, a.trace != nullptr, s, "lstm_rec_bwd");
 }
 
 }  // namespace zrb

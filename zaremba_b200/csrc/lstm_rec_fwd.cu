@@ -7,7 +7,7 @@
 // canonical no-swizzle K-major wgmma layout and stays there for all T steps (weight-stationary):
 //   SPLIT = false  the 4U gate rows of its own units x the whole contraction, M = 64 tiles   (H < 256)
 //   SPLIT = true   CTA PAIRS (clusters of 2): the 8U gate rows of the pair's units x ONE HALF of the contraction,
-//                  M = 128 tiles; see the note above RecFwdArgs.  The description below is the SPLIT = false flow;
+//                  M = 128 tiles; see the K-split note below.  The description below is the SPLIT = false flow;
 //                  with SPLIT the drain pushes rows to their owner instead of staging them.
 //
 // Per step:
@@ -41,27 +41,6 @@ namespace zrb {
 // only its half of the h image, runs half the K chain, and the MMA warpgroup pushes each accumulator pair straight from
 // registers into the shared memory of the CTA that owns the row's unit (st.async, bytes counted on the owner's mbarrier:
 // no fence, no staging pass); the owner adds the two partial sums in its cell math.
-struct RecFwdArgs {
-    const __half* w_img;      // [nCTA][KcS][G][8][8]  (K-split: CTA = (pair, K half))
-    const __half* h0_img;     // [Kc][GB][8][8] image of the state entering the window: the B operand of step 0
-    __half* h_img;            // [T+1][Kc][GB][8][8]; image t (t >= 1) is the B operand of step t, written by step t-1
-    float* gates;             // [N,4H] in: x-part pre-activations (+biases); out: activated gates
-    const float* c0;          // [B,H]
-    float* cst;               // [N,H]
-    float* h_last;            // [B,H] or null
-    float* c_last;            // [B,H] or null
-    __half* hprev_h;          // [N+B,Hp] row-major, rows B.. written here
-    __half* y_h;              // [N,Hp] row-major dropout(h)
-    float* h_f32;             // or null: [N,H] fp32 h_t (the unit-level entry point zrb_lstm_layer_fwd returns it)
-    unsigned int* counter;    // grid barrier: never reset, `base` is its value when this launch starts
-    unsigned int base;
-    int T, B, H, Hp, U, G, GB, Kc, nCTA;
-    int KcS, GBi;             // K chunks per CTA (Kc / KS); 8-row batch groups of the operand image (GB, or 4 when N = 32)
-    MaskSrc m;                // the output site's dropout (period B*H: variational mode, fixed over the window)
-    MaskSrc rm;               // variational mode: recurrent mask of element b*H + j on h_{t-1} (operand images, hprev_h)
-    RecWatch w;               // watchdog (rec_common.cuh)
-    long long* trace;         // optional (profiling): [8] launch stamps (rec_launch_stamps) + [T][8] clock64 stamps of CTA 0
-};
 
 __device__ __forceinline__ uint32_t fwd_cluster_ctarank() {
     uint32_t r;
@@ -505,22 +484,14 @@ int pack_whh_fwd(const float* W, __half* img, int H, const RecPlan& p, cudaStrea
     return ZRB_OK;
 }
 
-int lstm_rec_fwd(const RecPlan& p, const RecWatchdog& wd, const __half* w_img, const __half* h0_img, __half* h_img, float* gates,
-                 const float* c0, float* cst, float* h_last, float* c_last, __half* hprev_h, __half* y_h,
-                 unsigned int* counter, unsigned int counter_base, int T, int B, int H, int Hp, MaskSrc m, MaskSrc rm,
-                 cudaStream_t s, long long* trace, float* h_f32) {
-    RecFwdArgs a;
-    a.w_img = w_img; a.h0_img = h0_img; a.h_img = h_img; a.base = counter_base; a.gates = gates; a.c0 = c0; a.cst = cst; a.h_last = h_last; a.c_last = c_last;
-    a.hprev_h = hprev_h; a.y_h = y_h; a.counter = counter; a.h_f32 = h_f32;
-    a.T = T; a.B = B; a.H = H; a.Hp = Hp; a.U = p.U; a.G = p.G; a.GB = p.GB; a.Kc = p.Kc; a.nCTA = p.nCTA; a.m = m; a.rm = rm;
-    a.KcS = p.KcS; a.GBi = p.GBi;
-    a.trace = trace;
+int lstm_rec_fwd(const RecPlan& p, const RecWatchdog& wd, RecFwdArgs a, cudaStream_t s) {
+    a.U = p.U; a.G = p.G; a.GB = p.GB; a.Kc = p.Kc; a.nCTA = p.nCTA; a.KcS = p.KcS; a.GBi = p.GBi;
     ZRB_REQUIRE(wd.flag && wd.host, "lstm_rec_fwd needs the context's watchdog words");
     a.w = rec_watch_args(wd);
     a.base += rec_fault_base("fwd");   // (tests only)
-    if (trace) ZRB_CUDA(cudaMemsetAsync(trace + 4, 0x80, 2 * sizeof(long long), s));
+    if (a.trace) ZRB_CUDA(cudaMemsetAsync(a.trace + 4, 0x80, 2 * sizeof(long long), s));
     void* args[] = {&a};
-    return rec_launch(p, args, trace != nullptr, s, "lstm_rec_fwd");
+    return rec_launch(p, args, a.trace != nullptr, s, "lstm_rec_fwd");
 }
 
 }  // namespace zrb

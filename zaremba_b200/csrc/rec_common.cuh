@@ -23,11 +23,6 @@ constexpr int kRecMaxCell = 2;                        // (unit, batch) cells per
 // has seen the word set stops waiting for good), so the kernel runs to its end through its unchanged barrier skeleton --
 // producing garbage, but terminating, with the CUDA context intact.  The host finds the code in a mapped host word at its
 // next API call and fails the zrb context (api.cu: watchdog_check).  Nothing on the fast path but a register test.
-struct RecWatch {
-    unsigned int* flag;       // device word polled by the spinning threads (0 = healthy)
-    unsigned int* host;       // mapped host word the first thread to give up writes the code to
-    long long spin_cycles;    // ~3 s at 2 GHz unless ZRB_SPIN_CYCLES says otherwise
-};
 // host: the kernel argument for one launch (ZRB_SPIN_CYCLES shortens the time-out; read once), and the fault injection
 // of tests/test_gpu_watchdog.py: ZRB_FAULT_BARRIER_BASE="fwd" / "bwd" makes that kernel's launches expect one arrival
 // more than the grid will ever deliver -- every CTA then sits at its first grid barrier like after a lost wake-up.

@@ -73,24 +73,45 @@ int rec_plan_finish(RecPlan* plan, const void* kernel, int cluster);
 // launch the plan's kernel with args = {&RecFwdArgs} or {&RecBwdArgs}; the launch modes are described at the definition
 // (lstm_rec_fwd.cu).  trace: the launch records a trace (never programmatic); name: for error messages
 int rec_launch(const RecPlan& p, void** args, bool trace, cudaStream_t s, const char* name);
-// Where a persistent kernel that gave up on a wait (rec_common.cuh: RecWatch) reports it: `flag` is the device word the
+// Where a persistent kernel that gave up on a wait (rec_common.cuh: watchdog) reports it: `flag` is the device word the
 // spinning threads poll, `host` a mapped host word the host reads without synchronising.  Owned by the context.
 struct RecWatchdog {
     unsigned int* flag = nullptr;
     unsigned int* host = nullptr;
 };
+// ... and the kernels' copy of it, one per launch (rec_common.cuh: rec_watch_args)
+struct RecWatch {
+    unsigned int* flag;       // device word polled by the spinning threads (0 = healthy)
+    unsigned int* host;       // mapped host word the first thread to give up writes the code to
+    long long spin_cycles;    // ~3 s at 2 GHz unless ZRB_SPIN_CYCLES says otherwise
+};
 int rec_fwd_plan(int H, int B, RecPlan* plan);
 // m (weight drop, DESIGN.md section 15; inactive by default): the image of fp32(W[r, k] * multiplier of r*H + k)
 int pack_whh_fwd(const float* W, __half* img, int H, const RecPlan& p, cudaStream_t s, MaskSrc m = MaskSrc{});
-// h0_img: the B operand of step 0 (image of the state entering the window, built by fwd_prep); h_img slot t+1 is
-// written by step t.  The grid-barrier counter is never reset between launches: `counter_base` is its value when
-// the launch starts (engine_tc.cu: GridBarrier).
-int lstm_rec_fwd(const RecPlan& p, const RecWatchdog& wd, const __half* w_img, const __half* h0_img, __half* h_img, float* gates,
-                 const float* c0, float* cst, float* h_last, float* c_last, __half* hprev_h, __half* y_h,
-                 unsigned int* counter, unsigned int counter_base, int T, int B, int H, int Hp, MaskSrc m, MaskSrc rm,
-                 cudaStream_t s, long long* trace = nullptr, float* h_f32 = nullptr);   // h_f32: optional [N,H] fp32 copy of h_t
-// m: the output site's mask (period B*H in the variational mode); rm: the recurrent mask of element b*H + j, applied to
-// the operand images and hprev_h (never to h_last, h_f32 or the input of m).
+struct RecFwdArgs {
+    const __half* w_img;      // [nCTA][KcS][G][8][8]  (K-split: CTA = (pair, K half))
+    const __half* h0_img;     // [Kc][GB][8][8] image of the state entering the window: the B operand of step 0
+    __half* h_img;            // [T+1][Kc][GB][8][8]; image t (t >= 1) is the B operand of step t, written by step t-1
+    float* gates;             // [N,4H] in: x-part pre-activations (+biases); out: activated gates
+    const float* c0;          // [B,H]
+    float* cst;               // [N,H]
+    float* h_last;            // [B,H] or null
+    float* c_last;            // [B,H] or null
+    __half* hprev_h;          // [N+B,Hp] row-major, rows B.. written here
+    __half* y_h;              // [N,Hp] row-major dropout(h)
+    float* h_f32;             // or null: [N,H] fp32 h_t (the unit-level entry point zrb_lstm_layer_fwd returns it)
+    unsigned int* counter;    // grid barrier: never reset, `base` is its value when this launch starts
+    unsigned int base;
+    int T, B, H, Hp, U, G, GB, Kc, nCTA;
+    int KcS, GBi;             // K chunks per CTA (Kc / KS); 8-row batch groups of the operand image (GB, or 4 when N = 32)
+    MaskSrc m;                // the output site's dropout (period B*H: variational mode, fixed over the window)
+    MaskSrc rm;               // variational mode: recurrent mask of element b*H + j on h_{t-1} (operand images, hprev_h)
+    RecWatch w;               // watchdog (rec_common.cuh)
+    long long* trace;         // optional (profiling): [8] launch stamps (rec_launch_stamps) + [T][8] clock64 stamps of CTA 0
+};
+// Launch the forward recurrence with a's per-call fields; the launcher sets the plan's fields (U, G, GB, Kc, nCTA, KcS,
+// GBi) and the watchdog's.  rm is never applied to h_last, h_f32 or the input of m.
+int lstm_rec_fwd(const RecPlan& p, const RecWatchdog& wd, RecFwdArgs a, cudaStream_t s);
 // Everything the forward needs from the incoming state and tokens in ONE launch (it replaced 9: five device
 // copies, two fp16 conversions, two image packs): h0s/c0s = copies of the incoming (h, c) (the caller may pass
 // the same buffers for the outgoing state), hprev_h rows [0,B) = half(h0) with zeroed pad columns, h0_img = the
@@ -136,14 +157,34 @@ int update_pack_avg(float* p, float* g, float* a, float mu, bool first, int rows
 int swap_pack(float* p, float* a, int rows, int cols, const WeightImages& img, cudaStream_t s);
 int rec_bwd_plan(int H, int B, RecPlan* plan);   // U = units per CTA, nCTA = 4 * clusters
 int pack_whh_bwd(const float* W, __half* img, int H, const RecPlan& p, cudaStream_t s, MaskSrc m = MaskSrc{});
-int lstm_rec_bwd(const RecPlan& p, const RecWatchdog& wd, const __half* w_img, __half* g_img, const float* dy, const float* gates,
-                 const float* cst, const float* c0, __half* dG_h, unsigned int* counter, unsigned int counter_base, int T,
-                 int B, int H, int G4p, MaskSrc m, MaskSrc rm, cudaStream_t s, long long* trace = nullptr, float* db1 = nullptr,
-                 float* db2 = nullptr,    // db1 / db2: bias gradients sum_{t,b} dG [4H] written by the kernel (or null)
-                 unsigned int* resident_flag = nullptr, unsigned int resident_value = 0, float* db_scratch = nullptr,
-                 const float* r = nullptr);   // r [N,H] or null: the AR/TAR gradient, added to dh after the output mask
-// resident_flag: CTA 0 stores resident_value there once every CTA of the grid has arrived at the first grid barrier,
-// i.e. the whole persistent grid holds its SMs: a stream gated on it (cuStreamWaitValue32) can then start work that
-// must only take the SMs this kernel leaves free (the data-parallel bucket all-reduce).
+struct RecBwdArgs {
+    const __half* w_img;      // [nCluster][4][Kc][G][8][8]
+    __half* g_img;            // [2][4][Kc][GB][8][8] ring: slot (t & 1) holds kGradScale * dG_t per gate
+    const float* dy;          // [N,H] grad wrt the layer's dropout'ed output
+    const float* r;           // [N,H] or null: AR/TAR gradient added after the mask (DESIGN.md section 17)
+    const float* gates;       // [N,4H] activated (i,f,g,o)
+    const float* cst;         // [N,H]
+    const float* c0;          // [B,H]
+    __half* dG_h;             // [N,G4p] row-major, kGradScale * dG
+    float* db1;               // [4H] or null: bias gradient sum_{t,b} dG (model.py:35-36: b_ih and b_hh get the same
+    float* db2;               //      gradient), accumulated in registers over the window and reduced over the batch here
+    float* db_scratch;        // [4][B][H] fp32 scratch of that reduction (needed when db1 is set)
+    int push;                 // exchange of the cluster's partial products: 1 = st.async pushes into the owners' shared
+                              // memory (complete_tx on their mbarrier), 0 = stage + remote arrive + DSMEM pulls
+    unsigned int* res_flag;   // or null: CTA 0 publishes res_value here when the whole grid is resident
+    unsigned int res_value;
+    unsigned int* counter;    // grid barrier: never reset, `base` is its value when this launch starts
+    unsigned int base;
+    int T, B, H, G4p, U, G, GB, Kc, nCTA;
+    int KcS, GBi;             // K chunks per CTA (Kc / S); 8-row batch groups of the dG images (GB, or 4 when N = 32)
+    MaskSrc m;                // the output site's dropout (period B*H: variational mode, fixed over the window)
+    MaskSrc rm;               // variational mode: recurrent mask of element b*H + j; scales the recurrent gradient
+    RecWatch w;               // watchdog (rec_common.cuh)
+    long long* trace;         // optional (profiling): [8] launch stamps (rec_launch_stamps) + [T][8] clock64 stamps of CTA 0
+};
+// Launch the backward recurrence with a's per-call fields; the launcher sets push and the plan's and the watchdog's
+// fields.  res_flag: a stream gated on it (cuStreamWaitValue32) can start work that must only take the SMs this kernel
+// leaves free (the data-parallel bucket all-reduce).
+int lstm_rec_bwd(const RecPlan& p, const RecWatchdog& wd, RecBwdArgs a, cudaStream_t s);
 
 }  // namespace zrb
