@@ -134,6 +134,18 @@ int  zrb_ctx_create_mos(const zrb_config* cfg, const int32_t* widths, int32_t ex
 /* Latent dropout p_l of a Mixture-of-Softmaxes context (0 by default; train mode only).  ZRB_E_INVALID for p outside
  * [0, 1) or not finite and for a context without experts.  A change invalidates the saved forward. */
 int  zrb_set_mos_dropout(zrb_ctx* ctx, float p);
+/* Zoneout (Krueger et al. 2017; DESIGN.md section 20 states it bit for bit): each unit keeps its previous c with
+ * probability z_c and its previous h with probability z_h, instead of taking the new ones.  Off by default (z_c = z_h =
+ * 0 changes nothing).  Layer l, step t, row b, unit j: c~ and h~ are the LSTM cell's values.  Train mode: c_t = c_{t-1}
+ * where the dropped flag of element t*B*H_l + b*H_l + j of zrb_dropout_mask(seed, step, 3L + 3 + l, T*B*H_l, z_c) is
+ * set, else c~ (a select, no scaling); h_t likewise with site 4L + 3 + l and z_h.  `seed` is the activation-mask seed
+ * of the call; the flags are drawn per step in the variational mode too.  Eval mode (zrb_eval_step, the drop-in calls
+ * with train = 0, generation, beam search, the neural cache, dynamic evaluation): c_t = fma(fp32(z_c), c_{t-1},
+ * fp32(1 - z_c) * c~) and h_t likewise.  The layer output and the carried states are the zoned h and c; the states
+ * entering the window stay detached.  ZRB_E_INVALID for a value outside [0, 1) or not finite and for ZRB_ENGINE_SIMT;
+ * zrb_lstm_layer_fwd / _bwd have no zoneout and return ZRB_E_INVALID while it is on.  The first switch-on allocates
+ * 9 bytes per (t, b, j) and layer (zrb_ctx_workspace_bytes reports them).  A change invalidates the saved forward. */
+int  zrb_set_zoneout(zrb_ctx* ctx, float z_c, float z_h);
 void zrb_ctx_destroy(zrb_ctx* ctx);
 /* bytes of device memory the context holds */
 int64_t zrb_ctx_workspace_bytes(const zrb_ctx* ctx);

@@ -46,6 +46,10 @@ ap.add_argument("--experts", type=int, default=None,
                 help="a Mixture-of-Softmaxes head of this many softmaxes (Yang et al. 2018; e.g. 15 with --embed_size 280 "
                      "--layer_sizes 960,960,620 --tied)")
 ap.add_argument("--mos_dropout", type=float, default=0.0, help="latent dropout of the --experts head")
+ap.add_argument("--zoneout_cell", type=float, default=0.0,
+                help="zoneout of the cell state (Krueger et al. 2017; the paper's LSTM setting is 0.5)")
+ap.add_argument("--zoneout_hidden", type=float, default=0.0,
+                help="zoneout of the hidden state (Krueger et al. 2017; the paper's LSTM setting is 0.05)")
 ap.add_argument("--dropout", type=float, default=0.5)
 ap.add_argument("--winit", type=float, default=0.05)
 ap.add_argument("--batch_size", type=int, default=20)
@@ -97,6 +101,8 @@ if args.impl == "cudnn" and (args.experts is not None or args.mos_dropout):
     raise SystemExit("--experts / --mos_dropout are modes of --impl ours")
 if args.mos_dropout and args.experts is None:
     raise SystemExit("--mos_dropout needs --experts")
+if args.impl == "cudnn" and (args.zoneout_cell or args.zoneout_hidden):
+    raise SystemExit("--zoneout_cell / --zoneout_hidden are modes of --impl ours")
 if args.embed_size is not None or args.layer_sizes is not None:
     from zaremba_b200.model import _check_widths
     try:
@@ -140,7 +146,8 @@ if args.impl == "ours":
                                variational=args.variational, recurrent_dropout=args.recurrent_dropout,
                                tied=args.tied, weight_drop=args.weight_drop, embed_dropout=args.embed_dropout,
                                embed_size=args.embed_size, layer_sizes=args.layer_sizes, experts=args.experts,
-                               mos_dropout=args.mos_dropout).to(dev)
+                               mos_dropout=args.mos_dropout, zoneout_cell=args.zoneout_cell,
+                               zoneout_hidden=args.zoneout_hidden).to(dev)
     tr = zaremba_b200.Trainer(model, B, T, lazy_update=args.lazy_update, ar=args.ar, tar=args.tar)
     # the corpus is staged on the device once (SURVEY 8f#2): 3 x [n_batches, T, B] int64
     trn_x = torch.stack([x for x, _ in trn_b]).contiguous().to(dev)

@@ -61,6 +61,7 @@ _SIGNATURES = {
     "zrb_ctx_create_widths": (C.c_int, [C.POINTER(ZrbConfig), C.POINTER(C.c_int32), C.POINTER(_vp)]),
     "zrb_ctx_create_mos": (C.c_int, [C.POINTER(ZrbConfig), C.POINTER(C.c_int32), C.c_int32, C.POINTER(_vp)]),
     "zrb_set_mos_dropout": (C.c_int, [_vp, C.c_float]),
+    "zrb_set_zoneout": (C.c_int, [_vp, C.c_float, C.c_float]),
     "zrb_ctx_destroy": (None, [_vp]),
     "zrb_ctx_workspace_bytes": (C.c_int64, [_vp]),
     "zrb_params_changed": (C.c_int, [_vp]),

@@ -284,6 +284,28 @@ int zrb_set_mos_dropout(zrb_ctx* c, float p) {
     return ZRB_OK;
 }
 
+int zrb_set_zoneout(zrb_ctx* c, float z_c, float z_h) {
+    ZRB_REQUIRE(c, "null ctx");
+    ZRB_REQUIRE(isfinite(z_c) && z_c >= 0.f && z_c < 1.f, "zoneout z_c %f outside [0,1)", z_c);
+    ZRB_REQUIRE(isfinite(z_h) && z_h >= 0.f && z_h < 1.f, "zoneout z_h %f outside [0,1)", z_h);
+    ZRB_REQUIRE(c->cfg.engine == ZRB_ENGINE_TC, "zoneout needs the tensor-core engine");
+    if ((z_c > 0.f || z_h > 0.f) && !c->ctil[0]) {
+        const size_t N = (size_t)c->cfg.max_seq * c->cfg.max_batch;
+        for (int l = 0; l < c->cfg.layers; ++l) {
+            ZRB_TRY(dalloc(c, &c->ctil[l], N * c->width[l + 1]));
+            ZRB_TRY(dalloc(c, &c->zflags[l], N * c->width[l + 1]));
+        }
+        ZRB_TRY(dalloc(c, &c->zhcarry, (size_t)c->cfg.max_batch * c->max_width));
+    }
+    if (z_c != c->z_c || z_h != c->z_h) {
+        c->have_fwd = false;        // a backward must not apply another rule than its forward used
+        c->bwd_next_layer = -1;
+    }
+    c->z_c = z_c;
+    c->z_h = z_h;
+    return ZRB_OK;
+}
+
 void zrb_ctx_destroy(zrb_ctx* c) {
     if (!c) return;
     tc_ctx_free(c);
@@ -976,6 +998,7 @@ int zrb_lstm_layer_fwd(zrb_ctx* c, const float* w_ih, const float* w_hh, const f
     ZRB_REQUIRE(c->cfg.engine == ZRB_ENGINE_TC, "zrb_lstm_layer_fwd is an entry point of the tensor-core engine");
     ZRB_REQUIRE(c->cfg.hidden > 0, "zrb_lstm_layer_fwd needs a context of one width");
     ZRB_REQUIRE(h0 != hT && c0 != cT, "the unit-level entry point does not alias states");
+    ZRB_REQUIRE(!zoneout_on(c), "zrb_lstm_layer_fwd has no zoneout: switch it off (zrb_set_zoneout(ctx, 0, 0)) first");
     return tc_layer_fwd(c, w_ih, w_hh, b_ih, b_hh, x, T, B, h0, c0, y, hT, cT, (cudaStream_t)stream);
 }
 
@@ -984,6 +1007,7 @@ int zrb_lstm_layer_bwd(zrb_ctx* c, const float* dy, float* dx, float* dw_ih, flo
     ZRB_REQUIRE(c && dy && dw_ih && dw_hh && db_ih && db_hh, "null argument");
     ZRB_REQUIRE(c->cfg.engine == ZRB_ENGINE_TC, "zrb_lstm_layer_bwd is an entry point of the tensor-core engine");
     ZRB_REQUIRE(c->cfg.hidden > 0, "zrb_lstm_layer_bwd needs a context of one width");
+    ZRB_REQUIRE(!zoneout_on(c), "zrb_lstm_layer_bwd has no zoneout: switch it off (zrb_set_zoneout(ctx, 0, 0)) first");
     return tc_layer_bwd(c, dy, dx, dw_ih, dw_hh, db_ih, db_hh, (cudaStream_t)stream);
 }
 

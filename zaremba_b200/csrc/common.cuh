@@ -107,9 +107,10 @@ __host__ inline MaskSrc make_mask_src(const uint8_t* explicit_mask, uint64_t see
 //   key     = (seed lo32, seed hi32 XOR pos hi32)
 //   counter = (j / 4, b, 0xFFFFFFFF, pos lo32); entry j reads word r[j % 4]
 //   u       = ((r >> 9) + 0.5) * 2^-23: exact in float32, strictly inside (0, 1)
-// Counter word 2 of a dropout mask is its site (<= 3 * ZRB_MAX_LAYERS + 1 = 25 with the recurrent sites of the
-// variational mode, the weight-drop sites, the embedding-dropout site and the latent-dropout site 3L + 2 of a
-// Mixture-of-Softmaxes head, L <= 3), never 0xFFFFFFFF: the two streams cannot meet.
+// Counter word 2 of a dropout mask is its site (<= 5 * ZRB_MAX_LAYERS + 2 = 42 with the recurrent sites of the
+// variational mode, the weight-drop sites, the embedding-dropout site, the latent-dropout site 3L + 2 of a
+// Mixture-of-Softmaxes head and the zoneout sites 3L + 3 + l and 4L + 3 + l), never 0xFFFFFFFF: the two streams cannot
+// meet.
 struct SampleSrc {
     uint32_t k0, k1, c3;
 };

@@ -14,6 +14,10 @@ struct zrb_ctx {
     int max_width = 0;
     int experts = 0;                       // zrb_ctx_create_mos: K softmaxes in the head (DESIGN.md section 19), 0 = plain
     float p_mos = 0.f;                     // zrb_set_mos_dropout: latent dropout of the head
+    float z_c = 0.f, z_h = 0.f;            // zrb_set_zoneout: zoneout of the cell and hidden states (DESIGN.md section 20)
+    float* ctil[ZRB_MAX_LAYERS] = {};      // ... [N,H_l] c~_t of the last forward, allocated when first switched on
+    uint8_t* zflags[ZRB_MAX_LAYERS] = {};  // ... [N,H_l] train-mode flags of the last forward (zoneout_flags)
+    float* zhcarry = nullptr;              // ... [B,max width] the per-timestep backward's carried zh * dh
     std::vector<void*> allocs;
     int64_t bytes = 0;
 
@@ -115,6 +119,7 @@ MaskSrc rec_mask(const zrb_ctx* c, int layer);   // recurrent site L+1+layer of 
 MaskSrc wd_mask(const zrb_ctx* c, int layer);    // weight-drop site 2L+1+layer over W_hh's 4H*H elements (inactive:
                                                  // eval mode or p_wd = 0)
 bool reg_on(const zrb_ctx* c);                   // AR / TAR is switched on (alpha > 0 or beta > 0)
+inline bool zoneout_on(const zrb_ctx* c) { return c->z_c > 0.f || c->z_h > 0.f; }   // DESIGN.md section 20
 // AR / TAR of the last forward (train mode): r into reg_r and the two values into reg_val, then reg_use = true
 int reg_compute(zrb_ctx* c, cudaStream_t s);
 MaskSrc ed_mask(const zrb_ctx* c);               // embedding-dropout site 3L+1 over the V vocabulary rows (inactive:

@@ -160,6 +160,29 @@ static int tc_alloc(zrb_ctx* c, T** p, size_t count) {
     return ZRB_OK;
 }
 
+// zoneout of layer l in this call (DESIGN.md section 20): on or off, the train-mode flags zoneout_flags drew, or the
+// eval-mode constants
+static ZoneoutSrc zoneout_src(const zrb_ctx* c, int l) {
+    ZoneoutSrc z = {};
+    z.on = zoneout_on(c) ? 1 : 0;
+    z.flags = c->train ? c->zflags[l] : nullptr;
+    z.ec = c->z_c; z.ec1 = (float)(1.0 - (double)c->z_c);
+    z.eh = c->z_h; z.eh1 = (float)(1.0 - (double)c->z_h);
+    return z;
+}
+// train mode: every layer's flags of (seed, step): sites 3L + 3 + l (c) and 4L + 3 + l (h) over T*B*H_l, per step even in
+// the variational mode
+static int zoneout_draw(zrb_ctx* c, cudaStream_t s) {
+    if (!zoneout_on(c) || !c->train) return ZRB_OK;
+    const int L = c->cfg.layers;
+    for (int l = 0; l < L; ++l) {
+        const MaskSrc mc = make_mask_src(nullptr, c->seed, c->step, 3 * L + 3 + l, c->z_c, 1);
+        const MaskSrc mh = make_mask_src(nullptr, c->seed, c->step, 4 * L + 3 + l, c->z_h, 1);
+        ZRB_TRY(zoneout_flags(mc, mh, (int64_t)c->T * c->B * c->width[l + 1], c->zflags[l], s));
+    }
+    return ZRB_OK;
+}
+
 static inline RecWatchdog tc_watchdog(const zrb_ctx* c) {
     RecWatchdog wd;
     wd.flag = c->wd_flag; wd.host = c->wd_host;
@@ -468,6 +491,7 @@ int tc_forward(zrb_ctx* c, const zrb_params* p, const int64_t* x, const zrb_stat
         fp.L = L; fp.B = B; fp.N = N;
         ZRB_TRY(fwd_prep(fp, s));
     }
+    ZRB_TRY(zoneout_draw(c, s));
     {
         ProfScope ps(c, ZRB_PROF_EMBED_FWD, s);
         // tied: E's update (item L) is still deferred -> gather through it; the update itself rides beside the last
@@ -496,6 +520,7 @@ int tc_forward(zrb_ctx* c, const zrb_params* p, const int64_t* x, const zrb_stat
             ZRB_TRY(gemm_f16_tc(xw, s));
         }
         MaskSrc m = site_mask(c, l + 1), rm = rec_mask(c, l);
+        const ZoneoutSrc zo = zoneout_src(c, l);
         // AR / TAR (DESIGN.md section 17) reads the last layer's fp32 h (the per-timestep path always writes it)
         const bool reg_h = t->in_train_step && reg_on(c) && l == L - 1;
         ProfScope ps(c, ZRB_PROF_REC_FWD, s);
@@ -506,6 +531,7 @@ int tc_forward(zrb_ctx* c, const zrb_params* p, const int64_t* x, const zrb_stat
                 a.cst = c->cst[l]; a.h_last = out->h[l]; a.c_last = out->c[l]; a.hprev_h = t->hprev_h[l];
                 a.y_h = t->x_h[l + 1]; a.h_f32 = reg_h ? c->hraw[l] : nullptr; a.counter = word; a.base = base;
                 a.T = T; a.B = B; a.H = H; a.Hp = Hp; a.m = m; a.rm = rm; a.trace = t->trace;
+                a.zo = zo; a.h0 = c->h0s[l]; a.ctil = c->ctil[l];
                 return lstm_rec_fwd(fplan, tc_watchdog(c), a, s);
             }));
             // deferred update of the NEXT layer's matrices (or of fc.W after the last layer): on the idle SMs, beside
@@ -520,9 +546,11 @@ int tc_forward(zrb_ctx* c, const zrb_params* p, const int64_t* x, const zrb_stat
             hw.A = {t->hprev_h[l] + (size_t)tt * B * Hp, Hp}; hw.B = {t->w_hh_h[l], Hp};
             hw.C = Gt; hw.ldc = 4 * H; hw.M = B; hw.N = 4 * H; hw.K = H; hw.accumulate = true;
             ZRB_TRY(gemm_f16_tc(hw, s));
+            const float* h_prev = tt ? c->hraw[l] + (size_t)(tt - 1) * B * H : c->h0s[l];
             ZRB_TRY(lstm_cell_fwd_tc(Gt, c_prev, c->cst[l] + (size_t)tt * B * H, c->hraw[l] + (size_t)tt * B * H,
                                      t->hprev_h[l] + (size_t)(tt + 1) * B * Hp, t->x_h[l + 1] + (size_t)tt * B * Hp, Hp, B,
-                                     H, (int64_t)tt * B * H, (int64_t)N * H, m, rm, s));
+                                     H, (int64_t)tt * B * H, (int64_t)N * H, m, rm, s, zo.on ? &zo : nullptr, h_prev,
+                                     zo.on ? c->ctil[l] + (size_t)tt * B * H : nullptr));
         }
         ZRB_CUDA(cudaMemcpyAsync(out->h[l], c->hraw[l] + (size_t)(T - 1) * B * H, bh, cudaMemcpyDeviceToDevice, s));
         ZRB_CUDA(cudaMemcpyAsync(out->c[l], c->cst[l] + (size_t)(T - 1) * B * H, bh, cudaMemcpyDeviceToDevice, s));
@@ -700,6 +728,7 @@ static int tc_backward_layer(zrb_ctx* c, const zrb_params* p, const zrb_params* 
     const float* r = (c->reg_use && l == c->cfg.layers - 1) ? c->reg_r : nullptr;   // AR / TAR gradient (section 17)
     {
         MaskSrc m = site_mask(c, l + 1), rm = rec_mask(c, l);
+        const ZoneoutSrc zo = zoneout_src(c, l);
         if (bplan.ok) {
             ProfScope ps(c, ZRB_PROF_REC_BWD, s);
             ZRB_TRY(t->bwd_bar.claim(T, bplan.nCTA, s, [&](unsigned int* word, unsigned int base) {
@@ -710,18 +739,22 @@ static int tc_backward_layer(zrb_ctx* c, const zrb_params* p, const zrb_params* 
                 a.res_flag = c->resident_flag; a.res_value = ++c->resident_seq; a.counter = word; a.base = base;
                 a.T = T; a.B = B; a.H = H; a.G4p = G4p; a.m = m; a.rm = rm;
                 a.trace = t->trace ? t->trace + 8 + (size_t)c->cfg.max_seq * 8 : nullptr;
+                a.zo = zo; a.ctil = c->ctil[l];
                 return lstm_rec_bwd(bplan, tc_watchdog(c), a, s);
             }));
             ZRB_TRY(tc_issue_pending(c, g, s));   // runs on the SMs the cluster kernel leaves idle
         } else {
             ProfScope ps(c, ZRB_PROF_REC_BWD, s);
             ZRB_CUDA(cudaMemsetAsync(c->dc, 0, bh * sizeof(float), s));   // (the persistent kernel keeps dc in registers)
+            if (zo.on) ZRB_CUDA(cudaMemsetAsync(c->zhcarry, 0, bh * sizeof(float), s));
             for (int tt = T - 1; tt >= 0; --tt) {
                 const float* c_prev = tt ? c->cst[l] + (size_t)(tt - 1) * bh : c->c0s[l];
+                const float* c_t = (zo.on ? c->ctil[l] : c->cst[l]) + (size_t)tt * bh;   // (zoneout: c~_t)
                 ZRB_TRY(lstm_cell_bwd_tc(dY + (size_t)tt * bh, tt == T - 1 ? nullptr : c->dh_rec, c->dc,
-                                         c->gates[l] + (size_t)tt * B * 4 * H, c->cst[l] + (size_t)tt * bh, c_prev,
+                                         c->gates[l] + (size_t)tt * B * 4 * H, c_t, c_prev,
                                          c->dG + (size_t)tt * B * 4 * H, dG_h + (size_t)tt * B * G4p, G4p, B, H,
-                                         (int64_t)tt * bh, (int64_t)N * H, m, rm, s, r ? r + (size_t)tt * bh : nullptr));
+                                         (int64_t)tt * bh, (int64_t)N * H, m, rm, s, r ? r + (size_t)tt * bh : nullptr,
+                                         zo.on ? &zo : nullptr, c->zhcarry));
                 if (tt == 0) continue;
                 Gemm dh;   // dh_{t-1}[B,H] = dG_t[B,4H] * W_hh[4H,H]
                 dh.A = {dG_h + (size_t)tt * B * G4p, G4p}; dh.B = {t->w_hh_h[l], Hp, true};

@@ -5,10 +5,13 @@
 
 namespace zrb {
 
+// ZO: zoneout (DESIGN.md section 20), the persistent kernels' rule with h_{t-1} from h_prev and c~_t into c_til
+template <bool ZO>
 __global__ void lstm_cell_fwd_tc_kernel(float* __restrict__ pre, const float* __restrict__ c_prev,
                                         float* __restrict__ c_out, float* __restrict__ h_raw,
                                         __half* __restrict__ h_raw_h, __half* __restrict__ y_h, int64_t ld_h, int B,
-                                        int H, int64_t elem_off, int64_t n_total, MaskSrc m, MaskSrc rm) {
+                                        int H, int64_t elem_off, int64_t n_total, MaskSrc m, MaskSrc rm, ZoneoutSrc zo,
+                                        const float* __restrict__ h_prev, float* __restrict__ c_til) {
     int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (tid >= (int64_t)B * H) return;
     int b = (int)(tid / H), j = (int)(tid % H);
@@ -19,6 +22,17 @@ __global__ void lstm_cell_fwd_tc_kernel(float* __restrict__ pre, const float* __
     float o = sigmoidf_(row[3 * H + j]);
     float c = f * c_prev[tid] + i * g;
     float h = o * tanhf(c);
+    if constexpr (ZO) {
+        c_til[tid] = c;
+        if (zo.flags) {
+            const uint32_t z = zo.flags[elem_off + tid];
+            if (z & 1u) c = c_prev[tid];
+            if (z & 2u) h = h_prev[tid];
+        } else {
+            c = __fmaf_rn(zo.ec, c_prev[tid], __fmul_rn(zo.ec1, c));
+            h = __fmaf_rn(zo.eh, h_prev[tid], __fmul_rn(zo.eh1, h));
+        }
+    }
     row[j] = i; row[H + j] = f; row[2 * H + j] = g; row[3 * H + j] = o;
     c_out[tid] = c;
     h_raw[tid] = h;
@@ -27,10 +41,16 @@ __global__ void lstm_cell_fwd_tc_kernel(float* __restrict__ pre, const float* __
 }
 
 int lstm_cell_fwd_tc(float* pre, const float* c_prev, float* c_out, float* h_raw, __half* h_raw_h, __half* y_h,
-                     int64_t ld_h, int B, int H, int64_t elem_off, int64_t n_total, MaskSrc m, MaskSrc rm, cudaStream_t s) {
+                     int64_t ld_h, int B, int H, int64_t elem_off, int64_t n_total, MaskSrc m, MaskSrc rm, cudaStream_t s,
+                     const ZoneoutSrc* zo, const float* h_prev, float* c_til) {
     int64_t n = (int64_t)B * H;
-    lstm_cell_fwd_tc_kernel<<<cdiv(n, 256), 256, 0, s>>>(pre, c_prev, c_out, h_raw, h_raw_h, y_h, ld_h, B, H, elem_off,
-                                                         n_total, m, rm);
+    if (zo)
+        lstm_cell_fwd_tc_kernel<true><<<cdiv(n, 256), 256, 0, s>>>(pre, c_prev, c_out, h_raw, h_raw_h, y_h, ld_h, B, H,
+                                                                   elem_off, n_total, m, rm, *zo, h_prev, c_til);
+    else
+        lstm_cell_fwd_tc_kernel<false><<<cdiv(n, 256), 256, 0, s>>>(pre, c_prev, c_out, h_raw, h_raw_h, y_h, ld_h, B, H,
+                                                                    elem_off, n_total, m, rm, ZoneoutSrc{}, nullptr,
+                                                                    nullptr);
     ZRB_KERNEL_CHECK();
     return ZRB_OK;
 }
@@ -41,12 +61,14 @@ __device__ __forceinline__ __half to_half_scaled(float v) {
     return __float2half_rn(v);
 }
 
+// ZO: c_t is c~_t, and hcarry [B,H] carries zh * dh from step t to step t-1 (the persistent kernel's register)
+template <bool ZO>
 __global__ void lstm_cell_bwd_tc_kernel(const float* __restrict__ dy_post, const float* __restrict__ dh_rec,
                                         float* __restrict__ dc, const float* __restrict__ gates,
                                         const float* __restrict__ c_t, const float* __restrict__ c_prev,
                                         float* __restrict__ dG, __half* __restrict__ dG_h, int64_t ld_g, int B, int H,
                                         int64_t elem_off, int64_t n_total, MaskSrc m, MaskSrc rm,
-                                        const float* __restrict__ r) {
+                                        const float* __restrict__ r, ZoneoutSrc zo, float* __restrict__ hcarry) {
     int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (tid >= (int64_t)B * H) return;
     int b = (int)(tid / H), j = (int)(tid % H);
@@ -55,11 +77,29 @@ __global__ void lstm_cell_bwd_tc_kernel(const float* __restrict__ dy_post, const
     float dh = dy_post[tid] * mask_mul1(m, (uint64_t)(elem_off + tid), (uint64_t)n_total);
     if (r) dh += r[tid];
     if (dh_rec) dh += dh_rec[tid] * mask_mul1_at(rm, (uint64_t)tid, (uint64_t)B * H);
+    uint32_t z = 0;
+    if constexpr (ZO) {
+        dh += hcarry[tid];
+        if (zo.flags) z = zo.flags[elem_off + tid];
+        const float dht = zo.flags ? ((z & 2u) ? 0.f : dh) : __fmul_rn(zo.eh1, dh);
+        hcarry[tid] = zo.flags ? ((z & 2u) ? dh : 0.f) : __fmul_rn(zo.eh, dh);
+        dh = dht;
+    }
     float tc = tanhf(c_t[tid]);
     float d_o = dh * tc;
-    float dcc = dc[tid] + dh * o * (1.f - tc * tc);
+    float dcc;
+    if constexpr (ZO) {   // dc~: the carried dc times (1 - zc), plus the h~ path (h~ reads c~)
+        const float dt = __fmul_rn(__fmul_rn(dh, o), __fsub_rn(1.f, __fmul_rn(tc, tc)));
+        dcc = zo.flags ? ((z & 1u) ? dt : __fadd_rn(dc[tid], dt)) : __fmaf_rn(zo.ec1, dc[tid], dt);
+    } else {
+        dcc = dc[tid] + dh * o * (1.f - tc * tc);
+    }
     float d_i = dcc * g, d_g = dcc * i, d_f = dcc * c_prev[tid];
-    dc[tid] = dcc * f;
+    if constexpr (ZO)
+        dc[tid] = zo.flags ? ((z & 1u) ? __fmaf_rn(dcc, f, dc[tid]) : __fmul_rn(dcc, f))
+                           : __fmaf_rn(zo.ec, dc[tid], __fmul_rn(dcc, f));
+    else
+        dc[tid] = dcc * f;
     float gi = d_i * i * (1.f - i), gf = d_f * f * (1.f - f), gg = d_g * (1.f - g * g), go = d_o * o * (1.f - o);
     float* drow = dG + (int64_t)b * 4 * H;
     drow[j] = gi; drow[H + j] = gf; drow[2 * H + j] = gg; drow[3 * H + j] = go;
@@ -70,10 +110,34 @@ __global__ void lstm_cell_bwd_tc_kernel(const float* __restrict__ dy_post, const
 
 int lstm_cell_bwd_tc(const float* dy_post, const float* dh_rec, float* dc, const float* gates, const float* c_t,
                      const float* c_prev, float* dG, __half* dG_h, int64_t ld_g, int B, int H, int64_t elem_off,
-                     int64_t n_total, MaskSrc m, MaskSrc rm, cudaStream_t s, const float* r) {
+                     int64_t n_total, MaskSrc m, MaskSrc rm, cudaStream_t s, const float* r, const ZoneoutSrc* zo,
+                     float* hcarry) {
     int64_t n = (int64_t)B * H;
-    lstm_cell_bwd_tc_kernel<<<cdiv(n, 256), 256, 0, s>>>(dy_post, dh_rec, dc, gates, c_t, c_prev, dG, dG_h, ld_g, B, H,
-                                                         elem_off, n_total, m, rm, r);
+    if (zo)
+        lstm_cell_bwd_tc_kernel<true><<<cdiv(n, 256), 256, 0, s>>>(dy_post, dh_rec, dc, gates, c_t, c_prev, dG, dG_h, ld_g,
+                                                                   B, H, elem_off, n_total, m, rm, r, *zo, hcarry);
+    else
+        lstm_cell_bwd_tc_kernel<false><<<cdiv(n, 256), 256, 0, s>>>(dy_post, dh_rec, dc, gates, c_t, c_prev, dG, dG_h,
+                                                                    ld_g, B, H, elem_off, n_total, m, rm, r,
+                                                                    ZoneoutSrc{}, nullptr);
+    ZRB_KERNEL_CHECK();
+    return ZRB_OK;
+}
+
+__global__ void zoneout_flags_kernel(MaskSrc c, MaskSrc h, int64_t n, uint8_t* __restrict__ flags) {
+    for (int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; 4 * g < n; g += (int64_t)gridDim.x * blockDim.x) {
+        const uint32_t kc = c.active ? mask_keep4(c, (uint64_t)g, (uint64_t)n) : 0xFu;
+        const uint32_t kh = h.active ? mask_keep4(h, (uint64_t)g, (uint64_t)n) : 0xFu;
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+            if (4 * g + i < n) flags[4 * g + i] = (uint8_t)((~kc >> i & 1u) | (~kh >> i & 1u) << 1);
+    }
+}
+
+int zoneout_flags(MaskSrc c, MaskSrc h, int64_t n, uint8_t* flags, cudaStream_t s) {
+    const int64_t quads = (n + 3) / 4;
+    const int blocks = (int)(quads < 4096 * 256 ? cdiv(quads, 256) : 4096);
+    zoneout_flags_kernel<<<blocks > 0 ? blocks : 1, 256, 0, s>>>(c, h, n, flags);
     ZRB_KERNEL_CHECK();
     return ZRB_OK;
 }

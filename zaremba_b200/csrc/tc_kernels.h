@@ -41,12 +41,30 @@ int mos_vjp(const float* Z, const float* lse, const float* ua, int64_t ldu, int 
 
 // cell pointwise with fp16 side outputs (tc_cell.cu).  rm: recurrent mask of element b*H + j (variational mode), applied
 // to h_raw_h (the next step's operand) forward and to dh_rec backward
+struct ZoneoutSrc;
+// zo (or null: the mode off; zoneout, DESIGN.md section 20): h_prev [B,H] is h_{t-1} and c_til [B,H] receives c~_t
 int lstm_cell_fwd_tc(float* pre, const float* c_prev, float* c_out, float* h_raw, __half* h_raw_h, __half* y_h,
-                     int64_t ld_h, int B, int H, int64_t elem_off, int64_t n_total, MaskSrc m, MaskSrc rm, cudaStream_t s);
+                     int64_t ld_h, int B, int H, int64_t elem_off, int64_t n_total, MaskSrc m, MaskSrc rm, cudaStream_t s,
+                     const ZoneoutSrc* zo = nullptr, const float* h_prev = nullptr, float* c_til = nullptr);
+// zo (or null): c_t is c~_t and hcarry [B,H] the carried zh * dh (read, then overwritten; zero at t = T-1)
 int lstm_cell_bwd_tc(const float* dy_post, const float* dh_rec, float* dc, const float* gates, const float* c_t,
                      const float* c_prev, float* dG, __half* dG_h, int64_t ld_g, int B, int H, int64_t elem_off,
-                     int64_t n_total, MaskSrc m, MaskSrc rm, cudaStream_t s, const float* r = nullptr);
+                     int64_t n_total, MaskSrc m, MaskSrc rm, cudaStream_t s, const float* r = nullptr,
+                     const ZoneoutSrc* zo = nullptr, float* hcarry = nullptr);
 // r [B,H] (or null): the AR/TAR gradient of this step (DESIGN.md section 17), added to dh after the output mask
+
+// Zoneout of one layer (DESIGN.md section 20).  Train mode (flags non-null): unit (t, b, j) keeps c_{t-1} where bit 0 of
+// flags[t*B*H + b*H + j] is set, and h_{t-1} where bit 1 is (zoneout_flags).  Eval mode (flags null): the expectation
+// c_t = fma(ec, c_{t-1}, ec1 * c~_t) and h_t = fma(eh, h_{t-1}, eh1 * h~_t).
+struct ZoneoutSrc {
+    const uint8_t* flags;     // [T*B*H] or null
+    float ec, ec1, eh, eh1;   // fp32(z_c), fp32(1 - z_c), fp32(z_h), fp32(1 - z_h)
+    int on;                   // the mode is on (z_c > 0 or z_h > 0): the kernels take the zoneout instantiations
+};
+// flags[e] = (dropped flag of element e of c's stream) | (dropped flag of element e of h's stream) << 1, e < n: one
+// Philox call per site and quad of elements, drawn before the layer's recurrence so that neither recurrence kernel holds
+// the generator's registers
+int zoneout_flags(MaskSrc c, MaskSrc h, int64_t n, uint8_t* flags, cudaStream_t s);
 
 // ---- persistent recurrence (lstm_rec_fwd.cu / lstm_rec_bwd.cu) ---------------------------------------
 struct RecPlan {
@@ -73,6 +91,11 @@ int rec_plan_finish(RecPlan* plan, const void* kernel, int cluster);
 // launch the plan's kernel with args = {&RecFwdArgs} or {&RecBwdArgs}; the launch modes are described at the definition
 // (lstm_rec_fwd.cu).  trace: the launch records a trace (never programmatic); name: for error messages
 int rec_launch(const RecPlan& p, void** args, bool trace, cudaStream_t s, const char* name);
+// the zoneout instantiations of the two kernels (lstm_rec_zoneout.cu): the forward with or without the K split, the
+// backward for S = 1 or 2, with their shared-memory limit raised on the current device (null when that fails, the error
+// set); the plans' occupancy answers hold for them (same shared memory, one CTA per SM, no spill)
+const void* rec_fwd_zoneout_kernel(bool split);
+const void* rec_bwd_zoneout_kernel(int S);
 // Where a persistent kernel that gave up on a wait (rec_common.cuh: watchdog) reports it: `flag` is the device word the
 // spinning threads poll, `host` a mapped host word the host reads without synchronising.  Owned by the context.
 struct RecWatchdog {
@@ -108,6 +131,10 @@ struct RecFwdArgs {
     MaskSrc rm;               // variational mode: recurrent mask of element b*H + j on h_{t-1} (operand images, hprev_h)
     RecWatch w;               // watchdog (rec_common.cuh)
     long long* trace;         // optional (profiling): [8] launch stamps (rec_launch_stamps) + [T][8] clock64 stamps of CTA 0
+    // zoneout (zo.on: the launch takes the zoneout instantiation; appended, so the other fields keep their offsets)
+    ZoneoutSrc zo;
+    const float* h0;          // [B,H] h entering the window (h_{-1} of the select)
+    float* ctil;              // [N,H] c~_t, the cell value before the select (the backward reads it)
 };
 // Launch the forward recurrence with a's per-call fields; the launcher sets the plan's fields (U, G, GB, Kc, nCTA, KcS,
 // GBi) and the watchdog's.  rm is never applied to h_last, h_f32 or the input of m.
@@ -181,6 +208,8 @@ struct RecBwdArgs {
     MaskSrc rm;               // variational mode: recurrent mask of element b*H + j; scales the recurrent gradient
     RecWatch w;               // watchdog (rec_common.cuh)
     long long* trace;         // optional (profiling): [8] launch stamps (rec_launch_stamps) + [T][8] clock64 stamps of CTA 0
+    ZoneoutSrc zo;            // zoneout (zo.on: the zoneout instantiation; the forward's flags), appended like RecFwdArgs'
+    const float* ctil;        // [N,H] c~_t of the forward (zo.on)
 };
 // Launch the backward recurrence with a's per-call fields; the launcher sets push and the plan's and the watchdog's
 // fields.  res_flag: a stream gated on it (cuStreamWaitValue32) can start work that must only take the SMs this kernel

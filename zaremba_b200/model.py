@@ -219,11 +219,18 @@ class Model(nn.Module):
     `beam_search` sample from the mixture.  The three head tensors are registered after `fc`, so with the same seed the
     other tensors equal the plain model's.  `tied=True` needs nothing beyond E.  Not with engine "simt", lstm_type
     "custom", data parallel, the neural cache or dynamic evaluation (ValueError).
+
+    Extra keywords `zoneout_cell` / `zoneout_hidden`: zoneout (Krueger et al. 2017; DESIGN.md section 20).  In train
+    mode each unit of every layer keeps its previous c with probability `zoneout_cell` and its previous h with
+    probability `zoneout_hidden` at each time step, instead of taking the new values; eval mode (and `generate`,
+    `beam_search`) uses the expectation z * previous + (1 - z) * new.  The flags are seeded like dropout.  Not with
+    lstm_type "custom" or engine "simt" (ValueError).  `state_dict()` is unchanged.
     """
 
     def __init__(self, vocab_size, hidden_size, layer_num, dropout, winit, lstm_type="pytorch", engine="tc",
                  variational=False, recurrent_dropout=None, *, tied=False, weight_drop=0.0, embed_dropout=0.0,
-                 embed_size=None, layer_sizes=None, experts=None, mos_dropout=0.0):
+                 embed_size=None, layer_sizes=None, experts=None, mos_dropout=0.0, zoneout_cell=0.0,
+                 zoneout_hidden=0.0):
         super().__init__()
         E, sizes = _check_widths(hidden_size, layer_num, embed_size, layer_sizes)
         equal = all(w == E for w in sizes)
@@ -241,6 +248,14 @@ class Model(nn.Module):
             raise ValueError(f"mos_dropout must be a number in [0, 1), got {mos_dropout!r}")
         if mos_dropout and experts is None:
             raise ValueError("mos_dropout needs experts")
+        for name, z in (("zoneout_cell", zoneout_cell), ("zoneout_hidden", zoneout_hidden)):
+            if isinstance(z, bool) or not isinstance(z, (int, float)) or not 0.0 <= float(z) < 1.0:
+                raise ValueError(f"{name} must be a number in [0, 1), got {z!r}")
+        if zoneout_cell or zoneout_hidden:
+            if lstm_type == "custom":
+                raise ValueError("zoneout needs lstm_type 'pytorch'")
+            if engine == "simt":
+                raise ValueError("zoneout needs the tensor-core engine (engine='tc')")
         if not equal and lstm_type == "custom":
             raise ValueError("layers of unequal width need lstm_type 'pytorch'")
         if not equal and engine == "simt":
@@ -285,6 +300,8 @@ class Model(nn.Module):
         self._widths_given = embed_size is not None or layer_sizes is not None
         self.experts = experts
         self.mos_dropout = float(mos_dropout)
+        self.zoneout_cell = float(zoneout_cell)
+        self.zoneout_hidden = float(zoneout_hidden)
         self.embed = Embed(vocab_size, E)
         self.rnns = nn.ModuleList(LSTM(([E] + list(sizes))[l], sizes[l], lstm_type) for l in range(layer_num))
         self.fc = Linear(E if experts else sizes[-1], vocab_size)
@@ -543,6 +560,8 @@ class Model(nn.Module):
             _lib.check(lib.zrb_set_embed_dropout(h, self.embed_dropout, int(torch.initial_seed()) & 0xFFFFFFFFFFFFFFFF))
         if self.mos_dropout:
             _lib.check(lib.zrb_set_mos_dropout(h, self.mos_dropout))
+        if self.zoneout_cell or self.zoneout_hidden:
+            _lib.check(lib.zrb_set_zoneout(h, self.zoneout_cell, self.zoneout_hidden))
         if self._explicit_masks is not None:
             self._push_masks()
         return self._ctx
