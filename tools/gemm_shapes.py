@@ -29,7 +29,7 @@ def cdiv(a, b):
 
 
 def plan(M, N, K, can_split, nsm, sumsq, direct):
-    """gemm_tc.cu choose_tiles restated: (tile width, splits, work items, rounds)."""
+    """gemm_tc.cu choose_tiles and the pair plan restated: (tile width, splits, work items, rounds, tile rows)."""
     kb = cdiv(K, GBK)
     tm = cdiv(M, GBM)
     t256 = tm * cdiv(N, 256)
@@ -42,7 +42,15 @@ def plan(M, N, K, can_split, nsm, sumsq, direct):
             bn = 128
         sp = 2 if (can_split and tm * cdiv(N, bn) * 2 <= nsm and kb >= 8) else 1
     items = tm * cdiv(N, bn) * sp
-    return bn, sp, items, items / nsm
+    tm64 = cdiv(M, 64)
+    if sp == 2 and bn == 256 and not direct and tm64 > tm:
+        # the pair plan (gemm_f16_tc_pair_kernel): 64-row items, two per 2-CTA cluster, taken when all its clusters are
+        # resident at once (assumed here: nsm / 2 of them, as on a 132-SM H100); items = CTAs, a copy included
+        tn = cdiv(N, bn)
+        pairs = 2 * ((tm64 // 2) * tn + ((tn + 1) // 2 if tm64 % 2 else 0))
+        if pairs <= nsm // 2:
+            return bn, sp, 2 * pairs, 2 * pairs / nsm, 64
+    return bn, sp, items, items / nsm, GBM
 
 
 def calls(cfg):
@@ -168,18 +176,18 @@ def main():
             t = time_call(lib, _lib, M, N, K, a_mn, b_mn, bias, a.reps, sides)
             flop = 2.0 * M * N * K
             for side in sides:
-                bn, sp, items, rounds = plan(M, N, K, True, nsm, False, side == "direct")
+                bn, sp, items, rounds, bm = plan(M, N, K, True, nsm, False, side == "direct")
                 r = dict(config=cfg, cls=cls, what=what, M=M, N=N, K=K, side=side, ms=t[side],
-                         tflops=flop / t[side] / 1e9, tile_n=bn, splits=sp, work_items=items, rounds=rounds,
+                         tflops=flop / t[side] / 1e9, tile_m=bm, tile_n=bn, splits=sp, work_items=items, rounds=rounds,
                          calls_per_step=per_step)
                 rows.append(r)
                 print(f"{cfg:6s} {cls:10s} {M:5d}x{N:5d}x{K:5d} {side:6s} {t[side]*1e3:8.1f} us "
-                      f"{r['tflops']:6.1f} TFLOP/s  128x{bn} x{sp}: {items} items, {rounds:.2f} rounds  ({what})")
+                      f"{r['tflops']:6.1f} TFLOP/s  {bm}x{bn} x{sp}: {items} items, {rounds:.2f} rounds  ({what})")
     prof = {}
     if not a.no_profile:
         for side in sides:
             prof[side] = profile_step(side, a.out)
-            gemm = sum(v for k, v in prof[side].items() if "gemm_f16_tc_kernel" in k)
+            gemm = sum(v for k, v in prof[side].items() if "gemm_f16_tc_kernel" in k or "gemm_f16_tc_pair_kernel" in k)
             total = sum(prof[side].values())
             print(f"# profile Large step, {side}: GEMM kernels {gemm:.1f} us of {total:.1f} us kernel time per step")
             for k, v in sorted(prof[side].items(), key=lambda kv: -kv[1])[:12]:

@@ -10,6 +10,9 @@
 //                 flight, and stores its accumulators (alpha, bias, fp32 stores or split-K atomics) itself; the two
 //                 warpgroups run kStages-1 K blocks apart, so one's epilogue overlaps the other's wgmmas
 //
+// A split-K plan that leaves SMs idle runs instead as 64-row items in 2-CTA clusters that multicast the B tile they
+// share (gemm_f16_tc_pair_kernel, below), with the same arithmetic per output element.
+//
 // Every batched contraction of the path runs here: X*W_ih^T, the vocabulary projection, their
 // dgrads (weights read MN-major from the same fp16 image, no transposed copies) and the
 // wgrads (both operands MN-major: contraction over tokens).  Roofline: tensor pipe
@@ -268,6 +271,209 @@ gemm_f16_tc_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_const
     if (p.pdl_tail && blockIdx.x == 0 && threadIdx.x == 0) asm volatile("griddepcontrol.wait;" ::: "memory");
 }
 
+// ---- split-K in CTA pairs ----------------------------------------------------------------------
+// A split-K plan of 128-row tiles leaves SMs idle (the dgrads: 6 x 6 tiles x 2 K halves = 72 CTAs on 132 SMs; M = 700 is
+// 11 blocks of 64 rows, so 64-row items fill the machine).  This kernel runs the same plan as 64 x 256 x (one K half)
+// work items, two per 2-CTA cluster.  A pair shares its K half; usually it is the two 64-row halves of one 128-row tile
+// (same N block), and then each CTA loads its own A rows and one column half of the B tile, multicast into both.  Each
+// consumer warpgroup takes 128 columns of the 64 rows, one wgmma chain over the same K blocks as in the 128-row plan:
+// every output element gets the same k16 sequence, the same alpha and the same two atomically added partials, so the
+// bits are those of the 128-row plan.
+//
+// Pairs of one K half: first the vertical ones (64-row blocks 2i and 2i+1 of an N block), then, when the number of
+// 64-row blocks is odd, the last block's items two by two along N; those do not share B, and each CTA loads its whole
+// B tile itself.  An odd one left over is paired with a copy of itself that stores nothing.  Both CTAs of a pair run the
+// same K blocks, so their stage rings stay in step: a stage is refilled once the consumers of BOTH CTAs have released it
+// (the partner's multicast writes into this CTA's copy of the stage).
+//
+// The two consumer warpgroups read the same stages in lockstep (no staggered start): a CTA of this plan runs one work
+// item, so there is no epilogue to hide under the other warpgroup's wgmmas, and the producer can run a whole ring ahead
+// of both.  The stage count is what fits in 227 KB (the 64-row A tile frees 8 KB per stage).  Only split plans of
+// 256-wide tiles take it (gemm_f16_tc).
+constexpr int PBM = 64, PBN = 256;
+struct PairCfg {
+    static constexpr int kStages = 5;
+    static constexpr int kABytes = PBM * GBK * 2;
+    static constexpr int kBBytes = PBN * GBK * 2;
+    static constexpr int kSmem = kStages * (kABytes + kBBytes) + 1024 /*align slack*/ + 256 /*barriers*/;
+};
+
+// pairs per K half for tiles_m 64-row blocks and tiles_n N blocks
+__host__ __device__ inline int pairs_per_split(int tiles_m, int tiles_n) {
+    return (tiles_m / 2) * tiles_n + ((tiles_m & 1) ? (tiles_n + 1) / 2 : 0);
+}
+
+struct PairItem {
+    int split, m_blk, n_blk;
+    bool shared;   // both CTAs have this N block: each loads one column half of B for both
+    bool live;     // false: a copy of the partner's item, nothing stored
+};
+__device__ __forceinline__ PairItem pair_item(int tiles_m, int tiles_n, int pair, int rank) {
+    const int vert = (tiles_m / 2) * tiles_n, per = pairs_per_split(tiles_m, tiles_n);
+    const int q = pair % per;
+    PairItem it;
+    it.split = pair / per;
+    if (q < vert) {
+        it.n_blk = q / (tiles_m / 2);
+        it.m_blk = 2 * (q % (tiles_m / 2)) + rank;
+        it.shared = it.live = true;
+    } else {
+        const int n_first = 2 * (q - vert);   // rank 0's N block
+        it.m_blk = tiles_m - 1;
+        it.live = n_first + rank < tiles_n;
+        it.n_blk = it.live ? n_first + rank : n_first;
+        it.shared = n_first + 1 >= tiles_n;
+    }
+    return it;
+}
+
+// p.tiles_m counts 64-row blocks here; p.splits == 2, no sum-of-squares slots, no accumulate, no dual problem.
+template <bool A_MN, bool B_MN>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+gemm_f16_tc_pair_kernel(const __grid_constant__ CUtensorMap tma_a, const __grid_constant__ CUtensorMap tma_b,
+                        GemmArgs p) {
+    using Cfg = PairCfg;
+    constexpr int GBN = PBN;
+    constexpr int kStages = Cfg::kStages;
+    constexpr int kABytes = Cfg::kABytes;
+    constexpr int kBBytes = Cfg::kBBytes;
+    constexpr int kBHalf = kBBytes / 2;   // GBN/2 columns: K-major GBN/2 rows of 128 B, MN-major GBN/128 64-column boxes
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
+    uint8_t* sA = smem;
+    uint8_t* sB = smem + kStages * kABytes;
+    uint64_t* bars = (uint64_t*)(smem + kStages * (kABytes + kBBytes));
+    uint64_t* full = bars;                       // [kStages]
+    uint64_t* empty = bars + kStages;            // [kStages]: the consumer warps of both CTAs
+
+    const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
+    const int lane = threadIdx.x & 31;
+    const int rank = (int)cta_rank_in_cluster();
+    const int num_kb = (p.K + GBK - 1) / GBK;
+    const int kb_per = (num_kb + 1) / 2;
+    const int num_pairs = 2 * pairs_per_split(p.tiles_m, p.tiles_n);
+    const int cluster = blockIdx.x >> 1, num_clusters = gridDim.x >> 1;
+
+    if (threadIdx.x == 0) {
+        if (p.pdl_trigger) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+        tma_prefetch_desc(&tma_a);
+        tma_prefetch_desc(&tma_b);
+        for (int i = 0; i < kStages; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 2 * kEpiWarps); }
+        fence_mbar_init();
+    }
+    cluster_barrier();   // the partner's barriers exist before anything multicasts or arrives on them
+
+    if (warp < 4) {
+        // ===================== TMA producer =====================
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
+        if (warp == 0 && lane == 0) {
+            int s = 0; uint32_t ph = 0;
+            for (int pr = cluster; pr < num_pairs; pr += num_clusters) {
+                const PairItem it = pair_item(p.tiles_m, p.tiles_n, pr, rank);
+                const int kb0 = it.split * kb_per, kb1 = min(num_kb, kb0 + kb_per);
+                const int m0 = it.m_blk * PBM, n0 = it.n_blk * GBN;
+                for (int kb = kb0; kb < kb1; ++kb) {
+                    mbar_wait(&empty[s], ph ^ 1);
+                    mbar_expect_tx(&full[s], kABytes + kBBytes);
+                    uint8_t* a = sA + s * kABytes;
+                    uint8_t* b = sB + s * kBBytes;
+                    if (!A_MN) tma_load_2d(a, &tma_a, &full[s], kb * GBK, m0);
+                    else       tma_load_2d(a, &tma_a, &full[s], m0, kb * GBK);
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        if (it.shared && h != rank) continue;
+#pragma unroll
+                        for (int j = 0; j < (B_MN ? GBN / 128 : 1); ++j) {
+                            uint8_t* dst = b + h * kBHalf + j * (GBK * 128);
+                            const int c0 = B_MN ? n0 + h * (GBN / 2) + 64 * j : kb * GBK;
+                            const int c1 = B_MN ? kb * GBK : n0 + h * (GBN / 2);
+                            if (it.shared) tma_load_2d_multicast(dst, &tma_b, &full[s], c0, c1, 0x3);
+                            else           tma_load_2d(dst, &tma_b, &full[s], c0, c1);
+                        }
+                    }
+                    if (++s == kStages) { s = 0; ph ^= 1; }
+                }
+            }
+        }
+    } else {
+        // ===================== consumers: warpgroup wg takes columns [wg GBN/2, (wg + 1) GBN/2) =====================
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
+        const int cw = warp - 4;
+        const int wg = cw >> 2;
+        const int t = (int)threadIdx.x - 128 * (1 + wg);
+        int s = 0; uint32_t ph = 0;
+        float acc[GBN / 4];
+        const bool pair_store = (p.ldc & 1) == 0 && ((uintptr_t)p.C & 7) == 0;
+        for (int pr = cluster; pr < num_pairs; pr += num_clusters) {
+            const PairItem it = pair_item(p.tiles_m, p.tiles_n, pr, rank);
+            const int kb0 = it.split * kb_per, kb1 = min(num_kb, kb0 + kb_per);
+            const int m0 = it.m_blk * PBM, n0 = it.n_blk * GBN + wg * (GBN / 2);
+#pragma unroll
+            for (int i = 0; i < GBN / 4; ++i) acc[i] = 0.f;
+            wgmma_fence();
+            wgmma_fence_acc(acc);
+            int prev = -1;
+            for (int kb = kb0; kb < kb1; ++kb) {
+                mbar_wait(&full[s], ph);
+                const uint32_t a_addr = smem_u32(sA + s * kABytes);
+                const uint32_t b_addr = smem_u32(sB + s * kBBytes) + wg * kBHalf;   // 1024-byte aligned
+#pragma unroll
+                for (int k = 0; k < GBK / 16; ++k) {
+                    const uint64_t da = A_MN ? make_smem_desc(a_addr + k * 2048, GBK * 128, 1024, kSwizzle128B)
+                                             : make_smem_desc(a_addr + k * 32, 16, 1024, kSwizzle128B);
+                    const uint64_t db = B_MN ? make_smem_desc(b_addr + k * 2048, GBK * 128, 1024, kSwizzle128B)
+                                             : make_smem_desc(b_addr + k * 32, 16, 1024, kSwizzle128B);
+                    Wgmma<GBN / 2, A_MN ? 1 : 0, B_MN ? 1 : 0>::mma(acc, da, db, 1u);
+                }
+                wgmma_commit();
+                wgmma_wait<1>();
+                if (prev >= 0) {
+                    __syncwarp();
+                    if (lane < 2) mbar_arrive_rank(&empty[prev], lane);   // this CTA's and the partner's
+                }
+                prev = s;
+                if (++s == kStages) { s = 0; ph ^= 1; }
+            }
+            wgmma_wait<0>();
+            wgmma_fence_acc(acc);
+            if (prev >= 0) {
+                __syncwarp();
+                if (lane < 2) mbar_arrive_rank(&empty[prev], lane);
+            }
+            if (!it.live) continue;
+            // the epilogue of gemm_f16_tc_kernel's split-K path, element for element
+            const bool add_bias = p.bias != nullptr && it.split == 0;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int row = m0 + wgmma_row(t, h);
+                if (row >= p.M) continue;
+                float* const crow = p.C + (int64_t)row * p.ldc;
+#pragma unroll
+                for (int c8 = 0; c8 < GBN / 16; ++c8) {
+                    const int col0 = n0 + wgmma_col(t, c8);
+                    if (pair_store && col0 + 1 < p.N) {
+                        const float bv0 = add_bias ? p.bias[col0] + (p.bias2 ? p.bias2[col0] : 0.f) : 0.f;
+                        const float bv1 = add_bias ? p.bias[col0 + 1] + (p.bias2 ? p.bias2[col0 + 1] : 0.f) : 0.f;
+                        const float o0 = p.alpha * acc[4 * c8 + 2 * h] + bv0;
+                        const float o1 = p.alpha * acc[4 * c8 + 2 * h + 1] + bv1;
+                        atomicAdd(reinterpret_cast<float2*>(crow + col0), make_float2(o0, o1));
+                        continue;
+                    }
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const int col = col0 + e;
+                        if (col >= p.N) continue;
+                        const float bv = add_bias ? p.bias[col] + (p.bias2 ? p.bias2[col] : 0.f) : 0.f;
+                        atomicAdd(crow + col, p.alpha * acc[4 * c8 + 2 * h + e] + bv);
+                    }
+                }
+            }
+        }
+    }
+    __syncwarp();
+    cluster_barrier();   // no CTA leaves while its partner may still multicast into it or arrive on its barriers
+}
+
 // ---- host side ----------------------------------------------------------------------------------
 namespace {
 
@@ -367,6 +573,58 @@ static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const CUten
     return ZRB_OK;
 }
 
+// the gemm_f16_tc_pair_kernel instantiation for the operand layouts
+static const void* pair_kernel(bool a_mn, bool b_mn) {
+    if (!a_mn) return b_mn ? (const void*)gemm_f16_tc_pair_kernel<false, true> : (const void*)gemm_f16_tc_pair_kernel<false, false>;
+    return b_mn ? (const void*)gemm_f16_tc_pair_kernel<true, true> : (const void*)gemm_f16_tc_pair_kernel<true, false>;
+}
+
+static void pair_launch_config(cudaLaunchConfig_t* cfg, cudaLaunchAttribute* cluster, int grid) {
+    *cfg = {};
+    cfg->gridDim = dim3(grid); cfg->blockDim = dim3(kGemmThreads); cfg->dynamicSmemBytes = PairCfg::kSmem;
+    cluster->id = cudaLaunchAttributeClusterDimension;
+    cluster->val.clusterDim.x = 2; cluster->val.clusterDim.y = 1; cluster->val.clusterDim.z = 1;
+    cfg->attrs = cluster; cfg->numAttrs = 1;
+}
+
+// per device and layout: 1 + cudaOccupancyMaxActiveClusters of the pair kernel (0: not asked yet; a failed query
+// counts as none).  Asking also raises the kernel's shared-memory limit, which its launches rely on.
+static int g_pair_clusters[64][4] = {};
+
+// The pair plan when all its clusters are resident at once (one round of 64-row items instead of one of 128-row tiles);
+// false: the caller keeps the 128-row plan.
+static bool pair_plan_fits(int pairs, bool a_mn, bool b_mn) {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    int& slot = g_pair_clusters[dev & 63][(a_mn ? 2 : 0) + (b_mn ? 1 : 0)];
+    if (!slot) {
+        const void* kern = pair_kernel(a_mn, b_mn);
+        cudaLaunchConfig_t cfg;
+        cudaLaunchAttribute cluster;
+        pair_launch_config(&cfg, &cluster, tc_num_sms() & ~1);
+        int n = 0;
+        if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, PairCfg::kSmem) != cudaSuccess ||
+            cudaOccupancyMaxActiveClusters(&n, kern, &cfg) != cudaSuccess) {
+            (void)cudaGetLastError();
+            n = 0;
+        }
+        slot = 1 + n;
+    }
+    return pairs <= slot - 1;
+}
+
+static int launch_gemm_pair(const CUtensorMap& ta, const CUtensorMap& tb, const GemmArgs& a, int pairs, bool a_mn,
+                            bool b_mn, cudaStream_t s) {
+    cudaLaunchConfig_t cfg;
+    cudaLaunchAttribute cluster;
+    pair_launch_config(&cfg, &cluster, 2 * pairs);
+    cfg.stream = s;
+    void* args[] = {(void*)&ta, (void*)&tb, (void*)&a};
+    ZRB_CUDA(cudaLaunchKernelExC(&cfg, pair_kernel(a_mn, b_mn), args));
+    count_launch();
+    return ZRB_OK;
+}
+
 template <int GBN>
 static int dispatch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& tb2, const GemmArgs& a,
                          int a_mn, int b_mn, cudaStream_t s) {
@@ -440,10 +698,18 @@ int gemm_f16_tc(const Gemm& g, cudaStream_t s) {
     const TileChoice tc = gemm_tiles(g, g.sumsq != nullptr, direct);
     const int bn = tc.bn;
     const bool a_mn = g.A.mn_major, b_mn = g.B.mn_major;
+    // a split plan of 256-wide tiles runs in CTA pairs of 64-row items (gemm_f16_tc_pair_kernel) when that makes more
+    // work items and all the pairs are resident at once; never under ZRB_GEMM_EPI=direct, whose plan is the reference.
+    // (128-wide tiles stay: as pairs each warpgroup issues m64n64 wgmmas, and Medium's dS*W_fc measured 6% slower.)
+    const int tiles_m64 = cdiv(M, PBM);
+    const int pairs = 2 * pairs_per_split(tiles_m64, tc.tiles_n);
+    const bool paired = !direct && tc.splits == 2 && bn == 256 && !g.a_tiled && !g.b_tiled && tiles_m64 > tc.tiles_m &&
+                        pair_plan_fits(pairs, a_mn, b_mn);
+    const int box_m = paired ? PBM : GBM, box_n = paired ? bn / 2 : bn;   // (K-major boxes; MN-major ones are 64 wide)
     CUtensorMap ta, tb;
-    if (!a_mn) ZRB_TRY(tc_make_tmap_f16(&ta, g.A.ptr, K, M, g.A.ld, GBK, GBM, 1));
+    if (!a_mn) ZRB_TRY(tc_make_tmap_f16(&ta, g.A.ptr, K, M, g.A.ld, GBK, box_m, 1));
     else       ZRB_TRY(tc_make_tmap_f16(&ta, g.A.ptr, M, K, g.A.ld, 64, GBK, 1));
-    if (!b_mn) ZRB_TRY(tc_make_tmap_f16(&tb, g.B.ptr, K, N, g.B.ld, GBK, bn, 1));
+    if (!b_mn) ZRB_TRY(tc_make_tmap_f16(&tb, g.B.ptr, K, N, g.B.ld, GBK, box_n, 1));
     else       ZRB_TRY(tc_make_tmap_f16(&tb, g.B.ptr, N, K, g.B.ld, 64, GBK, 1));
     CUtensorMap tb2 = tb;
     if (d2.B) {
@@ -466,6 +732,10 @@ int gemm_f16_tc(const Gemm& g, cudaStream_t s) {
     a.epi_direct = direct ? 1 : 0;
     // split partials are added into a zeroed C: order-independent for two (a+b == b+a)
     if (a.splits > 1 && !g.accumulate) ZRB_CUDA(cudaMemsetAsync(g.C, 0, (size_t)M * N * sizeof(float), s));
+    if (paired) {
+        a.tiles_m = tiles_m64;
+        return launch_gemm_pair(ta, tb, a, pairs, a_mn, b_mn, s);
+    }
     return bn == 256 ? dispatch_gemm<256>(ta, tb, tb2, a, a_mn, b_mn, s) : dispatch_gemm<128>(ta, tb, tb2, a, a_mn, b_mn, s);
 }
 

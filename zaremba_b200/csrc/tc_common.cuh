@@ -37,6 +37,23 @@ __device__ __forceinline__ void fence_mbar_init() { asm volatile("fence.mbarrier
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
+// arrive on the mbarrier at `bar`'s offset in the shared memory of cluster rank `rank` (this CTA's own included), with
+// the default CTA-scope release: it hands back a stage whose reads (wgmma) have completed, and orders no memory writes.
+// (.release.cluster would put a MEMBAR.GPU in front of every arrive: ~1 us per stage, measured.)
+__device__ __forceinline__ void mbar_arrive_rank(uint64_t* bar, uint32_t rank) {
+    uint32_t a;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(a) : "r"(smem_u32(bar)), "r"(rank));
+    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(a) : "memory");
+}
+__device__ __forceinline__ uint32_t cta_rank_in_cluster() {
+    uint32_t r;
+    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+    return r;
+}
+// every thread of every CTA in the cluster (warp-converged)
+__device__ __forceinline__ void cluster_barrier() {
+    asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
@@ -73,6 +90,16 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* m, uin
     asm volatile(
         "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
         :: "r"(smem_u32(dst)), "l"((uint64_t)m), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
+        : "memory");
+}
+// the same box written to the same shared-memory offset of every CTA in `cta_mask` (cluster ranks), each of which has
+// its mbarrier at `bar`'s offset signalled with the box's bytes
+__device__ __forceinline__ void tma_load_2d_multicast(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1,
+                                                      uint16_t cta_mask) {
+    asm volatile(
+        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+        " [%0], [%1, {%3, %4}], [%2], %5;"
+        :: "r"(smem_u32(dst)), "l"((uint64_t)m), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask)
         : "memory");
 }
 // 1-D bulk copy global -> shared (bytes multiple of 16, 16-byte aligned both sides)
