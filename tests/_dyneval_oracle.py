@@ -1,6 +1,6 @@
 """Float64 restatement of dynamic evaluation (DESIGN.md section 14)  --  TEST INFRASTRUCTURE ONLY.
 
-Built on `oracle.lstm_lm_oracle` (untied) and `tests/_tied_oracle.py` (tied); nothing under oracle/ changes.
+Built on `oracle.lstm_lm_oracle` (untied) and `tests/_model_oracle.py` (tied); nothing under oracle/ changes.
   - the window loss and its gradient are the oracle's eval-mode (no dropout) loss and backward, entering states detached;
   - the update is theta += a * (theta_g - theta) - lr * u with the RMS rule (u = g / (r + eps), a = min(1, lam r / rbar))
     or the SGD rule (u = g, a = min(1, lam));
@@ -10,22 +10,28 @@ Built on `oracle.lstm_lm_oracle` (untied) and `tests/_tied_oracle.py` (tied); no
 from __future__ import annotations
 
 import numpy as np
+import torch
 
 from oracle import lstm_lm_oracle as O
-from tests import _tied_oracle as TO
+from tests import _model_oracle as MO
 
 
 def names(layer_num, tied=False):
     """The distinct parameter tensors (a tied E once, as "embed.W")."""
-    return TO.param_names(layer_num) if tied else O.param_names(layer_num)
+    return MO.names(layer_num, tied)
 
 
 def window_grads(params, x, y, states, layer_num, tied=False):
     """(loss, grads, new states) of the eval-mode window loss at params."""
-    M = TO if tied else O
-    scores, new_states, cache = M.model_fwd(params, x, states, layer_num)
+    if tied:
+        loss, _, grads, _, new_states, _ = MO.train_step(
+            {k: torch.as_tensor(v) for k, v in params.items()}, torch.as_tensor(x), torch.as_tensor(y),
+            [(torch.as_tensor(h), torch.as_tensor(c)) for h, c in states], layer_num, True, 0.0, float("inf"))
+        return (loss, {k: g.numpy() for k, g in grads.items()},
+                [(h.numpy(), c.numpy()) for h, c in new_states])
+    scores, new_states, cache = O.model_fwd(params, x, states, layer_num)
     loss = O.nll_loss(scores, y)
-    grads = M.model_bwd(params, cache, O.nll_loss_bwd(scores, y), layer_num)
+    grads = O.model_bwd(params, cache, O.nll_loss_bwd(scores, y), layer_num)
     return loss, grads, new_states
 
 

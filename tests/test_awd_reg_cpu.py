@@ -1,4 +1,4 @@
-"""Embedding dropout and AR/TAR without a GPU: their numpy restatement (tests/_awd_reg_oracle.py) against an
+"""Embedding dropout and AR/TAR without a GPU: the fp64 restatement (tests/_model_oracle.py) against an
 independent float64 torch-autograd loop written as AWD-LSTM writes it (`F.embedding(x, W * mask / (1 - p))`, then
 `alpha * y.pow(2).mean()` and `beta * (h[1:] - h[:-1]).pow(2).mean()`, times B), with Zaremba's dropout, the variational
 mode, weight drop, tied weights and T = 1; the mask's site; the C entry points in the header and the ctypes binding;
@@ -14,9 +14,7 @@ import torch.nn.functional as F
 
 from oracle import lstm_lm_oracle as O
 from oracle import philox as PH
-from tests import _awd_reg_oracle as AO
-from tests import _variational_oracle as VO
-from tests import _weight_drop_oracle as WO
+from tests import _model_oracle as MO
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 V, H, L, B = 23, 8, 2, 3
@@ -33,20 +31,40 @@ def _setup(T, variational, weight_drop, tied, seed=7):
     x = rng.integers(0, V, size=(T, B))
     y = rng.integers(0, V, size=(T, B))
     states = [(rng.uniform(-0.5, 0.5, (B, H)), rng.uniform(-1, 1, (B, H))) for _ in range(L)]   # non-zero entering
-    if variational:
-        masks, rmasks = VO.variational_masks(12345, STEP, L, T, B, H, P, P_REC)
-    else:
-        masks, rmasks = PH.site_masks(12345, STEP, L, T, B, H, P), None
-    wd = WO.weight_drop_masks(SEED, STEP, L, H, P_WD) if weight_drop else None
-    em = AO.embed_mask(SEED, STEP, L, V, P_E)
-    return params, x, y, states, masks, rmasks, wd, em
+    mk = MO.mode_masks(_modes(variational, weight_drop), [H] * (L + 1), T, B, V)
+    return params, x, y, states, mk.sites, mk.rec, mk.wd, mk.ed
+
+
+def _modes(variational, weight_drop, alpha=0.0, beta=0.0, p_e=P_E):
+    return MO.Modes(seed=12345, step=STEP, p=P, variational=variational, p_rec=P_REC if variational else 0.0,
+                    wd_seed=SEED, p_wd=P_WD if weight_drop else 0.0, ed_seed=SEED, p_e=p_e, alpha=alpha, beta=beta)
+
+
+def _embed_mask(step, V, p_e):
+    return MO.mode_masks(MO.Modes(ed_seed=SEED, step=step, p_e=p_e), [H] * (L + 1), 1, 1, V).ed
+
+
+def _tensors(params, x, y, states):
+    return ({k: torch.tensor(v) for k, v in params.items()}, torch.tensor(x), torch.tensor(y),
+            [(torch.tensor(h), torch.tensor(c)) for h, c in states])
+
+
+def _oracle(params, x, y, states, masks, rmasks, wd, em, md, tied):
+    """_model_oracle's NLL, scores, states, raw gradients of NLL + AR + TAR (autograd) and AR + TAR, as numpy"""
+    ps, x, y, states = _tensors(params, x, y, states)
+    ps = {k: v.requires_grad_(True) for k, v in ps.items()}
+    sc, st, reg = MO.forward(ps, x, states, L, tied, md, MO.Masks(sites=masks, rec=rmasks, wd=wd, ed=em))
+    loss = MO.loss_of(sc, y)
+    (loss + reg).backward()
+    return (loss.item(), sc.detach().numpy(), [(h.detach().numpy(), c.detach().numpy()) for h, c in st],
+            {k: v.grad.numpy() for k, v in ps.items()}, torch.as_tensor(reg).item())
 
 
 def _torch_restatement(params, x, y, states, masks, rmasks, wd, em, tied, alpha=0.0, beta=0.0):
     """model.py:103-110 as an explicit per-step loop in float64 torch with AWD-LSTM's embedded_dropout
     (F.embedding(x, W * mask / (1 - p))), the projection reading the raw E when tied; autograd for the gradients.
     The backward differentiates NLL + AR + TAR (AWD's main.py terms times B, the unit of the NLL).
-    Returns (NLL, scores, states, grads, (AR, TAR))."""
+    Returns (NLL, scores, states, grads, (AR, TAR), r = d(AR + TAR) / dh of the last layer's raw output)."""
     tp = {k: torch.tensor(v, dtype=torch.float64, requires_grad=True) for k, v in params.items()}
     T = x.shape[0]
     s, sr, sw = 1.0 / (1.0 - P), 1.0 / (1.0 - P_REC), 1.0 / (1.0 - P_WD)
@@ -78,9 +96,10 @@ def _torch_restatement(params, x, y, states, masks, rmasks, wd, em, tied, alpha=
     loss = -logp[torch.arange(T * B), torch.tensor(y).reshape(-1)].mean() * B
     ar = alpha * a.pow(2).mean() * B
     tar = beta * (hs[1:] - hs[:-1]).pow(2).mean() * B if T > 1 else torch.zeros((), dtype=torch.float64)
+    r = torch.autograd.grad(ar + tar, hs, retain_graph=True)[0] if alpha > 0 or beta > 0 else None
     (loss + ar + tar).backward()
     return (loss.item(), scores.detach().numpy(), out_states, {k: v.grad.numpy() for k, v in tp.items()},
-            (ar.item(), tar.item()))
+            (ar.item(), tar.item()), r)
 
 
 CASES = {   # name -> (T, variational, weight_drop, tied)
@@ -99,11 +118,9 @@ def test_embed_dropout_oracle_matches_torch_autograd(case):
     params, x, y, states, masks, rmasks, wd, em = _setup(T, variational, weight_drop, tied)
     assert not em.all() and em.any()
     assert (~em[x]).any() and em[x].any(), "the window should hold dropped and kept word types"
-    p_rec = P_REC if variational else 0.0
-    sc, st, cache = AO.model_fwd(params, x, states, L, P, masks, rmasks, p_rec, wd, P_WD, em, P_E, tied)
-    grads = AO.model_bwd(params, cache, O.nll_loss_bwd(sc, y), L, wd, P_WD, em, P_E, tied)
-    loss = O.nll_loss(sc, y)
-    t_loss, t_sc, t_st, t_grads, _ = _torch_restatement(params, x, y, states, masks, rmasks, wd, em, tied)
+    loss, sc, st, grads, _ = _oracle(params, x, y, states, masks, rmasks, wd, em, _modes(variational, weight_drop),
+                                     tied)
+    t_loss, t_sc, t_st, t_grads, _, _ = _torch_restatement(params, x, y, states, masks, rmasks, wd, em, tied)
     np.testing.assert_allclose(loss, t_loss, rtol=1e-12)
     np.testing.assert_allclose(sc, t_sc, rtol=1e-11, atol=1e-12)
     for l in range(L):
@@ -123,63 +140,62 @@ def test_activation_reg_oracle_matches_torch_autograd(case):
     scores and states are those without the penalties; R and all gradients match the loop's."""
     T, variational, weight_drop, tied = CASES[case]
     params, x, y, states, masks, rmasks, wd, em = _setup(T, variational, weight_drop, tied)
-    p_rec = P_REC if variational else 0.0
-    sc, st, cache = AO.model_fwd(params, x, states, L, P, masks, rmasks, p_rec, wd, P_WD, em, P_E, tied)
-    ar, tar, r = AO.activation_reg(cache, L, ALPHA, BETA)
-    grads = AO.model_bwd(params, cache, O.nll_loss_bwd(sc, y), L, wd, P_WD, em, P_E, tied, r)
-    t_loss, t_sc, t_st, t_grads, (t_ar, t_tar) = _torch_restatement(params, x, y, states, masks, rmasks, wd, em, tied,
-                                                                    ALPHA, BETA)
-    np.testing.assert_allclose(O.nll_loss(sc, y), t_loss, rtol=1e-12)
+    args = (params, x, y, states, masks, rmasks, wd, em)
+    nll, sc, st, grads, reg = _oracle(*args, _modes(variational, weight_drop, ALPHA, BETA), tied)
+    ar = _oracle(*args, _modes(variational, weight_drop, ALPHA, 0.0), tied)[4]
+    tar = _oracle(*args, _modes(variational, weight_drop, 0.0, BETA), tied)[4]
+    t_loss, t_sc, t_st, t_grads, (t_ar, t_tar), r = _torch_restatement(*args, tied, ALPHA, BETA)
+    np.testing.assert_allclose(nll, t_loss, rtol=1e-12)
     np.testing.assert_allclose(sc, t_sc, rtol=1e-11, atol=1e-12)
     assert ar > 0 and (tar > 0) == (T > 1)
     np.testing.assert_allclose(ar, t_ar, rtol=1e-12)
     np.testing.assert_allclose(tar, t_tar, rtol=1e-12, atol=1e-300)
     for k in grads:
         np.testing.assert_allclose(grads[k], t_grads[k], rtol=1e-9, atol=1e-12, err_msg=k)
-    # the penalties reach units whose output was dropped: r is not 0 everywhere the last site's mask drops
+    # the penalties reach units whose output was dropped (r is not 0 everywhere the last site's mask drops), so the
+    # gradients above tell TAR on the raw h from TAR on the masked output
     if T > 1:
         dropped = ~np.broadcast_to(masks[L], r.shape)
-        assert (r[dropped] != 0).any()
+        assert (r.numpy()[dropped] != 0).any()
     # the full train step carries the values
-    p1 = {k: v.copy() for k, v in params.items()}
-    out = AO.train_step(p1, x, y, states, L, 1.0, 0.25, P, masks, rmasks, p_rec, wd, P_WD, em, P_E, tied, ALPHA, BETA)
-    assert out[0] == O.nll_loss(sc, y) and out[5] == (ar, tar)
+    out = MO.train_step(*_tensors(params, x, y, states), L, tied, 1.0, 0.25,
+                        _modes(variational, weight_drop, ALPHA, BETA), MO.Masks(sites=masks, rec=rmasks, wd=wd, ed=em))
+    assert out[0] == nll and out[5] == reg == ar + tar
 
 
 def test_tied_projection_is_unmasked():
     """Tied: dE = G_proj + s_e * G_emb, with the projection reading the raw E."""
     params, x, y, states, masks, _, _, em = _setup(5, False, False, True)
-    sc, _, cache = AO.model_fwd(params, x, states, L, P, masks, ed_mask=em, p_e=P_E, tied=True)
+    md = _modes(False, False)
+    _, sc, _, g, _ = _oracle(params, x, y, states, masks, None, None, em, md, True)
     untied = dict(params, **{"fc.W": params["embed.W"].copy()})
-    sc2, _, cache2 = AO.model_fwd(untied, x, states, L, P, masks, ed_mask=em, p_e=P_E)
+    _, sc2, _, g2, _ = _oracle(untied, x, y, states, masks, None, None, em, md, False)
     np.testing.assert_array_equal(sc, sc2)
-    g = AO.model_bwd(params, cache, O.nll_loss_bwd(sc, y), L, ed_mask=em, p_e=P_E, tied=True)
-    g2 = AO.model_bwd(untied, cache2, O.nll_loss_bwd(sc2, y), L, ed_mask=em, p_e=P_E)
     np.testing.assert_allclose(g["embed.W"], g2["embed.W"] + g2["fc.W"], rtol=1e-13, atol=1e-15)
 
 
 def test_p0_is_the_weight_drop_oracle():
+    """p_e = 0 draws no mask and is the weight-drop step, bit for bit"""
     params, x, y, states, masks, _, wd, _ = _setup(5, False, True, False)
-    assert AO.embed_mask(SEED, STEP, L, V, 0.0) is None
-    p1 = {k: v.copy() for k, v in params.items()}
-    p2 = {k: v.copy() for k, v in params.items()}
-    got = AO.train_step(p1, x, y, states, L, 1.0, 0.25, P, masks, None, 0.0, wd, P_WD)
-    want = WO.train_step(p2, x, y, states, L, 1.0, 0.25, P, masks, None, 0.0, wd, P_WD)
-    assert got[0] == want[0] and got[1] == want[1] and got[5] == (0.0, 0.0)
-    for k in p1:
-        np.testing.assert_array_equal(p1[k], p2[k])
+    assert _embed_mask(STEP, V, 0.0) is None
+    got = MO.train_step(*_tensors(params, x, y, states), L, False, 1.0, 0.25, _modes(False, True, p_e=0.0))
+    want = MO.train_step(*_tensors(params, x, y, states), L, False, 1.0, 0.25,
+                         MO.Modes(p=P, p_wd=P_WD), MO.Masks(sites=masks, wd=wd))
+    assert got[0] == want[0] and got[1] == want[1] and got[5] == 0.0
+    for k in params:
+        assert torch.equal(got[3][k], want[3][k]), k
 
 
 def test_mask_is_site_3L_plus_1_over_the_vocabulary():
     """The keep flag of word v is element v of zrb_dropout_mask(seed, step, 3L + 1, V, p): the site after the
     weight-drop ones (2L + 1 .. 3L), far from the sampler's counter word 0xFFFFFFFF."""
-    em = AO.embed_mask(SEED, STEP, L, V, P_E)
+    em = _embed_mask(STEP, V, P_E)
     np.testing.assert_array_equal(em, PH.keep_mask(SEED, STEP, 3 * L + 1, V, P_E))
     wd_sites = {2 * L + 1 + l for l in range(L)}
     assert 3 * L + 1 not in wd_sites and 3 * L + 1 > max(wd_sites)
-    big = AO.embed_mask(SEED, STEP, L, 100000, P_E)
+    big = _embed_mask(STEP, 100000, P_E)
     assert abs((1 - big.mean()) - P_E) < 0.01
-    assert not np.array_equal(big, AO.embed_mask(SEED, STEP + 1, L, 100000, P_E))
+    assert not np.array_equal(big, _embed_mask(STEP + 1, 100000, P_E))
     assert 3 * 8 + 1 < 0xFFFFFFFF   # largest site with ZRB_MAX_LAYERS = 8
 
 

@@ -5,7 +5,7 @@ tests/test_gpu_dropout.py (every plan branch, the per-timestep path at B = 40, t
     (loss, scores, states and every other gradient), and dE = fp32(s_e * dE_off) -- on the fused Trainer and on the
     drop-in Model, alone and with the variational mode and weight drop;
   * two carried steps of the fused Trainer (and the drop-in Model) against the fp64 restatement of
-    tests/_awd_reg_oracle.py with masks computed by oracle/philox.py, alone and with everything on (variational,
+    tests/_model_oracle.py with masks computed by oracle/philox.py, alone and with everything on (variational,
     weight drop, tied);
   * AR/TAR: alpha = beta = 0 is the mode off bit for bit; with alpha, beta > 0 the returned loss and the states are
     bit-identical to the mode off, R matches the fp64 oracle, and the penalties' own gradient contribution (gradients
@@ -17,6 +17,7 @@ tests/test_gpu_dropout.py (every plan branch, the per-timestep path at B = 40, t
 Windows hold distinct tokens, so the embedding scatter is deterministic.
 """
 import ctypes as C
+import dataclasses
 import gc
 import math
 import os
@@ -25,9 +26,7 @@ import numpy as np
 import pytest
 import torch
 
-from tests import _awd_reg_oracle as AO
-from tests import _variational_oracle as VO
-from tests import _weight_drop_oracle as WO
+from tests import _model_oracle as MO
 from tests.test_gpu_dropout import L, P_DROP, ROW_IDS, Row
 from tests.test_gpu_parity import ENGINES, TOL, _caller_nll_loss, _scale_close
 
@@ -165,27 +164,33 @@ def test_composes_with_variational_and_weight_drop(mode):
 _oracle_cache = {}
 
 
+def _oracle_steps(row, tied, lr, modes):
+    """two carried fp64 steps from the row's model and states, as numpy: loss, norm, scores, states, raw grads,
+    params after and (AR, TAR) per step; modes(s) gives step s's Modes"""
+    m = _model(row, tied=tied)
+    params = {k: v.detach().cpu().double() for k, v in m.named_parameters()}
+    del m
+    states = [(h.double(), c.double()) for h, c in row.h0]
+    out = []
+    for s in range(2):
+        md = modes(s)
+        with torch.no_grad():
+            sc, _, ar = MO.forward(params, row.x[s], states, L, tied, dataclasses.replace(md, beta=0.0))
+            tar = MO.forward(params, row.x[s], states, L, tied, dataclasses.replace(md, alpha=0.0))[2]
+        loss, norm, grads, params, states, _ = MO.train_step(params, row.x[s], row.y[s], states, L, tied, lr,
+                                                             MAX_NORM, md)
+        out.append(dict(loss=loss, norm=norm, scores=sc.numpy(), states=[(h.numpy(), c.numpy()) for h, c in states],
+                        grads={k: v.numpy() for k, v in grads.items()},
+                        params={k: v.numpy() for k, v in params.items()}, reg=(float(ar), float(tar))))
+    return out
+
+
 def _oracle(row, seed, p_e, variational=False, p_wd=0.0, tied=False, alpha=0.0, beta=0.0):
     key = (row.name, seed, p_e, variational, p_wd, tied, alpha, beta)
     if key not in _oracle_cache:
-        m = _model(row, tied=tied)
-        params = {k: v.detach().cpu().numpy().astype(np.float64) for k, v in m.named_parameters()}
-        del m
-        states = [(h.numpy().astype(np.float64), c.numpy().astype(np.float64)) for h, c in row.h0]
-        p_rec = P_DROP if variational else 0.0
-        out = []
-        for s in range(2):
-            if variational:
-                masks, rmasks = VO.variational_masks(seed, s, L, row.T, row.B, row.H, P_DROP, p_rec)
-            else:
-                masks, rmasks = row.masks(seed, s), None
-            wd = WO.weight_drop_masks(row.torch_seed, s, L, row.H, p_wd)
-            em = AO.embed_mask(row.torch_seed, s, L, row.V, p_e)
-            x, y = row.x[s].numpy(), row.y[s].numpy()
-            loss, norm, states, sc, raw, reg = AO.train_step(params, x, y, states, L, LR, MAX_NORM, P_DROP, masks,
-                                                             rmasks, p_rec, wd, p_wd, em, p_e, tied, alpha, beta)
-            out.append(dict(loss=loss, norm=norm, scores=sc, states=[(h.copy(), c.copy()) for h, c in states],
-                            grads=raw, params={k: v.copy() for k, v in params.items()}, reg=reg))
+        out = _oracle_steps(row, tied, LR, lambda s: MO.Modes(
+            seed=seed, step=s, p=P_DROP, variational=variational, p_rec=P_DROP if variational else 0.0,
+            wd_seed=row.torch_seed, p_wd=p_wd, ed_seed=row.torch_seed, p_e=p_e, alpha=alpha, beta=beta))
         _oracle_cache.clear()
         _oracle_cache[key] = out
     return _oracle_cache[key]
@@ -377,16 +382,7 @@ def _oracle_lr0(row, seed, alpha, beta):
     """Two steps of the fp64 restatement at lr = 0 (the weights stay put; the states carry)."""
     key = (row.name, seed, alpha, beta)
     if key not in _oracle_lr0_cache:
-        m = _model(row)
-        params = {k: v.detach().cpu().numpy().astype(np.float64) for k, v in m.named_parameters()}
-        del m
-        states = [(h.numpy().astype(np.float64), c.numpy().astype(np.float64)) for h, c in row.h0]
-        out = []
-        for s in range(2):
-            loss, norm, states, sc, raw, reg = AO.train_step(params, row.x[s].numpy(), row.y[s].numpy(), states, L, 0.0,
-                                                             MAX_NORM, P_DROP, row.masks(seed, s), alpha=alpha,
-                                                             beta=beta)
-            out.append(dict(grads=raw, reg=reg))
+        out = _oracle_steps(row, False, 0.0, lambda s: MO.Modes(seed=seed, step=s, p=P_DROP, alpha=alpha, beta=beta))
         if len(_oracle_lr0_cache) > 2:
             _oracle_lr0_cache.clear()
         _oracle_lr0_cache[key] = out

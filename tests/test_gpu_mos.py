@@ -1,5 +1,5 @@
 """Mixture of Softmaxes (DESIGN.md section 19) through the tensor-core engine, against the fp64 restatement in
-tests/_mos_oracle.py.
+tests/_model_oracle.py.
 
 Shapes: MoS's PTB model (E = 280, 960-960-620, K = 15, T = 70, B = 12, tied), the recurrence-plan branches of
 test_gpu_widths.py with K = 3, the per-timestep path (B = 40), a vocabulary that is not a multiple of 4 (the scalar
@@ -12,7 +12,7 @@ import pytest
 import torch
 
 from oracle import philox as PH
-from tests import _mos_oracle as O
+from tests import _model_oracle as O
 from tests.test_gpu_parity import TOL
 
 pytestmark = pytest.mark.gpu
@@ -179,7 +179,7 @@ def test_dropin_forward_backward_matches_oracle(name):
         want_logp, want_states, _ = O.forward(ps, xs[0], z, L, tied)
         if upstream == "nll":
             (torch.nn.functional.cross_entropy(logp, ys[0].reshape(-1)) * B).backward()
-            O.loss_of(want_logp, ys[0]).backward()
+            O.loss_of(want_logp, ys[0], logp=True).backward()
         else:
             G = torch.randn(T * B, V, generator=torch.Generator().manual_seed(3)).cuda()
             (logp * G).sum().backward()
@@ -256,13 +256,13 @@ def test_modes_match_oracle(case):
     for s in range(2):
         md = O.Modes(seed=tr.seed, step=tr.step, p=mkw["dropout"], variational=mkw.get("variational", False),
                      p_rec=p_rec, wd_seed=key, p_wd=mkw["weight_drop"], ed_seed=key, p_e=mkw["embed_dropout"],
-                     alpha=tkw["ar"], beta=tkw["tar"])
+                     alpha=tkw["ar"], beta=tkw["tar"], p_l=mkw["mos_dropout"])
         if s == 1:
             tr.start_averaging()
         loss, norm = tr.train_step(xs[s], ys[s], LR, MAX_NORM)
         torch.cuda.synchronize()
         want_loss, want_norm, grads, params, states, _ = O.train_step(params, xs[s], ys[s], states, L, tied, LR,
-                                                                     MAX_NORM, md, mkw["mos_dropout"])
+                                                                     MAX_NORM, md)
         print(f"ERR {case} s{s} loss: {abs(loss.item() - want_loss) / abs(want_loss):.2e} "
               f"norm: {abs(norm.item() - want_norm) / want_norm:.2e}")
         assert abs(loss.item() - want_loss) <= tol["loss"] * abs(want_loss), (case, s, loss.item(), want_loss)

@@ -1,5 +1,5 @@
 """Tied embedding and softmax weights on the GPU (DESIGN.md section 13): Model(tied=True) and the fused Trainer against
-the float64 restatement tests/_tied_oracle.py, the fused clip norm and update, bit-reproducibility, lazy = strict, tied
+the float64 restatement tests/_model_oracle.py, the fused clip norm and update, bit-reproducibility, lazy = strict, tied
 against untied with equal weights, the variational mode, rejected arguments and the data-parallel step.
 
 Tolerances are test_gpu_parity's (TOL per engine, NORM_TOL for the fused norm)."""
@@ -10,10 +10,8 @@ import numpy as np
 import pytest
 import torch
 
-from oracle import lstm_lm_oracle as O
 from oracle import philox as PH
-from tests import _tied_oracle as TO
-from tests import _variational_oracle as VO
+from tests import _model_oracle as MO
 from tests._golden import StepCase
 from tests.test_gpu_parity import ENGINES, NORM_TOL, TOL, _caller_nll_loss, _record, _scale_close
 
@@ -66,21 +64,28 @@ def _masks(name, s, seed=SEED):
 
 @functools.lru_cache(maxsize=None)
 def _oracle(name):
-    """Two carried tied steps in float64: per step (loss, norm, raw grads, params after, states after)."""
+    """Two carried tied steps in float64: per step (loss, norm, raw grads, params after, states after), as numpy."""
     V, H, L, T, B, p, params, xs, ys, states, _, _ = _case(name)
-    P = {k: v.astype(np.float64) for k, v in params.items()}
-    st = [(h.astype(np.float64), c.astype(np.float64)) for h, c in states]
+    P = {k: _t64(v) for k, v in params.items()}
+    st = [(_t64(h), _t64(c)) for h, c in states]
     out = []
     for s in range(2):
-        masks = _masks(name, s)
-        sc, new_st, cache = TO.model_fwd(P, xs[s], st, L, p, masks)
-        loss = O.nll_loss(sc, ys[s])
-        grads = TO.model_bwd(P, cache, O.nll_loss_bwd(sc, ys[s]), L)
-        raw = {k: v.copy() for k, v in grads.items()}
-        norm = O.clip_sgd(P, grads, LR, MAX_NORM, TO.param_names(L))
-        out.append((loss, norm, raw, {k: v.copy() for k, v in P.items()}, new_st))
-        st = new_st
+        loss, norm, raw, P, st, _ = MO.train_step(P, _tok(xs[s]), _tok(ys[s]), st, L, True, LR, MAX_NORM,
+                                                  MO.Modes(p=p), MO.Masks(sites=_masks(name, s)))
+        out.append((loss, norm, _np(raw), _np(P), [(h.numpy(), c.numpy()) for h, c in st]))
     return out
+
+
+def _t64(a):
+    return torch.tensor(a, dtype=torch.float64)
+
+
+def _tok(a):
+    return torch.as_tensor(a, dtype=torch.int64)
+
+
+def _np(d):
+    return {k: v.numpy() for k, v in d.items()}
 
 
 def _tied_model(name, engine, **kw):
@@ -285,16 +290,16 @@ def test_tied_variational_against_oracle():
     m = zaremba_b200.Model(V, H, L, p, 0.08, variational=True, recurrent_dropout=p_rec, tied=True).to(DEV)
     m.train()
     m._seed, m._drop_step = SEED, 0
-    P = {k: q.detach().cpu().double().numpy().copy() for k, q in m.named_parameters()}
+    P = {k: q.detach().cpu().double() for k, q in m.named_parameters()}
     rng = np.random.default_rng(4)
-    st = [(rng.uniform(-0.3, 0.3, (B, H)), rng.uniform(-0.5, 0.5, (B, H))) for _ in range(L)]
-    sts = [(torch.tensor(h, dtype=torch.float32).view(1, B, H).to(DEV),
-            torch.tensor(c, dtype=torch.float32).view(1, B, H).to(DEV)) for h, c in st]
+    st = [(_t64(rng.uniform(-0.3, 0.3, (B, H))), _t64(rng.uniform(-0.5, 0.5, (B, H)))) for _ in range(L)]
+    sts = [(h.float().view(1, B, H).to(DEV), c.float().view(1, B, H).to(DEV)) for h, c in st]
     tol = TOL["tc"]
     for s in range(2):
         x, y = rng.integers(0, V, size=(T, B)), rng.integers(0, V, size=(T, B))
-        masks, rmasks = VO.variational_masks(SEED, s, L, T, B, H, p, p_rec)
-        loss_w, norm_w, st, _, grads_w = TO.train_step(P, x, y, st, L, LR, MAX_NORM, p, masks, rmasks, p_rec)
+        md = MO.Modes(seed=SEED, step=s, p=p, variational=True, p_rec=p_rec)
+        loss_w, norm_w, raw_w, P, st, _ = MO.train_step(P, _tok(x), _tok(y), st, L, True, LR, MAX_NORM, md)
+        coef = min(1.0, MAX_NORM / (norm_w + 1e-6))
         m.zero_grad()
         sts = m.detach(sts)
         scores, sts = m(torch.tensor(x), sts)
@@ -307,8 +312,8 @@ def test_tied_variational_against_oracle():
                 q -= LR * q.grad
         assert abs(float(norm) - norm_w) <= tol["grad"] * max(1.0, norm_w)
         for k, q in m.named_parameters():
-            _scale_close(q.grad.cpu().numpy(), grads_w[k], tol["grad"], f"s{s} clipped grad {k}")
-            _scale_close(q.detach().cpu().numpy(), P[k], tol["grad"], f"s{s} param {k}")
+            _scale_close(q.grad.cpu().numpy(), raw_w[k].numpy() * coef, tol["grad"], f"s{s} clipped grad {k}")
+            _scale_close(q.detach().cpu().numpy(), P[k].numpy(), tol["grad"], f"s{s} param {k}")
 
 
 def test_tied_rejected_arguments_leave_the_context_usable():

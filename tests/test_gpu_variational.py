@@ -3,7 +3,7 @@ applies a mask: the rows of tests/test_gpu_dropout.py (every plan branch, the pe
 embedding paths, the validation engine).
 
   * two carried train steps through the fused Trainer and the drop-in Model against the fp64 restatement of
-    tests/_variational_oracle.py, with masks computed by oracle/philox.py, never by the library;
+    tests/_model_oracle.py, with masks computed by oracle/philox.py, never by the library;
   * with p_rec = 0 the mode is bit for bit Zaremba's path fed the step-0 masks tiled over the window (the
     fixed-over-window indexing of every kernel and branch, the rows-out embedding gradient included);
   * a lazy-update Trainer equals a strict one bit for bit; inference is untouched by the mode;
@@ -19,7 +19,7 @@ import pytest
 import torch
 
 from oracle import lstm_lm_oracle as O
-from tests import _variational_oracle as VO
+from tests import _model_oracle as MO
 from tests.test_gpu_dropout import L, P_DROP, ROW_IDS, Row
 from tests.test_gpu_parity import ENGINES, TOL, _caller_nll_loss, _scale_close
 
@@ -52,24 +52,29 @@ def _model(row, variational=True, p_rec=None):
 _oracle_cache = {}
 
 
+def _tiled_masks(seed, step, T, B, H):
+    """the variational mode's site masks: the step-0 mask of every site tiled over the window"""
+    return MO.mode_masks(MO.Modes(seed=seed, step=step, p=P_DROP, variational=True), [H] * (L + 1), T, B, 0).sites
+
+
 def _oracle(row, seed, p_rec):
-    """fp64 oracle of two carried steps: per step loss, norm, states, unclipped grads, updated params."""
+    """fp64 oracle of two carried steps: per step loss, norm, states, unclipped grads, updated params (numpy)."""
     key = (row.name, seed, p_rec)
     if key not in _oracle_cache:
         m = _model(row, False)
-        params = {k: v.detach().cpu().numpy().astype(np.float64) for k, v in m.named_parameters()}
+        params = {k: v.detach().cpu().double() for k, v in m.named_parameters()}
         del m
-        states = [(h.numpy().astype(np.float64), c.numpy().astype(np.float64)) for h, c in row.h0]
+        states = [(h.double(), c.double()) for h, c in row.h0]
         out = []
         for s in range(2):
-            masks, rmasks = VO.variational_masks(seed, s, L, row.T, row.B, row.H, P_DROP, p_rec)
-            x, y = row.x[s].numpy(), row.y[s].numpy()
-            sc, states, cache = VO.model_fwd(params, x, states, L, P_DROP, masks, rmasks, p_rec)
-            grads = VO.model_bwd(params, cache, O.nll_loss_bwd(sc, y), L)
-            raw = {k: v.copy() for k, v in grads.items()}
-            norm = O.clip_sgd(params, grads, LR, MAX_NORM, O.param_names(L))
-            out.append(dict(loss=O.nll_loss(sc, y), norm=norm, scores=sc, states=[(h.copy(), c.copy()) for h, c in states],
-                            grads=raw, params={k: v.copy() for k, v in params.items()}))
+            md = MO.Modes(seed=seed, step=s, p=P_DROP, variational=True, p_rec=p_rec)
+            with torch.no_grad():
+                sc = MO.forward(params, row.x[s], states, L, False, md)[0]
+            loss, norm, grads, params, states, _ = MO.train_step(params, row.x[s], row.y[s], states, L, False, LR,
+                                                                 MAX_NORM, md)
+            out.append(dict(loss=loss, norm=norm, scores=sc.numpy(), states=[(h.numpy(), c.numpy()) for h, c in states],
+                            grads={k: v.numpy() for k, v in grads.items()},
+                            params={k: v.numpy() for k, v in params.items()}))
         _oracle_cache.clear()
         _oracle_cache[key] = out
     return _oracle_cache[key]
@@ -90,7 +95,7 @@ def _trainer_run(row, variational=True, p_rec=None, explicit=False, lazy=False):
     out = []
     for s in range(2):
         if explicit:
-            masks, _ = VO.variational_masks(tr.seed, s, L, row.T, row.B, row.H, P_DROP, 0.0)
+            masks = _tiled_masks(tr.seed, s, row.T, row.B, row.H)
             m.set_explicit_dropout_masks([torch.tensor(mk).to(_dev()) for mk in masks])
         loss, norm = tr.train_step(row.x[s].to(_dev()), row.y[s].to(_dev()), LR, MAX_NORM)
         tr.flush()
@@ -113,7 +118,7 @@ def _dropin_run(row, variational=True, p_rec=None, explicit=False):
     out = []
     for s in range(2):
         if explicit:
-            masks, _ = VO.variational_masks(seed, s, L, row.T, row.B, row.H, P_DROP, 0.0)
+            masks = _tiled_masks(seed, s, row.T, row.B, row.H)
             m.set_explicit_dropout_masks([torch.tensor(mk).to(_dev()) for mk in masks])
         m.zero_grad(set_to_none=True)
         scores, states = m(row.x[s], states)
@@ -216,7 +221,7 @@ def test_embed_rows_out_fixed_over_window(H, engine):
         m.train()
         tr = zaremba_b200.Trainer(m, B, T)
         if not variational:
-            masks, _ = VO.variational_masks(tr.seed, tr.step, L, T, B, H, P_DROP, 0.0)
+            masks = _tiled_masks(tr.seed, tr.step, T, B, H)
             m.set_explicit_dropout_masks([torch.tensor(mk).to(_dev()) for mk in masks])
         rows = torch.full((T * B, H), float("nan"), device=_dev())
         _lib.check(lib.zrb_set_embed_rows_out(tr.ctx, _lib.ptr(rows)))
@@ -228,7 +233,7 @@ def test_embed_rows_out_fixed_over_window(H, engine):
         finally:
             _lib.check(lib.zrb_set_embed_rows_out(tr.ctx, None))
         out.append(rows.clone())
-        keep = VO.variational_masks(tr.seed, tr.step, L, T, B, H, P_DROP, 0.0)[0][0].reshape(T * B, H)
+        keep = _tiled_masks(tr.seed, tr.step, T, B, H)[0].reshape(T * B, H)
         tr.close()
         del tr, m
         gc.collect()

@@ -5,7 +5,7 @@ tests/test_gpu_dropout.py (every plan branch, the per-timestep path at B = 40, t
     fp32(W_hh * m * scale) (loss, scores, states and every other gradient), and dW_hh = fp32(scale * m * dW_eff) -- this
     pins the masked fp16 images and the gradient mask with no tolerance; the fused clip norm against the fp64 norm;
   * two carried steps of the fused Trainer and the drop-in Model against the fp64 restatement of
-    tests/_weight_drop_oracle.py with masks computed by oracle/philox.py;
+    tests/_model_oracle.py with masks computed by oracle/philox.py;
   * lazy equals strict; eval untouched; p = 0 is the mode off; rejected arguments and call orders; two GPUs.
 Windows hold distinct tokens, so the embedding scatter is deterministic.
 """
@@ -19,8 +19,7 @@ import pytest
 import torch
 
 from oracle import lstm_lm_oracle as O
-from tests import _variational_oracle as VO
-from tests import _weight_drop_oracle as WO
+from tests import _model_oracle as MO
 from tests.test_gpu_dropout import L, P_DROP, ROW_IDS, Row
 from tests.test_gpu_parity import ENGINES, NORM_TOL, TOL, _caller_nll_loss, _scale_close
 
@@ -175,22 +174,20 @@ def _oracle(row, seed, p_wd, variational):
     key = (row.name, seed, p_wd, variational)
     if key not in _oracle_cache:
         m = _model(row)
-        params = {k: v.detach().cpu().numpy().astype(np.float64) for k, v in m.named_parameters()}
+        params = {k: v.detach().cpu().double() for k, v in m.named_parameters()}
         del m
-        states = [(h.numpy().astype(np.float64), c.numpy().astype(np.float64)) for h, c in row.h0]
-        p_rec = P_DROP if variational else 0.0
+        states = [(h.double(), c.double()) for h, c in row.h0]
         out = []
         for s in range(2):
-            if variational:
-                masks, rmasks = VO.variational_masks(seed, s, L, row.T, row.B, row.H, P_DROP, p_rec)
-            else:
-                masks, rmasks = row.masks(seed, s), None
-            wd = WO.weight_drop_masks(row.torch_seed, s, L, row.H, p_wd)
-            x, y = row.x[s].numpy(), row.y[s].numpy()
-            loss, norm, states, sc, raw = WO.train_step(params, x, y, states, L, LR, MAX_NORM, P_DROP, masks, rmasks,
-                                                        p_rec, wd, p_wd)
-            out.append(dict(loss=loss, norm=norm, scores=sc, states=[(h.copy(), c.copy()) for h, c in states],
-                            grads=raw, params={k: v.copy() for k, v in params.items()}))
+            md = MO.Modes(seed=seed, step=s, p=P_DROP, variational=variational,
+                          p_rec=P_DROP if variational else 0.0, wd_seed=row.torch_seed, p_wd=p_wd)
+            with torch.no_grad():
+                sc = MO.forward(params, row.x[s], states, L, False, md)[0]
+            loss, norm, grads, params, states, _ = MO.train_step(params, row.x[s], row.y[s], states, L, False, LR,
+                                                                 MAX_NORM, md)
+            out.append(dict(loss=loss, norm=norm, scores=sc.numpy(), states=[(h.numpy(), c.numpy()) for h, c in states],
+                            grads={k: v.numpy() for k, v in grads.items()},
+                            params={k: v.numpy() for k, v in params.items()}))
         _oracle_cache.clear()
         _oracle_cache[key] = out
     return _oracle_cache[key]

@@ -1,5 +1,5 @@
 """Layers of unequal width (DESIGN.md section 18) through the tensor-core engine, against the fp64 restatement in
-tests/_widths_oracle.py, and the equal-width path through zrb_ctx_create_widths against zrb_ctx_create, bit for bit.
+tests/_model_oracle.py, and the equal-width path through zrb_ctx_create_widths against zrb_ctx_create, bit for bit.
 
 Shapes: AWD-LSTM's PTB model (E = 400, 1150-1150-400, tied), a growing stack (E = 200, 650-1500), the recurrence-plan
 branches (H < 256 unsplit, K-split, pitches that are not multiples of 64), the per-timestep path (B = 40) and one layer
@@ -10,7 +10,7 @@ import numpy as np
 import pytest
 import torch
 
-from tests import _widths_oracle as O
+from tests import _model_oracle as O
 from tests.test_gpu_parity import NORM_TOL, TOL
 
 pytestmark = pytest.mark.gpu
@@ -316,7 +316,7 @@ def test_explicit_masks_take_each_sites_width():
         m.train()
         tr = zaremba_b200.Trainer(m, B, T)
         if explicit:
-            masks = O.site_masks(tr.seed, tr.step, [E, *sizes], T, B, 0.3)
+            masks = O.mode_masks(O.Modes(seed=tr.seed, step=tr.step, p=0.3), [E, *sizes], T, B, V).sites
             m.set_explicit_dropout_masks([torch.as_tensor(mk).cuda() for mk in masks])
         xs, ys = _data("branches", 1)
         loss, norm = tr.train_step(xs[0], ys[0], LR, MAX_NORM)

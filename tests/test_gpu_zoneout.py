@@ -1,4 +1,4 @@
-"""Zoneout (DESIGN.md section 20) on the GPU against the fp64 restatement of tests/_zoneout_oracle.py, with the flags
+"""Zoneout (DESIGN.md section 20) on the GPU against the fp64 restatement of tests/_model_oracle.py, with the flags
 fetched through zrb_dropout_mask.
 
   * two carried fused steps, alone and under Zaremba dropout: loss, clip norm, the raw gradient of every tensor (each
@@ -24,7 +24,7 @@ import torch
 
 from oracle import lstm_lm_oracle as O
 from oracle import philox
-from tests import _zoneout_oracle as ZO
+from tests import _model_oracle as MO
 
 pytestmark = pytest.mark.gpu
 
@@ -83,6 +83,33 @@ def _np(t):
     return t.detach().cpu().double().numpy()
 
 
+def _t64(states):
+    return [(torch.tensor(h), torch.tensor(c)) for h, c in states]
+
+
+def _oracle_step(params, x, y, states, md, masks):
+    """one fp64 train step of the oracle on numpy params (updated in place) and states: loss, norm, states after, raw
+    gradients"""
+    loss, norm, grads, after, st, _ = MO.train_step({k: torch.tensor(v) for k, v in params.items()}, x, y, _t64(states),
+                                                    L, False, LR, MAX_NORM, md, masks)
+    params.update({k: v.numpy() for k, v in after.items()})
+    return loss, norm, [(h.numpy(), c.numpy()) for h, c in st], {k: v.numpy() for k, v in grads.items()}
+
+
+def _eval_oracle(params, x, y, states, z, G):
+    """the oracle in eval mode at rates z, as numpy: scores, states, the gradients of sum(G * scores) and of the
+    loss, and the loss"""
+    grads = []
+    for upstream in (G, None):
+        ps = {k: torch.tensor(v, requires_grad=True) for k, v in params.items()}
+        scores, st, _ = MO.forward(ps, x, _t64(states), L, False, MO.Modes(z_c=z[0], z_h=z[1]), train=False)
+        loss = MO.loss_of(scores, y)
+        (loss if upstream is None else (scores * torch.tensor(upstream)).sum()).backward()
+        grads.append({k: v.grad.numpy() for k, v in ps.items()})
+    return (scores.detach().numpy(), [(h.detach().numpy(), c.detach().numpy()) for h, c in st], grads[0], grads[1],
+            loss.item())
+
+
 def fused_errors(shape, p, steps=2):
     """the fused Trainer's errors against the oracle with the right flags, without zoneout, and with the next step's
     flags: {check: [err_right, err_no_zoneout, err_wrong_flags]} (the largest over the steps)"""
@@ -111,8 +138,9 @@ def fused_errors(shape, p, steps=2):
         got_p = {k: _np(v) for k, v in m.named_parameters()}
         rows = []
         for r, zf in enumerate((right, none, wrong)):
-            want_loss, want_norm, states[r], raw = ZO.train_step(refs[r], x.numpy(), y.numpy(), states[r], L, LR,
-                                                                 MAX_NORM, z_c, z_h, zf, p, masks)
+            mk = MO.Masks(sites=masks, zc=[f[0] for f in zf], zh=[f[1] for f in zf])
+            want_loss, want_norm, states[r], raw = _oracle_step(refs[r], x, y, states[r],
+                                                                MO.Modes(p=p, z_c=z_c, z_h=z_h), mk)
             rows.append((want_loss, want_norm, raw))
         note("loss", [abs(loss.item() - w[0]) / w[0] for w in rows])
         note("norm", [abs(norm.item() - w[1]) / w[1] for w in rows])
@@ -159,30 +187,29 @@ def eval_errors(shape):
     x, y = _tokens(V, T, B, 9)
     zeros = O.zero_states(L, B, H, np.float64)
     errs = {}
-    refs = [ZO.model_fwd(params, x.numpy(), zeros, L, zc, zh) for zc, zh in ((z_c, z_h), (0.0, 0.0))]
     # the drop-in forward and backward (a fixed upstream gradient)
     m.eval()
     st = m.state_init(B)
     scores, st = m(x.to(_dev()), st)
     G = torch.randn(scores.shape, generator=torch.Generator().manual_seed(3)).to(_dev())
     scores.backward(G)
+    refs = [_eval_oracle(params, x, y, zeros, z, _np(G)) for z in ((z_c, z_h), (0.0, 0.0))]
     errs["dropin scores"] = [_rel(_np(scores), r[0]) for r in refs]
     errs["dropin state c"] = [max(_rel(_np(st[l][1]), r[1][l][1]) for l in range(L)) for r in refs]
     errs["dropin state h"] = [max(_rel(_np(st[l][0]), r[1][l][0]) for l in range(L)) for r in refs]
     for k, v in m.named_parameters():
-        errs["dropin grad " + k] = [_rel(_np(v.grad), ZO.model_bwd(r[2], _np(G), L)[k]) for r in refs]
+        errs["dropin grad " + k] = [_rel(_np(v.grad), r[2][k]) for r in refs]
     # eval_step, perplexity and the raw gradient of a dynamic-evaluation step (lr = 0: the weights stay put)
     m.zero_grad(set_to_none=True)
     tr = zaremba_b200.Trainer(m, B, T)
-    want = [ZO.eval_loss(params, x.numpy(), y.numpy(), zeros, L, zc, zh)[0] for zc, zh in ((z_c, z_h), (0.0, 0.0))]
+    want = [r[4] for r in refs]
     errs["eval_step"] = [abs(tr.eval_step(x.to(_dev()), y.to(_dev())).item() - w) / w for w in want]
     ppl = tr.perplexity([(x, y)])
     errs["perplexity"] = [abs(ppl - math.exp(w / B)) / math.exp(w / B) for w in want]
     tr.reset_states()
     tr.dynamic_eval_step(x.to(_dev()), y.to(_dev()), tr.flat_p.clone(), 0.0)
     for k, v in m.named_parameters():
-        wants = [ZO.model_bwd(r[2], O.nll_loss_bwd(r[0], y.numpy()), L)[k] for r in refs]
-        errs["dyneval grad " + k] = [_rel(_np(v.grad), w) for w in wants]
+        errs["dyneval grad " + k] = [_rel(_np(v.grad), r[3][k]) for r in refs]
     return errs
 
 

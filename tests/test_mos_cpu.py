@@ -1,4 +1,4 @@
-"""Mixture of Softmaxes without a GPU: the fp64 restatement (tests/_mos_oracle.py) against torch autograd of a literal
+"""Mixture of Softmaxes without a GPU: the fp64 restatement (tests/_model_oracle.py) against torch autograd of a literal
 transcription of Yang et al.'s head on a stack of nn.LSTM, the drop-in backward's formulas against autograd, Model's
 parameters, initialisation, checkpoints and argument checks, and the C declarations of the new entry points."""
 import ctypes as C
@@ -11,7 +11,7 @@ from torch import nn
 
 import zaremba_b200
 from zaremba_b200 import _lib
-from tests import _mos_oracle as O
+from tests import _model_oracle as O
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 MOS_PTB = dict(tied=True, embed_size=280, layer_sizes=(960, 960, 620), experts=15)

@@ -1,4 +1,4 @@
-"""The tied embedding mode without a GPU: its float64 restatement (tests/_tied_oracle.py) against torch autograd over a
+"""The tied embedding mode without a GPU: the float64 restatement (tests/_model_oracle.py) against torch autograd over a
 genuinely shared nn.Parameter, the host side of Model(tied=True), and the flag in the header and the ctypes binding."""
 import ctypes as C
 import os
@@ -11,7 +11,7 @@ from torch import nn
 
 from oracle import lstm_lm_oracle as O
 from oracle import philox as PH
-from tests import _tied_oracle as TO
+from tests import _model_oracle as MO
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 V, H, L, T, B = 23, 8, 2, 5, 3
@@ -28,6 +28,18 @@ def _setup(seed=7):
     states = [(rng.uniform(-0.5, 0.5, (B, H)), rng.uniform(-1, 1, (B, H))) for _ in range(L)]   # non-zero entering
     masks = [PH.keep_mask(99, 1, s, T * B * H, P).reshape(T, B, H) for s in range(L + 1)]
     return params, x, y, states, masks
+
+
+def _oracle(params, x, y, states, masks, lr=0.0, max_norm=float("inf")):
+    """_model_oracle's tied step as numpy: (NLL, norm, raw grads, params after, states after, scores)"""
+    ps = {k: torch.tensor(v) for k, v in params.items()}
+    x, y = torch.tensor(x), torch.tensor(y)
+    states = [(torch.tensor(h), torch.tensor(c)) for h, c in states]
+    md, mk = MO.Modes(p=P), MO.Masks(sites=masks)
+    loss, norm, grads, after, st, _ = MO.train_step(ps, x, y, states, L, True, lr, max_norm, md, mk)
+    sc = MO.forward(ps, x, states, L, True, md, mk)[0]
+    return (loss, norm, {k: v.numpy() for k, v in grads.items()}, {k: v.numpy() for k, v in after.items()},
+            [(h.numpy(), c.numpy()) for h, c in st], sc.numpy())
 
 
 class _TorchTied(nn.Module):
@@ -64,7 +76,7 @@ class _TorchTied(nn.Module):
         return loss, scores, out
 
     def named(self):
-        names = TO.param_names(L)
+        names = MO.names(L, True)
         return dict(zip(names, [self.E, *self.lstm, self.b]))
 
 
@@ -76,22 +88,20 @@ def test_tied_oracle_matches_torch_autograd_with_a_shared_parameter():
     t_loss.backward()
     t_grads = {k: p.grad.numpy().copy() for k, p in tm.named().items()}
 
-    p_or = {k: v.copy() for k, v in params.items()}
-    loss, norm, st, sc, grads = TO.train_step(p_or, x, y, states, L, lr, max_norm, P, masks)
+    loss, norm, grads, p_or, st, sc = _oracle(params, x, y, states, masks, lr, max_norm)
     np.testing.assert_allclose(loss, t_loss.item(), rtol=1e-12)
     np.testing.assert_allclose(sc, t_sc.detach().numpy(), rtol=1e-11, atol=1e-12)
     for l in range(L):
         np.testing.assert_allclose(st[l][0], t_st[l][0], rtol=1e-11, atol=1e-12)
         np.testing.assert_allclose(st[l][1], t_st[l][1], rtol=1e-11, atol=1e-12)
-    assert sorted(t_grads) == sorted(TO.param_names(L)) and len(t_grads) == 2 + 4 * L
+    assert sorted(t_grads) == sorted(MO.names(L, True)) and len(t_grads) == 2 + 4 * L
 
-    # grads were clipped in place by O.clip_sgd: undo the coefficient to compare the raw ones
     t_norm = torch.nn.utils.clip_grad_norm_(tm.parameters(), max_norm).item()
     np.testing.assert_allclose(norm, t_norm, rtol=1e-12)
     coef = min(1.0, max_norm / (norm + 1e-6))
     assert coef < 1.0, "the clip must be active"
-    for k in TO.param_names(L):
-        np.testing.assert_allclose(grads[k] / coef, t_grads[k], rtol=1e-10, atol=1e-13, err_msg=k)
+    for k in MO.names(L, True):
+        np.testing.assert_allclose(grads[k], t_grads[k], rtol=1e-10, atol=1e-13, err_msg=k)
     with torch.no_grad():
         for p in tm.parameters():
             p -= lr * p.grad
@@ -100,14 +110,14 @@ def test_tied_oracle_matches_torch_autograd_with_a_shared_parameter():
 
 
 def test_tied_gradient_is_the_sum_of_the_untied_pair():
+    """against the numpy oracle's untied pair, to 1e-12 relative (two separate implementations)"""
     params, x, y, states, masks = _setup(3)
     untied = dict(params, **{"fc.W": params["embed.W"].copy()})
     sc, _, cache = O.model_fwd(untied, x, states, L, P, masks)
     g_u = O.model_bwd(untied, cache, O.nll_loss_bwd(sc, y), L)
-    sc_t, _, cache_t = TO.model_fwd(params, x, states, L, P, masks)
-    np.testing.assert_array_equal(sc, sc_t)
-    g_t = TO.model_bwd(params, cache_t, O.nll_loss_bwd(sc_t, y), L)
-    np.testing.assert_array_equal(g_t["embed.W"], g_u["embed.W"] + g_u["fc.W"])
+    _, _, g_t, _, _, sc_t = _oracle(params, x, y, states, masks)
+    np.testing.assert_allclose(sc_t, sc, rtol=1e-12)
+    np.testing.assert_allclose(g_t["embed.W"], g_u["embed.W"] + g_u["fc.W"], rtol=1e-12)
     assert "fc.W" not in g_t
 
 
@@ -121,7 +131,7 @@ def test_model_tied_on_the_host():
     m = zaremba_b200.Model(V, H, L, 0.5, 0.1, tied=True)
     assert m.fc.W is m.embed.W
     assert len(list(m.parameters())) == 2 + 4 * L
-    assert _names(m) == TO.param_names(L)
+    assert _names(m) == MO.names(L, True)
     assert [id(p) for p in m.ordered_parameters()] == [id(p) for p in m.parameters()]
     assert sum(p.numel() for p in m.parameters()) == V * H + 4 * L * (2 * H * H + 2 * H) + V
     sd = m.state_dict()
@@ -161,7 +171,7 @@ def test_tied_init_is_seed_for_seed_the_untied_one():
     torch.manual_seed(11)
     t = zaremba_b200.Model(V, H, L, 0.5, 0.1, tied=True)
     su, st = u.state_dict(), t.state_dict()
-    for k in TO.param_names(L)[:-1]:
+    for k in MO.names(L, True)[:-1]:
         assert torch.equal(su[k], st[k]), k
     # replay Model's draws: the LSTM constructors (as nn.LSTM's), then reset_parameters up to where fc.W would be drawn
     torch.manual_seed(11)

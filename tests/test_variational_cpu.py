@@ -1,6 +1,6 @@
-"""The variational dropout mode without a GPU: its numpy restatement (tests/_variational_oracle.py) against an
-independent float64 torch-autograd restatement, its reduction to the oracle when there is no recurrent mask, and the
-new C entry point in the header and the ctypes binding."""
+"""The variational dropout mode without a GPU: the fp64 restatement (tests/_model_oracle.py) against an independent
+float64 torch-autograd restatement, its agreement with the oracle when there is no recurrent mask, and the new C entry
+point in the header and the ctypes binding."""
 import os
 import re
 
@@ -9,7 +9,7 @@ import torch
 
 from oracle import lstm_lm_oracle as O
 from oracle import philox as PH
-from tests import _variational_oracle as VO
+from tests import _model_oracle as MO
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 V, H, L, T, B = 23, 8, 2, 5, 3
@@ -22,8 +22,23 @@ def _setup(seed=7):
     x = rng.integers(0, V, size=(T, B))
     y = rng.integers(0, V, size=(T, B))
     states = [(rng.uniform(-0.5, 0.5, (B, H)), rng.uniform(-1, 1, (B, H))) for _ in range(L)]   # non-zero entering
-    masks, rmasks = VO.variational_masks(12345, 3, L, T, B, H, P, P_REC)
-    return params, x, y, states, masks, rmasks
+    mk = _masks(P_REC)
+    return params, x, y, states, mk.sites, mk.rec
+
+
+def _masks(p_rec):
+    return MO.mode_masks(MO.Modes(seed=12345, step=3, p=P, variational=True, p_rec=p_rec), [H] * (L + 1), T, B, V)
+
+
+def _oracle(params, x, y, states, masks, rmasks, p_rec):
+    """_model_oracle's loss, scores, states and raw gradients (autograd) as numpy"""
+    ps = {k: torch.tensor(v, requires_grad=True) for k, v in params.items()}
+    sc, st, _ = MO.forward(ps, torch.tensor(x), [(torch.tensor(h), torch.tensor(c)) for h, c in states], L, False,
+                           MO.Modes(p=P, variational=True, p_rec=p_rec), MO.Masks(sites=masks, rec=rmasks))
+    loss = MO.loss_of(sc, torch.tensor(y))
+    loss.backward()
+    return (loss.item(), sc.detach().numpy(), [(h.detach().numpy(), c.detach().numpy()) for h, c in st],
+            {k: v.grad.numpy() for k, v in ps.items()})
 
 
 def _torch_restatement(params, x, y, states, masks, rmasks):
@@ -58,9 +73,7 @@ def _torch_restatement(params, x, y, states, masks, rmasks):
 def test_variational_oracle_matches_torch_autograd():
     params, x, y, states, masks, rmasks = _setup()
     assert rmasks is not None and not all(m.all() for m in rmasks)
-    sc, st, cache = VO.model_fwd(params, x, states, L, P, masks, rmasks, P_REC)
-    grads = VO.model_bwd(params, cache, O.nll_loss_bwd(sc, y), L)
-    loss = O.nll_loss(sc, y)
+    loss, sc, st, grads = _oracle(params, x, y, states, masks, rmasks, P_REC)
     t_loss, t_sc, t_st, t_grads = _torch_restatement(params, x, y, states, masks, rmasks)
     np.testing.assert_allclose(loss, t_loss, rtol=1e-12)
     np.testing.assert_allclose(sc, t_sc, rtol=1e-11, atol=1e-12)
@@ -75,30 +88,38 @@ def test_variational_oracle_matches_torch_autograd():
 def test_recurrent_masks_change_the_result():
     """The recurrent masks are not a no-op (guards the torch comparison above against a restatement that ignores them)."""
     params, x, y, states, masks, rmasks = _setup()
-    a, _, _ = VO.model_fwd(params, x, states, L, P, masks, rmasks, P_REC)
-    b, _, _ = VO.model_fwd(params, x, states, L, P, masks, None, 0.0)
+    a = _oracle(params, x, y, states, masks, rmasks, P_REC)[1]
+    b = _oracle(params, x, y, states, masks, None, 0.0)[1]
     assert np.abs(a - b).max() > 1e-3
 
 
 def test_without_recurrent_masks_equals_the_oracle_with_tiled_masks():
     params, x, y, states, masks, _ = _setup()
-    masks0, rm0 = VO.variational_masks(12345, 3, L, T, B, H, P, 0.0)
-    assert rm0 is None
+    """p_rec = 0: the numpy oracle given the tiled masks, to 1e-12 relative (two separate implementations)"""
+    params, x, y, states, masks, _ = _setup()
+    mk = _masks(0.0)
+    masks0 = mk.sites
+    assert mk.rec is None
     for s in range(L + 1):   # the step-0 slice of the site's per-step mask, reused for every t
         want = PH.keep_mask(12345, 3, s, T * B * H, P).reshape(T, B, H)[0]
         assert all(np.array_equal(masks0[s][t], want) for t in range(T))
-    p1 = {k: v.copy() for k, v in params.items()}
+    loss, sc, st, _ = _oracle(params, x, y, states, masks0, None, 0.0)
+    tp = {k: torch.tensor(v) for k, v in params.items()}
+    _, norm, grads, after, _, _ = MO.train_step(tp, torch.tensor(x), torch.tensor(y),
+                                                [(torch.tensor(h), torch.tensor(c)) for h, c in states], L, False, 1.0,
+                                                0.25, MO.Modes(p=P, variational=True), MO.Masks(sites=masks0))
     p2 = {k: v.copy() for k, v in params.items()}
-    got = VO.train_step(p1, x, y, states, L, 1.0, 0.25, P, masks0, None, 0.0)
     want = O.train_step(p2, x, y, states, L, 1.0, 0.25, P, masks0)
-    assert got[0] == want[0] and got[1] == want[1]
-    np.testing.assert_array_equal(got[3], want[3])
-    for (h, c), (h2, c2) in zip(got[2], want[2]):
-        np.testing.assert_array_equal(h, h2)
-        np.testing.assert_array_equal(c, c2)
-    for k in p1:
-        np.testing.assert_array_equal(got[4][k], want[4][k])
-        np.testing.assert_array_equal(p1[k], p2[k])
+    np.testing.assert_allclose(loss, want[0], rtol=1e-12)
+    np.testing.assert_allclose(norm, want[1], rtol=1e-12)
+    np.testing.assert_allclose(sc, want[3], rtol=1e-12)
+    for (h, c), (h2, c2) in zip(st, want[2]):
+        np.testing.assert_allclose(h, h2, rtol=1e-12)
+        np.testing.assert_allclose(c, c2, rtol=1e-12)
+    coef = min(1.0, 0.25 / (norm + 1e-6))
+    for k in p2:
+        np.testing.assert_allclose(grads[k].numpy() * coef, want[4][k], rtol=1e-12, err_msg=k)
+        np.testing.assert_allclose(after[k].numpy(), p2[k], rtol=1e-12, err_msg=k)
 
 
 def test_entry_point_declared_and_bound():

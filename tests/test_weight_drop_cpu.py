@@ -1,4 +1,4 @@
-"""The weight-dropped LSTM without a GPU: its numpy restatement (tests/_weight_drop_oracle.py) against an independent
+"""The weight-dropped LSTM without a GPU: the fp64 restatement (tests/_model_oracle.py) against an independent
 float64 torch-autograd restatement with a masked W_hh, with Zaremba's dropout and with the variational mode; the masks'
 definition; the new C entry point in the header and the ctypes binding; Model(weight_drop=) argument checks."""
 import ctypes as C
@@ -11,8 +11,7 @@ import torch
 
 from oracle import lstm_lm_oracle as O
 from oracle import philox as PH
-from tests import _variational_oracle as VO
-from tests import _weight_drop_oracle as WO
+from tests import _model_oracle as MO
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 V, H, L, T, B = 23, 8, 2, 5, 3
@@ -26,12 +25,24 @@ def _setup(variational, seed=7):
     x = rng.integers(0, V, size=(T, B))
     y = rng.integers(0, V, size=(T, B))
     states = [(rng.uniform(-0.5, 0.5, (B, H)), rng.uniform(-1, 1, (B, H))) for _ in range(L)]   # non-zero entering
-    if variational:
-        masks, rmasks = VO.variational_masks(12345, STEP, L, T, B, H, P, P_REC)
-    else:
-        masks, rmasks = PH.site_masks(12345, STEP, L, T, B, H, P), None
-    wd = WO.weight_drop_masks(WD_SEED, STEP, L, H, P_WD)
-    return params, x, y, states, masks, rmasks, wd
+    mk = MO.mode_masks(_modes(variational, P_WD), [H] * (L + 1), T, B, V)
+    return params, x, y, states, mk.sites, mk.rec, mk.wd
+
+
+def _modes(variational, p_wd):
+    return MO.Modes(seed=12345, step=STEP, p=P, variational=variational, p_rec=P_REC if variational else 0.0,
+                    wd_seed=WD_SEED, p_wd=p_wd)
+
+
+def _oracle(params, x, y, states, masks, rmasks, wd, variational):
+    """_model_oracle's loss, scores, states and raw gradients (autograd) as numpy"""
+    ps = {k: torch.tensor(v, requires_grad=True) for k, v in params.items()}
+    sc, st, _ = MO.forward(ps, torch.tensor(x), [(torch.tensor(h), torch.tensor(c)) for h, c in states], L, False,
+                           _modes(variational, P_WD), MO.Masks(sites=masks, rec=rmasks, wd=wd))
+    loss = MO.loss_of(sc, torch.tensor(y))
+    loss.backward()
+    return (loss.item(), sc.detach().numpy(), [(h.detach().numpy(), c.detach().numpy()) for h, c in st],
+            {k: v.grad.numpy() for k, v in ps.items()})
 
 
 def _torch_restatement(params, x, y, states, masks, rmasks, wd):
@@ -67,9 +78,7 @@ def _torch_restatement(params, x, y, states, masks, rmasks, wd):
 def test_weight_drop_oracle_matches_torch_autograd(variational):
     params, x, y, states, masks, rmasks, wd = _setup(variational)
     assert wd is not None and all(not w.all() and w.any() for w in wd)
-    sc, st, cache = WO.model_fwd(params, x, states, L, P, masks, rmasks, P_REC if variational else 0.0, wd, P_WD)
-    grads = WO.model_bwd(params, cache, O.nll_loss_bwd(sc, y), L, wd, P_WD)
-    loss = O.nll_loss(sc, y)
+    loss, sc, st, grads = _oracle(params, x, y, states, masks, rmasks, wd, variational)
     t_loss, t_sc, t_st, t_grads = _torch_restatement(params, x, y, states, masks, rmasks, wd)
     np.testing.assert_allclose(loss, t_loss, rtol=1e-12)
     np.testing.assert_allclose(sc, t_sc, rtol=1e-11, atol=1e-12)
@@ -84,24 +93,28 @@ def test_weight_drop_oracle_matches_torch_autograd(variational):
 
 
 def test_weight_drop_changes_the_result_and_p0_is_the_identity():
+    """p_wd = 0 is the numpy oracle, to 1e-12 relative (two separate implementations)"""
     params, x, y, states, masks, _, wd = _setup(False)
-    a, _, _ = WO.model_fwd(params, x, states, L, P, masks, None, 0.0, wd, P_WD)
-    b, _, _ = WO.model_fwd(params, x, states, L, P, masks)
+    a = _oracle(params, x, y, states, masks, None, wd, False)[1]
+    b = _oracle(params, x, y, states, masks, None, None, False)[1]
     assert np.abs(a - b).max() > 1e-3
-    assert WO.weight_drop_masks(WD_SEED, STEP, L, H, 0.0) is None
-    p1 = {k: v.copy() for k, v in params.items()}
+    assert MO.mode_masks(_modes(False, 0.0), [H] * (L + 1), T, B, V).wd is None
+    tp = {k: torch.tensor(v) for k, v in params.items()}
+    loss, norm, _, after, _, _ = MO.train_step(tp, torch.tensor(x), torch.tensor(y),
+                                               [(torch.tensor(h), torch.tensor(c)) for h, c in states], L, False, 1.0,
+                                               0.25, _modes(False, 0.0), MO.Masks(sites=masks))
     p2 = {k: v.copy() for k, v in params.items()}
-    got = WO.train_step(p1, x, y, states, L, 1.0, 0.25, P, masks)
     want = O.train_step(p2, x, y, states, L, 1.0, 0.25, P, masks)
-    assert got[0] == want[0] and got[1] == want[1]
-    for k in p1:
-        np.testing.assert_array_equal(p1[k], p2[k])
+    np.testing.assert_allclose(loss, want[0], rtol=1e-12)
+    np.testing.assert_allclose(norm, want[1], rtol=1e-12)
+    for k in p2:
+        np.testing.assert_allclose(after[k].numpy(), p2[k], rtol=1e-12, err_msg=k)
 
 
 def test_masks_are_site_2L_plus_1_plus_l_over_w_hh():
     """The mask of layer l is zrb_dropout_mask(wd_seed, step, 2L + 1 + l, 4H*H, p) read in W_hh's row-major order; the
     sites follow the variational mode's recurrent ones and stay far from the sampler's counter word 0xFFFFFFFF."""
-    wd = WO.weight_drop_masks(WD_SEED, STEP, L, H, P_WD)
+    wd = MO.mode_masks(_modes(False, P_WD), [H] * (L + 1), T, B, V).wd
     for l in range(L):
         want = PH.keep_mask(WD_SEED, STEP, 2 * L + 1 + l, 4 * H * H, P_WD).reshape(4 * H, H)
         np.testing.assert_array_equal(wd[l], want)

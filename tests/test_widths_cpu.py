@@ -1,5 +1,5 @@
 """Layers of unequal width without a GPU: Model's parameters, initialisation and argument checks against a torch stack of
-nn.LSTM(In_l, H_l), the fp64 restatement (tests/_widths_oracle.py) against torch autograd on such a stack, and the
+nn.LSTM(In_l, H_l), the fp64 restatement (tests/_model_oracle.py) against torch autograd on such a stack, and the
 C declarations of the new entry points."""
 import math
 
@@ -8,7 +8,7 @@ import torch
 from torch import nn
 
 import zaremba_b200
-from tests import _widths_oracle as O
+from tests import _model_oracle as O
 
 AWD = dict(tied=True, embed_size=400, layer_sizes=(1150, 1150, 400))
 
@@ -155,61 +155,28 @@ def test_new_entry_points_are_bound():
 
 
 def test_mask_helpers_match_the_equal_width_oracles():
-    """at equal widths the per-site helpers draw exactly the masks of oracle.philox and the mode oracles"""
+    """at equal widths mode_masks draws exactly the masks of oracle.philox's site_masks and keep_mask"""
     import numpy as np
     from oracle import philox as PH
-    from tests import _variational_oracle as VO
-    from tests import _weight_drop_oracle as WO
     L, T, B, H, V = 2, 3, 4, 24, 50
-    got = O.site_masks(9, 5, [H] * (L + 1), T, B, 0.3)
+    got = O.mode_masks(O.Modes(seed=9, step=5, p=0.3), [H] * (L + 1), T, B, V).sites
     assert all(np.array_equal(a, b) for a, b in zip(got, PH.site_masks(9, 5, L, T, B, H, 0.3)))
     md = O.Modes(seed=9, step=5, p=0.3, variational=True, p_rec=0.2, wd_seed=11, p_wd=0.4, ed_seed=13, p_e=0.1)
-    sites, rec, wd, ed = O.mode_masks(md, [H] * (L + 1), T, B, V)
-    vs, vr = VO.variational_masks(9, 5, L, T, B, H, 0.3, 0.2)
-    assert all(np.array_equal(a, b) for a, b in zip(sites, vs)) and all(np.array_equal(a, b) for a, b in zip(rec, vr))
-    assert all(np.array_equal(a, b) for a, b in zip(wd, WO.weight_drop_masks(11, 5, L, H, 0.4)))
-    assert np.array_equal(ed, PH.keep_mask(13, 5, 3 * L + 1, V, 0.1))
+    mk = O.mode_masks(md, [H] * (L + 1), T, B, V)
+    for s in range(L + 1):   # variational: the site's first B*H elements at every t
+        want = PH.keep_mask(9, 5, s, B * H, 0.3).reshape(B, H)
+        assert all(np.array_equal(mk.sites[s][t], want) for t in range(T))
+    for l in range(L):
+        assert np.array_equal(mk.rec[l], PH.keep_mask(9, 5, L + 1 + l, B * H, 0.2).reshape(B, H))
+        assert np.array_equal(mk.wd[l], PH.keep_mask(11, 5, 2 * L + 1 + l, 4 * H * H, 0.4).reshape(4 * H, H))
+    assert np.array_equal(mk.ed, PH.keep_mask(13, 5, 3 * L + 1, V, 0.1))
     # unequal widths: each site's stream is over its own width
-    sites, rec, wd, _ = O.mode_masks(md, [8, 16, 24], T, B, V)
+    mk = O.mode_masks(md, [8, 16, 24], T, B, V)
+    sites, rec, wd = mk.sites, mk.rec, mk.wd
     assert [m.shape for m in sites] == [(T, B, 8), (T, B, 16), (T, B, 24)]
     assert np.array_equal(sites[1][2], PH.keep_mask(9, 5, 1, B * 16, 0.3).reshape(B, 16))
     assert [m.shape for m in rec] == [(B, 16), (B, 24)] and [m.shape for m in wd] == [(64, 16), (96, 24)]
     assert np.array_equal(wd[1].reshape(-1), PH.keep_mask(11, 5, 2 * L + 2, 4 * 24 * 24, 0.4))
-
-
-@pytest.mark.parametrize("tied", [False, True])
-@pytest.mark.parametrize("variational", [False, True])
-def test_oracle_modes_match_numpy_restatement_at_equal_widths(tied, variational):
-    """the torch restatement of every mode against the numpy one of DESIGN sections 11, 15 and 17 (a separate
-    implementation with hand-written gradients) where both apply: equal widths"""
-    import numpy as np
-    from tests import _awd_reg_oracle as AR
-    L, T, B, H, V = 2, 4, 3, 12, 29
-    g = np.random.default_rng(0)
-    names = O.names(L, tied)
-    shapes = {"embed.W": (V, H), "fc.W": (V, H), "fc.b": (V,)}
-    for l in range(L):
-        shapes.update({f"rnns.{l}.weight_ih_l0": (4 * H, H), f"rnns.{l}.weight_hh_l0": (4 * H, H),
-                       f"rnns.{l}.bias_ih_l0": (4 * H,), f"rnns.{l}.bias_hh_l0": (4 * H,)})
-    pn = {k: g.uniform(-0.3, 0.3, shapes[k]) for k in names}
-    x, y = g.integers(0, V, (T, B)), g.integers(0, V, (T, B))
-    st = [(g.uniform(-0.2, 0.2, (B, H)), g.uniform(-0.2, 0.2, (B, H))) for _ in range(L)]
-    md = O.Modes(seed=3, step=7, p=0.3, variational=variational, p_rec=0.25 if variational else 0.0, wd_seed=4,
-                 p_wd=0.5, ed_seed=5, p_e=0.2, alpha=2.0, beta=1.0)
-    sites, rec, wd, ed = O.mode_masks(md, [H] * (L + 1), T, B, V)
-    pt = {k: torch.tensor(v) for k, v in pn.items()}
-    loss, norm, grads, _, st_out, reg = O.train_step(pt, torch.tensor(x), torch.tensor(y),
-                                                     [(torch.tensor(h), torch.tensor(c)) for h, c in st], L, tied, 1.0,
-                                                     0.5, md)
-    pa = {k: v.copy() for k, v in pn.items()}
-    nl, nn_, nst, _, nraw, (ar, tar) = AR.train_step(pa, x, y, st, L, 1.0, 0.5, 0.3, sites, rec, md.p_rec, wd, 0.5,
-                                                     ed, 0.2, tied, 2.0, 1.0)
-    assert abs(loss - nl) < 1e-10 * abs(nl) and abs(reg - (ar + tar)) < 1e-10 * max(1.0, ar + tar)
-    assert abs(norm - nn_) < 1e-9 * nn_
-    for k in names:
-        assert np.allclose(grads[k].numpy(), nraw[k], rtol=1e-8, atol=1e-12), k
-    for (h, c), (nh, nc) in zip(st_out, nst):
-        assert np.allclose(h.numpy(), nh) and np.allclose(c.numpy(), nc)
 
 
 def _train_ptb(*args):

@@ -1,4 +1,4 @@
-"""Zoneout (DESIGN.md section 20) without a GPU: the fp64 restatement of tests/_zoneout_oracle.py against torch autograd of
+"""Zoneout (DESIGN.md section 20) without a GPU: the fp64 restatement of tests/_model_oracle.py against torch autograd of
 a literal transcription of Krueger et al.'s LSTM equations, its flags, the Model's arguments, the ABI, and what ptxas
 makes of the zoneout instantiations of the persistent recurrence kernels."""
 import os
@@ -10,7 +10,7 @@ import torch
 
 from oracle import lstm_lm_oracle as O
 from oracle import philox
-from tests import _zoneout_oracle as ZO
+from tests import _model_oracle as MO
 from tests.test_rec_codegen_cpu import _stack_frames, ptxas_logs  # noqa: F401  (the module fixture)
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -19,6 +19,21 @@ V, H, L, T, B = 23, 6, 2, 5, 3
 
 def _params(seed=0):
     return O.init_params(V, H, L, 0.3, seed, dtype=np.float64)
+
+
+def _masks(seed, step, z_c, z_h, Lm=L):
+    return MO.mode_masks(MO.Modes(seed=seed, step=step, z_c=z_c, z_h=z_h), [H] * (Lm + 1), T, B, V)
+
+
+def _oracle(params, x, y, states, z_c, z_h, train):
+    """_model_oracle's loss, states and gradients (autograd) as numpy, flags of seed 7 at step 3 in train mode"""
+    P = {k: torch.tensor(v, requires_grad=True) for k, v in params.items()}
+    scores, st, _ = MO.forward(P, torch.as_tensor(x), [tuple(torch.tensor(v) for v in s) for s in states], L, False,
+                               MO.Modes(seed=7, step=3, z_c=z_c, z_h=z_h), train=train)
+    loss = MO.loss_of(scores, torch.as_tensor(y))
+    loss.backward()
+    return (loss.item(), scores.detach().numpy(), [(h.detach().numpy(), c.detach().numpy()) for h, c in st],
+            {k: v.grad.numpy() for k, v in P.items()})
 
 
 def _krueger(params, x, y, states, z_c, z_h, zflags):
@@ -38,8 +53,8 @@ def _krueger(params, x, y, states, z_c, z_h, zflags):
             if zflags is None:
                 dc, dh = z_c, z_h
             else:
-                dc = torch.tensor(zflags[l][0][t], dtype=torch.float64)
-                dh = torch.tensor(zflags[l][1][t], dtype=torch.float64)
+                dc = 0.0 if zflags.zc is None else torch.tensor(zflags.zc[l][t], dtype=torch.float64)
+                dh = 0.0 if zflags.zh is None else torch.tensor(zflags.zh[l][t], dtype=torch.float64)
             c = dc * c + (1 - dc) * c_new
             h = dh * h + (1 - dh) * h_new
             ys.append(h)
@@ -60,11 +75,10 @@ def test_oracle_equals_autograd_of_krueger(train, z):
     x, y = rng.integers(0, V, (T, B)), rng.integers(0, V, (T, B))
     states = [(rng.standard_normal((B, H)) * 0.5, rng.standard_normal((B, H))) for _ in range(L)]
     params = _params()
-    zflags = [ZO.flags(7, 3, L, l, T, B, H, z_c, z_h) for l in range(L)] if train else None
+    zflags = _masks(7, 3, z_c, z_h) if train else None
     want_loss, want_states, want = _krueger(params, x, y, states, z_c, z_h, zflags)
-    scores, got_states, cache = ZO.model_fwd(params, x, states, L, z_c, z_h, zflags)
-    got = ZO.model_bwd(cache, O.nll_loss_bwd(scores, y), L)
-    assert abs(O.nll_loss(scores, y) - want_loss) < 1e-12
+    loss, _, got_states, got = _oracle(params, x, y, states, z_c, z_h, train)
+    assert abs(loss - want_loss) < 1e-12
     for (h, c), (wh, wc) in zip(got_states, want_states):
         np.testing.assert_allclose(h, wh, atol=1e-13)
         np.testing.assert_allclose(c, wc, atol=1e-13)
@@ -73,15 +87,14 @@ def test_oracle_equals_autograd_of_krueger(train, z):
 
 
 def test_zero_rates_are_the_plain_lstm():
+    """against the numpy oracle, to 1e-12 relative (two separate implementations)"""
     rng = np.random.default_rng(2)
     x, y = rng.integers(0, V, (T, B)), rng.integers(0, V, (T, B))
     states = O.zero_states(L, B, H, np.float64)
     params = _params()
-    zflags = [ZO.flags(7, 3, L, l, T, B, H, 0.0, 0.0) for l in range(L)]
-    scores, _, cache = ZO.model_fwd(params, x, states, L, 0.0, 0.0, zflags)
+    _, scores, _, got = _oracle(params, x, y, states, 0.0, 0.0, True)
     want_scores, _, want_cache = O.model_fwd(params, x, states, L)
-    np.testing.assert_array_equal(scores, want_scores)
-    got = ZO.model_bwd(cache, O.nll_loss_bwd(scores, y), L)
+    np.testing.assert_allclose(scores, want_scores, rtol=1e-12)
     want = O.model_bwd(params, want_cache, O.nll_loss_bwd(want_scores, y), L)
     for k in O.param_names(L):
         np.testing.assert_allclose(got[k], want[k], rtol=1e-12, atol=1e-15, err_msg=k)
@@ -93,12 +106,13 @@ def test_flags_take_their_own_sites():
     Lm = 3
     sites = {(3 * Lm + 3 + l) for l in range(Lm)} | {(4 * Lm + 3 + l) for l in range(Lm)}
     assert len(sites) == 2 * Lm and min(sites) == 3 * Lm + 3 and max(sites) == 5 * Lm + 2
-    zc, zh = ZO.flags(11, 4, Lm, 1, T, B, H, 0.5, 0.25)
+    mk = _masks(11, 4, 0.5, 0.25, Lm)
+    zc, zh = mk.zc[1], mk.zh[1]
     np.testing.assert_array_equal(zc.reshape(-1), ~philox.keep_mask(11, 4, 3 * Lm + 4, T * B * H, 0.5))
     np.testing.assert_array_equal(zh.reshape(-1), ~philox.keep_mask(11, 4, 4 * Lm + 4, T * B * H, 0.25))
     assert 0.3 < zc.mean() < 0.7 and 0.05 < zh.mean() < 0.5
-    zc0, zh0 = ZO.flags(11, 4, Lm, 1, T, B, H, 0.0, 0.0)
-    assert not zc0.any() and not zh0.any()
+    mk0 = _masks(11, 4, 0.0, 0.0, Lm)
+    assert mk0.zc is None and mk0.zh is None          # no flag: no unit is zoned
 
 
 @pytest.mark.parametrize("kw, msg", [
