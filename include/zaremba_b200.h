@@ -353,15 +353,6 @@ int    zrb_dp_allreduce_bucket(zrb_dp* dp, int32_t bucket, int64_t lo, int64_t h
 /* join: `stream` waits for all bucket reductions enqueued in this step (alternative to last = 1) */
 int    zrb_dp_finish_step(zrb_dp* dp, void* stream);
 
-/* Co-scheduling hook for work that must only use the SMs the persistent backward recurrence leaves idle (the
- * data-parallel bucket all-reduce of a communicator limited to <= 16 CTAs): the kernel's CTA 0 stores a sequence
- * number into a device flag once every CTA of its grid is resident.  zrb_resident_flag returns the flag and the value
- * the NEXT backward-recurrence launch of this context will publish (0: this context does not use the persistent
- * kernel, do not wait); zrb_stream_wait_value32 makes `stream` wait until *d_flag >= value (cuStreamWaitValue32). */
-/* CAUTION: a stream blocked in cuStreamWaitValue32 on a value that a kernel enqueued LATER on another stream of the same
- * process will write can deadlock when the two streams share a hardware work queue (observed: a 2-GPU run hung).  Use the
- * flag only from a stream that provably does not alias the launching stream's queue, or poll it from a kernel. */
-int  zrb_resident_flag(zrb_ctx* ctx, uint32_t** d_flag, uint32_t* next_value);
 /* The plans the persistent recurrence kernels of a tensor-core context run with, chosen at creation for its max_batch
  * (so a smaller window reuses them) from the shape and the device's SM count.  h_out[0..7] = forward, h_out[8..15] =
  * backward, each {ok, KS, U, G, nCTA, GBi, Kc, KcS}: ok = 0 means that direction takes the per-timestep path (the other
@@ -373,7 +364,6 @@ int  zrb_resident_flag(zrb_ctx* ctx, uint32_t** d_flag, uint32_t* next_value);
 int  zrb_rec_plans(const zrb_ctx* ctx, int32_t* h_out);
 /* zrb_rec_plans for layer `layer` (0 <= layer < L, else ZRB_E_INVALID). */
 int  zrb_rec_plans_layer(const zrb_ctx* ctx, int32_t layer, int32_t* h_out);
-int  zrb_stream_wait_value32(void* stream, const uint32_t* d_flag, uint32_t value);
 
 /* perplexity's inner step (main.py:91-94) without materialising scores for the caller:
  * forward in eval mode + loss (+ per-token target probabilities for the ensemble). */

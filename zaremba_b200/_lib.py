@@ -121,8 +121,6 @@ _SIGNATURES = {
     "zrb_average_count": (C.c_int, [_vp, C.POINTER(C.c_int64)]),
     "zrb_swap_average": (C.c_int, [_vp, C.POINTER(ZrbParams), _vp]),
     "zrb_check_health": (C.c_int, [_vp]),
-    "zrb_resident_flag": (C.c_int, [_vp, C.POINTER(_vp), C.POINTER(C.c_uint32)]),
-    "zrb_stream_wait_value32": (C.c_int, [_vp, _vp, C.c_uint32]),
     "zrb_rec_plans": (C.c_int, [_vp, _vp]),
     "zrb_rec_plans_layer": (C.c_int, [_vp, C.c_int32, _vp]),
     "zrb_dp_create": (C.c_int, [C.c_int32, C.c_int32, C.c_int64, C.POINTER(_vp)]),

@@ -42,8 +42,7 @@ static int dalloc(zrb_ctx* c, T** p, size_t count) {
 // A persistent recurrence kernel that ran out of patience (lost wake-up, grid not co-resident) finished with garbage and
 // left a code in the mapped host word: every later call on this context fails -- the CUDA context is intact, a new zrb
 // context works.  Costs one host load.
-static const char* const kWaitNames[] = {"?", "weight slice", "operand image", "accumulators", "partner rows", "grid barrier",
-                                         "cluster partials"};
+static const char* const kWaitNames[] = {"?", "weight slice", "operand image", "accumulators", "partner rows", "grid barrier"};
 static int watchdog_check(const zrb_ctx* c) {
     if (!c->wd_host) return ZRB_OK;
     const unsigned int code = *(volatile const unsigned int*)c->wd_host;
@@ -191,10 +190,9 @@ static int ctx_create(const zrb_config* cfg, const int* widths, zrb_ctx** out, i
     if (rc == ZRB_OK) rc = dalloc(c, &c->x_saved, N);
     if (rc == ZRB_OK) rc = dalloc(c, &c->emb_prev_ids, N);
     if (rc == ZRB_OK) c->emb_prev_cap = (int64_t)N;
-    if (rc == ZRB_OK) rc = dalloc(c, &c->resident_flag, 4);
-    if (rc == ZRB_OK && cudaMemset(c->resident_flag, 0, 4 * sizeof(unsigned int)) != cudaSuccess) rc = ZRB_E_CUDA;
+    if (rc == ZRB_OK) rc = dalloc(c, &c->wd_flag, 1);
+    if (rc == ZRB_OK && cudaMemset(c->wd_flag, 0, sizeof(unsigned int)) != cudaSuccess) rc = ZRB_E_CUDA;
     if (rc == ZRB_OK) {
-        c->wd_flag = c->resident_flag + 2;
         void* hp = nullptr;
         if (cudaHostAlloc(&hp, sizeof(unsigned int), cudaHostAllocMapped) != cudaSuccess) {
             set_error("cudaHostAlloc of the watchdog word failed");
@@ -658,13 +656,6 @@ int zrb_set_embed_sparse(zrb_ctx* c, int32_t on) {
     c->emb_sparse = on != 0;
     c->fused_norm = on == 1;
     c->emb_prev_grad = nullptr;
-    return ZRB_OK;
-}
-
-int zrb_resident_flag(zrb_ctx* c, uint32_t** flag, uint32_t* next_value) {
-    ZRB_REQUIRE(c && flag && next_value, "null argument");
-    *flag = c->resident_flag;
-    *next_value = (c->cfg.engine == ZRB_ENGINE_TC && tc_persistent_bwd(c)) ? c->resident_seq + 1 : 0;
     return ZRB_OK;
 }
 

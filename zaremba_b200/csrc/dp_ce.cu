@@ -112,13 +112,6 @@ using namespace zrb;
 
 extern "C" {
 
-int zrb_stream_wait_value32(void* stream, const uint32_t* d_flag, uint32_t value) {
-    ZRB_REQUIRE(d_flag, "null flag");
-    ZRB_TRY(load_stream_memops());
-    ZRB_CU(g_wait32((CUstream)stream, (CUdeviceptr)d_flag, value, CU_STREAM_WAIT_VALUE_GEQ));
-    return ZRB_OK;
-}
-
 int zrb_dp_create(int32_t rank, int32_t world, int64_t n_grad, zrb_dp** out) {
     ZRB_REQUIRE(out && world >= 1 && rank >= 0 && rank < world && n_grad > 0, "bad arguments");
     ZRB_TRY(load_stream_memops());

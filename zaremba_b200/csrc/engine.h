@@ -82,9 +82,7 @@ struct zrb_ctx {
     bool fused_norm = false;               // single process: matrices' part of the clip norm from the wgrad GEMM epilogues
     bool tied = false;                     // ZRB_TIED_EMBEDDING: embed_w == fc_w in every zrb_params (DESIGN.md section 13)
     int64_t emb_prev_cap = 0;              // capacity of emb_prev_ids (tokens)
-    unsigned int* resident_flag = nullptr; // written by the backward recurrence kernel once all its CTAs are resident
-    unsigned int resident_seq = 0;         // value the last launch publishes there
-    unsigned int* wd_flag = nullptr;       // watchdog of the persistent kernels (rec_common.cuh): device word, = resident_flag + 2
+    unsigned int* wd_flag = nullptr;       // watchdog of the persistent kernels (rec_common.cuh): device word
     unsigned int* wd_host = nullptr;       // ... and the mapped host word the host polls (watchdog_check)
     int64_t* emb_prev_ids = nullptr;       // token ids whose gradient rows are non-zero in emb_prev_grad
     int emb_prev_n = 0;
@@ -157,7 +155,6 @@ int tc_train_step_begin(zrb_ctx* c, const zrb_params* p, const zrb_params* g, co
 int tc_train_step_layer(zrb_ctx* c, const zrb_params* p, const zrb_params* g, int l, cudaStream_t s);
 int tc_rec_trace(zrb_ctx* c, long long* h_out, int max_entries);
 int tc_flush_updates(zrb_ctx* c, cudaStream_t s);   // apply deferred weight updates now (zrb_set_lazy_update)
-bool tc_persistent_bwd(const zrb_ctx* c);
 const __half* tc_last_layer_image(const zrb_ctx* c);   // x_h[L]: fp16 last-layer output of the last forward, pitch
                                                        // pad64(H_{L-1})
 // zrb_rec_plans_layer: layer l's 2 x {ok, KS, U, G, nCTA, GBi, Kc, KcS}

@@ -136,12 +136,8 @@ struct zrb_tc_state {
 namespace zrb {
 
 // whether work may run as a programmatic dependent beside a recurrence kernel: not while zrb_prof_enable brackets the
-// kernel classes with events (a record would sit between the two launches), unless ZRB_PROF_KEEP_PDL=1
-static bool pdl_beside_rec(const zrb_ctx* c) {
-    if (!c->prof_on) return true;
-    static const bool keep = getenv("ZRB_PROF_KEEP_PDL") != nullptr;
-    return keep;
-}
+// kernel classes with events (a record would sit between the two launches)
+static bool pdl_beside_rec(const zrb_ctx* c) { return !c->prof_on; }
 static int pad64(int n) { return (n + 63) / 64 * 64; }
 
 template <typename T>
@@ -696,7 +692,7 @@ static int tc_issue_pending(zrb_ctx* c, const zrb_params* g, cudaStream_t s) {
     const int kind = t->pending;
     t->pending = 0;
     // (no event bracket here: an event record between the recurrence kernel and its programmatic dependent would sit
-    // between the two launches; while profiling with ZRB_PROF_KEEP_PDL=1 the time lands in the enclosing REC_BWD class)
+    // between the two launches; while profiling, pdl_beside_rec defers nothing)
     if (kind == 1) {
         Gemm dw = fc_w_wgrad(c, g);
         dw.pdl = true;
@@ -736,7 +732,7 @@ static int tc_backward_layer(zrb_ctx* c, const zrb_params* p, const zrb_params* 
                 a.w_img = t->w_img_b[l]; a.g_img = t->g_img; a.dy = dY; a.r = r; a.gates = c->gates[l];
                 a.cst = c->cst[l]; a.c0 = c->c0s[l]; a.dG_h = dG_h; a.db1 = g->b_ih[l]; a.db2 = g->b_hh[l];
                 a.db_scratch = c->dG;   // [N,4H] fp32, idle on this path
-                a.res_flag = c->resident_flag; a.res_value = ++c->resident_seq; a.counter = word; a.base = base;
+                a.counter = word; a.base = base;
                 a.T = T; a.B = B; a.H = H; a.G4p = G4p; a.m = m; a.rm = rm;
                 a.trace = t->trace ? t->trace + 8 + (size_t)c->cfg.max_seq * 8 : nullptr;
                 a.zo = zo; a.ctil = c->ctil[l];
@@ -811,8 +807,7 @@ static int tc_backward_layer(zrb_ctx* c, const zrb_params* p, const zrb_params* 
 }
 
 static int tc_backward_from_image(zrb_ctx* c, const zrb_params* p, const zrb_params* g, cudaStream_t s) {
-    static const bool no_overlap = getenv("ZRB_NO_OVERLAP") != nullptr;    // A/B switch
-    c->tc->defer_wgrad = !no_overlap;
+    c->tc->defer_wgrad = true;
     ZRB_TRY(tc_backward_head(c, p, g, s));
     for (int l = c->cfg.layers - 1; l >= 0; --l) ZRB_TRY(tc_backward_layer(c, p, g, l, s));
     return ZRB_OK;
@@ -907,8 +902,6 @@ int tc_train_step_layer(zrb_ctx* c, const zrb_params* p, const zrb_params* g, in
     return tc_backward_layer(c, p, g, l, s);
 }
 
-bool tc_persistent_bwd(const zrb_ctx* c) { return c->tc && c->tc->persistent(); }
-
 void tc_rec_plans(const zrb_ctx* c, int l, int32_t* h_out) {
     const RecPlan* plans[2] = {&c->tc->fplan[l], &c->tc->bplan[l]};
     for (int d = 0; d < 2; ++d) {
@@ -977,7 +970,7 @@ int tc_layer_bwd(zrb_ctx* c, const float* dy, float* dx, float* dw_ih, float* dw
         RecBwdArgs a = {};
         a.w_img = t->w_img_b[0]; a.g_img = t->g_img; a.dy = dy; a.gates = c->gates[0]; a.cst = c->cst[0];
         a.c0 = c->c0s[0]; a.dG_h = t->dG_h; a.db1 = db_ih; a.db2 = db_hh; a.db_scratch = c->dG;
-        a.res_flag = c->resident_flag; a.res_value = ++c->resident_seq; a.counter = word; a.base = base;
+        a.counter = word; a.base = base;
         a.T = T; a.B = B; a.H = H; a.G4p = G4p; a.m = m; a.rm = m;
         return lstm_rec_bwd(bplan, tc_watchdog(c), a, s);
     }));

@@ -654,9 +654,7 @@ static TileChoice choose_tiles(int M, int N, int num_kb, bool can_split, bool re
         return c;
     }
     c.bn = (t256 >= (nsm * 9) / 10) ? 256 : 128;
-    static const int force_bn = [] { const char* e = getenv("ZRB_GEMM_BN"); return e ? atoi(e) : 0; }();   // experiment switch
-    if (force_bn == 128 || force_bn == 256) c.bn = force_bn;
-    else if (retile && c.bn == 256 && cdiv(t256, nsm) * 2 > cdiv(c.tiles_m * cdiv(N, 128), nsm) &&
+    if (retile && c.bn == 256 && cdiv(t256, nsm) * 2 > cdiv(c.tiles_m * cdiv(N, 128), nsm) &&
              c.tiles_m * cdiv(N, 128) * 2 > nsm)   // (never turns a whole plan into a split one)
         c.bn = 128;
     c.tiles_n = cdiv(N, c.bn);

@@ -14,8 +14,7 @@
 // The partial products D_r[UC x B] are exchanged as a reduce-scatter by PUSHING: the MMA warpgroup writes each
 // accumulator pair straight from registers into the shared memory of the CTA that owns the row's unit
 // (st.async, the bytes are counted on the owner's mbarrier: no fence, no staging pass), and the owner adds
-// the partials in fixed order in its cell math.  (The alternative stages them locally, announces them with a
-// cluster-scope release arrive and pulls them through DSMEM; selectable for S = 1 with ZRB_BWD_PULL=1.)
+// the partials in fixed order in its cell math.
 // dc lives in registers for the whole window; the bias
 // gradients sum_{t,b} dG are accumulated in registers and reduced over the batch at the end of the kernel.
 //
@@ -80,9 +79,8 @@ int rec_bwd_plan(int H, int B, RecPlan* plan) {
     plan->ok = 0;
     plan->KS = 1;
     if (plan->GB * 8 > 32) return ZRB_OK;
-    static const bool no_split = getenv("ZRB_REC_NOSPLIT") != nullptr;   // A/B switch
     // clusters of 8, half a gate block per CTA (see the kernel header); image batch groups padded to an even count
-    if (!no_split && H >= 256) {
+    if (H >= 256) {
         const int Kp = (H + 31) / 32 * 32, Kc = Kp / 8, KcS = Kc / 2, GBi = (plan->GB + 1) / 2 * 2;
         // first choice: at most one (unit, batch) cell per epilogue thread (see rec_fwd_plan)
         for (int pass = 0; pass < 2; ++pass)
@@ -132,8 +130,6 @@ int pack_whh_bwd(const float* W, __half* img, int H, const RecPlan& p, cudaStrea
 
 int lstm_rec_bwd(const RecPlan& p, const RecWatchdog& wd, RecBwdArgs a, cudaStream_t s) {
     ZRB_REQUIRE(!a.db1 || a.db_scratch, "bias gradients need the scratch buffer");
-    static const bool pull = getenv("ZRB_BWD_PULL") != nullptr;   // A/B switch: the r01 staging + DSMEM-pull exchange (S = 1)
-    a.push = pull ? 0 : 1;
     a.U = p.U; a.G = p.G; a.GB = p.GB; a.Kc = p.Kc; a.nCTA = p.nCTA; a.KcS = p.KcS; a.GBi = p.GBi;
     if (!a.rm.active) a.rm.scale = 1.f;   // (the epilogue multiplies by it unconditionally)
     ZRB_REQUIRE(wd.flag && wd.host, "lstm_rec_bwd needs the context's watchdog words");

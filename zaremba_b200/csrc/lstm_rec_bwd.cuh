@@ -15,38 +15,18 @@ __device__ __forceinline__ uint32_t mapa_shared(uint32_t local_addr, uint32_t ra
     asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_addr), "r"(rank));
     return r;
 }
-__device__ __forceinline__ float ld_dsmem_f32(uint32_t cluster_addr) {
-    float v;
-    asm volatile("ld.shared::cluster.f32 %0, [%1];" : "=f"(v) : "r"(cluster_addr));
-    return v;
-}
 __device__ __forceinline__ void st_dsmem_f32(uint32_t cluster_addr, float v) {
     asm volatile("st.shared::cluster.f32 [%0], %1;" ::"r"(cluster_addr), "f"(v) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_remote_release(uint32_t cluster_addr) {
-    asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-__device__ __forceinline__ bool mbar_try_wait_acq_cluster(uint64_t* bar, uint32_t parity) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(smem_u32(bar)), "r"(parity)
-        : "memory");
-    return ok != 0;
 }
 __device__ __forceinline__ void cluster_sync_all() {
     asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
 
-// S = 1: clusters of 4 (CTA rank = gate), one M = 64 tile, the whole gate block as contraction (S = 1 also keeps the
-//        staging + DSMEM-pull exchange selectable with a.push = 0).
+// S = 1: clusters of 4 (CTA rank = gate), one M = 64 tile, the whole gate block as contraction.
 // S = 2: clusters of 8.  The cluster owns twice the units (8U = 96 rows, two M = 64 tiles, N = 32) and CTA rank
 //        r = 2*gate + half multiplies only HALF of its gate's rows: 47 K steps per step instead of 94, half the operand
-//        image to fetch; the eight partial products are pushed (st.async) into the owners' shared memory and summed in
-//        fixed order.
+//        image to fetch.
+// Both push their CS partial products (st.async) into the owners' shared memory, where they are summed in fixed order.
 // ZO: zoneout (DESIGN.md section 20): tanh of c~_t (the forward's store), dh~ = (1 - zh) dh, dc~ = (1 - zc) dc +
 // dh~ o (1 - tanh^2 c~), and the carries dc <- zc dc + f dc~ and hcarry <- zh dh in registers; hcarry joins dh with the upstream gradient in the
 // prefetch, so that it holds no register across the waits.  Under `if constexpr` like the forward's.
@@ -60,19 +40,17 @@ __global__ void __launch_bounds__(kRecThreads, 1) lstm_rec_bwd_kernel(RecBwdArgs
     const int a_bytes = a.KcS * a.G * 128;     // this CTA's weight slice
     const int b_bytes = a.KcS * a.GBi * 128;   // the part of its gate's dG image this CTA multiplies with
     const int Bp = a.GBi * 8;                  // N of the MMA
-    const int ldd = Bp + 1;
     uint8_t* sA = smem;
     uint8_t* sB = smem + a_bytes;
-    float* sD = (float*)(sB + b_bytes);  // [64][Bp+1] this CTA's partial product, all issuers' accumulators summed (sized for two)
-    uint64_t* bars = (uint64_t*)((uint8_t*)sD + 2 * 64 * ldd * 4);
+    // receive buffer sR[source rank][unit][batch (pitch ldr, 16-byte rows)], in the 2 x 64 x (Bp + 1) floats that
+    // rec_smem_bytes sets aside (the plans check that it fits)
+    const int ldr = Bp + 4;
+    float* sR = (float*)(sB + b_bytes);
+    uint64_t* bars = (uint64_t*)((uint8_t*)sR + 2 * 64 * (Bp + 1) * 4);
     uint64_t* bar_a = bars;
     uint64_t* bar_b = bars + 1;                    // [kRecPieces]
     uint64_t* bar_mma = bars + 1 + kRecPieces;
-    uint64_t* bar_part = bar_mma + 1;              // 4 arrivals per step: every CTA of the cluster staged its partial
-    uint64_t* bar_recv = bar_part + 1;             // push mode: all four CTAs' partials of this CTA's units have landed
-    // push mode reuses the staging buffer as the receive buffer sR[source rank][unit][batch (pitch ldr, 16-byte rows)]
-    const int ldr = Bp + 4;
-    float* sR = sD;
+    uint64_t* bar_recv = bar_mma + 1;              // all CS CTAs' partials of this CTA's units have landed
 
     const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);   // warp-uniform for the compiler
     const int lane = threadIdx.x & 31;
@@ -94,7 +72,6 @@ __global__ void __launch_bounds__(kRecThreads, 1) lstm_rec_bwd_kernel(RecBwdArgs
         mbar_init(bar_a, 1);
         for (int i = 0; i < kRecPieces; ++i) mbar_init(&bar_b[i], 1);
         mbar_init(bar_mma, kRecMmaThreads);
-        mbar_init(bar_part, CS);
         mbar_init(bar_recv, 1);
         fence_mbar_init();
     }
@@ -110,13 +87,9 @@ __global__ void __launch_bounds__(kRecThreads, 1) lstm_rec_bwd_kernel(RecBwdArgs
         bool dead = false;
         const int lbo_b = a.GBi * 128;
         const size_t gate_bytes = (size_t)a.Kc * a.GBi * 128;   // one gate's whole dG image
-        const bool publish = a.res_flag != nullptr && blockIdx.x == 0;
-        if (publish && T == 1) asm volatile("st.relaxed.sys.global.u32 [%0], %1;" ::"l"(a.res_flag), "r"(a.res_value) : "memory");
         for (int s = 1; s < T; ++s) {
             const int t = T - 1 - s;                      // step being computed; needs dG_{t+1}
             grid_counter_wait(a.counter, a.base + (unsigned int)s * a.nCTA, a.w, dead, s);
-            if (publish && s == 1)   // every CTA arrived once: the whole grid is resident (or gave up: a stream gated on this must not hang)
-                asm volatile("st.relaxed.sys.global.u32 [%0], %1;" ::"l"(a.res_flag), "r"(a.res_value) : "memory");
             if (dead) break;   // (watchdog: a thread that gave up starts no further asynchronous operation)
             if (tr) trs[s * 8 + 0] = clock64();
             fence_proxy_async_global();
@@ -135,10 +108,9 @@ __global__ void __launch_bounds__(kRecThreads, 1) lstm_rec_bwd_kernel(RecBwdArgs
         const uint32_t a_addr = smem_u32(sA), b_addr = smem_u32(sB);
         const uint32_t lbo_a = a.G * 128, lbo_b = a.GBi * 128;
         const int mt = S == 2 && UC > 64 ? 2 : 1;
-        const bool push = S == 2 || a.push != 0;
         const uint32_t sR_addr = smem_u32(sR), bar_recv_addr = smem_u32(bar_recv);
         // accumulator row = cluster-local unit.  Where each of this thread's (at most four) rows goes, worked out once:
-        // its first float in the staging buffer, or its receive row in the owner's shared memory and the owner's mbarrier
+        // its receive row in the owner's shared memory and the owner's mbarrier
         const int tm = (int)threadIdx.x - kRecMmaWarp * 32;
         uint32_t row_dst[2][2], row_owner[2][2], row_bar[2][2];
         bool row_ok[2][2];
@@ -147,16 +119,11 @@ __global__ void __launch_bounds__(kRecThreads, 1) lstm_rec_bwd_kernel(RecBwdArgs
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 const int row = rec_acc_row(tm, m, h);
-                if (!push) {
-                    row_dst[m][h] = (uint32_t)(row * ldd * 4);
-                    row_owner[m][h] = 0u; row_bar[m][h] = 0u; row_ok[m][h] = true;
-                } else {
-                    const int owner = row / a.U, uo = row - owner * a.U;
-                    row_ok[m][h] = row < UC;
-                    row_owner[m][h] = row_ok[m][h] ? (uint32_t)owner : 0u;   // (rows past the cluster's are never sent)
-                    row_dst[m][h] = sR_addr + (uint32_t)(((int)rank * a.U + uo) * ldr * 4);
-                    row_bar[m][h] = mapa_shared(bar_recv_addr, row_owner[m][h]);
-                }
+                const int owner = row / a.U, uo = row - owner * a.U;
+                row_ok[m][h] = row < UC;
+                row_owner[m][h] = row_ok[m][h] ? (uint32_t)owner : 0u;   // (rows past the cluster's are never sent)
+                row_dst[m][h] = sR_addr + (uint32_t)(((int)rank * a.U + uo) * ldr * 4);
+                row_bar[m][h] = mapa_shared(bar_recv_addr, row_owner[m][h]);
             }
         // variational mode: the recurrent mask of each (unit = row, batch = column) value this thread emits, drawn once.
         // Bit 16 m + 4 (col / 8) + 2 h + e (e: column col + e) set = dropped; none set with the mode off.  Every
@@ -183,11 +150,7 @@ __global__ void __launch_bounds__(kRecThreads, 1) lstm_rec_bwd_kernel(RecBwdArgs
             const int bit = 16 * m + 4 * (col >> 3) + 2 * h;
             v0 *= ((rdrop >> bit) & 1u) ? 0.f : rscale;
             v1 *= ((rdrop >> (bit + 1)) & 1u) ? 0.f : rscale;
-            if (!push) {
-                float* dst = (float*)((uint8_t*)sD + row_dst[m][h]) + col;
-                dst[0] = v0;
-                dst[1] = v1;
-            } else if (row_ok[m][h]) {
+            if (row_ok[m][h]) {
                 // straight from the registers into the shared memory of the CTA that owns this unit
                 st_async_v2(mapa_shared(row_dst[m][h] + (uint32_t)col * 4u, row_owner[m][h]), v0, v1, row_bar[m][h]);
             }
@@ -217,16 +180,9 @@ __global__ void __launch_bounds__(kRecThreads, 1) lstm_rec_bwd_kernel(RecBwdArgs
             for (int q = 0; q < 4; ++q) bsum[k][q] = 0.f;
         }
         const uint64_t n_total = (uint64_t)T * B * H;
-        const uint32_t sD_addr = smem_u32(sD);
-        uint32_t part_addr[4];
-#pragma unroll
-        for (int rr = 0; rr < 4; ++rr) part_addr[rr] = mapa_shared(sD_addr, rr);   // (pull exchange: S == 1 only)
-        const uint32_t bar_part_addr = smem_u32(bar_part);
-        const uint32_t sR_addr = smem_u32(sR), bar_recv_addr = smem_u32(bar_recv);
         const uint32_t recv_bytes = (uint32_t)CS * (uint32_t)a.U * (uint32_t)Bp * 4u;   // CS sources x U units x Bp columns
         const float inv = 1.f / kGradScale;
         const size_t img_gate = (size_t)a.Kc * a.GBi * 64;
-        const bool push = S == 2 || a.push != 0;
 
         for (int s = 0; s < T; ++s) {
             const int t = T - 1 - s;
@@ -263,21 +219,10 @@ __global__ void __launch_bounds__(kRecThreads, 1) lstm_rec_bwd_kernel(RecBwdArgs
                 }
             }
             if (s > 0) {
-                if (push && tid == 0 && !dead) mbar_expect_tx(bar_recv, recv_bytes);
+                if (tid == 0 && !dead) mbar_expect_tx(bar_recv, recv_bytes);
                 bounded_mbar_wait(bar_mma, (s - 1) & 1, a.w, dead, kWaitAcc, s);
-                if (tr && tid == 0) trs[s * 8 + 3] = clock64();   // staged partial / my pushes are out
-                if (!push) {
-                    asm volatile("bar.sync 1, 256;" ::: "memory");
-                    if (tid < 4) mbar_arrive_remote_release(mapa_shared(bar_part_addr, tid));
-                    {   // wait until all four CTAs of the cluster staged their partials
-                        uint32_t n = 0; long long t0 = 0;
-                        while (!dead && !mbar_try_wait_acq_cluster(bar_part, (s - 1) & 1)) {
-                            if ((++n & 0xFFFu) == 0 && rec_spin_check(a.w, t0, kWaitPart, s)) dead = true;
-                        }
-                    }
-                } else {
-                    bounded_mbar_wait(bar_recv, (s - 1) & 1, a.w, dead, kWaitRecv, s);   // all CS x U x Bp partial sums of my units have landed
-                }
+                if (tr && tid == 0) trs[s * 8 + 3] = clock64();   // my pushes are out
+                bounded_mbar_wait(bar_recv, (s - 1) & 1, a.w, dead, kWaitRecv, s);   // all CS x U x Bp partial sums of my units have landed
                 if (tr && tid == 0) trs[s * 8 + 4] = clock64();
             }
             __half hv[kRecMaxCell][4];
@@ -288,14 +233,8 @@ __global__ void __launch_bounds__(kRecThreads, 1) lstm_rec_bwd_kernel(RecBwdArgs
                 float dh = dyv[k];
                 if (s > 0) {
                     float pp[CS];
-                    if (!push) {
-                        const uint32_t off = (uint32_t)(((int)rank * a.U + u) * ldd + b) * 4u;
-#pragma unroll             // issue all four DSMEM loads before the first use (each is ~200+ clk)
-                        for (int rr = 0; rr < 4; ++rr) pp[rr] = ld_dsmem_f32(part_addr[rr] + off);
-                    } else {
 #pragma unroll
-                        for (int rr = 0; rr < CS; ++rr) pp[rr] = sR[(rr * a.U + u) * ldr + b];
-                    }
+                    for (int rr = 0; rr < CS; ++rr) pp[rr] = sR[(rr * a.U + u) * ldr + b];
                     float r = (pp[0] + pp[1]) + (pp[2] + pp[3]);
                     if constexpr (S == 2) r += (pp[4] + pp[5]) + (pp[6] + pp[7]);
                     dh += r * inv;
@@ -356,9 +295,8 @@ __global__ void __launch_bounds__(kRecThreads, 1) lstm_rec_bwd_kernel(RecBwdArgs
             }
         }
         if (a.db1) {
-            // bias gradients: per-cell sums over the window -> a global scratch [4][B][H] (no shared-memory region of
-            // a guaranteed size is free: peers may still read the staging buffer) -> fixed-order sum over the batch by
-            // one thread per (gate, unit) of this CTA.  bar.sync orders the CTA's own global writes for its readers.
+            // bias gradients: per-cell sums over the window -> a global scratch [4][B][H] -> fixed-order sum over the
+            // batch by one thread per (gate, unit) of this CTA.  bar.sync orders the CTA's own global writes for its readers.
             // (ZO: nu and cells computed afresh from an opaque copy of U: held across the step loop, the two values
             // would be the zoneout epilogue's only spills)
             int nu_db = nu, cells_db = cells;
@@ -390,7 +328,7 @@ __global__ void __launch_bounds__(kRecThreads, 1) lstm_rec_bwd_kernel(RecBwdArgs
         }
     }
     __syncthreads();
-    cluster_sync_all();   // no CTA leaves while a peer may still read its staged partial
+    cluster_sync_all();   // no CTA leaves while a peer could still address its shared memory
     if (a.trace && threadIdx.x == 0) rec_launch_stamps(a.trace, tr, true);
 }
 

@@ -197,9 +197,8 @@ int rec_fwd_plan(int H, int B, RecPlan* plan) {
     plan->ok = 0;
     plan->KS = 1;
     if (plan->GB * 8 > 32) return ZRB_OK;  // accumulators / staging sized for N <= 32
-    static const bool no_split = getenv("ZRB_REC_NOSPLIT") != nullptr;   // A/B switch
     // K-split pairs (see the kernel header): image batch groups padded to an even count
-    if (!no_split && H >= 256) {
+    if (H >= 256) {
         const int Kp = (H + 31) / 32 * 32, Kc = Kp / 8, KcS = Kc / 2, GBi = (plan->GB + 1) / 2 * 2;
         // first choice: at most one (unit, batch) cell per epilogue thread -- a second pass of the cell loop for a handful
         // of cells doubles the critical path of that warp (measured: U = 13, 260 cells, was slower than U = 12)

@@ -36,7 +36,7 @@ static inline unsigned int rec_fault_base(const char* which) {
     static const char* fault = getenv("ZRB_FAULT_BARRIER_BASE");
     return (fault && !strcmp(fault, which)) ? 1u : 0u;
 }
-enum { kWaitWeights = 1, kWaitOperand = 2, kWaitAcc = 3, kWaitRecv = 4, kWaitGrid = 5, kWaitPart = 6 };
+enum { kWaitWeights = 1, kWaitOperand = 2, kWaitAcc = 3, kWaitRecv = 4, kWaitGrid = 5 };
 
 __device__ __forceinline__ unsigned int ld_relaxed_gpu(const unsigned int* p) {
     unsigned int v;

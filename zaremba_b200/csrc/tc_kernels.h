@@ -196,10 +196,6 @@ struct RecBwdArgs {
     float* db1;               // [4H] or null: bias gradient sum_{t,b} dG (model.py:35-36: b_ih and b_hh get the same
     float* db2;               //      gradient), accumulated in registers over the window and reduced over the batch here
     float* db_scratch;        // [4][B][H] fp32 scratch of that reduction (needed when db1 is set)
-    int push;                 // exchange of the cluster's partial products: 1 = st.async pushes into the owners' shared
-                              // memory (complete_tx on their mbarrier), 0 = stage + remote arrive + DSMEM pulls
-    unsigned int* res_flag;   // or null: CTA 0 publishes res_value here when the whole grid is resident
-    unsigned int res_value;
     unsigned int* counter;    // grid barrier: never reset, `base` is its value when this launch starts
     unsigned int base;
     int T, B, H, G4p, U, G, GB, Kc, nCTA;
@@ -211,9 +207,7 @@ struct RecBwdArgs {
     ZoneoutSrc zo;            // zoneout (zo.on: the zoneout instantiation; the forward's flags), appended like RecFwdArgs'
     const float* ctil;        // [N,H] c~_t of the forward (zo.on)
 };
-// Launch the backward recurrence with a's per-call fields; the launcher sets push and the plan's and the watchdog's
-// fields.  res_flag: a stream gated on it (cuStreamWaitValue32) can start work that must only take the SMs this kernel
-// leaves free (the data-parallel bucket all-reduce).
+// Launch the backward recurrence with a's per-call fields; the launcher sets the plan's and the watchdog's fields.
 int lstm_rec_bwd(const RecPlan& p, const RecWatchdog& wd, RecBwdArgs a, cudaStream_t s);
 
 }  // namespace zrb

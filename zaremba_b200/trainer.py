@@ -38,31 +38,6 @@ def minibatch(data, batch_size, seq_length):
     return out
 
 
-class _NullCtx:
-    def __enter__(self):
-        return None
-
-    def __exit__(self, *a):
-        return False
-
-
-class _SideStream:
-    """`with` block that runs on `side`, ordered after everything already on `cur`; `cur` then waits for it."""
-
-    def __init__(self, cur, side):
-        self.cur, self.side = cur, side
-        self.ctx = torch.cuda.stream(side)
-
-    def __enter__(self):
-        self.side.wait_stream(self.cur)
-        self.ctx.__enter__()
-
-    def __exit__(self, *a):
-        self.ctx.__exit__(*a)
-        self.cur.wait_stream(self.side)
-        return False
-
-
 class Trainer:
     def __init__(self, model: Model, batch_size: int, seq_length: int, process_group=None,
                  keep_clipped_grads: bool = False, data_parallel: bool = True, lazy_update: bool = False, *,
@@ -172,7 +147,6 @@ class Trainer:
         # (reducing finished buckets with NCCL underneath the rest of backward was removed: NCCL's channels evict part
         # of the persistent recurrence grid; the copy-engine transport is the one that overlaps)
         self._ctx_cached = None
-        self._step_stream = None
         _ = self.ctx
         # single process: the fused step owns the gradient buffers -> touch only the window's embedding rows and take
         # the matrices' clip norm from the wgrad epilogues (mode 1).  Data parallel with the sparse embedding exchange
@@ -339,26 +313,10 @@ class Trainer:
     def _stream(self):
         return torch.cuda.current_stream(self.dev).cuda_stream
 
-    def _own_stream(self):
-        """Optional (ZRB_OWN_STREAM=1): when the caller is on the legacy default stream, run the step on a stream of
-        the Trainer's own, ordered after the caller's stream and joined back into it afterwards.  Off by default:
-        programmatic dependent launches overlap on the legacy default stream as well (tools/micro/pdl_overlap.cu)
-        and the two event hops cost ~10 us per step."""
-        cur = torch.cuda.current_stream(self.dev)
-        if cur.cuda_stream != 0 or os.environ.get("ZRB_OWN_STREAM", "0") != "1":
-            return _NullCtx()
-        if self._step_stream is None:
-            self._step_stream = torch.cuda.Stream(device=self.dev)
-        return _SideStream(cur, self._step_stream)
-
     # ---- main.py:109-117 -----------------------------------------------------------------
     def train_step(self, x, y, lr, max_norm):
         """x, y: [T,B] int64 CUDA tensors (contiguous).  Returns (loss, norm) as 0-d CUDA
         tensors (no host sync)."""
-        with self._own_stream():
-            return self._train_step(x, y, lr, max_norm)
-
-    def _train_step(self, x, y, lr, max_norm):
         lib = _lib.load()
         T, B = x.shape
         self._check_not_swapped()
@@ -424,22 +382,18 @@ class Trainer:
         self._check_not_swapped()
         if self.world == 1:
             self._check_versions()
-            with self._own_stream():
-                return self._train_step_host1(lib, hx, hy, T, B, lr, max_norm)
+            _lib.check(lib.zrb_train_step_host(self.ctx, C.byref(self._ps), C.byref(self._gs),
+                                               C.c_void_p(hx.data_ptr()), C.c_void_p(hy.data_ptr()), T, B,
+                                               C.byref(self._st), C.byref(self._st), self.seed, self.step,
+                                               float(lr), float(max_norm), C.c_void_p(self._hloss.data_ptr()),
+                                               C.c_void_p(self._hloss.data_ptr() + 4), self._stream()))
+            self.step += 1
+            self._pending = True
+            return float(self._hloss[0]), float(self._hloss[1])
         xd = hx.to(self.dev, non_blocking=True); yd = hy.to(self.dev, non_blocking=True)
         loss, norm = self.train_step(xd, yd, lr, max_norm)
         both = torch.stack([loss, norm]).cpu()
         return float(both[0]), float(both[1])
-
-    def _train_step_host1(self, lib, hx, hy, T, B, lr, max_norm):
-        _lib.check(lib.zrb_train_step_host(self.ctx, C.byref(self._ps), C.byref(self._gs),
-                                           C.c_void_p(hx.data_ptr()), C.c_void_p(hy.data_ptr()), T, B,
-                                           C.byref(self._st), C.byref(self._st), self.seed, self.step,
-                                           float(lr), float(max_norm), C.c_void_p(self._hloss.data_ptr()),
-                                           C.c_void_p(self._hloss.data_ptr() + 4), self._stream()))
-        self.step += 1
-        self._pending = True
-        return float(self._hloss[0]), float(self._hloss[1])
 
     # ---- main.py:91-94 --------------------------------------------------------------------
     def eval_step(self, x, y, want_probs=False, cache=None, theta=0.0, lam=0.0):
