@@ -18,6 +18,7 @@ import torch
 
 from oracle import lstm_lm_oracle as O
 from tests._golden import GOLDEN
+from tests._rounded_oracle import rounded_operand_fwd
 
 MEDIUM = dict(V=10000, H=650, L=2, T=35, B=20, p=0.5, winit=0.05, lr=1.0, clip=5.0)    # bench.py CONFIGS["medium"]
 SMALL = dict(V=10000, H=200, L=2, T=20, B=20, p=0.0, winit=0.1, lr=1.0, clip=5.0)      # bench.py CONFIGS["small"]
@@ -293,27 +294,6 @@ def layer_unit(pt, T):
         h0, c0 = pt.states[l]
         out.update({f"l{l} {k}": v for k, v in layer_against_oracle(lib, ctx, W_ih, W_hh, b_ih, b_hh, x, h0, c0, dy).items()})
     return out
-
-
-def rounded_operand_fwd(x, h0, c0, W_ih, W_hh, b_ih, b_hh, h_dev):
-    """fp64 forward of one layer fed exactly what the tensor-core kernels multiply -- fp16-rounded x, W_ih, W_hh and
-    h_{t-1} -- with exact activations.  h_{t-1} is the DEVICE's h (h_dev [T,B,H]; h0 at t = 0), so that a rounding flip
-    of one fp16 h image cannot propagate: what remains between the device and this is fp32 accumulation and the
-    activation functions.  Returns y [T,B,H], c_T and the largest |pre-activation|."""
-    r = lambda a: np.asarray(a, dtype=np.float64).astype(np.float16).astype(np.float64)
-    T, B, H = x.shape
-    pre = r(x) @ r(W_ih).T + b_ih + b_hh
-    Wh = r(W_hh).T
-    c, h, ys, zmax = np.asarray(c0, dtype=np.float64), h0, [], 0.0
-    sig = lambda v: 1.0 / (1.0 + np.exp(-v))
-    for t in range(T):
-        z = pre[t] + r(h) @ Wh
-        zmax = max(zmax, float(np.abs(z).max()))
-        zi, zf, zg, zo = np.split(z, 4, axis=1)
-        c = sig(zf) * c + sig(zi) * np.tanh(zg)
-        ys.append(sig(zo) * np.tanh(c))
-        h = h_dev[t]
-    return np.stack(ys), c, zmax
 
 
 def layer_against_oracle(lib, ctx, W_ih, W_hh, b_ih, b_hh, x, h0, c0, dy):
