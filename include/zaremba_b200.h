@@ -320,6 +320,28 @@ int  zrb_average_count(const zrb_ctx* ctx, int64_t* n);
  * the average and swapping back would corrupt both).  ZRB_E_INVALID when n = 0 and when an average tensor overlaps p. */
 int  zrb_swap_average(zrb_ctx* ctx, const zrb_params* p, void* stream);
 
+/* Adam (Kingma & Ba 2015; DESIGN.md section 21 states it bit for bit).  Opt-in; off (the default, and m = NULL),
+ * nothing changes.  zrb_set_adam(ctx, m, v, beta1, beta2, eps, step) with m and v non-NULL (laid out like the
+ * parameters; tied: m->fc_w == m->embed_w, likewise v; a context with experts takes a zrb_mos_params base) makes every
+ * zrb_train_step_update (and zrb_train_step_host) apply Adam after the global-norm clip, in place of SGD.  step = the
+ * updates already applied, so the next is number t = step + 1; the context counts on.  Each update computes on the host,
+ * in double and rounded once to fp32, step_size = lr / (1 - beta1^t), bc2s = sqrt(1 - beta2^t), omb1 = 1 - beta1 and
+ * omb2 = 1 - beta2, then for every element of every parameter, with g' = coef * g (clip_grad_norm_'s scaled gradient)
+ * and every fp32 operation rounded on its own in this order:
+ *     m = beta1 * m + omb1 * g';  v = beta2 * v + omb2 * (g' * g');  denom = sqrt(v) / bc2s + eps;
+ *     p = p - step_size * (m / denom)
+ * (torch.optim.Adam with weight_decay = 0, amsgrad = False).  The embedding is updated densely (its moments decay in
+ * every row); the rows-only norm and gradient clearing of zrb_set_embed_sparse stay.  g' is stored back as by SGD when
+ * zrb_set_keep_clipped_grads is on.  Under lazy update the deferred matrices apply the scalars of their own step (a tied
+ * E is applied at once).  zrb_clip_sgd, zrb_dyneval_step, the gradient statistics and every eval call leave m, v and t
+ * alone.  Pending lazy updates are applied first (on the legacy default stream).  ZRB_E_INVALID, before anything is
+ * launched, for beta1 or beta2 outside [0, 1) or not finite, eps <= 0 or not finite, step < 0, exactly one of m and v,
+ * a NULL tensor, moment tensors that overlap each other, an untied pair in a tied context, and while averaging is on or
+ * swapped; zrb_set_average refuses to start while Adam is on; zrb_train_step_update returns ZRB_E_INVALID when a
+ * moment tensor overlaps a parameter or gradient it was given. */
+int  zrb_set_adam(zrb_ctx* ctx, const zrb_params* m, const zrb_params* v, float beta1, float beta2, float eps,
+                  int64_t step);
+
 /* Watchdog of the persistent recurrence kernels.  Every wait inside them is bounded (~3 s; ZRB_SPIN_CYCLES overrides).  A
  * wait that runs out -- a lost wake-up, or a grid that never became co-resident -- does not trap: the kernel stops
  * waiting everywhere, finishes with garbage in its outputs and leaves a code in a host-mapped word.  The next call on

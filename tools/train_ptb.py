@@ -82,6 +82,12 @@ ap.add_argument("--nonmono", type=int, default=5,
                      "of all but the last NONMONO")
 ap.add_argument("--asgd_from", type=int, default=None,
                 help="start averaging at the start of this epoch (1-based), whatever validation does")
+ap.add_argument("--optimizer", choices=["sgd", "adam"], default="sgd",
+                help="adam: torch.optim.Adam after the clip, in place of SGD (DESIGN.md section 21); --learning_rate is "
+                     "its lr and the schedule divides it as it divides SGD's.  --impl cudnn runs torch.optim.Adam(fused=True)")
+ap.add_argument("--beta1", type=float, default=0.9, help="--optimizer adam: beta1 (Melis et al. 2018 use 0)")
+ap.add_argument("--beta2", type=float, default=0.999, help="--optimizer adam: beta2")
+ap.add_argument("--adam_eps", type=float, default=1e-8, help="--optimizer adam: eps (Melis et al. 2018 use 1e-9)")
 ap.add_argument("--lazy_update", action="store_true",
                 help="Trainer(lazy_update=True): upper-layer / fc weight updates run beside the next step's forward")
 ap.add_argument("--eval_batch_size", type=int, default=None,
@@ -148,7 +154,10 @@ if args.impl == "ours":
                                embed_size=args.embed_size, layer_sizes=args.layer_sizes, experts=args.experts,
                                mos_dropout=args.mos_dropout, zoneout_cell=args.zoneout_cell,
                                zoneout_hidden=args.zoneout_hidden).to(dev)
-    tr = zaremba_b200.Trainer(model, B, T, lazy_update=args.lazy_update, ar=args.ar, tar=args.tar)
+    if args.optimizer == "adam" and (args.asgd or args.asgd_from is not None):
+        raise SystemExit("--asgd / --asgd_from average SGD iterates: not with --optimizer adam")
+    tr = zaremba_b200.Trainer(model, B, T, lazy_update=args.lazy_update, ar=args.ar, tar=args.tar,
+                              optimizer=args.optimizer, betas=(args.beta1, args.beta2), eps=args.adam_eps)
     # the corpus is staged on the device once (SURVEY 8f#2): 3 x [n_batches, T, B] int64
     trn_x = torch.stack([x for x, _ in trn_b]).contiguous().to(dev)
     trn_y = torch.stack([y for _, y in trn_b]).contiguous().to(dev)
@@ -196,13 +205,31 @@ else:
     from oracle import torch_port as P
     model = P.TorchLstmLm(vocab, args.hidden_size, args.layer_num, args.dropout, args.winit).to(dev)
     trn_d = [(x.to(dev), y.to(dev)) for x, y in trn_b]
+    adam = (torch.optim.Adam(model.parameters(), lr=args.learning_rate, betas=(args.beta1, args.beta2),
+                             eps=args.adam_eps, fused=True) if args.optimizer == "adam" else None)
+
+    def adam_step(x, y, states, lr):
+        """main.py:109-117 with torch.optim.Adam in place of the SGD loop"""
+        adam.zero_grad(set_to_none=True)
+        states = [(h.detach(), c.detach()) for h, c in states]
+        logits, states = model(x, states)
+        loss = P.softmax_nll_times_batch(logits, y)
+        loss.backward()
+        norm = torch.nn.utils.clip_grad_norm_(model.parameters(), args.max_grad_norm)
+        for g in adam.param_groups:
+            g["lr"] = lr
+        adam.step()
+        return loss, norm, states
 
     def train_epoch(lr, log):
         model.train()
         states = model.zero_state(B)
         every = max(1, len(trn_b) // 10)
         for i, (x, y) in enumerate(trn_d):
-            loss, norm, states = P.train_step(model, x, y, states, lr, args.max_grad_norm)
+            if adam is not None:
+                loss, norm, states = adam_step(x, y, states, lr)
+            else:
+                loss, norm, states = P.train_step(model, x, y, states, lr, args.max_grad_norm)
             if i % every == 0:
                 log(i, loss.item(), float(norm))
 

@@ -120,6 +120,8 @@ _SIGNATURES = {
     "zrb_set_average": (C.c_int, [_vp, C.POINTER(ZrbParams)]),
     "zrb_average_count": (C.c_int, [_vp, C.POINTER(C.c_int64)]),
     "zrb_swap_average": (C.c_int, [_vp, C.POINTER(ZrbParams), _vp]),
+    "zrb_set_adam": (C.c_int, [_vp, C.POINTER(ZrbParams), C.POINTER(ZrbParams), C.c_float, C.c_float, C.c_float,
+                               C.c_int64]),
     "zrb_check_health": (C.c_int, [_vp]),
     "zrb_rec_plans": (C.c_int, [_vp, _vp]),
     "zrb_rec_plans_layer": (C.c_int, [_vp, C.c_int32, _vp]),

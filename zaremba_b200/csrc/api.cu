@@ -1,6 +1,7 @@
 // C ABI of libzaremba_b200.so: context, orchestration of the forward / backward / loss /
 // update kernels.  See include/zaremba_b200.h for the contract of every entry point.
 #include <math.h>
+#include <cmath>
 #include <stdarg.h>
 #include <string.h>
 
@@ -513,6 +514,16 @@ static int check_avg_alias(const TensorList& ta, const TensorList& tl, bool with
     return ZRB_OK;
 }
 
+// ZRB_E_INVALID when a moment tensor (tm.p) overlaps a parameter or gradient of `tl`
+static int check_moment_alias(const TensorList& tm, const TensorList& tl) {
+    for (int i = 0; i < tm.count; ++i)
+        for (int j = 0; j < tl.count; ++j)
+            ZRB_REQUIRE(!ranges_overlap(tm.p[i], tm.n[i], tl.p[j], tl.n[j]) &&
+                            !ranges_overlap(tm.p[i], tm.n[i], tl.g[j], tl.n[j]),
+                        "moment tensor %d overlaps a parameter or gradient tensor %d", i, j);
+    return ZRB_OK;
+}
+
 static int check_not_swapped(const zrb_ctx* c) {
     ZRB_REQUIRE(!c->avg_swapped, "the parameters hold the average (zrb_swap_average): swap back before training");
     return ZRB_OK;
@@ -521,6 +532,7 @@ static int check_not_swapped(const zrb_ctx* c) {
 int zrb_set_average(zrb_ctx* c, const zrb_params* avg) {
     ZRB_REQUIRE(c, "null ctx");
     ZRB_REQUIRE(!c->avg_swapped, "the parameters hold the average (zrb_swap_average): swap back first");
+    ZRB_REQUIRE(!avg || !c->adam_on, "iterate averaging is an SGD scheme: switch Adam off (zrb_set_adam) first");
     if (avg) {
         ZRB_REQUIRE(avg->embed_w && avg->fc_w && avg->fc_b, "null average tensor");
         ZRB_REQUIRE(!c->experts || (mos_of(avg)->prior_w && mos_of(avg)->latent_w && mos_of(avg)->latent_b),
@@ -538,6 +550,56 @@ int zrb_set_average(zrb_ctx* c, const zrb_params* avg) {
     c->avg_on = avg != nullptr;
     if (avg) memcpy(&c->avg, avg, c->experts ? sizeof(zrb_mos_params) : sizeof(zrb_params));
     c->avg_n = 0;
+    return ZRB_OK;
+}
+
+// ---- Adam (DESIGN.md section 21) -------------------------------------------------------------------------------------
+// every tensor of a zrb_params (with the head's in a context with experts) is non-null
+static int check_complete(const zrb_ctx* c, const zrb_params* p, const char* what) {
+    ZRB_REQUIRE(p->embed_w && p->fc_w && p->fc_b, "null %s tensor", what);
+    ZRB_REQUIRE(!c->experts || (mos_of(p)->prior_w && mos_of(p)->latent_w && mos_of(p)->latent_b),
+                "null %s tensor of the Mixture-of-Softmaxes head", what);
+    for (int l = 0; l < c->cfg.layers; ++l)
+        ZRB_REQUIRE(p->w_ih[l] && p->w_hh[l] && p->b_ih[l] && p->b_hh[l], "null %s tensor of layer %d", what, l);
+    return ZRB_OK;
+}
+
+int zrb_set_adam(zrb_ctx* c, const zrb_params* m, const zrb_params* v, float beta1, float beta2, float eps,
+                 int64_t step) {
+    ZRB_REQUIRE(c, "null ctx");
+    ZRB_REQUIRE(!c->avg_swapped, "the parameters hold the average (zrb_swap_average): swap back first");
+    ZRB_REQUIRE(!m == !v, "give both moment tensors m and v, or neither");
+    if (m) {
+        ZRB_REQUIRE(!c->avg_on, "iterate averaging is an SGD scheme: stop it (zrb_set_average(ctx, NULL)) first");
+        ZRB_REQUIRE(std::isfinite(beta1) && beta1 >= 0.f && beta1 < 1.f, "beta1 = %g outside [0, 1)", (double)beta1);
+        ZRB_REQUIRE(std::isfinite(beta2) && beta2 >= 0.f && beta2 < 1.f, "beta2 = %g outside [0, 1)", (double)beta2);
+        ZRB_REQUIRE(std::isfinite(eps) && eps > 0.f, "eps = %g must be finite and > 0", (double)eps);
+        ZRB_REQUIRE(step >= 0, "step = %lld must be >= 0", (long long)step);
+        ZRB_TRY(check_complete(c, m, "first-moment"));
+        ZRB_TRY(check_complete(c, v, "second-moment"));
+        ZRB_TRY(check_tied(c, m));
+        ZRB_TRY(check_tied(c, v));
+        const TensorList tm = param_list(c, m, v);   // p: the first moments, g: the second
+        for (int i = 0; i < tm.count; ++i)
+            for (int j = 0; j < tm.count; ++j) {
+                ZRB_REQUIRE(j <= i || !ranges_overlap(tm.p[i], tm.n[i], tm.p[j], tm.n[j]),
+                            "first-moment tensors %d and %d overlap", i, j);
+                ZRB_REQUIRE(j <= i || !ranges_overlap(tm.g[i], tm.n[i], tm.g[j], tm.n[j]),
+                            "second-moment tensors %d and %d overlap", i, j);
+                ZRB_REQUIRE(!ranges_overlap(tm.p[i], tm.n[i], tm.g[j], tm.n[j]),
+                            "first-moment tensor %d overlaps second-moment tensor %d", i, j);
+            }
+    }
+    // deferred updates belong to the steps before: they apply the rule (and the t) they were issued with
+    if (c->cfg.engine == ZRB_ENGINE_TC) ZRB_TRY(tc_flush_updates(c, nullptr));
+    c->adam_on = m != nullptr;
+    if (m) {
+        const size_t sz = c->experts ? sizeof(zrb_mos_params) : sizeof(zrb_params);
+        memcpy(&c->adam_m, m, sz);
+        memcpy(&c->adam_v, v, sz);
+        c->adam_b1 = beta1; c->adam_b2 = beta2; c->adam_eps = eps;
+        c->adam_t = step;
+    }
     return ZRB_OK;
 }
 
@@ -732,11 +794,32 @@ int zrb_train_step_update(zrb_ctx* c, const zrb_params* p, const zrb_params* g, 
         as.first = c->avg_n == 0;
         avg = &as;
     }
+    // Adam: this update is number t = adam_t + 1; each scalar computed in double and rounded once to fp32
+    AdamStep ad{};
+    const AdamStep* adam = nullptr;
+    if (c->adam_on) {
+        const TensorList tm = param_list(c, &c->adam_m.base, &c->adam_v.base);
+        TensorList tv = tm;
+        for (int i = 0; i < tm.count; ++i) tv.p[i] = tm.g[i];
+        ZRB_TRY(check_moment_alias(tm, tl));
+        ZRB_TRY(check_moment_alias(tv, tl));
+        for (int i = 0; i < tm.count; ++i) { ad.m[i] = tm.p[i]; ad.v[i] = tm.g[i]; }
+        const double b1 = c->adam_b1, b2 = c->adam_b2, t = (double)(c->adam_t + 1);
+        ad.k.beta1 = c->adam_b1; ad.k.beta2 = c->adam_b2; ad.k.eps = c->adam_eps;
+        ad.k.omb1 = (float)(1.0 - b1);
+        ad.k.omb2 = (float)(1.0 - b2);
+        ad.k.step_size = (float)((double)lr / (1.0 - std::pow(b1, t)));
+        ad.k.bc2s = (float)std::sqrt(1.0 - std::pow(b2, t));
+        adam = &ad;
+    }
     if (c->cfg.engine == ZRB_ENGINE_TC) {
-        ZRB_TRY(tc_update(c, p, tl, lr, max_norm, norm_out, avg, s));
+        ZRB_TRY(tc_update(c, p, tl, lr, max_norm, norm_out, avg, adam, s));
     } else {
         ProfScope ps(c, ZRB_PROF_CLIP_SGD, s);
-        if (avg) {
+        if (adam) {
+            ZRB_TRY(grad_norm(tl, max_norm, c->partials, c->scalars, norm_out, s));
+            ZRB_TRY(adam_apply(tl, *adam, c->scalars, c->keep_clipped, s));
+        } else if (avg) {
             ZRB_TRY(grad_norm(tl, max_norm, c->partials, c->scalars, norm_out, s));
             ZRB_TRY(sgd_avg_apply(tl, avg->a, lr, c->scalars, c->keep_clipped, avg->mu, avg->first, s));
         } else {
@@ -745,6 +828,7 @@ int zrb_train_step_update(zrb_ctx* c, const zrb_params* p, const zrb_params* g, 
         c->weights_version++;
     }
     if (avg) c->avg_n++;
+    if (adam) c->adam_t++;
     return ZRB_OK;
 }
 

@@ -25,7 +25,8 @@ struct AvgRule : SgdRule {
     template <int VEC> __device__ __forceinline__ void load(int64_t off, int e, Tile<VEC>& t) const {
         load_vec<VEC>(a + off, t.v[e]);
     }
-    template <int VEC> __device__ __forceinline__ void finish(int e, const float (&pv)[VEC], Tile<VEC>& t) const {
+    template <int VEC>
+    __device__ __forceinline__ void finish(int e, float (&pv)[VEC], float (&)[VEC], Tile<VEC>& t) const {
 #pragma unroll
         for (int x = 0; x < VEC; ++x) t.v[e][x] = avg_elem(t.v[e][x], pv[x], mu, first);
     }

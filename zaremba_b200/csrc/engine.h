@@ -70,6 +70,10 @@ struct zrb_ctx {
     zrb_mos_params avg{};                  // (the head tensors only in a context with experts)
     int64_t avg_n = 0;                     // train-step updates averaged so far
     bool avg_swapped = false;              // zrb_swap_average: the parameters hold the average
+    bool adam_on = false;                  // zrb_set_adam: Adam in place of SGD, moments in adam_m / adam_v (section 21)
+    zrb_mos_params adam_m{}, adam_v{};     // (the head tensors only in a context with experts)
+    float adam_b1 = 0.f, adam_b2 = 0.f, adam_eps = 0.f;
+    int64_t adam_t = 0;                    // updates applied so far: the next train-step update is number adam_t + 1
     float* bwd_dy = nullptr;               // phased backward: grad wrt the next layer's output / scratch
     float* bwd_dx = nullptr;
     int bwd_next_layer = -1;
@@ -164,7 +168,7 @@ int tc_layer_fwd(zrb_ctx* c, const float* w_ih, const float* w_hh, const float* 
 int tc_layer_bwd(zrb_ctx* c, const float* dy, float* dx, float* dw_ih, float* dw_hh, float* db_ih, float* db_hh,
                  cudaStream_t s);   // the persistent backward recurrence kernel is in use for this context
 int tc_update(zrb_ctx* c, const zrb_params* p, const TensorList& tl, float lr, float max_norm, float* norm_out,
-              const AvgStep* avg, cudaStream_t s);
+              const AvgStep* avg, const AdamStep* adam, cudaStream_t s);
 // iterate averaging (DESIGN.md section 16): exchange the tensors of tl (param_list() over p) with a, images rebuilt
 int tc_swap_average(zrb_ctx* c, const zrb_params* p, const TensorList& tl, float* const* a, cudaStream_t s);
 // dynamic evaluation (DESIGN.md section 14): eval-mode gradients, and the update with the dynamic rule

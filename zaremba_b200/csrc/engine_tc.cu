@@ -61,6 +61,8 @@ struct zrb_tc_state {
     zrb::TensorList upd_tl{};
     bool upd_avg_on = false;      // ... and averaged with upd_avg, the average step of that train step (section 16)
     zrb::AvgStep upd_avg{};
+    bool upd_adam_on = false;     // ... or under Adam with upd_adam, the moments and scalars of that step (section 21)
+    zrb::AdamStep upd_adam{};
     bool in_train_step = false;   // tc_forward is running as the first half of a fused train step
     float* colsum_scratch = nullptr;   // row-split partials of the bias-gradient column sums
     int64_t packed_version = 0;
@@ -412,15 +414,18 @@ static void tc_images_current(zrb_ctx* c, const zrb_params* p) {
 }
 
 // The train step's update of one matrix: update_pack, or with iterate averaging on (avg non-null) update_pack_avg,
-// which also averages the new p into a (DESIGN.md section 16).  Both rebuild the matrix's fp16 images from registers, so
-// the next forward needs no pack.  The exception is W_hh in the weight-drop mode: p (and g) only, and the next forward
-// packs the images with its own mask.
+// which also averages the new p into a (DESIGN.md section 16), or under Adam (adam non-null) update_pack_adam (section
+// 21).  All rebuild the matrix's fp16 images from registers, so the next forward needs no pack.  The exception is W_hh
+// in the weight-drop mode: p (and g) only, and the next forward packs the images with its own mask.
 static int tc_update_matrix(zrb_ctx* c, const WeightMatrix& m, const TensorList& tl, float lr, const AvgStep* avg,
-                            bool pdl, cudaStream_t s) {
+                            const AdamStep* adam, bool pdl, cudaStream_t s) {
     zrb_tc_state::WhhImage whh;
     if (c->p_wd > 0.f) whh.kind = zrb_tc_state::kWhhStale;
     const WeightImages img = tc_images(c, m, whh);
     float *p = tl.p[m.i], *g = tl.g[m.i];
+    if (adam)
+        return update_pack_adam(p, g, adam->m[m.i], adam->v[m.i], adam->k, m.rows, m.cols, c->scalars, img,
+                                c->keep_clipped, s, pdl);
     if (!avg) return update_pack(p, g, m.rows, m.cols, lr, c->scalars, img, c->keep_clipped, s, pdl);
     return update_pack_avg(p, g, avg->a[m.i], avg->mu, avg->first, m.rows, m.cols, lr, c->scalars, img, c->keep_clipped,
                            s, pdl);
@@ -433,8 +438,9 @@ static int tc_issue_update(zrb_ctx* c, int item, bool pdl, cudaStream_t s) {
     if (!(t->upd_pending & (1u << item))) return ZRB_OK;
     t->upd_pending &= ~(1u << item);
     const AvgStep* avg = t->upd_avg_on ? &t->upd_avg : nullptr;
+    const AdamStep* adam = t->upd_adam_on ? &t->upd_adam : nullptr;
     for (const WeightMatrix& m : tc_matrices(c))
-        if (m.item == item) ZRB_TRY(tc_update_matrix(c, m, t->upd_tl, t->upd_lr, avg, pdl, s));
+        if (m.item == item) ZRB_TRY(tc_update_matrix(c, m, t->upd_tl, t->upd_lr, avg, adam, pdl, s));
     return ZRB_OK;
 }
 
@@ -1001,15 +1007,20 @@ int tc_rec_trace(zrb_ctx* c, long long* h_out, int max_entries) {
 
 // clip + SGD (main.py:114-117).  The update pass also writes the fp16 operand images of the new weights,
 // so the next forward needs no pack pass.  avg (or null): iterate averaging, every tensor's new value averaged into
-// avg->a[i] in the same passes (DESIGN.md section 16).
+// avg->a[i] in the same passes (DESIGN.md section 16).  adam (or null; never with avg): Adam in place of SGD, with the
+// moments in the same passes (section 21).  Adam updates the embedding densely: its moments decay in every row.
 int tc_update(zrb_ctx* c, const zrb_params* p, const TensorList& tl, float lr, float max_norm, float* norm_out,
-              const AvgStep* avg, cudaStream_t s) {
+              const AvgStep* avg, const AdamStep* adam, cudaStream_t s) {
     zrb_tc_state* t = c->tc;
-    const int E = c->width[0], V = c->cfg.vocab;
+    const int E = c->width[0], V = c->cfg.vocab, L = c->cfg.layers;
     ZRB_TRY(tc_flush_updates(c, s));   // (a second update without a forward in between)
     ProfScope ps(c, ZRB_PROF_CLIP_SGD, s);
-    if (!tc_streams_aligned(tl, avg ? avg->a : nullptr)) {   // images rebuilt by the next forward's pack
-        if (avg) {
+    if (!tc_streams_aligned(tl, avg ? avg->a : adam ? adam->m : nullptr, adam ? adam->v : nullptr)) {
+        // images rebuilt by the next forward's pack
+        if (adam) {
+            ZRB_TRY(grad_norm(tl, max_norm, c->partials, c->scalars, norm_out, s));
+            ZRB_TRY(adam_apply(tl, *adam, c->scalars, c->keep_clipped, s));
+        } else if (avg) {
             ZRB_TRY(grad_norm(tl, max_norm, c->partials, c->scalars, norm_out, s));
             ZRB_TRY(sgd_avg_apply(tl, avg->a, lr, c->scalars, c->keep_clipped, avg->mu, avg->first, s));
         } else {
@@ -1023,7 +1034,7 @@ int tc_update(zrb_ctx* c, const zrb_params* p, const TensorList& tl, float lr, f
     // gemm_norm: the matrices' sums of squares are in the wgrad epilogue slots: no read of their gradients
     const bool gemm_norm = t->wg_ok && t->wg_key == tl.g[tc_matrices(c).fc_w().i];
     TensorList rest = tc_without_matrices(c, tl);   // what the list kernel updates ...
-    if (rows_only) rest.n[0] = 0;
+    if (rows_only && !adam) rest.n[0] = 0;
     TensorList dense = gemm_norm ? rest : tl;       // ... and what the norm reads
     if (rows_only) dense.n[0] = 0;
     if (c->tied && gemm_norm) {
@@ -1034,8 +1045,9 @@ int tc_update(zrb_ctx* c, const zrb_params* p, const TensorList& tl, float lr, f
         ZRB_TRY(embed_rows_sumsq(tl.g[0], c->emb_prev_ids, c->emb_first, c->emb_prev_n, E, V,
                                  c->partials + norm_partials_base(), kNormExtra, s));   // one token per block
         ZRB_TRY(grad_norm(dense, max_norm, c->partials, c->scalars, norm_out, s, true, gemm_norm ? t->wg_slots : 0));
-        ZRB_TRY(embed_rows_update(tl.p[0], tl.g[0], c->emb_prev_ids, c->emb_first, c->emb_prev_n, E, V, lr, c->scalars,
-                                  c->keep_clipped, s));
+        if (!adam)
+            ZRB_TRY(embed_rows_update(tl.p[0], tl.g[0], c->emb_prev_ids, c->emb_first, c->emb_prev_n, E, V, lr,
+                                      c->scalars, c->keep_clipped, s));
         if (avg) {   // the average is dense: every row moves toward the new embedding
             TensorList e{};
             e.p[0] = tl.p[0]; e.n[0] = tl.n[0]; e.count = 1;
@@ -1052,12 +1064,17 @@ int tc_update(zrb_ctx* c, const zrb_params* p, const TensorList& tl, float lr, f
         t->upd_lr = lr;
         t->upd_avg_on = avg != nullptr;
         if (avg) t->upd_avg = *avg;
+        t->upd_adam_on = adam != nullptr;
+        if (adam) t->upd_adam = *adam;
     }
     for (const WeightMatrix& m : tc_matrices(c)) {
-        if (lazy && m.item >= 1) t->upd_pending |= 1u << m.item;
-        else ZRB_TRY(tc_update_matrix(c, m, tl, lr, avg, false, s));
+        // a tied E under Adam is never deferred: the next forward's gather through a pending update (tc_forward) knows
+        // only the SGD rule
+        if (lazy && m.item >= 1 && !(adam && c->tied && m.item == L)) t->upd_pending |= 1u << m.item;
+        else ZRB_TRY(tc_update_matrix(c, m, tl, lr, avg, adam, false, s));
     }
-    if (avg) ZRB_TRY(sgd_avg_apply(rest, avg->a, lr, c->scalars, c->keep_clipped, avg->mu, avg->first, s));
+    if (adam) ZRB_TRY(adam_apply(rest, *adam, c->scalars, c->keep_clipped, s));
+    else if (avg) ZRB_TRY(sgd_avg_apply(rest, avg->a, lr, c->scalars, c->keep_clipped, avg->mu, avg->first, s));
     else ZRB_TRY(sgd_apply(rest, lr, c->scalars, c->keep_clipped, s));
     tc_images_current(c, p);
     return ZRB_OK;

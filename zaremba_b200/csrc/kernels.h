@@ -108,6 +108,25 @@ int avg_apply(const TensorList& tl, float* const* a, float mu, bool first, cudaS
 // exchange tl.p[i] and a[i] element by element
 int swap_apply(const TensorList& tl, float* const* a, cudaStream_t s);
 
+// ---- adam_tc.cu: Adam (DESIGN.md section 21) -------------------------------------------------------------------------
+// The per-step scalars of update t, each computed in double on the host and rounded once to fp32
+struct AdamScalars {
+    float beta1, beta2;
+    float omb1, omb2;    // 1 - beta1, 1 - beta2
+    float eps;
+    float step_size;     // lr / (1 - beta1^t)
+    float bc2s;          // sqrt(1 - beta2^t)
+};
+// One train-step update under Adam: m[i], v[i] are tl.p[i]'s moments (param_list() order)
+struct AdamStep {
+    float* m[kMaxTensors];
+    float* v[kMaxTensors];
+    AdamScalars k;
+};
+// g' = scalars[1] * g, then Adam's element rule over every tensor of tl (zero-length entries skipped); g' stored back
+// when write_g
+int adam_apply(const TensorList& tl, const AdamStep& a, const float* scalars, bool write_g, cudaStream_t s);
+
 // ---- sample.cu ---------------------------------------------------------------------------
 // ZRB_E_INVALID for the arguments zrb_sample rejects (checked before anything is enqueued)
 int sample_check(const zrb_sampling* cfg, int B, int V);

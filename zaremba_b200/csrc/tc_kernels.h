@@ -180,6 +180,10 @@ int update_pack_dyn(float* p, float* g, const float* tg, const float* r, int row
 // over the new p in the same pass; the same images
 int update_pack_avg(float* p, float* g, float* a, float mu, bool first, int rows, int cols, float lr,
                     const float* scalars, const WeightImages& img, bool write_g, cudaStream_t s, bool pdl = false);
+// Adam (adam_tc.cu, DESIGN.md section 21): adam_apply's element rule with the moments m and v at p's offsets, in place of
+// update_pack's SGD; the same images
+int update_pack_adam(float* p, float* g, float* m, float* v, const AdamScalars& k, int rows, int cols,
+                     const float* scalars, const WeightImages& img, bool write_g, cudaStream_t s, bool pdl = false);
 // exchange p and a, and write the images of the new p (update_pack's image stores)
 int swap_pack(float* p, float* a, int rows, int cols, const WeightImages& img, cudaStream_t s);
 int rec_bwd_plan(int H, int B, RecPlan* plan);   // U = units per CTA, nCTA = 4 * clusters

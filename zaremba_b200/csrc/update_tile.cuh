@@ -1,7 +1,7 @@
 // The tile kernels of the fused weight update: each thread updates a tile of 8 rows of one matrix with a rule (SGD,
-// dynamic evaluation, SGD + iterate averaging, the average swap) and writes the fp16 operand images of the new weights
-// from registers.  Shared by optim_tc.cu (SgdRule, DynRule) and average_tc.cu (AvgRule, SwapRule); every translation
-// unit instantiates the kernels of its own rules.
+// dynamic evaluation, SGD + iterate averaging, the average swap, Adam) and writes the fp16 operand images of the new
+// weights from registers.  Shared by optim_tc.cu (SgdRule, DynRule), average_tc.cu (AvgRule, SwapRule) and adam_tc.cu
+// (AdamRule); every translation unit instantiates the kernels of its own rules.
 #pragma once
 #include "tc_kernels.h"
 
@@ -87,14 +87,14 @@ __device__ __forceinline__ void store_vec(float* p, const float (&v)[VEC]) {
 constexpr int kTileRows = 8;
 constexpr int kUpdThreads = 128;
 
-// A rule is init(), apply(off, p row, g row) (the new p, and g as the kernel may store it), and three hooks for a
-// stream of its own that the kernel stores (iterate averaging): load(off, e, tile) with the tile's loads,
-// finish(e, new p row, tile) after apply, store(off, e, tile) after the tile's p / g stores.  A rule without such a
-// stream derives from NoTileRule.
+// A rule is init(), apply(off, p row, g row) (the new p, and g as the kernel may store it), and three hooks for
+// streams of its own that the kernel stores (iterate averaging, Adam's moments): load(off, e, tile) with the tile's
+// loads, finish(e, p row, g row, tile) after apply (it may still change p and g: Adam's update needs the tile),
+// store(off, e, tile) after the tile's p / g stores.  A rule without such a stream derives from NoTileRule.
 struct NoTileRule {
     template <int VEC> struct Tile {};
     template <int VEC> __device__ __forceinline__ void load(int64_t, int, Tile<VEC>&) const {}
-    template <int VEC> __device__ __forceinline__ void finish(int, const float (&)[VEC], Tile<VEC>&) const {}
+    template <int VEC> __device__ __forceinline__ void finish(int, float (&)[VEC], float (&)[VEC], Tile<VEC>&) const {}
     template <int VEC> __device__ __forceinline__ void store(int64_t, int, const Tile<VEC>&) const {}
 };
 
@@ -131,7 +131,7 @@ __device__ __forceinline__ void tile_update(const float* __restrict__ p, const f
     for (int e = 0; e < kTileRows; ++e) {
         if (e < n) {
             rule.template apply<VEC>(off + (int64_t)e * stride, pv[e], gv[e]);
-            rule.template finish<VEC>(e, pv[e], tile);
+            rule.template finish<VEC>(e, pv[e], gv[e], tile);
         }
     }
 }

@@ -38,10 +38,73 @@ def minibatch(data, batch_size, seq_length):
     return out
 
 
+def _adam_hyper(betas, eps):
+    """(betas, eps) as floats, ValueError outside torch.optim.Adam's domain of the fused rule: 0 <= beta < 1, eps > 0."""
+    try:
+        b1, b2 = (float(b) for b in betas)
+        eps = float(eps)
+    except (TypeError, ValueError):
+        raise ValueError(f"betas must be two numbers and eps a number, got {betas!r}, {eps!r}") from None
+    for name, b in (("beta1", b1), ("beta2", b2)):
+        if not (math.isfinite(b) and 0.0 <= b < 1.0):
+            raise ValueError(f"{name} must be in [0, 1), got {b!r}")
+    if not (math.isfinite(eps) and eps > 0.0):
+        raise ValueError(f"eps must be finite and > 0, got {eps!r}")
+    return (b1, b2), eps
+
+
+def adam_state_to_torch(flat_m, flat_v, step, layout, lr, betas, eps):
+    """torch.optim.Adam's state_dict() from flat moments: layout = [(state index, shape, offset into the flat
+    buffers)].  Per index `step` (a float tensor, as torch keeps it), `exp_avg` and `exp_avg_sq` (copies); no state
+    before the first step, as a fresh torch.optim.Adam has none."""
+    state = {}
+    if step > 0:
+        for i, shape, off in layout:
+            n = math.prod(shape)
+            state[i] = {"step": torch.tensor(float(step)), "exp_avg": flat_m[off:off + n].view(shape).clone(),
+                        "exp_avg_sq": flat_v[off:off + n].view(shape).clone()}
+    group = {"lr": float(lr), "betas": tuple(betas), "eps": float(eps), "weight_decay": 0, "amsgrad": False,
+             "maximize": False, "foreach": None, "capturable": False, "differentiable": False, "fused": None,
+             "decoupled_weight_decay": False, "params": [i for i, _, _ in layout]}
+    return {"state": state, "param_groups": [group]}
+
+
+def adam_state_from_torch(sd, layout, flat_m, flat_v):
+    """The inverse of adam_state_to_torch: copies the moments into flat_m / flat_v (zeros for an empty state) and
+    returns (step, betas, eps, lr).  ValueError unless sd has one param group over the layout's indices in order, with
+    weight_decay, amsgrad and maximize off, and a state for every parameter with one common step, or none at all."""
+    groups = sd.get("param_groups", [])
+    if len(groups) != 1 or list(groups[0]["params"]) != [i for i, _, _ in layout]:
+        raise ValueError("expected one param group over model.parameters() in order")
+    g = groups[0]
+    if g.get("weight_decay", 0) or g.get("amsgrad", False) or g.get("maximize", False):
+        raise ValueError("weight_decay, amsgrad and maximize are not part of the fused Adam")
+    betas, eps = _adam_hyper(tuple(g["betas"]), g["eps"])
+    state = sd.get("state", {})
+    steps = {float(st["step"]) for st in state.values()}
+    if state and (set(state) != {i for i, _, _ in layout} or len(steps) != 1):
+        raise ValueError("every parameter needs a state, all with one common step")
+    step = steps.pop() if state else 0.0
+    if step != int(step) or step < 0:
+        raise ValueError(f"step must be a whole number >= 0, got {step}")
+    for i, shape, _ in layout if state else []:
+        for key in ("exp_avg", "exp_avg_sq"):
+            if tuple(state[i][key].shape) != shape:
+                raise ValueError(f"state {i} {key}: shape {tuple(state[i][key].shape)}, expected {shape}")
+    with torch.no_grad():
+        if not state:
+            flat_m.zero_(); flat_v.zero_()
+        for i, shape, off in layout if state else []:
+            n = math.prod(shape)
+            flat_m[off:off + n].view(shape).copy_(state[i]["exp_avg"])
+            flat_v[off:off + n].view(shape).copy_(state[i]["exp_avg_sq"])
+    return int(step), betas, eps, float(g.get("lr", 1e-3))
+
+
 class Trainer:
     def __init__(self, model: Model, batch_size: int, seq_length: int, process_group=None,
                  keep_clipped_grads: bool = False, data_parallel: bool = True, lazy_update: bool = False, *,
-                 ar: float = 0.0, tar: float = 0.0):
+                 ar: float = 0.0, tar: float = 0.0, optimizer: str = "sgd", betas=(0.9, 0.999), eps: float = 1e-8):
         """lazy_update: let the SGD update of the upper layers' matrices and of fc.W (HBM-bound, no consumer until the
         next forward reaches them) run beside the NEXT step's forward recurrence kernels instead of at the end of this
         step (zrb_set_lazy_update).  Same arithmetic; every Trainer entry point that reads parameters applies what is
@@ -58,11 +121,20 @@ class Trainer:
         and beta >= 0.  Every fused train step adds alpha/(T*H) * sum(y^2) over the last layer's dropped output y and
         beta/((T-1)*H) * sum((h_t - h_{t-1})^2) over its raw output h (AWD's main.py terms, times B) to the loss it
         differentiates; the clip norm and `.grad` include their gradient.  The returned loss stays the NLL;
-        `activation_reg` holds the two penalty values of the last step.  Eval calls ignore them."""
+        `activation_reg` holds the two penalty values of the last step.  Eval calls ignore them.
+        optimizer / betas / eps (keyword only): "sgd" (default) or "adam" (Kingma & Ba 2015; DESIGN.md section 21), the
+        update every train step applies after the global-norm clip, lr being the train step's own.  Adam is
+        torch.optim.Adam(betas=betas, eps=eps, weight_decay=0): the moments live in `flat_m` and `flat_v` (flat_p's
+        layout), the update count in `adam_step`; `optimizer_state_dict()` / `load_optimizer_state_dict()` move them
+        to and from torch.optim.Adam's format.  Iterate averaging is an SGD scheme and refuses to start under Adam."""
         for name, v in (("ar", ar), ("tar", tar)):
             if isinstance(v, bool) or not isinstance(v, (int, float)) or not math.isfinite(v) or v < 0:
                 raise ValueError(f"{name} must be a finite number >= 0, got {v!r}")
         self._ar, self._tar = float(ar), float(tar)
+        if optimizer not in ("sgd", "adam"):
+            raise ValueError(f"optimizer must be 'sgd' or 'adam', got {optimizer!r}")
+        self.optimizer = optimizer
+        self._betas, self._eps = _adam_hyper(betas, eps)
         if model.lstm_type != "pytorch":
             raise ValueError("Trainer drives the --lstm_type pytorch layout")
         dev = model.embed.W.device
@@ -147,6 +219,12 @@ class Trainer:
         # (reducing finished buckets with NCCL underneath the rest of backward was removed: NCCL's channels evict part
         # of the persistent recurrence grid; the copy-engine transport is the one that overlaps)
         self._ctx_cached = None
+        self.adam_step = 0             # Adam: the updates applied so far (torch.optim.Adam's state "step")
+        if optimizer == "adam":
+            self.flat_m = torch.zeros_like(self.flat_p)
+            self.flat_v = torch.zeros_like(self.flat_p)
+            self._m_s = self._flat_params_struct(self.flat_m)
+            self._v_s = self._flat_params_struct(self.flat_v)
         _ = self.ctx
         # single process: the fused step owns the gradient buffers -> touch only the window's embedding rows and take
         # the matrices' clip norm from the wgrad epilogues (mode 1).  Data parallel with the sparse embedding exchange
@@ -244,12 +322,19 @@ class Trainer:
             _lib.check(_lib.load().zrb_set_keep_clipped_grads(c, 1 if self._keep_clipped else 0))
             _lib.check(_lib.load().zrb_set_lazy_update(c, 1 if getattr(self, "_lazy", False) else 0))
             _lib.check(_lib.load().zrb_set_activation_reg(c, self._ar, self._tar))
+            if getattr(self, "optimizer", "sgd") == "adam":
+                self._set_adam(c)
             self._ctx_cached = self.model._ctx_serial
             if getattr(self, "_averaging", False):
                 self._set_averaging(False)
                 raise RuntimeError("the model's library context was re-created while averaging was on: the average "
                                    "stops here (flat_avg holds it as it was); call start_averaging() to restart")
         return c
+
+    def _set_adam(self, c):
+        """Hand Adam's moments, hyper-parameters and update count to the context c."""
+        _lib.check(_lib.load().zrb_set_adam(c, C.byref(self._m_s), C.byref(self._v_s), self._betas[0], self._betas[1],
+                                            self._eps, self.adam_step))
 
     def _set_averaging(self, on):
         """Whether averaging is on; while it is, the model keeps its library context (the average's count lives there)."""
@@ -346,8 +431,14 @@ class Trainer:
         _lib.check(lib.zrb_train_step_update(self.ctx, C.byref(self._ps), C.byref(self._gs), float(lr),
                                              float(max_norm), _lib.ptr(self.norm), self._stream()))
         self.step += 1
-        self._pending = True
+        self._updated(lr)
         return self.loss, self.norm
+
+    def _updated(self, lr):
+        self._pending = True
+        self._lr = float(lr)
+        if self.optimizer == "adam":
+            self.adam_step += 1
 
     def _ce_join(self, lib):
         """Tied model on the copy-engine transport: E's gradient lies in bucket 0, which the transport reduces on its
@@ -388,7 +479,7 @@ class Trainer:
                                                float(lr), float(max_norm), C.c_void_p(self._hloss.data_ptr()),
                                                C.c_void_p(self._hloss.data_ptr() + 4), self._stream()))
             self.step += 1
-            self._pending = True
+            self._updated(lr)
             return float(self._hloss[0]), float(self._hloss[1])
         xd = hx.to(self.dev, non_blocking=True); yd = hy.to(self.dev, non_blocking=True)
         loss, norm = self.train_step(xd, yd, lr, max_norm)
@@ -453,7 +544,10 @@ class Trainer:
         """Average the weights over every following train step (zrb_set_average): after n steps `flat_avg` holds the
         mean of the n weight vectors those steps produced, as torch.optim.ASGD(lambd=0, t0=0) created now would.  The
         weights themselves train exactly as without averaging.  Calling it again restarts at n = 0.  Under data
-        parallelism every rank calls it at the same step (the ranks' averages stay identical; nothing is exchanged)."""
+        parallelism every rank calls it at the same step (the ranks' averages stay identical; nothing is exchanged).
+        ValueError under Adam: NT-ASGD averages SGD iterates."""
+        if self.optimizer == "adam":
+            raise ValueError("iterate averaging (NT-ASGD) is an SGD scheme: it does not run with optimizer='adam'")
         self._check_not_swapped()
         if getattr(self, "flat_avg", None) is None:
             self.flat_avg = torch.zeros_like(self.flat_p)
@@ -522,6 +616,33 @@ class Trainer:
                 v = src[off:off + v.numel()].view_as(v)
             out[k] = v.detach().clone()
         return out
+
+    # ---- Adam (DESIGN.md section 21) ---------------------------------------------------------------------------------
+    def _adam_layout(self):
+        """(index, shape, offset into flat_p) in model.parameters() order: torch.optim.Adam's state indices."""
+        if self.optimizer != "adam":
+            raise ValueError("the Trainer was created with optimizer='sgd': there is no Adam state")
+        base = self.flat_p.data_ptr()
+        return [(i, tuple(p.shape), (p.data_ptr() - base) // 4) for i, p in enumerate(self.model.parameters())]
+
+    def optimizer_state_dict(self):
+        """Adam's state in torch.optim.Adam's state_dict() format for an Adam over model.parameters() (copies on the
+        parameters' device), with one param group of the betas, eps and the last train step's lr.  Pending lazy updates
+        are applied first."""
+        layout = self._adam_layout()
+        self.flush()
+        return adam_state_to_torch(self.flat_m, self.flat_v, self.adam_step, layout, getattr(self, "_lr", 1e-3),
+                                   self._betas, self._eps)
+
+    def load_optimizer_state_dict(self, sd):
+        """Load a torch.optim.Adam state_dict() over model.parameters() (or one from optimizer_state_dict()): the
+        moments, the update count, and the group's betas, eps and lr (see adam_state_from_torch).  Pending lazy updates
+        are applied first."""
+        layout = self._adam_layout()
+        self.flush()
+        self.adam_step, self._betas, self._eps, lr = adam_state_from_torch(sd, layout, self.flat_m, self.flat_v)
+        self._lr = lr
+        self._set_adam(self.ctx)
 
     # ---- dynamic evaluation (DESIGN.md section 14) -------------------------------------------------------------------
     def _no_experts(self, what):
