@@ -52,10 +52,10 @@ struct AdamRule : NoTileRule {
 };
 
 int update_pack_adam(float* p, float* g, float* m, float* v, const AdamScalars& k, int rows, int cols,
-                     const float* scalars, const WeightImages& img, bool write_g, cudaStream_t s, bool pdl) {
+                     const float* scalars, const WeightImages& img, bool write_g, cudaStream_t s, int pdl_smem) {
     AdamRule rule;
     rule.m = m; rule.v = v; rule.k = k; rule.scalars = scalars; rule.coef = 0.f;
-    return update_pack_rule(p, g, rows, cols, rule, (uintptr_t)m | (uintptr_t)v, img, write_g, s, pdl);
+    return update_pack_rule(p, g, rows, cols, rule, (uintptr_t)m | (uintptr_t)v, img, write_g, s, pdl_smem);
 }
 
 // ---- tensors without an fp16 image (and every tensor on the validation engine / the unaligned fallback) ------------

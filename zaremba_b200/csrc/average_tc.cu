@@ -50,11 +50,11 @@ struct SwapRule : NoTileRule {
 };
 
 int update_pack_avg(float* p, float* g, float* a, float mu, bool first, int rows, int cols, float lr,
-                    const float* scalars, const WeightImages& img, bool write_g, cudaStream_t s, bool pdl) {
+                    const float* scalars, const WeightImages& img, bool write_g, cudaStream_t s, int pdl_smem) {
     AvgRule rule;
     rule.lr = lr; rule.scalars = scalars; rule.coef = 0.f;
     rule.a = a; rule.mu = mu; rule.first = first ? 1 : 0;
-    return update_pack_rule(p, g, rows, cols, rule, (uintptr_t)a, img, write_g, s, pdl);
+    return update_pack_rule(p, g, rows, cols, rule, (uintptr_t)a, img, write_g, s, pdl_smem);
 }
 
 int swap_pack(float* p, float* a, int rows, int cols, const WeightImages& img, cudaStream_t s) {

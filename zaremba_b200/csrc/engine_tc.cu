@@ -418,29 +418,29 @@ static void tc_images_current(zrb_ctx* c, const zrb_params* p) {
 // 21).  All rebuild the matrix's fp16 images from registers, so the next forward needs no pack.  The exception is W_hh
 // in the weight-drop mode: p (and g) only, and the next forward packs the images with its own mask.
 static int tc_update_matrix(zrb_ctx* c, const WeightMatrix& m, const TensorList& tl, float lr, const AvgStep* avg,
-                            const AdamStep* adam, bool pdl, cudaStream_t s) {
+                            const AdamStep* adam, int pdl_smem, cudaStream_t s) {
     zrb_tc_state::WhhImage whh;
     if (c->p_wd > 0.f) whh.kind = zrb_tc_state::kWhhStale;
     const WeightImages img = tc_images(c, m, whh);
     float *p = tl.p[m.i], *g = tl.g[m.i];
     if (adam)
         return update_pack_adam(p, g, adam->m[m.i], adam->v[m.i], adam->k, m.rows, m.cols, c->scalars, img,
-                                c->keep_clipped, s, pdl);
-    if (!avg) return update_pack(p, g, m.rows, m.cols, lr, c->scalars, img, c->keep_clipped, s, pdl);
+                                c->keep_clipped, s, pdl_smem);
+    if (!avg) return update_pack(p, g, m.rows, m.cols, lr, c->scalars, img, c->keep_clipped, s, pdl_smem);
     return update_pack_avg(p, g, avg->a[m.i], avg->mu, avg->first, m.rows, m.cols, lr, c->scalars, img, c->keep_clipped,
-                           s, pdl);
+                           s, pdl_smem);
 }
 
-// apply deferred update item `item` (see zrb_tc_state::upd_pending); pdl: as a programmatic dependent of the forward
-// recurrence kernel just enqueued on `s`
-static int tc_issue_update(zrb_ctx* c, int item, bool pdl, cudaStream_t s) {
+// apply deferred update item `item` (see zrb_tc_state::upd_pending); pdl_smem > 0: as a programmatic dependent of the
+// forward recurrence kernel just enqueued on `s`, requesting its plan's beside_smem
+static int tc_issue_update(zrb_ctx* c, int item, int pdl_smem, cudaStream_t s) {
     zrb_tc_state* t = c->tc;
     if (!(t->upd_pending & (1u << item))) return ZRB_OK;
     t->upd_pending &= ~(1u << item);
     const AvgStep* avg = t->upd_avg_on ? &t->upd_avg : nullptr;
     const AdamStep* adam = t->upd_adam_on ? &t->upd_adam : nullptr;
     for (const WeightMatrix& m : tc_matrices(c))
-        if (m.item == item) ZRB_TRY(tc_update_matrix(c, m, t->upd_tl, t->upd_lr, avg, adam, pdl, s));
+        if (m.item == item) ZRB_TRY(tc_update_matrix(c, m, t->upd_tl, t->upd_lr, avg, adam, pdl_smem, s));
     return ZRB_OK;
 }
 
@@ -448,7 +448,7 @@ int tc_flush_updates(zrb_ctx* c, cudaStream_t s) {
     zrb_tc_state* t = c->tc;
     if (!t || !t->upd_pending) return ZRB_OK;
     ProfScope ps(c, ZRB_PROF_CLIP_SGD, s);
-    for (int item = 1; item <= c->cfg.layers; ++item) ZRB_TRY(tc_issue_update(c, item, false, s));
+    for (int item = 1; item <= c->cfg.layers; ++item) ZRB_TRY(tc_issue_update(c, item, 0, s));
     return ZRB_OK;
 }
 
@@ -538,7 +538,7 @@ int tc_forward(zrb_ctx* c, const zrb_params* p, const int64_t* x, const zrb_stat
             }));
             // deferred update of the NEXT layer's matrices (or of fc.W after the last layer): on the idle SMs, beside
             // this recurrence; their consumers (the next input GEMM / the projection) are enqueued behind them
-            if (ride) ZRB_TRY(tc_issue_update(c, l + 1, true, s));
+            if (ride) ZRB_TRY(tc_issue_update(c, l + 1, fplan.beside_smem, s));
             continue;
         }
         for (int tt = 0; tt < T; ++tt) {
@@ -1071,7 +1071,7 @@ int tc_update(zrb_ctx* c, const zrb_params* p, const TensorList& tl, float lr, f
         // a tied E under Adam is never deferred: the next forward's gather through a pending update (tc_forward) knows
         // only the SGD rule
         if (lazy && m.item >= 1 && !(adam && c->tied && m.item == L)) t->upd_pending |= 1u << m.item;
-        else ZRB_TRY(tc_update_matrix(c, m, tl, lr, avg, adam, false, s));
+        else ZRB_TRY(tc_update_matrix(c, m, tl, lr, avg, adam, 0, s));
     }
     if (adam) ZRB_TRY(adam_apply(rest, *adam, c->scalars, c->keep_clipped, s));
     else if (avg) ZRB_TRY(sgd_avg_apply(rest, avg->a, lr, c->scalars, c->keep_clipped, avg->mu, avg->first, s));

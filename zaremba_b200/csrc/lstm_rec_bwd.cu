@@ -79,17 +79,18 @@ int rec_bwd_plan(int H, int B, RecPlan* plan) {
     plan->ok = 0;
     plan->KS = 1;
     if (plan->GB * 8 > 32) return ZRB_OK;
-    // clusters of 8, half a gate block per CTA (see the kernel header); image batch groups padded to an even count
+    // clusters of 8, half a gate block per CTA (see the kernel header); the dG images' batch groups: rec_split_groups
     if (H >= 256) {
-        const int Kp = (H + 31) / 32 * 32, Kc = Kp / 8, KcS = Kc / 2, GBi = (plan->GB + 1) / 2 * 2;
-        // first choice: at most one (unit, batch) cell per epilogue thread (see rec_fwd_plan)
+        const int Kp = (H + 31) / 32 * 32, Kc = Kp / 8, KcS = Kc / 2, GBi = rec_split_groups(plan->GB);
+        // first choice: as in rec_fwd_plan (rec_split_first_choice)
         for (int pass = 0; pass < 2; ++pass)
             for (int U = 16; U >= 1; --U) {
                 const int UC = 8 * U;
                 if (UC > 128) continue;
                 const int ncl = (H + UC - 1) / UC;
                 if (ncl * 8 > nsm) break;
-                if (U * B > (pass == 0 ? 1 : kRecMaxCell) * kRecEpiThreads) continue;
+                if (U * B > kRecMaxCell * kRecEpiThreads || (pass == 0 && !rec_split_first_choice(U, B, 8 * ncl, nsm)))
+                    continue;
                 const int G = UC / 8;
                 const size_t smem = rec_smem_bytes(KcS, G, GBi);
                 if (smem <= 227 * 1024 && 8 * U * (GBi * 8 + 4) <= 2 * 64 * (GBi * 8 + 1)) {

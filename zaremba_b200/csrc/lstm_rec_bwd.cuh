@@ -23,7 +23,7 @@ __device__ __forceinline__ void cluster_sync_all() {
 }
 
 // S = 1: clusters of 4 (CTA rank = gate), one M = 64 tile, the whole gate block as contraction.
-// S = 2: clusters of 8.  The cluster owns twice the units (8U = 96 rows, two M = 64 tiles, N = 32) and CTA rank
+// S = 2: clusters of 8.  The cluster owns twice the units (8U = 120 rows at Large, two M = 64 tiles, N = pad8(B)) and CTA rank
 //        r = 2*gate + half multiplies only HALF of its gate's rows: 47 K steps per step instead of 94, half the operand
 //        image to fetch.
 // Both push their CS partial products (st.async) into the owners' shared memory, where they are summed in fixed order.

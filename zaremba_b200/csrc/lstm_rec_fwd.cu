@@ -84,6 +84,12 @@ size_t rec_smem_bytes(int Kc, int G, int GB) {
     return (size_t)Kc * G * 128 + (size_t)Kc * GB * 128 + 2 * 64 * (GB * 8 + 1) * 4 + 128 /*align*/ + 128 /*bars*/;
 }
 
+// 8-row batch groups of the K-split plans' operand images: the real ones (wgmma's m64nNk16 takes any N that is a multiple
+// of 8), but two at B <= 8.  The receive area (2 x 64 x (8 GBi + 1) floats, rows of pitch 8 GBi + 4) holds the 8U rows a
+// CTA receives for U <= 13 at N = 16, for U <= 12 only at N = 8; at H = 1500, U = 12 would need 16 backward clusters of 8,
+// more than the GPCs hold, and the backward would fall back to clusters of 4
+int rec_split_groups(int GB) { return GB < 2 ? 2 : GB; }
+
 int rec_max_clusters(const void* kernel, int cluster, int smem, int nCTA) {
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(nCTA);
@@ -106,6 +112,11 @@ int rec_plan_finish(RecPlan* plan, const void* kernel, int cluster) {
     plan->kernel = kernel;
     plan->cluster = cluster;
     plan->max_clusters = rec_max_clusters(kernel, cluster, plan->smem, plan->nCTA);
+    int dev = 0, per_sm = 0, reserved = 0;
+    ZRB_CUDA(cudaGetDevice(&dev));
+    ZRB_CUDA(cudaDeviceGetAttribute(&per_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev));
+    ZRB_CUDA(cudaDeviceGetAttribute(&reserved, cudaDevAttrReservedSharedMemoryPerBlock, dev));
+    plan->beside_smem = per_sm - 2 * reserved - plan->smem + 1;
     plan->ok = 1;
     return ZRB_OK;
 }
@@ -197,16 +208,17 @@ int rec_fwd_plan(int H, int B, RecPlan* plan) {
     plan->ok = 0;
     plan->KS = 1;
     if (plan->GB * 8 > 32) return ZRB_OK;  // accumulators / staging sized for N <= 32
-    // K-split pairs (see the kernel header): image batch groups padded to an even count
+    // K-split pairs (see the kernel header); the operand image's batch groups: rec_split_groups
     if (H >= 256) {
-        const int Kp = (H + 31) / 32 * 32, Kc = Kp / 8, KcS = Kc / 2, GBi = (plan->GB + 1) / 2 * 2;
-        // first choice: at most one (unit, batch) cell per epilogue thread -- a second pass of the cell loop for a handful
-        // of cells doubles the critical path of that warp (measured: U = 13, 260 cells, was slower than U = 12)
+        const int Kp = (H + 31) / 32 * 32, Kc = Kp / 8, KcS = Kc / 2, GBi = rec_split_groups(plan->GB);
+        // first choice (rec_split_first_choice): one (unit, batch) cell per epilogue thread, and SMs left for the work
+        // beside the recurrence; else the largest U that fits, up to kRecMaxCell cells per thread
         for (int pass = 0; pass < 2; ++pass)
             for (int U = 16; U >= 1; --U) {
                 const int npair = (H + 2 * U - 1) / (2 * U);
                 if (2 * npair > nsm) break;
-                if (U * B > (pass == 0 ? 1 : kRecMaxCell) * kRecEpiThreads) continue;
+                if (U * B > kRecMaxCell * kRecEpiThreads || (pass == 0 && !rec_split_first_choice(U, B, 2 * npair, nsm)))
+                    continue;
                 const int G = U;                              // 8U gate rows of the pair / 8
                 const size_t smem = rec_smem_bytes(KcS, G, GBi);
                 // two M = 64 tiles read 16 row groups per K chunk: the last chunk reaches (16-G)*128 B past the slice, into the h buffer

@@ -7,7 +7,7 @@ namespace zrb {
 
 // K-split variant (RecPlan::KS == 2, used when the shape allows): a CTA that owns 4U = 48 gate rows and the whole
 // contraction issues H/16 = 94 chained, three-quarters-full M=64 wgmmas per step.  A CLUSTER OF TWO CTAs instead owns 2U
-// units = 96 gate rows (two M = 64 tiles, N = 32): CTA r keeps the K half r of all 96 rows resident (same 144 KB), loads
+// units = 8U gate rows (two M = 64 tiles, N = pad8(B)): CTA r keeps the K half r of all 8U rows resident (168 KB at U = 14), loads
 // only its half of the h image, runs half the K chain, and the MMA warpgroup pushes each accumulator pair straight from
 // registers into the shared memory of the CTA that owns the row's unit (st.async, bytes counted on the owner's mbarrier:
 // no fence, no staging pass); the owner adds the two partial sums in its cell math.

@@ -31,10 +31,10 @@ struct DynRule : NoTileRule {
 };
 
 int update_pack(float* p, float* g, int rows, int cols, float lr, const float* scalars, const WeightImages& img,
-                bool write_g, cudaStream_t s, bool pdl) {
+                bool write_g, cudaStream_t s, int pdl_smem) {
     SgdRule rule;
     rule.lr = lr; rule.scalars = scalars; rule.coef = 0.f;
-    return update_pack_rule(p, g, rows, cols, rule, 0, img, write_g, s, pdl);
+    return update_pack_rule(p, g, rows, cols, rule, 0, img, write_g, s, pdl_smem);
 }
 
 int update_pack_dyn(float* p, float* g, const float* tg, const float* r, int rows, int cols, const DynArgs& a,

@@ -17,6 +17,13 @@ constexpr int kRecThreads = (kRecLoadWarp + 1) * 32;
 constexpr int kRecPieces = 4;                         // operand image arrives in this many bulk copies, so that the MMAs
                                                       // start when the first quarter of K has landed
 constexpr int kRecMaxCell = 2;                        // (unit, batch) cells per epilogue thread
+// The K-split plans' first choice of U (rec_fwd_plan / rec_bwd_plan): each of the 256 epilogue threads owns at most one
+// (unit, batch) cell, and the grid of nCTA leaves at least an eighth of the SMs to the kernels launched beside it (the
+// deferred weight update, the weight gradients).  When no U meets both, the plans take the largest U that fits: two
+// cells for some threads cost less than a grid that leaves the work beside it a handful of SMs (DESIGN.md section 4.1)
+inline bool rec_split_first_choice(int U, int B, int nCTA, int nsm) {
+    return U * B <= kRecEpiThreads && nCTA <= nsm - nsm / 8;
+}
 // ---- watchdog -------------------------------------------------------------------------------------
 // Every wait of the persistent kernels is bounded.  A wait that runs out (a lost wake-up, a grid that is not co-resident)
 // publishes a code in the context's abort word; from then on EVERY wait of EVERY thread returns at once (a thread that

@@ -77,16 +77,20 @@ struct RecPlan {
     int smem;
     int KS;      // K-split: CTAs that share one set of output rows, each holding 1/KS of the contraction (clusters)
     int KcS;     // K chunks per CTA (Kc / KS)
-    int GBi;     // 8-row batch groups of the operand images (GB, or padded so that the MMA's N is a multiple of 16)
+    int GBi;     // 8-row batch groups of the operand images (GB; the K-split plans: rec_split_groups(GB))
     const void* kernel;   // the instantiation launched: lstm_rec_fwd_kernel<KS == 2> / lstm_rec_bwd_kernel<KS>
     int cluster;          // CTAs per thread-block cluster: 1 (unsplit forward), 2, 4 or 8
     int max_clusters;     // cudaOccupancyMaxActiveClusters at this cluster size and smem (0: the query failed)
+    int beside_smem;      // dynamic shared memory per block that keeps a kernel launched beside this grid off its SMs:
+                          // one byte more than an SM has left after one of its CTAs (the SM's shared memory less smem
+                          // and two blocks' reserved shares)
 };
 size_t rec_smem_bytes(int Kc, int G, int GB);
+int rec_split_groups(int GB);   // GBi of the K-split plans (see the definition)
 // cudaOccupancyMaxActiveClusters of `kernel` on a grid of nCTA in clusters of `cluster`, after raising its dynamic
 // shared-memory limit; 0 if either call fails, with the error cleared
 int rec_max_clusters(const void* kernel, int cluster, int smem, int nCTA);
-// the plan fits: record the kernel it launches, its cluster size and occupancy answer, and set ok
+// the plan fits: record the kernel it launches, its cluster size, occupancy answer and beside_smem, and set ok
 int rec_plan_finish(RecPlan* plan, const void* kernel, int cluster);
 // launch the plan's kernel with args = {&RecFwdArgs} or {&RecBwdArgs}; the launch modes are described at the definition
 // (lstm_rec_fwd.cu).  trace: the launch records a trace (never programmatic); name: for error messages
@@ -126,7 +130,7 @@ struct RecFwdArgs {
     unsigned int* counter;    // grid barrier: never reset, `base` is its value when this launch starts
     unsigned int base;
     int T, B, H, Hp, U, G, GB, Kc, nCTA;
-    int KcS, GBi;             // K chunks per CTA (Kc / KS); 8-row batch groups of the operand image (GB, or 4 when N = 32)
+    int KcS, GBi;             // K chunks per CTA (Kc / KS); 8-row batch groups of the operand image (RecPlan::GBi)
     MaskSrc m;                // the output site's dropout (period B*H: variational mode, fixed over the window)
     MaskSrc rm;               // variational mode: recurrent mask of element b*H + j on h_{t-1} (operand images, hprev_h)
     RecWatch w;               // watchdog (rec_common.cuh)
@@ -171,7 +175,8 @@ struct WeightImages {
 // SGD update of one matrix fused with its fp16 image rebuild (optim_tc.cu)
 int update_pack(float* p, float* g, int rows, int cols, float lr, const float* scalars, const WeightImages& img,
                 bool write_g, cudaStream_t s,
-                bool pdl = false);   // pdl: programmatic dependent of the (forward recurrence) kernel enqueued before it
+                int pdl_smem = 0);   // > 0: programmatic dependent of the forward recurrence kernel enqueued before it,
+                                     // each block requesting this much dynamic shared memory (rec_beside_smem)
 // the same kernels with the dynamic-evaluation rule (dyneval_elem): theta_g tg and r at p's offsets (r unused under the
 // SGD rule, a.rbar null); g is read, never written; the same images
 int update_pack_dyn(float* p, float* g, const float* tg, const float* r, int rows, int cols, const DynArgs& a,
@@ -179,11 +184,11 @@ int update_pack_dyn(float* p, float* g, const float* tg, const float* r, int row
 // iterate averaging (average_tc.cu, DESIGN.md section 16): update_pack's update, then a = first ? p : a + (p - a) * mu
 // over the new p in the same pass; the same images
 int update_pack_avg(float* p, float* g, float* a, float mu, bool first, int rows, int cols, float lr,
-                    const float* scalars, const WeightImages& img, bool write_g, cudaStream_t s, bool pdl = false);
+                    const float* scalars, const WeightImages& img, bool write_g, cudaStream_t s, int pdl_smem = 0);
 // Adam (adam_tc.cu, DESIGN.md section 21): adam_apply's element rule with the moments m and v at p's offsets, in place of
 // update_pack's SGD; the same images
 int update_pack_adam(float* p, float* g, float* m, float* v, const AdamScalars& k, int rows, int cols,
-                     const float* scalars, const WeightImages& img, bool write_g, cudaStream_t s, bool pdl = false);
+                     const float* scalars, const WeightImages& img, bool write_g, cudaStream_t s, int pdl_smem = 0);
 // exchange p and a, and write the images of the new p (update_pack's image stores)
 int swap_pack(float* p, float* a, int rows, int cols, const WeightImages& img, cudaStream_t s);
 int rec_bwd_plan(int H, int B, RecPlan* plan);   // U = units per CTA, nCTA = 4 * clusters
@@ -203,7 +208,7 @@ struct RecBwdArgs {
     unsigned int* counter;    // grid barrier: never reset, `base` is its value when this launch starts
     unsigned int base;
     int T, B, H, G4p, U, G, GB, Kc, nCTA;
-    int KcS, GBi;             // K chunks per CTA (Kc / S); 8-row batch groups of the dG images (GB, or 4 when N = 32)
+    int KcS, GBi;             // K chunks per CTA (Kc / S); 8-row batch groups of the dG images (RecPlan::GBi)
     MaskSrc m;                // the output site's dropout (period B*H: variational mode, fixed over the window)
     MaskSrc rm;               // variational mode: recurrent mask of element b*H + j; scales the recurrent gradient
     RecWatch w;               // watchdog (rec_common.cuh)

@@ -286,7 +286,7 @@ __global__ void __launch_bounds__(kUpdThreads, Rule::kWhhMinBlocks) update_pack_
 
 template <int VEC, class Rule>
 static int update_pack_launch(float* p, float* g, int rows, int cols, const Rule& rule, const PackSpec& sp, bool whh,
-                              cudaStream_t s) {
+                              int pdl_smem, cudaStream_t s) {
     // one tile per thread, the grid sized to the tiles: W_hh 8 rows of the 4 gates x 8 * VEC columns per warp, other
     // matrices 8 rows x VEC columns per thread (narrower blocks when the matrix is narrow)
     const int cv = cols / VEC;
@@ -298,18 +298,25 @@ static int update_pack_launch(float* p, float* g, int rows, int cols, const Rule
         col_tiles = (cv + threads - 1) / threads;
     }
     const dim3 grid((unsigned)(((rows / (whh ? 4 : 1)) + kTileRows - 1) / kTileRows * col_tiles));
-    if (sp.pdl) {
-        // beside the persistent forward recurrence: a dynamic shared-memory request larger than what that kernel leaves
-        // free on its SMs keeps these blocks on the SMs it does not occupy, off the latency-critical ones.  On a 132-SM
-        // H100 the forward plan holds 126 SMs at Large (6 free), 56 at Medium (76 free) and 13 at Small (119 free)
+    if (pdl_smem > 0) {
+        // beside the persistent forward recurrence: pdl_smem is more dynamic shared memory than that kernel leaves free
+        // on its SMs (rec_beside_smem), which keeps these blocks on the SMs it does not occupy, off the latency-critical
+        // ones
         cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = grid; cfg.blockDim = dim3(threads); cfg.dynamicSmemBytes = 12 * 1024; cfg.stream = s;
+        cfg.gridDim = grid; cfg.blockDim = dim3(threads); cfg.dynamicSmemBytes = (size_t)pdl_smem; cfg.stream = s;
         cudaLaunchAttribute at[1];
         at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
         at[0].val.programmaticStreamSerializationAllowed = 1;
         cfg.attrs = at; cfg.numAttrs = 1;
-        if (whh) ZRB_CUDA(cudaLaunchKernelEx(&cfg, update_pack_whh_kernel<VEC, Rule>, p, g, cols, col_tiles, rule, sp));
-        else ZRB_CUDA(cudaLaunchKernelEx(&cfg, update_pack_kernel<VEC, Rule>, p, g, rows, cols, col_tiles, rule, sp));
+        if (whh) {
+            ZRB_CUDA(cudaFuncSetAttribute(update_pack_whh_kernel<VEC, Rule>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                          pdl_smem));
+            ZRB_CUDA(cudaLaunchKernelEx(&cfg, update_pack_whh_kernel<VEC, Rule>, p, g, cols, col_tiles, rule, sp));
+        } else {
+            ZRB_CUDA(cudaFuncSetAttribute(update_pack_kernel<VEC, Rule>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                          pdl_smem));
+            ZRB_CUDA(cudaLaunchKernelEx(&cfg, update_pack_kernel<VEC, Rule>, p, g, rows, cols, col_tiles, rule, sp));
+        }
         count_launch();
         return ZRB_OK;
     }
@@ -322,11 +329,11 @@ static int update_pack_launch(float* p, float* g, int rows, int cols, const Rule
 // align: OR of every pointer the rule streams besides p and g (their alignment picks the access width too)
 template <class Rule>
 static int update_pack_rule(float* p, float* g, int rows, int cols, const Rule& rule, uintptr_t align,
-                            const WeightImages& img, bool write_g, cudaStream_t s, bool pdl) {
+                            const WeightImages& img, bool write_g, cudaStream_t s, int pdl_smem) {
     const RecPlan *fp = img.fplan, *bp = img.bplan;
     PackSpec sp;
     sp.write_g = write_g ? 1 : 0;
-    sp.pdl = pdl ? 1 : 0;
+    sp.pdl = pdl_smem > 0 ? 1 : 0;
     sp.row_img = img.row; sp.ld = img.ld;
     sp.fwd_img = img.fwd; sp.fKS = fp ? fp->KS : 1; sp.fU = fp ? fp->KS * fp->U : 1; sp.fG = fp ? fp->G : 1;
     sp.fKc = fp ? fp->KcS : 1;
@@ -335,9 +342,9 @@ static int update_pack_rule(float* p, float* g, int rows, int cols, const Rule& 
     const bool whh = (img.fwd || img.bwd) && rows == 4 * cols;
     const uintptr_t all = ((uintptr_t)p) | ((uintptr_t)g) | align;
     const bool al16 = (all & 15) == 0, al8 = (all & 7) == 0;
-    if (cols % 4 == 0 && al16) return update_pack_launch<4>(p, g, rows, cols, rule, sp, whh, s);
-    if (cols % 2 == 0 && al8) return update_pack_launch<2>(p, g, rows, cols, rule, sp, whh, s);
-    return update_pack_launch<1>(p, g, rows, cols, rule, sp, whh, s);
+    if (cols % 4 == 0 && al16) return update_pack_launch<4>(p, g, rows, cols, rule, sp, whh, pdl_smem, s);
+    if (cols % 2 == 0 && al8) return update_pack_launch<2>(p, g, rows, cols, rule, sp, whh, pdl_smem, s);
+    return update_pack_launch<1>(p, g, rows, cols, rule, sp, whh, pdl_smem, s);
 }
 
 }  // namespace zrb
