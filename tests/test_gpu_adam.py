@@ -420,6 +420,14 @@ def test_refusals(monkeypatch):
     assert set_adam(ms, vs, step=-1) == E
     assert set_adam(ms, None) == E and set_adam(None, vs) == E
     assert set_adam(ms, ms) == E                     # m and v overlap
+    # a moment tensor that is not 4-byte aligned (in a buffer of its own, so it overlaps nothing); never left installed
+    spare = torch.zeros(tr.flat_m.numel() + 1, device=_dev())
+    odd = _lib.ZrbParams.from_buffer_copy(ms)
+    odd.w_hh[0] = spare.data_ptr() + 2
+    try:
+        assert set_adam(odd, vs) == E
+    finally:
+        set_adam(None, None)
     # moments that alias the parameters pass zrb_set_adam but stop the train step before anything is launched
     assert set_adam(tr._ps, vs) == 0
     before = tr.flat_p.clone()

@@ -287,6 +287,15 @@ def test_refusals(monkeypatch):
     C.memmove(C.byref(bad), C.byref(tr._avg_s), C.sizeof(bad))
     bad.b_hh[0] = bad.b_ih[0]
     assert lib.zrb_set_average(tr.ctx, C.byref(bad)) == -1
+    # an average tensor that is not 4-byte aligned (in a buffer of its own, so it overlaps nothing); never left installed
+    spare = torch.zeros(tr.flat_avg.numel() + 1, device=_dev())
+    odd = _lib.ZrbParams()
+    C.memmove(C.byref(odd), C.byref(tr._avg_s), C.sizeof(odd))
+    odd.w_hh[0] = spare.data_ptr() + 2
+    try:
+        assert lib.zrb_set_average(tr.ctx, C.byref(odd)) == -1
+    finally:
+        lib.zrb_set_average(tr.ctx, None)
     tr.close()
     del tr, m
     gc.collect()

@@ -135,6 +135,18 @@ ProfScope::~ProfScope() {
     if (b) cudaEventRecord(b, s);
 }
 
+int update_list(const zrb_ctx* c, const UpdateStep& st, const TensorList& tl, cudaStream_t s) {
+    switch (st.kind) {
+        case UpdateStep::kSgd: return sgd_apply(tl, st.lr, c->scalars, c->keep_clipped, s);
+        case UpdateStep::kSgdAvg:
+            return sgd_avg_apply(tl, st.avg.a, st.lr, c->scalars, c->keep_clipped, st.avg.mu, st.avg.first, s);
+        case UpdateStep::kAdam: return adam_apply(tl, st.adam, c->scalars, c->keep_clipped, s);
+        case UpdateStep::kDyn: return dyneval_apply(tl, st.tg, st.r, st.dyn, s);
+        case UpdateStep::kSwap: return swap_apply(tl, st.avg.a, s);
+    }
+    return ZRB_E_INVALID;
+}
+
 }  // namespace zrb
 
 using namespace zrb;
@@ -524,6 +536,13 @@ static int check_moment_alias(const TensorList& tm, const TensorList& tl) {
     return ZRB_OK;
 }
 
+// ZRB_E_INVALID when a tensor of `tl` (its p or g) is not 4-byte aligned: the update kernels stream them as floats
+static int check_aligned(const TensorList& tl, const char* what) {
+    for (int i = 0; i < tl.count; ++i)
+        ZRB_REQUIRE((((uintptr_t)tl.p[i] | (uintptr_t)tl.g[i]) & 3) == 0, "%s tensor %d is not 4-byte aligned", what, i);
+    return ZRB_OK;
+}
+
 static int check_not_swapped(const zrb_ctx* c) {
     ZRB_REQUIRE(!c->avg_swapped, "the parameters hold the average (zrb_swap_average): swap back before training");
     return ZRB_OK;
@@ -544,6 +563,7 @@ int zrb_set_average(zrb_ctx* c, const zrb_params* avg) {
         for (int i = 0; i < ta.count; ++i)
             for (int j = i + 1; j < ta.count; ++j)
                 ZRB_REQUIRE(!ranges_overlap(ta.p[i], ta.n[i], ta.p[j], ta.n[j]), "average tensors %d and %d overlap", i, j);
+        ZRB_TRY(check_aligned(ta, "average"));
     }
     // deferred updates belong to the steps before: they average (or not) with the n they were issued with
     if (c->cfg.engine == ZRB_ENGINE_TC) ZRB_TRY(tc_flush_updates(c, nullptr));
@@ -589,6 +609,7 @@ int zrb_set_adam(zrb_ctx* c, const zrb_params* m, const zrb_params* v, float bet
                 ZRB_REQUIRE(!ranges_overlap(tm.p[i], tm.n[i], tm.g[j], tm.n[j]),
                             "first-moment tensor %d overlaps second-moment tensor %d", i, j);
             }
+        ZRB_TRY(check_aligned(tm, "moment"));
     }
     // deferred updates belong to the steps before: they apply the rule (and the t) they were issued with
     if (c->cfg.engine == ZRB_ENGINE_TC) ZRB_TRY(tc_flush_updates(c, nullptr));
@@ -609,21 +630,30 @@ int zrb_average_count(const zrb_ctx* c, int64_t* n) {
     return ZRB_OK;
 }
 
+// st's update of p on either engine; on the validation engine the clip norm of a train-step kind, then the list
+// kernels over every tensor.  max_norm / norm_out: the clip norm (unused by the other kinds)
+static int apply_update(zrb_ctx* c, const zrb_params* p, const UpdateStep& st, float max_norm, float* norm_out,
+                        cudaStream_t s) {
+    if (c->cfg.engine == ZRB_ENGINE_TC) return tc_apply_update(c, p, st, max_norm, norm_out, s);
+    ProfScope ps(c, st.kind == UpdateStep::kSwap ? ZRB_PROF_PACK : ZRB_PROF_CLIP_SGD, s);
+    if (st.train()) ZRB_TRY(grad_norm(st.tl, max_norm, c->partials, c->scalars, norm_out, s));
+    ZRB_TRY(update_list(c, st, st.tl, s));
+    c->weights_version++;
+    return ZRB_OK;
+}
+
 int zrb_swap_average(zrb_ctx* c, const zrb_params* p, void* stream) {
     ZRB_REQUIRE(c && p, "null argument");
     ZRB_TRY(watchdog_check(c));
     ZRB_TRY(check_tied(c, p));
     ZRB_REQUIRE(c->avg_on && c->avg_n > 0, "no average to swap in: no train step has been averaged since zrb_set_average");
-    const TensorList tl = param_list(c, p, p), ta = param_list(c, &c->avg.base, &c->avg.base);
-    ZRB_TRY(check_avg_alias(ta, tl, false));
-    cudaStream_t s = (cudaStream_t)stream;
-    if (c->cfg.engine == ZRB_ENGINE_TC) {
-        ZRB_TRY(tc_swap_average(c, p, tl, ta.p, s));
-    } else {
-        ProfScope ps(c, ZRB_PROF_PACK, s);
-        ZRB_TRY(swap_apply(tl, ta.p, s));
-        c->weights_version++;
-    }
+    UpdateStep st;
+    st.kind = UpdateStep::kSwap;
+    st.tl = param_list(c, p, p);
+    const TensorList ta = param_list(c, &c->avg.base, &c->avg.base);
+    ZRB_TRY(check_avg_alias(ta, st.tl, false));
+    for (int i = 0; i < ta.count; ++i) st.avg.a[i] = ta.p[i];
+    ZRB_TRY(apply_update(c, p, st, 0.f, nullptr, (cudaStream_t)stream));
     c->avg_swapped = !c->avg_swapped;
     return ZRB_OK;
 }
@@ -781,28 +811,26 @@ int zrb_train_step_update(zrb_ctx* c, const zrb_params* p, const zrb_params* g, 
     ZRB_TRY(check_tied(c, p));
     ZRB_TRY(check_tied(c, g));
     ZRB_TRY(check_not_swapped(c));
-    TensorList tl = param_list(c, p, g);
-    cudaStream_t s = (cudaStream_t)stream;
-    // iterate averaging: this update is number n = avg_n + 1, mu = fp32(1 / n) rounded once from double
-    AvgStep as{};
-    const AvgStep* avg = nullptr;
+    UpdateStep st;
+    st.tl = param_list(c, p, g);
+    st.lr = lr;
     if (c->avg_on) {
+        // iterate averaging: this update is number n = avg_n + 1, mu = fp32(1 / n) rounded once from double
+        st.kind = UpdateStep::kSgdAvg;
         const TensorList ta = param_list(c, &c->avg.base, &c->avg.base);
-        ZRB_TRY(check_avg_alias(ta, tl, true));
-        for (int i = 0; i < ta.count; ++i) as.a[i] = ta.p[i];
-        as.mu = (float)(1.0 / (double)(c->avg_n + 1));
-        as.first = c->avg_n == 0;
-        avg = &as;
-    }
-    // Adam: this update is number t = adam_t + 1; each scalar computed in double and rounded once to fp32
-    AdamStep ad{};
-    const AdamStep* adam = nullptr;
-    if (c->adam_on) {
+        ZRB_TRY(check_avg_alias(ta, st.tl, true));
+        for (int i = 0; i < ta.count; ++i) st.avg.a[i] = ta.p[i];
+        st.avg.mu = (float)(1.0 / (double)(c->avg_n + 1));
+        st.avg.first = c->avg_n == 0;
+    } else if (c->adam_on) {
+        // Adam: this update is number t = adam_t + 1; each scalar computed in double and rounded once to fp32
+        st.kind = UpdateStep::kAdam;
         const TensorList tm = param_list(c, &c->adam_m.base, &c->adam_v.base);
         TensorList tv = tm;
         for (int i = 0; i < tm.count; ++i) tv.p[i] = tm.g[i];
-        ZRB_TRY(check_moment_alias(tm, tl));
-        ZRB_TRY(check_moment_alias(tv, tl));
+        ZRB_TRY(check_moment_alias(tm, st.tl));
+        ZRB_TRY(check_moment_alias(tv, st.tl));
+        AdamStep& ad = st.adam;
         for (int i = 0; i < tm.count; ++i) { ad.m[i] = tm.p[i]; ad.v[i] = tm.g[i]; }
         const double b1 = c->adam_b1, b2 = c->adam_b2, t = (double)(c->adam_t + 1);
         ad.k.beta1 = c->adam_b1; ad.k.beta2 = c->adam_b2; ad.k.eps = c->adam_eps;
@@ -810,25 +838,10 @@ int zrb_train_step_update(zrb_ctx* c, const zrb_params* p, const zrb_params* g, 
         ad.k.omb2 = (float)(1.0 - b2);
         ad.k.step_size = (float)((double)lr / (1.0 - std::pow(b1, t)));
         ad.k.bc2s = (float)std::sqrt(1.0 - std::pow(b2, t));
-        adam = &ad;
     }
-    if (c->cfg.engine == ZRB_ENGINE_TC) {
-        ZRB_TRY(tc_update(c, p, tl, lr, max_norm, norm_out, avg, adam, s));
-    } else {
-        ProfScope ps(c, ZRB_PROF_CLIP_SGD, s);
-        if (adam) {
-            ZRB_TRY(grad_norm(tl, max_norm, c->partials, c->scalars, norm_out, s));
-            ZRB_TRY(adam_apply(tl, *adam, c->scalars, c->keep_clipped, s));
-        } else if (avg) {
-            ZRB_TRY(grad_norm(tl, max_norm, c->partials, c->scalars, norm_out, s));
-            ZRB_TRY(sgd_avg_apply(tl, avg->a, lr, c->scalars, c->keep_clipped, avg->mu, avg->first, s));
-        } else {
-            ZRB_TRY(clip_sgd(tl, lr, max_norm, c->partials, c->scalars, norm_out, c->keep_clipped, s));
-        }
-        c->weights_version++;
-    }
-    if (avg) c->avg_n++;
-    if (adam) c->adam_t++;
+    ZRB_TRY(apply_update(c, p, st, max_norm, norm_out, (cudaStream_t)stream));
+    if (st.kind == UpdateStep::kSgdAvg) c->avg_n++;
+    if (st.kind == UpdateStep::kAdam) c->adam_t++;
     return ZRB_OK;
 }
 
@@ -903,20 +916,21 @@ int zrb_dyneval_step(zrb_ctx* c, const zrb_params* p, const zrb_params* g, const
     ZRB_TRY(check_tied(c, g));
     ZRB_TRY(check_tied(c, global));
     ZRB_TRY(check_tied(c, rms));
+    UpdateStep st;
+    st.kind = UpdateStep::kDyn;
+    st.tl = param_list(c, p, g);
+    const TensorList tg = param_list(c, global, global);
+    ZRB_TRY(check_aligned(tg, "theta_g"));
+    for (int i = 0; i < tg.count; ++i) st.tg[i] = tg.p[i];
+    if (rms) {
+        const TensorList tr = param_list(c, rms, rms);
+        ZRB_TRY(check_aligned(tr, "RMS statistic"));
+        for (int i = 0; i < tr.count; ++i) st.r[i] = tr.p[i];
+    }
+    st.dyn.lr = lr; st.dyn.lam = lambda; st.dyn.eps = eps; st.dyn.rbar = rms ? rms_mean : nullptr;
     cudaStream_t s = (cudaStream_t)stream;
     ZRB_TRY(eval_grads(c, p, g, x, y, T, B, in, out, loss, s));
-    const TensorList tl = param_list(c, p, g), tg = param_list(c, global, global);
-    TensorList tr = tl;
-    if (rms) tr = param_list(c, rms, rms);
-    DynArgs a;
-    a.lr = lr; a.lam = lambda; a.eps = eps; a.rbar = rms ? rms_mean : nullptr;
-    if (c->cfg.engine == ZRB_ENGINE_TC) return tc_dyneval_update(c, p, tl, tg.p, rms ? tr.p : nullptr, a, s);
-    {
-        ProfScope ps(c, ZRB_PROF_CLIP_SGD, s);
-        ZRB_TRY(dyneval_apply(tl, tg.p, rms ? tr.p : nullptr, a, s));
-    }
-    c->weights_version++;
-    return ZRB_OK;
+    return apply_update(c, p, st, 0.f, nullptr, s);
 }
 
 int zrb_sample(const float* scores, int64_t ld, int32_t B, int32_t V, const zrb_sampling* cfg, uint64_t pos,

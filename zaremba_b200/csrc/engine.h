@@ -167,14 +167,15 @@ int tc_layer_fwd(zrb_ctx* c, const float* w_ih, const float* w_hh, const float* 
                  int T, int B, const float* h0, const float* c0, float* y, float* hT, float* cT, cudaStream_t s);
 int tc_layer_bwd(zrb_ctx* c, const float* dy, float* dx, float* dw_ih, float* dw_hh, float* db_ih, float* db_hh,
                  cudaStream_t s);   // the persistent backward recurrence kernel is in use for this context
-int tc_update(zrb_ctx* c, const zrb_params* p, const TensorList& tl, float lr, float max_norm, float* norm_out,
-              const AvgStep* avg, const AdamStep* adam, cudaStream_t s);
-// iterate averaging (DESIGN.md section 16): exchange the tensors of tl (param_list() over p) with a, images rebuilt
-int tc_swap_average(zrb_ctx* c, const zrb_params* p, const TensorList& tl, float* const* a, cudaStream_t s);
-// dynamic evaluation (DESIGN.md section 14): eval-mode gradients, and the update with the dynamic rule
+// st's update of p (st.tl = param_list() over p): the matrices fused with their fp16 image rebuild, the other tensors
+// by the list kernels.  max_norm / norm_out: the clip norm of a train-step kind (unused otherwise)
+int tc_apply_update(zrb_ctx* c, const zrb_params* p, const UpdateStep& st, float max_norm, float* norm_out,
+                    cudaStream_t s);
+// st's rule by the list kernels over tl (st.tl, or the part of it without an fp16 image), no norm: it reads the clip
+// coefficient in c->scalars[1]
+int update_list(const zrb_ctx* c, const UpdateStep& st, const TensorList& tl, cudaStream_t s);
+// dynamic evaluation (DESIGN.md section 14): eval-mode gradients
 int tc_eval_grads(zrb_ctx* c, const zrb_params* p, const zrb_params* g, const int64_t* x, const int64_t* y, int T, int B,
                   const zrb_states* in, const zrb_states* out, float* loss, cudaStream_t s);
-int tc_dyneval_update(zrb_ctx* c, const zrb_params* p, const TensorList& tl, float* const* tg, float* const* r,
-                      const DynArgs& a, cudaStream_t s);
 
 }  // namespace zrb

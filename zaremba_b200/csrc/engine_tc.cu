@@ -55,14 +55,10 @@ struct zrb_tc_state {
     int pending = 0, pending_layer = 0;
     bool defer_wgrad = false;
     // deferred weight updates (zrb_set_lazy_update): items 1..L-1 = (w_ih, w_hh) of that layer, item L = fc.W; bit i of
-    // upd_pending set = item i still to be applied with the (lr, coef in c->scalars[1]) of the step that deferred it
+    // upd_pending set = item i still to be applied with `upd`, the update of the step that deferred it (its rule and
+    // constants; the clip coefficient in c->scalars[1])
     unsigned upd_pending = 0;
-    float upd_lr = 0.f;
-    zrb::TensorList upd_tl{};
-    bool upd_avg_on = false;      // ... and averaged with upd_avg, the average step of that train step (section 16)
-    zrb::AvgStep upd_avg{};
-    bool upd_adam_on = false;     // ... or under Adam with upd_adam, the moments and scalars of that step (section 21)
-    zrb::AdamStep upd_adam{};
+    zrb::UpdateStep upd{};
     bool in_train_step = false;   // tc_forward is running as the first half of a fused train step
     float* colsum_scratch = nullptr;   // row-split partials of the bias-gradient column sums
     int64_t packed_version = 0;
@@ -397,14 +393,6 @@ static TensorList tc_without_matrices(const zrb_ctx* c, const TensorList& tl) {
     for (const WeightMatrix& m : tc_matrices(c)) rest.n[m.i] = 0;
     return rest;
 }
-// every pointer the tile kernels would stream is 4-byte aligned (they pick 16 / 8 / 4-byte accesses from the matrix
-// width and the alignment); x1, x2: further per-tensor streams in tl's order, or null
-static bool tc_streams_aligned(const TensorList& tl, float* const* x1 = nullptr, float* const* x2 = nullptr) {
-    uintptr_t all = 0;
-    for (int i = 0; i < tl.count; ++i)
-        all |= (uintptr_t)tl.p[i] | (uintptr_t)tl.g[i] | (x1 ? (uintptr_t)x1[i] : 0) | (x2 ? (uintptr_t)x2[i] : 0);
-    return (all & 3) == 0;
-}
 // after a fused update of every matrix (applied or pending): the images are current, the next forward needs no pack
 static void tc_images_current(zrb_ctx* c, const zrb_params* p) {
     zrb_tc_state* t = c->tc;
@@ -413,22 +401,31 @@ static void tc_images_current(zrb_ctx* c, const zrb_params* p) {
     note_packed(c, p);
 }
 
-// The train step's update of one matrix: update_pack, or with iterate averaging on (avg non-null) update_pack_avg,
-// which also averages the new p into a (DESIGN.md section 16), or under Adam (adam non-null) update_pack_adam (section
-// 21).  All rebuild the matrix's fp16 images from registers, so the next forward needs no pack.  The exception is W_hh
-// in the weight-drop mode: p (and g) only, and the next forward packs the images with its own mask.
-static int tc_update_matrix(zrb_ctx* c, const WeightMatrix& m, const TensorList& tl, float lr, const AvgStep* avg,
-                            const AdamStep* adam, int pdl_smem, cudaStream_t s) {
+// st's update of one matrix, with the tile kernels of its rule: update_pack (SGD), update_pack_avg (which also averages
+// the new p, DESIGN.md section 16), update_pack_adam (section 21), update_pack_dyn (section 14) or swap_pack.  All
+// rebuild the matrix's fp16 images from registers, so the next forward needs no pack.  The exception is W_hh under a
+// train-step rule in the weight-drop mode: p (and g) only, and the next forward packs the images with its own mask.
+// Dynamic evaluation and the swap leave the raw weights in the W_hh images: evaluation applies no weight drop.
+static int tc_update_matrix(zrb_ctx* c, const WeightMatrix& m, const UpdateStep& st, int pdl_smem, cudaStream_t s) {
     zrb_tc_state::WhhImage whh;
-    if (c->p_wd > 0.f) whh.kind = zrb_tc_state::kWhhStale;
+    if (st.train() && c->p_wd > 0.f) whh.kind = zrb_tc_state::kWhhStale;
     const WeightImages img = tc_images(c, m, whh);
-    float *p = tl.p[m.i], *g = tl.g[m.i];
-    if (adam)
-        return update_pack_adam(p, g, adam->m[m.i], adam->v[m.i], adam->k, m.rows, m.cols, c->scalars, img,
-                                c->keep_clipped, s, pdl_smem);
-    if (!avg) return update_pack(p, g, m.rows, m.cols, lr, c->scalars, img, c->keep_clipped, s, pdl_smem);
-    return update_pack_avg(p, g, avg->a[m.i], avg->mu, avg->first, m.rows, m.cols, lr, c->scalars, img, c->keep_clipped,
-                           s, pdl_smem);
+    float *p = st.tl.p[m.i], *g = st.tl.g[m.i];
+    switch (st.kind) {
+        case UpdateStep::kSgd:
+            return update_pack(p, g, m.rows, m.cols, st.lr, c->scalars, img, c->keep_clipped, s, pdl_smem);
+        case UpdateStep::kSgdAvg:
+            return update_pack_avg(p, g, st.avg.a[m.i], st.avg.mu, st.avg.first, m.rows, m.cols, st.lr, c->scalars, img,
+                                   c->keep_clipped, s, pdl_smem);
+        case UpdateStep::kAdam:
+            return update_pack_adam(p, g, st.adam.m[m.i], st.adam.v[m.i], st.adam.k, m.rows, m.cols, c->scalars, img,
+                                    c->keep_clipped, s, pdl_smem);
+        case UpdateStep::kDyn:
+            return update_pack_dyn(p, g, st.tg[m.i], st.r[m.i], m.rows, m.cols, st.dyn, img, s);
+        case UpdateStep::kSwap:
+            return swap_pack(p, st.avg.a[m.i], m.rows, m.cols, img, s);
+    }
+    return ZRB_E_INVALID;
 }
 
 // apply deferred update item `item` (see zrb_tc_state::upd_pending); pdl_smem > 0: as a programmatic dependent of the
@@ -437,10 +434,8 @@ static int tc_issue_update(zrb_ctx* c, int item, int pdl_smem, cudaStream_t s) {
     zrb_tc_state* t = c->tc;
     if (!(t->upd_pending & (1u << item))) return ZRB_OK;
     t->upd_pending &= ~(1u << item);
-    const AvgStep* avg = t->upd_avg_on ? &t->upd_avg : nullptr;
-    const AdamStep* adam = t->upd_adam_on ? &t->upd_adam : nullptr;
     for (const WeightMatrix& m : tc_matrices(c))
-        if (m.item == item) ZRB_TRY(tc_update_matrix(c, m, t->upd_tl, t->upd_lr, avg, adam, pdl_smem, s));
+        if (m.item == item) ZRB_TRY(tc_update_matrix(c, m, t->upd, pdl_smem, s));
     return ZRB_OK;
 }
 
@@ -500,7 +495,7 @@ int tc_forward(zrb_ctx* c, const zrb_params* p, const int64_t* x, const zrb_stat
         // recurrence, before the projection reads fc_w_h
         const bool through = ride && c->tied && (t->upd_pending & (1u << L));
         ZRB_TRY(embed_dropout_fwd(p->embed_w, x, nullptr, t->x_h[0], t->Xp[0], N, c->width[0], V, site_mask(c, 0), ed_mask(c), s,
-                                  through ? t->upd_tl.g[tc_matrices(c).fc_w().i] : nullptr, t->upd_lr, c->scalars));
+                                  through ? t->upd.tl.g[tc_matrices(c).fc_w().i] : nullptr, t->upd.lr, c->scalars));
     }
     for (int l = 0; l < L; ++l) {
         const int In = c->width[l], H = c->width[l + 1], Xi = t->Xp[l], Hp = t->Xp[l + 1];
@@ -1005,113 +1000,61 @@ int tc_rec_trace(zrb_ctx* c, long long* h_out, int max_entries) {
     return n;
 }
 
-// clip + SGD (main.py:114-117).  The update pass also writes the fp16 operand images of the new weights,
-// so the next forward needs no pack pass.  avg (or null): iterate averaging, every tensor's new value averaged into
-// avg->a[i] in the same passes (DESIGN.md section 16).  adam (or null; never with avg): Adam in place of SGD, with the
-// moments in the same passes (section 21).  Adam updates the embedding densely: its moments decay in every row.
-int tc_update(zrb_ctx* c, const zrb_params* p, const TensorList& tl, float lr, float max_norm, float* norm_out,
-              const AvgStep* avg, const AdamStep* adam, cudaStream_t s) {
+// One update: the train step's clip + SGD (main.py:114-117), SGD with iterate averaging (every tensor's new value
+// averaged in the same passes, DESIGN.md section 16) or Adam (the moments in the same passes, section 21); the
+// dynamic-evaluation update (section 14); or the exchange of the weights with their average (section 16).  The
+// matrices' passes also write the fp16 operand images of the new weights, so the next forward needs no pack pass.
+// Adam updates the embedding densely: its moments decay in every row.  Only a train step's update is deferred.
+int tc_apply_update(zrb_ctx* c, const zrb_params* p, const UpdateStep& st, float max_norm, float* norm_out,
+                    cudaStream_t s) {
     zrb_tc_state* t = c->tc;
+    const TensorList& tl = st.tl;
     const int E = c->width[0], V = c->cfg.vocab, L = c->cfg.layers;
+    const bool adam = st.kind == UpdateStep::kAdam;
     ZRB_TRY(tc_flush_updates(c, s));   // (a second update without a forward in between)
-    ProfScope ps(c, ZRB_PROF_CLIP_SGD, s);
-    if (!tc_streams_aligned(tl, avg ? avg->a : adam ? adam->m : nullptr, adam ? adam->v : nullptr)) {
-        // images rebuilt by the next forward's pack
-        if (adam) {
-            ZRB_TRY(grad_norm(tl, max_norm, c->partials, c->scalars, norm_out, s));
-            ZRB_TRY(adam_apply(tl, *adam, c->scalars, c->keep_clipped, s));
-        } else if (avg) {
-            ZRB_TRY(grad_norm(tl, max_norm, c->partials, c->scalars, norm_out, s));
-            ZRB_TRY(sgd_avg_apply(tl, avg->a, lr, c->scalars, c->keep_clipped, avg->mu, avg->first, s));
+    ProfScope ps(c, st.kind == UpdateStep::kSwap ? ZRB_PROF_PACK : ZRB_PROF_CLIP_SGD, s);
+    TensorList rest = tc_without_matrices(c, tl);   // what the list kernel updates
+    bool lazy = false;
+    if (st.train()) {
+        // rows_only: only the embedding rows of the last window can be non-zero -> norm and update over those rows
+        const bool rows_only = !c->tied && c->emb_sparse && c->emb_prev_grad == tl.g[0] && c->emb_prev_n > 0;
+        // gemm_norm: the matrices' sums of squares are in the wgrad epilogue slots: no read of their gradients
+        const bool gemm_norm = t->wg_ok && t->wg_key == tl.g[tc_matrices(c).fc_w().i];
+        if (rows_only && !adam) rest.n[0] = 0;
+        TensorList dense = gemm_norm ? rest : tl;   // what the norm reads
+        if (rows_only) dense.n[0] = 0;
+        if (c->tied && gemm_norm) {
+            // E's slots describe G_proj; the extra slots hold the merge's correction to dE (tc_backward_layer)
+            ZRB_TRY(grad_norm(dense, max_norm, c->partials, c->scalars, norm_out, s, true, t->wg_slots));
+        } else if (rows_only) {
+            ZRB_TRY(embed_first_table(c->emb_prev_ids, c->emb_first, c->emb_prev_n, V, s));
+            ZRB_TRY(embed_rows_sumsq(tl.g[0], c->emb_prev_ids, c->emb_first, c->emb_prev_n, E, V,
+                                     c->partials + norm_partials_base(), kNormExtra, s));   // one token per block
+            ZRB_TRY(grad_norm(dense, max_norm, c->partials, c->scalars, norm_out, s, true, gemm_norm ? t->wg_slots : 0));
+            if (!adam)
+                ZRB_TRY(embed_rows_update(tl.p[0], tl.g[0], c->emb_prev_ids, c->emb_first, c->emb_prev_n, E, V, st.lr,
+                                          c->scalars, c->keep_clipped, s));
+            if (st.kind == UpdateStep::kSgdAvg) {   // the average is dense: every row moves toward the new embedding
+                TensorList e{};
+                e.p[0] = tl.p[0]; e.n[0] = tl.n[0]; e.count = 1;
+                ZRB_TRY(avg_apply(e, st.avg.a, st.avg.mu, st.avg.first, s));
+            }
         } else {
-            ZRB_TRY(clip_sgd(tl, lr, max_norm, c->partials, c->scalars, norm_out, c->keep_clipped, s));
+            ZRB_TRY(grad_norm(tl, max_norm, c->partials, c->scalars, norm_out, s));
         }
-        c->weights_version++;
-        return ZRB_OK;
-    }
-    // rows_only: only the embedding rows of the last window can be non-zero -> norm and update over those rows
-    const bool rows_only = !c->tied && c->emb_sparse && c->emb_prev_grad == tl.g[0] && c->emb_prev_n > 0;
-    // gemm_norm: the matrices' sums of squares are in the wgrad epilogue slots: no read of their gradients
-    const bool gemm_norm = t->wg_ok && t->wg_key == tl.g[tc_matrices(c).fc_w().i];
-    TensorList rest = tc_without_matrices(c, tl);   // what the list kernel updates ...
-    if (rows_only && !adam) rest.n[0] = 0;
-    TensorList dense = gemm_norm ? rest : tl;       // ... and what the norm reads
-    if (rows_only) dense.n[0] = 0;
-    if (c->tied && gemm_norm) {
-        // E's slots describe G_proj; the extra slots hold the merge's correction to dE (tc_backward_layer)
-        ZRB_TRY(grad_norm(dense, max_norm, c->partials, c->scalars, norm_out, s, true, t->wg_slots));
-    } else if (rows_only) {
-        ZRB_TRY(embed_first_table(c->emb_prev_ids, c->emb_first, c->emb_prev_n, V, s));
-        ZRB_TRY(embed_rows_sumsq(tl.g[0], c->emb_prev_ids, c->emb_first, c->emb_prev_n, E, V,
-                                 c->partials + norm_partials_base(), kNormExtra, s));   // one token per block
-        ZRB_TRY(grad_norm(dense, max_norm, c->partials, c->scalars, norm_out, s, true, gemm_norm ? t->wg_slots : 0));
-        if (!adam)
-            ZRB_TRY(embed_rows_update(tl.p[0], tl.g[0], c->emb_prev_ids, c->emb_first, c->emb_prev_n, E, V, lr,
-                                      c->scalars, c->keep_clipped, s));
-        if (avg) {   // the average is dense: every row moves toward the new embedding
-            TensorList e{};
-            e.p[0] = tl.p[0]; e.n[0] = tl.n[0]; e.count = 1;
-            ZRB_TRY(avg_apply(e, avg->a, avg->mu, avg->first, s));
-        }
-    } else {
-        ZRB_TRY(grad_norm(tl, max_norm, c->partials, c->scalars, norm_out, s));
-    }
-    // lazy update: layer 0 (needed by the very next kernels) now; layers >= 1 and fc.W beside the forward recurrences of
-    // the next step (tc_forward), or at the next call that is not a fused train step (tc_flush_updates)
-    const bool lazy = c->lazy_update && t->persistent() && pdl_beside_rec(c);
-    if (lazy) {
-        t->upd_tl = tl;
-        t->upd_lr = lr;
-        t->upd_avg_on = avg != nullptr;
-        if (avg) t->upd_avg = *avg;
-        t->upd_adam_on = adam != nullptr;
-        if (adam) t->upd_adam = *adam;
+        // lazy update: layer 0 (needed by the very next kernels) now; layers >= 1 and fc.W beside the forward
+        // recurrences of the next step (tc_forward), or at the next call that is not a fused train step
+        // (tc_flush_updates)
+        lazy = c->lazy_update && t->persistent() && pdl_beside_rec(c);
+        if (lazy) t->upd = st;
     }
     for (const WeightMatrix& m : tc_matrices(c)) {
         // a tied E under Adam is never deferred: the next forward's gather through a pending update (tc_forward) knows
         // only the SGD rule
         if (lazy && m.item >= 1 && !(adam && c->tied && m.item == L)) t->upd_pending |= 1u << m.item;
-        else ZRB_TRY(tc_update_matrix(c, m, tl, lr, avg, adam, 0, s));
+        else ZRB_TRY(tc_update_matrix(c, m, st, 0, s));
     }
-    if (adam) ZRB_TRY(adam_apply(rest, *adam, c->scalars, c->keep_clipped, s));
-    else if (avg) ZRB_TRY(sgd_avg_apply(rest, avg->a, lr, c->scalars, c->keep_clipped, avg->mu, avg->first, s));
-    else ZRB_TRY(sgd_apply(rest, lr, c->scalars, c->keep_clipped, s));
-    tc_images_current(c, p);
-    return ZRB_OK;
-}
-
-// The dynamic-evaluation update (DESIGN.md section 14): tc_update's schedule with the dynamic rule, no norm and no lazy
-// deferral.  tg / r: theta_g and the RMS statistic in param_list() order (r null: the SGD rule).  The W_hh images then
-// hold the raw weights: evaluation applies no weight drop.
-int tc_dyneval_update(zrb_ctx* c, const zrb_params* p, const TensorList& tl, float* const* tg, float* const* r,
-                      const DynArgs& a, cudaStream_t s) {
-    ZRB_TRY(tc_flush_updates(c, s));
-    ProfScope ps(c, ZRB_PROF_CLIP_SGD, s);
-    if (!tc_streams_aligned(tl, tg, r)) {   // images rebuilt by the next forward's pack
-        ZRB_TRY(dyneval_apply(tl, tg, r, a, s));
-        c->weights_version++;
-        return ZRB_OK;
-    }
-    for (const WeightMatrix& m : tc_matrices(c))
-        ZRB_TRY(update_pack_dyn(tl.p[m.i], tl.g[m.i], tg[m.i], r ? r[m.i] : nullptr, m.rows, m.cols, a,
-                                tc_images(c, m, {}), s));
-    ZRB_TRY(dyneval_apply(tc_without_matrices(c, tl), tg, r, a, s));
-    tc_images_current(c, p);
-    return ZRB_OK;
-}
-
-// Exchange the weights with their average (DESIGN.md section 16), tl = param_list() over p, a = the averages in its
-// order.  The W_hh images then hold the raw weights, as after the dynamic-evaluation update.
-int tc_swap_average(zrb_ctx* c, const zrb_params* p, const TensorList& tl, float* const* a, cudaStream_t s) {
-    ZRB_TRY(tc_flush_updates(c, s));
-    ProfScope ps(c, ZRB_PROF_PACK, s);
-    if (!tc_streams_aligned(tl, a)) {   // images rebuilt by the next forward's pack
-        ZRB_TRY(swap_apply(tl, a, s));
-        c->weights_version++;
-        return ZRB_OK;
-    }
-    for (const WeightMatrix& m : tc_matrices(c)) ZRB_TRY(swap_pack(tl.p[m.i], a[m.i], m.rows, m.cols, tc_images(c, m, {}), s));
-    ZRB_TRY(swap_apply(tc_without_matrices(c, tl), a, s));
+    ZRB_TRY(update_list(c, st, rest, s));
     tc_images_current(c, p);
     return ZRB_OK;
 }

@@ -127,6 +127,22 @@ struct AdamStep {
 // when write_g
 int adam_apply(const TensorList& tl, const AdamStep& a, const float* scalars, bool write_g, cudaStream_t s);
 
+// ---- one update of the parameters: its rule and that rule's per-step constants ----------------------------------------
+struct UpdateStep {
+    // the train-step rules (clip + SGD, SGD with iterate averaging, Adam), dynamic evaluation (section 14), and the
+    // exchange of the weights with their average (section 16)
+    enum Kind { kSgd, kSgdAvg, kAdam, kDyn, kSwap } kind = kSgd;
+    TensorList tl{};                 // param_list() over the parameters and their gradients (kSwap: g unused)
+    float lr = 0.f;                  // train kinds (Adam's is in adam.k.step_size)
+    AvgStep avg{};                   // kSgdAvg; kSwap: avg.a, the averages exchanged with the parameters
+    AdamStep adam{};                 // kAdam
+    float* tg[kMaxTensors] = {};     // kDyn: theta_g, and the RMS statistic r (all null under the SGD rule)
+    float* r[kMaxTensors] = {};
+    DynArgs dyn{};
+    // a train-step kind takes the clip norm first, writes g back under keep_clipped and may be deferred (lazy update)
+    bool train() const { return kind <= kAdam; }
+};
+
 // ---- sample.cu ---------------------------------------------------------------------------
 // ZRB_E_INVALID for the arguments zrb_sample rejects (checked before anything is enqueued)
 int sample_check(const zrb_sampling* cfg, int B, int V);
