@@ -58,7 +58,7 @@ LAYER_TOL = dict(fwd=2e-3, grad=1.6e-3, l2=9e-4)
 # (|dz| ~ 2^-12 |z|, and |z| is ten times init's); the activations are isolated by ACT_TOL below.
 SAT_TOL = dict(fwd=4e-2, grad=2.6e-2, l2=1.2e-2)
 # the forward against an oracle fed the same fp16-rounded operands and the device's own h_{t-1} (R.rounded_operand_fwd):
-# what remains is fp32 accumulation, which grows with H, and the activation functions (SFU fast_sigmoid / fast_tanh in
+# what remains is fp32 accumulation, which grows with H, and the activation functions (lstm_cell.cuh: the SFU FastAct in
 # the persistent kernels, expf / tanhf in the per-timestep path), with pre-activations up to |z| = 122.  Measured y
 # (absolute) <= 3.3e-8 * H over every case (1.2e-7 at H = 40, 4.1e-5 at H = 1500), c_T <= 1.5e-6 of max(|c|, 1)
 ACT_TOL_PER_H = 1e-7
@@ -249,7 +249,7 @@ def _saturated(H, T, B, seed):
     b_ih, b_hh = rng.normal(size=4 * H), np.zeros(4 * H)
     b_hh[H:2 * H] = 4.0
     # planted units: every gate of PLANTED units driven to |z| in 48..92, where __expf overflows or its result exceeds
-    # 2^126 (the large-denominator rule of __fdividef) in fast_sigmoid / fast_tanh
+    # 2^126 (the large-denominator rule of __fdividef) in FastAct's sigmoid / tanh (lstm_cell.cuh)
     j = rng.choice(H, size=min(PLANTED, H), replace=False)
     for k in range(4):
         b_ih[k * H + j] = rng.choice([-1.0, 1.0], size=j.size) * rng.uniform(48.0, 92.0, size=j.size)

@@ -182,7 +182,8 @@ __device__ inline float mask_mul1(const MaskSrc& m, uint64_t e, uint64_t n_total
     return mask_mul1_at(m, mask_elem(m, e), n_total);
 }
 
-__device__ inline float sigmoidf_(float z) { return 1.f / (1.f + expf(-z)); }
+// fp16 of v, saturated at +-65504 instead of overflowing to inf (the scaled gradient images)
+__device__ __forceinline__ __half f16_sat(float v) { return __float2half_rn(fminf(fmaxf(v, -65504.f), 65504.f)); }
 
 // one SGD element (main.py:117) with the clipped gradient g = coef * grad: the ONE expression update_pack stores and the
 // tied embedding's gather through a deferred update reads, so that the two agree bit for bit

@@ -1,6 +1,7 @@
 // The persistent backward recurrence kernel (see lstm_rec_bwd.cu for the flow), included by the sources that
 // instantiate it: lstm_rec_bwd.cu (the mode off) and lstm_rec_zoneout.cu (zoneout, DESIGN.md section 20).
 #pragma once
+#include "lstm_cell.cuh"
 #include "rec_common.cuh"
 
 namespace zrb {
@@ -27,9 +28,9 @@ __device__ __forceinline__ void cluster_sync_all() {
 //        r = 2*gate + half multiplies only HALF of its gate's rows: 47 K steps per step instead of 94, half the operand
 //        image to fetch.
 // Both push their CS partial products (st.async) into the owners' shared memory, where they are summed in fixed order.
-// ZO: zoneout (DESIGN.md section 20): tanh of c~_t (the forward's store), dh~ = (1 - zh) dh, dc~ = (1 - zc) dc +
-// dh~ o (1 - tanh^2 c~), and the carries dc <- zc dc + f dc~ and hcarry <- zh dh in registers; hcarry joins dh with the upstream gradient in the
-// prefetch, so that it holds no register across the waits.  Under `if constexpr` like the forward's.
+// ZO: zoneout (DESIGN.md section 20): the cell rule (lstm_cell.cuh) reads c~_t (the forward's store) and keeps the carries
+// dc and hcarry in registers; hcarry joins dh with the upstream gradient in the prefetch, so that it holds no register
+// across the waits.  Under `if constexpr` like the forward's.
 template <int S, bool ZO>
 __global__ void __launch_bounds__(kRecThreads, 1) lstm_rec_bwd_kernel(RecBwdArgs a) {
     constexpr int CS = 4 * S;   // cluster size
@@ -175,7 +176,7 @@ __global__ void __launch_bounds__(kRecThreads, 1) lstm_rec_bwd_kernel(RecBwdArgs
         for (int k = 0; k < kRecMaxCell; ++k) {
             cb[k] = (tid + kRecEpiThreads * k) / a.U;
             dcreg[k] = 0.f;
-            if constexpr (ZO) hcarry[k] = 0.f;
+            hcarry[k] = 0.f;
 #pragma unroll
             for (int q = 0; q < 4; ++q) bsum[k][q] = 0.f;
         }
@@ -239,40 +240,16 @@ __global__ void __launch_bounds__(kRecThreads, 1) lstm_rec_bwd_kernel(RecBwdArgs
                     if constexpr (S == 2) r += (pp[4] + pp[5]) + (pp[6] + pp[7]);
                     dh += r * inv;
                 }
-                if constexpr (ZO) {
-                    const float dht = a.zo.flags ? (((zbits >> (2 * k)) & 2u) ? 0.f : dh) : __fmul_rn(a.zo.eh1, dh);
-                    hcarry[k] = a.zo.flags ? (((zbits >> (2 * k)) & 2u) ? dh : 0.f) : __fmul_rn(a.zo.eh, dh);
-                    dh = dht;
-                }
-                const float tc = fast_tanh(ct[k]);
-                const float d_o = dh * tc;
-                float dcc;
-                if constexpr (ZO) {   // dc~: the carried dc times (1 - zc), plus the h~ path (h~ reads c~)
-                    const float dt = __fmul_rn(__fmul_rn(dh, go[k]), __fsub_rn(1.f, __fmul_rn(tc, tc)));
-                    const bool kc = ((zbits >> (2 * k)) & 1u) != 0;
-                    dcc = a.zo.flags ? (kc ? dt : __fadd_rn(dcreg[k], dt)) : __fmaf_rn(a.zo.ec1, dcreg[k], dt);
-                } else {
-                    dcc = dcreg[k] + dh * go[k] * (1.f - tc * tc);
-                }
-                const float d_i = dcc * gg[k], d_g = dcc * gi[k], d_f = dcc * cp[k];
-                if constexpr (ZO)
-                    dcreg[k] = a.zo.flags ? (((zbits >> (2 * k)) & 1u) ? __fmaf_rn(dcc, gf[k], dcreg[k]) : __fmul_rn(dcc, gf[k]))
-                                          : __fmaf_rn(a.zo.ec, dcreg[k], __fmul_rn(dcc, gf[k]));
-                else
-                    dcreg[k] = dcc * gf[k];
-                float dg4[4];
-                dg4[0] = d_i * gi[k] * (1.f - gi[k]);
-                dg4[1] = d_f * gf[k] * (1.f - gf[k]);
-                dg4[2] = d_g * (1.f - gg[k] * gg[k]);
-                dg4[3] = d_o * go[k] * (1.f - go[k]);
+                const CellGrad d = cell_bwd<FastAct, ZO>(gi[k], gf[k], gg[k], go[k], ct[k], cp[k], dh, dcreg[k], hcarry[k],
+                                                          (zbits >> (2 * k)) & 1u, (zbits >> (2 * k)) & 2u, a.zo);
+                const float dg4[4] = {d.i, d.f, d.g, d.o};
                 const int j = j0 + u;
                 // critical path: the four gate images the next step multiplies with
                 __half* img = a.g_img + (size_t)(t & 1) * 4 * img_gate + ((size_t)(j >> 3) * a.GBi + (b >> 3)) * 64 +
                               (b & 7) * 8 + (j & 7);
 #pragma unroll
                 for (int q = 0; q < 4; ++q) {
-                    float v = fminf(fmaxf(dg4[q] * kGradScale, -65504.f), 65504.f);
-                    hv[k][q] = __float2half_rn(v);
+                    hv[k][q] = f16_sat(dg4[q] * kGradScale);
                     img[(size_t)q * img_gate] = hv[k][q];
                     bsum[k][q] += dg4[q];
                 }

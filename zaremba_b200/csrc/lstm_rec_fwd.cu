@@ -19,7 +19,7 @@
 //   MMA warpgroup   H/16 wgmma m64nNk16 (N = pad8(B)) chained into register accumulators, then each
 //                   accumulator row is staged in shared memory (rec_common.cuh: rec_mma_step)
 //   8 epilogue warps add the x-part pre-activations prefetched during the MMAs to the staged rows,
-//                   apply sigmoid/tanh/cell update/dropout (variational mode: the operand image holds h * rm, rm
+//                   apply the cell rule (lstm_cell.cuh) and dropout (variational mode: the operand image holds h * rm, rm
 //                   the cell's recurrent multiplier drawn once before the step loop and kept in a register).
 //                   The next step's operand image is stored FIRST and published (one red.release.gpu on the grid-barrier counter, which is never reset:
 //                   the launch gets its starting value); everything backward needs (activated gates, c_t,

@@ -1,6 +1,7 @@
 // The persistent forward recurrence kernel (see lstm_rec_fwd.cu for the flow), included by the sources that
 // instantiate it: lstm_rec_fwd.cu (the mode off) and lstm_rec_zoneout.cu (zoneout, DESIGN.md section 20).
 #pragma once
+#include "lstm_cell.cuh"
 #include "rec_common.cuh"
 
 namespace zrb {
@@ -156,7 +157,7 @@ __global__ void __launch_bounds__(kRecThreads, 1) lstm_rec_fwd_kernel(RecFwdArgs
         const uint64_t n_total = (uint64_t)a.T * B * H;
         int cb[kRecMaxCell];   // rec_cell
         float creg[kRecMaxCell];
-        float hreg[kRecMaxCell];   // (ZO only)
+        float hreg[kRecMaxCell];   // (ZO only; 0 and unused otherwise)
         // the cell's mask multipliers held fixed over the window, drawn once here (variational mode; else 1 and unused):
         // recurrent rm on the next step's operand, ym on the output when the output site's mask has a period
         float rm[kRecMaxCell], ym[kRecMaxCell];
@@ -166,7 +167,7 @@ __global__ void __launch_bounds__(kRecThreads, 1) lstm_rec_fwd_kernel(RecFwdArgs
             cb[k] = (tid + kRecEpiThreads * k) / a.U;
             const auto [b, u, ok] = rec_cell(tid, k, cb[k], a.U, cells, nu);
             creg[k] = ok ? a.c0[(size_t)b * H + j0 + u] : 0.f;
-            if constexpr (ZO) hreg[k] = ok ? a.h0[(size_t)b * H + j0 + u] : 0.f;
+            hreg[k] = ZO && ok ? a.h0[(size_t)b * H + j0 + u] : 0.f;
             const uint64_t e = (uint64_t)b * H + j0 + u;
             rm[k] = ok ? mask_mul1_at(a.rm, e, bh) : 1.f;
             ym[k] = ok && a.m.period ? mask_mul1_at(a.m, e, bh) : 1.f;
@@ -220,26 +221,18 @@ __global__ void __launch_bounds__(kRecThreads, 1) lstm_rec_fwd_kernel(RecFwdArgs
                     zg = pre[k][2] + (r0[2 * gs] + r1[2 * gs]);
                     zo = pre[k][3] + (r0[3 * gs] + r1[3 * gs]);
                 }
-                float gi = fast_sigmoid(zi), gf = fast_sigmoid(zf), gg = fast_tanh(zg), go = fast_sigmoid(zo);
-                float c = gf * creg[k] + gi * gg;
-                float h = go * fast_tanh(c);
+                const CellFwd cf = cell_fwd<FastAct, ZO>(zi, zf, zg, zo, creg[k], hreg[k], (zbits >> (2 * k)) & 1u,
+                                                          (zbits >> (2 * k)) & 2u, a.zo);
                 if constexpr (ZO) {
-                    a.ctil[((size_t)t * B + b) * H + j0 + u] = c;
-                    if (a.zo.flags) {   // a select: no scaling, no rounding
-                        if ((zbits >> (2 * k)) & 1u) c = creg[k];
-                        if ((zbits >> (2 * k)) & 2u) h = hreg[k];
-                    } else {            // the expectation
-                        c = __fmaf_rn(a.zo.ec, creg[k], __fmul_rn(a.zo.ec1, c));
-                        h = __fmaf_rn(a.zo.eh, hreg[k], __fmul_rn(a.zo.eh1, h));
-                    }
-                    hreg[k] = h;
+                    a.ctil[((size_t)t * B + b) * H + j0 + u] = cf.ctil;
+                    hreg[k] = cf.h;
                 }
-                creg[k] = c;
-                o_i[k] = gi; o_f[k] = gf; o_g[k] = gg; o_o[k] = go; o_h[k] = h;
+                creg[k] = cf.c;
+                o_i[k] = cf.i; o_f[k] = cf.f; o_g[k] = cf.g; o_o[k] = cf.o; o_h[k] = cf.h;
                 // critical path: the next step's operand image [kc][g][r][e], kc = j/8, e = j%8, g = b/8, r = b%8
                 const int j = j0 + u;
                 __half* img = a.h_img + (size_t)(t + 1) * ((size_t)a.Kc * a.GBi * 64);
-                img[((size_t)(j >> 3) * a.GBi + (b >> 3)) * 64 + (b & 7) * 8 + (j & 7)] = __float2half_rn(h * rm[k]);
+                img[((size_t)(j >> 3) * a.GBi + (b >> 3)) * 64 + (b & 7) * 8 + (j & 7)] = __float2half_rn(cf.h * rm[k]);
             }
             if (tr && tid == 0) trs[t * 8 + 5] = clock64();
             asm volatile("bar.sync 1, 256;" ::: "memory");

@@ -18,18 +18,14 @@ __global__ void convert_pad_kernel(const float* __restrict__ src, int64_t ld_src
             mask_mul4_at(m, (uint64_t)r * ld_src + c0, mul);
 #pragma unroll
             for (int k = 0; k < 4; ++k) {
-                float v = c0 + k < cols ? src[(int64_t)r * ld_src + c0 + k] * mul[k] * scale : 0.f;
-                v = fminf(fmaxf(v, -65504.f), 65504.f);
-                dst[i + k] = __float2half_rn(v);
+                dst[i + k] = f16_sat(c0 + k < cols ? src[(int64_t)r * ld_src + c0 + k] * mul[k] * scale : 0.f);
             }
         }
         return;
     }
     for (; i < total; i += (int64_t)gridDim.x * blockDim.x) {
         int r = (int)(i / ld_dst), c = (int)(i % ld_dst);
-        float v = c < cols ? src[(int64_t)r * ld_src + c] * scale : 0.f;
-        v = fminf(fmaxf(v, -65504.f), 65504.f);
-        dst[i] = __float2half_rn(v);
+        dst[i] = f16_sat(c < cols ? src[(int64_t)r * ld_src + c] * scale : 0.f);
     }
 }
 

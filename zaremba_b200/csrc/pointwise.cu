@@ -2,6 +2,7 @@
 // math (validation engine), bias/column sums, softmax-NLL.  Coalesced row-major access;
 // no tensor-core work here.
 #include "kernels.h"
+#include "lstm_cell.cuh"
 
 namespace zrb {
 
@@ -102,7 +103,7 @@ int embed_dropout_bwd(const float* dA, const int64_t* idx, float* dW, int N, int
 }
 
 // ----------------------------------------------------------------------------------------
-// LSTM cell pointwise (validation engine).  model.py:37-45 in nn.LSTM's (i,f,g,o) order.
+// LSTM cell pointwise (validation engine): the cell rule of lstm_cell.cuh with expf / tanhf.
 // ----------------------------------------------------------------------------------------
 __global__ void lstm_cell_fwd_kernel(float* __restrict__ pre, const float* __restrict__ c_prev,
                                      float* __restrict__ c_out, float* __restrict__ h_raw, float* __restrict__ y_out,
@@ -112,17 +113,13 @@ __global__ void lstm_cell_fwd_kernel(float* __restrict__ pre, const float* __res
     if (tid >= (int64_t)B * H) return;
     int b = (int)(tid / H), j = (int)(tid % H);
     float* row = pre + (int64_t)b * 4 * H;
-    float i = sigmoidf_(row[j]);
-    float f = sigmoidf_(row[H + j]);
-    float g = tanhf(row[2 * H + j]);
-    float o = sigmoidf_(row[3 * H + j]);
-    float c = f * c_prev[tid] + i * g;
-    float h = o * tanhf(c);
-    row[j] = i; row[H + j] = f; row[2 * H + j] = g; row[3 * H + j] = o;
-    c_out[tid] = c;
-    h_raw[tid] = h;
-    y_out[tid] = h * mask_mul1(m, (uint64_t)(elem_off + tid), (uint64_t)n_total);
-    if (h_rec) h_rec[tid] = h * mask_mul1_at(rm, (uint64_t)tid, (uint64_t)B * H);   // the next step's recurrent operand
+    const CellFwd cf = cell_fwd<PreciseAct, false>(row[j], row[H + j], row[2 * H + j], row[3 * H + j], c_prev[tid], 0.f,
+                                                   false, false, ZoneoutSrc{});
+    row[j] = cf.i; row[H + j] = cf.f; row[2 * H + j] = cf.g; row[3 * H + j] = cf.o;
+    c_out[tid] = cf.c;
+    h_raw[tid] = cf.h;
+    y_out[tid] = cf.h * mask_mul1(m, (uint64_t)(elem_off + tid), (uint64_t)n_total);
+    if (h_rec) h_rec[tid] = cf.h * mask_mul1_at(rm, (uint64_t)tid, (uint64_t)B * H);   // the next step's recurrent operand
 }
 
 int lstm_cell_fwd(float* pre, const float* c_prev, float* c_out, float* h_raw, float* y_out, float* h_rec, int B, int H,
@@ -134,7 +131,7 @@ int lstm_cell_fwd(float* pre, const float* c_prev, float* c_out, float* h_raw, f
     return ZRB_OK;
 }
 
-// SURVEY 8a backward: dh = mask*dy + dh_rec; do = dh*tanh(c); dc += dh*o*(1-tanh^2 c); ...
+// SURVEY 8a backward: dh = mask*dy + dh_rec, then the cell rule
 __global__ void lstm_cell_bwd_kernel(const float* __restrict__ dy_post, const float* __restrict__ dh_rec,
                                      float* __restrict__ dc, const float* __restrict__ gates,
                                      const float* __restrict__ c_t, const float* __restrict__ c_prev,
@@ -144,22 +141,15 @@ __global__ void lstm_cell_bwd_kernel(const float* __restrict__ dy_post, const fl
     if (tid >= (int64_t)B * H) return;
     int b = (int)(tid / H), j = (int)(tid % H);
     const float* row = gates + (int64_t)b * 4 * H;
-    float i = row[j], f = row[H + j], g = row[2 * H + j], o = row[3 * H + j];
+    const float i = row[j], f = row[H + j], g = row[2 * H + j], o = row[3 * H + j];
     float dh = dy_post[tid] * mask_mul1(m, (uint64_t)(elem_off + tid), (uint64_t)n_total);
     if (r) dh += r[tid];
     if (dh_rec) dh += dh_rec[tid] * mask_mul1_at(rm, (uint64_t)tid, (uint64_t)B * H);
-    float tc = tanhf(c_t[tid]);
-    float d_o = dh * tc;
-    float dcc = dc[tid] + dh * o * (1.f - tc * tc);
-    float d_i = dcc * g;
-    float d_g = dcc * i;
-    float d_f = dcc * c_prev[tid];
-    dc[tid] = dcc * f;
+    float unused;
+    const CellGrad d = cell_bwd<PreciseAct, false>(i, f, g, o, c_t[tid], c_prev[tid], dh, dc[tid], unused, false, false,
+                                                   ZoneoutSrc{});
     float* drow = dG + (int64_t)b * 4 * H;
-    drow[j] = d_i * i * (1.f - i);
-    drow[H + j] = d_f * f * (1.f - f);
-    drow[2 * H + j] = d_g * (1.f - g * g);
-    drow[3 * H + j] = d_o * o * (1.f - o);
+    drow[j] = d.i; drow[H + j] = d.f; drow[2 * H + j] = d.g; drow[3 * H + j] = d.o;
 }
 
 int lstm_cell_bwd(const float* dy_post, const float* dh_rec, float* dc, const float* gates, const float* c_t,
@@ -397,7 +387,7 @@ __global__ void softmax_nll_kernel(const float* __restrict__ scores, const int64
             if (v == tgt) p -= 1.f;
             p *= gscale;
             if (drow) drow[v] = p;
-            if (hrow) hrow[v] = __float2half_rn(fminf(fmaxf(p * h_scale, -65504.f), 65504.f));
+            if (hrow) hrow[v] = f16_sat(p * h_scale);
         }
     }
 }

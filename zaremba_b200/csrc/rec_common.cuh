@@ -235,10 +235,6 @@ __device__ __forceinline__ void rec_launch_stamps(long long* slots, bool cta0, b
     atomicMax(slots + (exit ? 5 : 4), exit ? gt : -gt);
 }
 
-// sigmoid / tanh on the SFU exp path (abs error ~1e-7, far below the fp16 operand noise of this engine)
-__device__ __forceinline__ float fast_sigmoid(float x) { return __fdividef(1.f, 1.f + __expf(-x)); }
-__device__ __forceinline__ float fast_tanh(float x) { return 1.f - __fdividef(2.f, 1.f + __expf(2.f * x)); }
-
 // Publish this CTA's global writes of the step and arrive on the grid barrier: one release-RED at gpu scope
 // (the bar.sync before it made the other epilogue threads' writes visible to this thread; release is
 // cumulative).  The consumers' TMA reads are ordered by THEIR acquire + fence.proxy.async.

@@ -1,11 +1,11 @@
-// Pointwise kernels of the tensor-core engine: same math as pointwise.cu, plus the fp16 operand
+// Pointwise kernels of the tensor-core engine: the cell rule of lstm_cell.cuh, as in pointwise.cu, plus the fp16 operand
 // images the tensor-core GEMMs consume (h_t for the next step / wgrad, dropout(h_t) for the next
 // layer, scaled dG and dS).  HBM/L2-bound, fully coalesced.
-#include "tc_kernels.h"
+#include "lstm_cell.cuh"
 
 namespace zrb {
 
-// ZO: zoneout (DESIGN.md section 20), the persistent kernels' rule with h_{t-1} from h_prev and c~_t into c_til
+// ZO: zoneout (DESIGN.md section 20), with h_{t-1} from h_prev and c~_t into c_til
 template <bool ZO>
 __global__ void lstm_cell_fwd_tc_kernel(float* __restrict__ pre, const float* __restrict__ c_prev,
                                         float* __restrict__ c_out, float* __restrict__ h_raw,
@@ -16,28 +16,15 @@ __global__ void lstm_cell_fwd_tc_kernel(float* __restrict__ pre, const float* __
     if (tid >= (int64_t)B * H) return;
     int b = (int)(tid / H), j = (int)(tid % H);
     float* row = pre + (int64_t)b * 4 * H;
-    float i = sigmoidf_(row[j]);
-    float f = sigmoidf_(row[H + j]);
-    float g = tanhf(row[2 * H + j]);
-    float o = sigmoidf_(row[3 * H + j]);
-    float c = f * c_prev[tid] + i * g;
-    float h = o * tanhf(c);
-    if constexpr (ZO) {
-        c_til[tid] = c;
-        if (zo.flags) {
-            const uint32_t z = zo.flags[elem_off + tid];
-            if (z & 1u) c = c_prev[tid];
-            if (z & 2u) h = h_prev[tid];
-        } else {
-            c = __fmaf_rn(zo.ec, c_prev[tid], __fmul_rn(zo.ec1, c));
-            h = __fmaf_rn(zo.eh, h_prev[tid], __fmul_rn(zo.eh1, h));
-        }
-    }
-    row[j] = i; row[H + j] = f; row[2 * H + j] = g; row[3 * H + j] = o;
-    c_out[tid] = c;
-    h_raw[tid] = h;
-    h_raw_h[(int64_t)b * ld_h + j] = __float2half_rn(h * mask_mul1_at(rm, (uint64_t)tid, (uint64_t)B * H));   // next step's operand
-    y_h[(int64_t)b * ld_h + j] = __float2half_rn(h * mask_mul1(m, (uint64_t)(elem_off + tid), (uint64_t)n_total));
+    const uint32_t z = ZO && zo.flags ? zo.flags[elem_off + tid] : 0u;
+    const CellFwd cf = cell_fwd<PreciseAct, ZO>(row[j], row[H + j], row[2 * H + j], row[3 * H + j], c_prev[tid],
+                                                ZO ? h_prev[tid] : 0.f, z & 1u, z & 2u, zo);
+    if constexpr (ZO) c_til[tid] = cf.ctil;
+    row[j] = cf.i; row[H + j] = cf.f; row[2 * H + j] = cf.g; row[3 * H + j] = cf.o;
+    c_out[tid] = cf.c;
+    h_raw[tid] = cf.h;
+    h_raw_h[(int64_t)b * ld_h + j] = __float2half_rn(cf.h * mask_mul1_at(rm, (uint64_t)tid, (uint64_t)B * H));   // next step's operand
+    y_h[(int64_t)b * ld_h + j] = __float2half_rn(cf.h * mask_mul1(m, (uint64_t)(elem_off + tid), (uint64_t)n_total));
 }
 
 int lstm_cell_fwd_tc(float* pre, const float* c_prev, float* c_out, float* h_raw, __half* h_raw_h, __half* y_h,
@@ -55,12 +42,6 @@ int lstm_cell_fwd_tc(float* pre, const float* c_prev, float* c_out, float* h_raw
     return ZRB_OK;
 }
 
-__device__ __forceinline__ __half to_half_scaled(float v) {
-    v *= kGradScale;
-    v = fminf(fmaxf(v, -65504.f), 65504.f);
-    return __float2half_rn(v);
-}
-
 // ZO: c_t is c~_t, and hcarry [B,H] carries zh * dh from step t to step t-1 (the persistent kernel's register)
 template <bool ZO>
 __global__ void lstm_cell_bwd_tc_kernel(const float* __restrict__ dy_post, const float* __restrict__ dh_rec,
@@ -73,39 +54,20 @@ __global__ void lstm_cell_bwd_tc_kernel(const float* __restrict__ dy_post, const
     if (tid >= (int64_t)B * H) return;
     int b = (int)(tid / H), j = (int)(tid % H);
     const float* row = gates + (int64_t)b * 4 * H;
-    float i = row[j], f = row[H + j], g = row[2 * H + j], o = row[3 * H + j];
+    const float i = row[j], f = row[H + j], g = row[2 * H + j], o = row[3 * H + j];
     float dh = dy_post[tid] * mask_mul1(m, (uint64_t)(elem_off + tid), (uint64_t)n_total);
     if (r) dh += r[tid];
     if (dh_rec) dh += dh_rec[tid] * mask_mul1_at(rm, (uint64_t)tid, (uint64_t)B * H);
-    uint32_t z = 0;
-    if constexpr (ZO) {
-        dh += hcarry[tid];
-        if (zo.flags) z = zo.flags[elem_off + tid];
-        const float dht = zo.flags ? ((z & 2u) ? 0.f : dh) : __fmul_rn(zo.eh1, dh);
-        hcarry[tid] = zo.flags ? ((z & 2u) ? dh : 0.f) : __fmul_rn(zo.eh, dh);
-        dh = dht;
-    }
-    float tc = tanhf(c_t[tid]);
-    float d_o = dh * tc;
-    float dcc;
-    if constexpr (ZO) {   // dc~: the carried dc times (1 - zc), plus the h~ path (h~ reads c~)
-        const float dt = __fmul_rn(__fmul_rn(dh, o), __fsub_rn(1.f, __fmul_rn(tc, tc)));
-        dcc = zo.flags ? ((z & 1u) ? dt : __fadd_rn(dc[tid], dt)) : __fmaf_rn(zo.ec1, dc[tid], dt);
-    } else {
-        dcc = dc[tid] + dh * o * (1.f - tc * tc);
-    }
-    float d_i = dcc * g, d_g = dcc * i, d_f = dcc * c_prev[tid];
-    if constexpr (ZO)
-        dc[tid] = zo.flags ? ((z & 1u) ? __fmaf_rn(dcc, f, dc[tid]) : __fmul_rn(dcc, f))
-                           : __fmaf_rn(zo.ec, dc[tid], __fmul_rn(dcc, f));
-    else
-        dc[tid] = dcc * f;
-    float gi = d_i * i * (1.f - i), gf = d_f * f * (1.f - f), gg = d_g * (1.f - g * g), go = d_o * o * (1.f - o);
+    if constexpr (ZO) dh += hcarry[tid];
+    const uint32_t z = ZO && zo.flags ? zo.flags[elem_off + tid] : 0u;
+    float unused;
+    const CellGrad d = cell_bwd<PreciseAct, ZO>(i, f, g, o, c_t[tid], c_prev[tid], dh, dc[tid], ZO ? hcarry[tid] : unused,
+                                                z & 1u, z & 2u, zo);
     float* drow = dG + (int64_t)b * 4 * H;
-    drow[j] = gi; drow[H + j] = gf; drow[2 * H + j] = gg; drow[3 * H + j] = go;
+    drow[j] = d.i; drow[H + j] = d.f; drow[2 * H + j] = d.g; drow[3 * H + j] = d.o;
     __half* hrow = dG_h + (int64_t)b * ld_g;
-    hrow[j] = to_half_scaled(gi); hrow[H + j] = to_half_scaled(gf);
-    hrow[2 * H + j] = to_half_scaled(gg); hrow[3 * H + j] = to_half_scaled(go);
+    hrow[j] = f16_sat(d.i * kGradScale); hrow[H + j] = f16_sat(d.f * kGradScale);
+    hrow[2 * H + j] = f16_sat(d.g * kGradScale); hrow[3 * H + j] = f16_sat(d.o * kGradScale);
 }
 
 int lstm_cell_bwd_tc(const float* dy_post, const float* dh_rec, float* dc, const float* gates, const float* c_t,
